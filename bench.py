@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """bench.py — env-steps/s of the batched Simulator.step() hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--envs E] [--map M]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--envs E] [--map M] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 A "step" is one pass of the hot path over one batch: `env.step(actions)` for all E envs of the
@@ -24,7 +24,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-METRIC = "env-steps/sec (obs+reward+done) at N envs, 1/2/4/8 B200 vs CPU ref"
+METRIC = "env-steps/sec (obs+reward+done) at N envs, 1/2/4/8 H100 vs CPU ref"
 UNIT = "env-steps/s"
 
 
@@ -56,11 +56,11 @@ def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s), not measured"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -159,10 +159,42 @@ def workload_text(c):
             f"distortion={c['distortion']}, device-side auto-reset")
 
 
-def run_config(c, K, Wm, rank, world, local_rank, obs_format="hwc_uint8", sampler=None, gather=True, gather_impl="fused"):
+DUMP_OBS_BYTES = 48 << 20     # --dump-outputs: float32 observations of a seeded sample of envs
+DUMP_ENV_BYTES = 15 << 20     # reward, done and the state arrays of a seeded sample of envs (all of them up to ~100 k)
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, obs, reward, done, state):
+    """What the last timed step returned, as .npy (float32 / float64): the observations of a fixed, seeded sample of
+    envs (obs_env_index.npy says which), and reward, done and every per-env state array for every env, or for a fixed,
+    seeded sample (env_index.npy) where all envs would not fit in 64 MB."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    n = obs.shape[0]
+
+    def sample(seed, budget, bytes_per_env):
+        k = min(n, max(1, budget // bytes_per_env))
+        return np.arange(n) if k == n else np.sort(np.random.default_rng(seed).choice(n, k, replace=False))
+
+    oi = sample(0, DUMP_OBS_BYTES, 4 * int(np.prod(obs.shape[1:])))
+    ei = sample(1, DUMP_ENV_BYTES, 4 + 4 + 8 * len(state))
+    pick = lambda t, i: t[torch.as_tensor(i, device=t.device)]
+    arrays = {"obs": pick(obs, oi).float(), "obs_env_index": oi.astype(np.float64), "env_index": ei.astype(np.float64),
+              "reward": pick(reward, ei).float(), "done": pick(done, ei).float()}
+    arrays.update({f"state_{k}": pick(v, ei).double() for k, v in state.items()})
+    arrays = {k: v.cpu().numpy() if hasattr(v, "cpu") else v for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_LIMIT_BYTES, f"--dump-outputs would write {total} B"
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
+def run_config(c, K, Wm, rank, world, local_rank, obs_format="hwc_uint8", sampler=None, gather=True, gather_impl="fused",
+               dump_dir=None):
     """Device-resident arm of one workload: W warm-up steps, K timed steps (k_step_logic + render) bracketed by
     barrier + synchronize, + the end-of-rollout NCCL all-gather when world > 1.  Returns (result dict, env) —
-    the env is left alive for the caller's end-to-end arm."""
+    the env is left alive for the caller's end-to-end arm.  With `dump_dir`, what the last timed step returned is
+    written there before anything else steps the env."""
     import torch
     import torch.distributed as dist
     from gym_duckietown_b200.batched_env import BatchedDuckietownEnv
@@ -224,7 +256,7 @@ def run_config(c, K, Wm, rank, world, local_rank, obs_format="hwc_uint8", sample
     for t in range(K):
         if fg is not None and t == K - 1:
             fg.arm()                              # the rollout's last step also fills every rank's gather buffer
-        env.step(actions[Wm + t])                 # dts_step: k_step_logic (+ device auto-reset) + the render kernels
+        last = env.step(actions[Wm + t])          # dts_step: k_step_logic (+ device auto-reset) + the render kernels
     if ag is not None:
         ag.all_gather(gathered)                   # baseline: the single end-of-rollout NCCL all-gather (SURVEY 8e)
     ev1.record()
@@ -232,6 +264,8 @@ def run_config(c, K, Wm, rank, world, local_rank, obs_format="hwc_uint8", sample
     env.sim.profile(0)
     launches = env.launch_count() - launches0
     env.check()   # no frame hit a capacity limit
+    if dump_dir is not None:
+        dump_outputs(dump_dir if world == 1 else os.path.join(dump_dir, f"rank{rank}"), *last)
     raster_ms_sum, raster_frames = env.sim.profile_read()
     # per-kernel breakdown: a few extra (untimed) steps with an event at every kernel boundary
     env.sim.profile(2)
@@ -279,7 +313,9 @@ def bind_numa(local_rank):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=200,
+                    help="timed steps (>= 1) of every device-resident workload (headline and --configs); the end-to-end "
+                         "arms time max(5, min(steps, 50)) and the CPU baseline 4; every arm reports its own \"steps\"")
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="dtsim", choices=["dtsim", "reference"])
     ap.add_argument("--envs", type=int, default=4096)
@@ -300,7 +336,11 @@ def main():
     ap.add_argument("--c4-envs", type=int, default=8192)
     ap.add_argument("--gather", default="fused", choices=["fused", "nccl"],
                     help="N>1: end-of-rollout observation exchange fused into the last step's rasteriser (peer memory), or NCCL")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step of the headline workload returned to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -312,7 +352,7 @@ def main():
                 cycle=args.cycle_maps)
     config = {"workload": workload_text(head), "envs_per_gpu": E, "width": W, "height": H, "map": args.map,
               "tile_mode": "1 (one quad per road tile + analytic 8x8 lattice lighting); vs mode 0 (the literal 98 triangles, DTS_FLAG_TESSELLATE): > 1 LSB on < 1 % of the channel values, all at tile outlines (tests/test_oracle_raster.py)",
-              "l2": "obs batch written per step (%.0f MB) exceeds the 126 MB L2; no flush needed" % (E * W * H * 3 / 1e6)}
+              "l2": "obs batch written per step (%.0f MB) exceeds the 50 MB L2; no flush needed" % (E * W * H * 3 / 1e6)}
 
     if args.impl == "reference":
         # The reference's own Pyglet/OpenGL path cannot run in this image (no pyglet, GL, display,
@@ -325,7 +365,8 @@ def main():
                 "ms_per_step": 1000 * secs / k, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": "f64 logic / f32 raster / u8 obs", "data": "synthetic", "config": config, "impl": "reference",
                 "baseline_is": "C port of the reference's CPU path (oracle/), NOT the Pyglet reference itself (cannot run here)",
-                "cpu_baseline": {"value": val, "unit": UNIT, "cores": cores, "kind": "port", "sample": desc},
+                "cpu_baseline": {"value": val, "unit": UNIT, "cores": cores, "kind": "port", "sample": desc, "steps": k,
+                                 "warmup": w_},
                 "e2e": {"value": val, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
                 "gpu_launches": 0}
         print(json.dumps(line))
@@ -348,7 +389,8 @@ def main():
 
     # ---- device-resident arm: `value` -------------------------------------------------------------
     sampler = ClockSampler(local_rank) if rank == 0 else None
-    res, env = run_config(head, K, Wm, rank, world, local_rank, args.obs_format, sampler, gather_impl=args.gather)
+    res, env = run_config(head, K, Wm, rank, world, local_rank, args.obs_format, sampler, gather_impl=args.gather,
+                          dump_dir=args.dump_outputs)
     config["gather"] = res.get("gather")
     if args.obs_format != "hwc_uint8":
         config["obs_format"] = args.obs_format
@@ -434,13 +476,6 @@ def main():
         if world > 1:
             dist.destroy_process_group()
         return
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "render_traffic.json")
-    if os.path.exists(tp):
-        tj = json.load(open(tp))
-        if tj.get("envs") == E and tj.get("width") == W and tj.get("map") == args.map:
-            traffic = tj.get("dram_bytes_per_launch")
-    res["roofline"]["traffic"] = traffic
     line = {
         "metric": METRIC, "value": res["value"], "unit": UNIT, "n_gpus": world, "steps": K, "warmup": Wm,
         "ms_per_step": res["ms_per_step"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -455,7 +490,8 @@ def main():
         line["configs"] = extra
     if not args.no_cpu_baseline:
         val, secs, used, desc = cpu_reference_run(args.map.split(",")[0], W, H, 4, 1, args.cpu_sample_envs, cores)
-        line["cpu_baseline"] = {"value": val, "unit": UNIT, "cores": used, "kind": "port", "sample": desc}
+        line["cpu_baseline"] = {"value": val, "unit": UNIT, "cores": used, "kind": "port", "sample": desc, "steps": 4,
+                                "warmup": 1}
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()

@@ -1,4 +1,4 @@
-"""dtsim-b200: batched Duckietown `Simulator.step()` hot path as sm_100a CUDA kernels.
+"""dtsim-b200: batched Duckietown `Simulator.step()` hot path as sm_90a (H100) CUDA kernels.
 
 Public surface (mirrors gym_duckietown's, SURVEY.md 8b):
   Simulator, DuckietownEnv, MultiMapEnv      single-env gym.Env adapters (old 4-tuple API)

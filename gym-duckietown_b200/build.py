@@ -1,4 +1,4 @@
-"""Build libdtsim.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libdtsim.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python gym-duckietown_b200/build.py [--force]
 """
@@ -12,7 +12,7 @@ LIB = os.path.join(HERE, "libdtsim.so")
 SOURCES = ["dts_api.cu", "dts_kernels_logic.cu", "dts_render.cu"]
 # -fmad=false: no implicit FMA contraction, so fp32/fp64 arithmetic is exactly what the source says
 # (the render kernels spell out fmaf() where an FMA is wanted; the CPU oracle is built the same way).
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-fmad=false",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-fmad=false",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v"]
 
 

@@ -594,7 +594,7 @@ int dts_reset_random(dts_sim* sim, const uint8_t* mask_dev, void* stream) {
 
 static int ensure_render(dts_sim* sim) {
   if (sim->render_scratch) return 0;
-  int sms = 148;
+  int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, sim->cfg.device);
   const bool tess = (sim->cfg.flags & DTS_FLAG_TESSELLATE) != 0;
   int max_tris = 2, max_lat = 1, items_max = 1;

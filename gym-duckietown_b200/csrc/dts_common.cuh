@@ -1,4 +1,4 @@
-// dts_common.cuh — device-side data layout shared by the dtsim kernels (sm_100a only).
+// dts_common.cuh — device-side data layout shared by the dtsim kernels (sm_90a only).
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>

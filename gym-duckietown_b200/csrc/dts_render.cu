@@ -1,5 +1,5 @@
 // dts_render.cu — batched software rasteriser for the agent camera (Simulator._render_img,
-// simulator.py:1707-1951) on sm_100a.  No tensor cores: there is no dense contraction here.
+// simulator.py:1707-1951) on sm_90a (H100).  No tensor cores: there is no dense contraction here.
 //
 // Stream-ordered kernels per frame batch (k_cull, a work-list pre-pass for k_geometry, and k_raster_solo, the lean
 // rasteriser of coarse bins lying inside one prim, are described at their definitions):
@@ -69,9 +69,9 @@ namespace {
 #define DTS_COPLANAR 1      // fine bins whose prims are all road tiles (coplanar, disjoint) resolve visibility by coverage alone (A/B switch)
 #endif
 #ifndef DTS_COARSE_FAST
-#define DTS_COARSE_FAST 0   // 1: coarse bins lying inside one prim skip visibility and fetch the prim once.  Measured
-                            // (profiles/README.md, r2d): +5 % k_raster time — the extra code and registers cost more
-                            // than the skipped flag tests save; kept as an A/B switch only
+#define DTS_COARSE_FAST 0   // 1: coarse bins lying inside one prim skip visibility and fetch the prim once.  The extra
+                            // code and registers cost more than the skipped flag tests save (k_raster_solo does this
+                            // job instead); kept as an A/B switch only
 #endif
 constexpr int kThreads = DTS_RENDER_THREADS;
 constexpr int kWarps = kThreads / 32;
@@ -95,9 +95,8 @@ struct Vtx { float cx, cy, cz, cw, r, g, b, u, v; };
 #define DTS_GEO_INLINE 5
 #endif
 // which of the geometry pass's big device functions are inlined: bit 0 shade_vertex, bit 1 setup_and_emit, bit 2 the clipper.
-// The kernel is instruction-fetch bound (ncu: 6.9 stall_no_instruction cycles per issue, 174 KB of SASS against a 32 KB
-// L1.5 I-cache): with everything inlined setup_and_emit alone is 107 KB in a dozen copies.  Measured k_geometry at c2 / c3:
-// 7 (all inline) 198 / 466 us, 5 (one copy of setup_and_emit) 177 / 424 us, 1: 188 / 435, 3: 220 / 493, 0: 221 / 447.
+// With everything inlined setup_and_emit alone is a dozen copies of a large function, more SASS than the instruction cache
+// holds; 5 keeps one out-of-line copy of it.
 #define DTS_GEO_FN_SHADE __forceinline__
 #define DTS_GEO_FN_SETUP __forceinline__
 #define DTS_GEO_FN_CLIP __forceinline__
@@ -1923,10 +1922,18 @@ __global__ void __launch_bounds__(256) k_blend4(const uint8_t* __restrict__ f0, 
     out[i] = a / scl;
   }
 }
+// SMs of the current device: grid-stride kernels cap their grid at a multiple of it
+static size_t device_sms() {
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms > 0 ? (size_t)sms : 1;
+}
+
 void launch_blend4(const uint8_t* const f[4], const double w[4], double* out, size_t n, cudaStream_t st) {
   const double scl = ((w[0] + w[1]) + w[2]) + w[3];   // numpy: wgt.sum() of four float64 (pairwise == sequential below 8 terms)
-  const size_t blocks = (n + 255) / 256;
-  k_blend4<<<(unsigned)(blocks < 148 * 32 ? blocks : 148 * 32), 256, 0, st>>>(f[0], f[1], f[2], f[3], w[0], w[1], w[2], w[3], scl, out, n);
+  const size_t blocks = (n + 255) / 256, cap = device_sms() * 32;
+  k_blend4<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, st>>>(f[0], f[1], f[2], f[3], w[0], w[1], w[2], w[3], scl, out, n);
 }
 
 // The same resize, tiled: a CTA per (band of `R` output rows, env).  The band's source rows (contiguous bytes of the
@@ -2035,7 +2042,8 @@ void launch_resize(const uint8_t* src, int W, int H, int ow, int oh, int n_envs,
     return;
   }
   const size_t total = (size_t)n_envs * ow * oh;
-  const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const size_t cap = device_sms() * 16;
+  const int blocks = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
   k_resize<<<blocks, 256, 0, st>>>(src, W, H, ow, oh, n_envs, xtab, ytab, dst, layout, dtype);
 }
 
@@ -2099,7 +2107,7 @@ int launch_render(const DState& S, const DMap* maps, const RenderCfg& rc, void* 
   mark();
   const size_t bin_smem_bytes = (size_t)2 * cbins * sizeof(int);
   const int bin_grid = rc.n_envs;   // CTA per env: one warp where a frame has few bins and prims (160x120: 75 bins — more warps
-  // only add barriers and CTA launches, measured 58 -> 88 us), four for large cameras (640x480: 9.0 -> 3.3 ms)
+  // only add barriers and CTA launches), four for large cameras (640x480)
   static const int bin_warps_env = getenv("DTS_BIN_WARPS") ? atoi(getenv("DTS_BIN_WARPS")) : 0;   // A/B override: 1..4
   const int bin_threads = bin_warps_env >= 1 && bin_warps_env <= kBinWarps ? bin_warps_env * 32 : (cbins > 128 ? kBinWarps * 32 : 32);
   if (fisheye) {

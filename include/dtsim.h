@@ -1,4 +1,4 @@
-/* dtsim.h — C ABI of libdtsim.so, the B200-native batched Duckietown step() hot path.
+/* dtsim.h — C ABI of libdtsim.so, the H100-native batched Duckietown step() hot path.
  *
  * The reference (duckietown/gym-duckietown @5c2a586) has no FFI for this path: Simulator.step()
  * is Python all the way down to the OpenGL driver.  This header is the boundary we introduce

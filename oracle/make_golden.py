@@ -10,6 +10,7 @@ Files written
   action_map.npz       DuckietownEnv.step [vel, steer] -> wheel duty  (envs/duckietown_env.py:36-59)
   reset_<map>.npz      Simulator.reset() outputs per seed, domain_rand off/on (simulator.py:528-763)
   fisheye.npz          Distortion LUT digest, sub-sampled LUT, one remapped test image (distortion.py)
+  objmesh_prop.npz     ObjMesh's extents and vertex lists for the synthetic OBJ of tests/test_obj_loader.py (objmesh.py)
   gltrace_<map>.npz    what the reference's own _render_img / _init_vlists / WorldObj.render / reset() lighting ask
                        OpenGL to do, recorded call by call (oracle/gltrace.py): per frame the projection arguments,
                        look-at, model-view of every draw, GL_LIGHT0 (eye-space position, ambient, diffuse), current
@@ -466,6 +467,45 @@ def gen_wrappers(seed=21):
     print("wrappers:", sorted(out))
 
 
+def gen_objmesh():
+    """The reference's ObjMesh loader (objmesh.py:65-293) on the synthetic OBJ / MTL pair of tests/test_obj_loader.py
+    -> tests/golden/objmesh_prop.npz: extents and the per-triangle vertex lists it hands pyglet."""
+    import importlib.util
+    import tempfile
+    spec = importlib.util.spec_from_file_location("t_obj", os.path.join(ROOT, "tests", "test_obj_loader.py"))
+    t = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(t)
+    refstub.install()
+    import gym_duckietown.objmesh as M
+    captured = []
+
+    def vertex_list(n, *attrs):
+        captured.append({name: np.array(data, dtype=np.float32) for name, data in attrs})
+        return object()
+
+    with tempfile.TemporaryDirectory() as d:
+        with open(os.path.join(d, "prop.obj"), "w") as f:
+            f.write(t.OBJ)
+        with open(os.path.join(d, "prop.mtl"), "w") as f:
+            f.write(t.MTL)
+
+        def resource(name):
+            p = os.path.join(d, name)
+            if not os.path.exists(p):
+                raise KeyError(name)
+            return p
+
+        M.pyglet.graphics.vertex_list = vertex_list
+        M.get_resource_path = resource
+        ref = M.ObjMesh(os.path.join(d, "prop.obj"), "prop")
+    np.savez_compressed(os.path.join(OUT, "objmesh_prop.npz"), min_coords=np.asarray(ref.min_coords),
+                        max_coords=np.asarray(ref.max_coords),
+                        tri_pos=np.concatenate([c["v3f"].reshape(-1, 3, 3) for c in captured]),
+                        tri_nrm=np.concatenate([c["n3f"].reshape(-1, 3, 3) for c in captured]),
+                        tri_uv=np.concatenate([c["t2f"].reshape(-1, 3, 2) for c in captured]),
+                        tri_col=np.concatenate([c["c3f"].reshape(-1, 3, 3) for c in captured]))
+
+
 def gen_gltrace(name: str, seeds=(11, 12, 13), poses_per_episode=8, width=160, height=120):
     """Run the reference's render path against the recording GL (oracle/gltrace.py): reset() + a short walk, twice per
     seed (the second episode captures GL_LIGHT0 under the previous frame's model-view, S:581), domain_rand off and on."""
@@ -573,6 +613,10 @@ if __name__ == "__main__":
         os.makedirs(OUT, exist_ok=True)
         gen_wrappers()
         sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "objmesh":
+        os.makedirs(OUT, exist_ok=True)
+        gen_objmesh()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "gltrace":
         os.makedirs(OUT, exist_ok=True)
         for m in MAPS:
@@ -592,5 +636,6 @@ if __name__ == "__main__":
     gen_reset_custom()
     gen_helpers()
     gen_wrappers()
+    gen_objmesh()
     for m in MAPS:
         gen_gltrace(m)

@@ -24,9 +24,12 @@ def test_library_exports_every_declared_symbol():
     assert declared == set(L.EXPORTS), declared ^ set(L.EXPORTS)
     for name in declared:
         assert hasattr(lib, name), name
-    # cuobjdump: the library carries sm_100a code only
+    # cuobjdump: the library carries sm_90a code only — every embedded cubin is sm_90a, and no PTX to JIT elsewhere
     out = subprocess.run(["cuobjdump", "-lelf", path], capture_output=True, text=True).stdout
-    assert "sm_100a" in out and "sm_90" not in out
+    elfs = [l for l in out.splitlines() if l.startswith("ELF file")]
+    assert elfs and all(re.findall(r"\.(sm_\w+)\.cubin", l) == ["sm_90a"] for l in elfs), out
+    ptx = subprocess.run(["cuobjdump", "-lptx", path], capture_output=True, text=True)
+    assert not re.search(r"^PTX file\s+\d+:", ptx.stdout, re.M), ptx.stdout
 
 
 def test_ctypes_struct_layout_matches_header():

@@ -6,7 +6,6 @@ the numpy semantics the GPU tests rely on are those outputs.  GPU part (-m gpu):
 (dts_set_resize) against cv2.INTER_CUBIC as the reference wrapper called it."""
 import hashlib
 import os
-import sys
 
 import numpy as np
 import pytest
@@ -49,43 +48,6 @@ def test_reward_and_action_wrapper_semantics_are_the_reference_classes():
     assert np.array_equal(g["dt_rewards"], np.where(r == -1000, -10.0, np.where(r > 0, r + 10, r + 4)))   # DtRewardWrapper LW:94-102
     assert np.array_equal(g["scaled_actions"], g["actions"] * [0.8, 1.0])                                # ActionWrapper LW:110-112
     assert np.array_equal(g["discrete_actions"], [[0.6, 1.0], [0.6, -1.0], [0.7, 0.0]])                   # DiscreteWrapper W:18-30
-
-
-def test_unmodified_reference_wrappers_accept_the_product_env_interface():
-    """The reference's wrappers.py, imported unmodified, wraps an object with the product Simulator's spaces and
-    step/reset signature and reproduces the PyTorchObsWrapper block of run_tests.py:28-34.  (Needs /root/reference;
-    the product env itself needs a GPU, so a shape-faithful stand-in carries its declared spaces here.)"""
-    sys.path.insert(0, os.path.join(ROOT, "oracle"))
-    import refstub
-    if not refstub.reference_available():
-        pytest.skip("reference tree not present")
-    refstub.install()
-    import importlib
-    Wm = importlib.import_module("gym_duckietown.wrappers")
-    import gym_duckietown_b200.simulator as PS
-    from gym_duckietown_b200.gymshim import spaces as pspaces
-
-    class StandIn:   # the attributes gym_duckietown_b200.Simulator.__init__ sets (simulator.py), no CUDA
-        metadata, reward_range = PS.Simulator.metadata, (-1000, 1000)
-        action_space = pspaces.Box(low=-1, high=1, shape=(2,), dtype=np.float32)
-        observation_space = pspaces.Box(low=0, high=255, shape=(120, 160, 3), dtype=np.uint8)
-
-        @property
-        def unwrapped(self):
-            return self
-
-        def reset(self):
-            return np.zeros((120, 160, 3), np.uint8)
-
-        def step(self, a):
-            return np.ones((120, 160, 3), np.uint8), 0.0, False, {}
-
-    env = Wm.PyTorchObsWrapper(StandIn())
-    first = env.reset()
-    second, _, _, _ = env.step([0, 0])
-    assert first.shape == tuple(env.observation_space.shape) == second.shape == (3, 160, 120)
-    rz = Wm.ResizeWrapper(env, resize_w=84, resize_h=84)
-    assert rz.reset().shape == (3, 84, 84)
 
 
 @pytest.mark.gpu
