@@ -1,8 +1,9 @@
 // dts_render.cu — batched software rasteriser for the agent camera (Simulator._render_img,
 // simulator.py:1707-1951) on sm_90a (H100).  No tensor cores: there is no dense contraction here.
 //
-// Stream-ordered kernels per frame batch (k_cull, a work-list pre-pass for k_geometry, and k_raster_solo, the lean
-// rasteriser of coarse bins lying inside one prim, are described at their definitions):
+// Stream-ordered kernels per frame batch (k_cull, a work-list pre-pass for k_geometry, and k_raster_solo / k_raster_flat,
+// the lean rasterisers of coarse bins lying inside one prim / holding only road tiles and ground, are described at their
+// definitions):
 //   k_frame_setup  thread per env: camera matrices (f64), gluPerspective, counters -> FrameCtx[env]
 //   k_geometry     warp per (env, draw item) over the whole GPU: ground / map tile / placed mesh.  Model-view
 //                  f64->f32, fixed-function per-vertex lighting, frustum cull, near + guard-band clip, snap to
@@ -64,6 +65,9 @@ namespace {
 #endif
 #ifndef DTS_SOLO_MIN_CTAS
 #define DTS_SOLO_MIN_CTAS 3   // resident CTAs per SM of k_raster_solo (register budget 65536 / (256 * this))
+#endif
+#ifndef DTS_FLAT_MIN_CTAS
+#define DTS_FLAT_MIN_CTAS 4   // resident CTAs per SM of k_raster_flat (register budget 65536 / (256 * this))
 #endif
 #ifndef DTS_COPLANAR
 #define DTS_COPLANAR 1      // fine bins whose prims are all road tiles (coplanar, disjoint) resolve visibility by coverage alone (A/B switch)
@@ -508,7 +512,8 @@ __device__ __forceinline__ bool bin_overlaps(const int qx[4], const int qy[4], i
 // trivial-accept bits for each of the bin's 8 fine bins, depth plane, draw id.
 // With `fb` (fused fisheye) the bin's pixels are wherever the LUT sends its output pixels: (ox, oy) is the corner of
 // their source bounding box and fb[f] the source box of fine bin f; the bits then speak about every pixel of that box.
-// Returns the fine bins every sample of which the prim covers (bits 0-7) | ground quad << 8.
+// Returns the fine bins every sample of which the prim covers (bits 0-7) | ground quad << 8 | (flat road tile or ground
+// quad, and not drawn by the tiny-triangle path) << 9.
 __device__ __forceinline__ unsigned build_binrec(const PrimRec* __restrict__ pr, int p, int ox, int oy, BinRec* __restrict__ out,
                                                  const short4* __restrict__ fb = nullptr) {
   const int4 w0 = __ldg(reinterpret_cast<const int4*>(pr));
@@ -583,7 +588,7 @@ __device__ __forceinline__ unsigned build_binrec(const PrimRec* __restrict__ pr,
   o[2] = make_int4(B[0], B[1], B[2], B[3]);
   o[3] = make_int4(__float_as_int(w2.x), __float_as_int(w2.y), __float_as_int(w2.z), id);
   o[4] = make_int4(qx[0] - ox, qy[0] - oy, (int)((unsigned)p | (live << 16) | ((inside & live) << 24)), quad | (id < 2 ? 2 : 0) | tiny | flat);
-  return (inside & live) | (id < 2 ? 0x100u : 0u);
+  return (inside & live) | (id < 2 ? 0x100u : 0u) | ((flat || id < 2) && !tiny ? 0x200u : 0u);
 }
 
 // Fragment colour of prim `w` of the env's slab at the pixel whose centre is (pxa + 32, pya + 32) sub-pixels (spec steps
@@ -817,7 +822,9 @@ struct FrameMem {
   float4* lat;          // [N][max_lat][64]
   uint2* geo_list;      // [N * items_max] (env, draw item) pairs that passed k_cull
   uint2* solo;          // [N * cbins] (env, coarse bin | prim << 16): coarse bins lying inside one prim (k_bin -> k_raster_solo)
-  int* work;            // global counters: [0] k_raster work items, [1] pair-pool cursor, [2] geo_list length, [3] solo list length
+  uint2* flat;          // [N * cbins] (env, coarse bin | record count << 16): flat bins, only road tiles and ground (k_bin -> k_raster_flat)
+  int* work;            // global counters: [0] k_raster work items, [1] pair-pool cursor, [2] geo_list length, [3] solo list length,
+                        // [4] flat list length
   int32_t* status;      // mapped host word (dts_status): bit 0 = a frame ran out of frame memory
 };
 
@@ -836,6 +843,7 @@ __host__ FrameMem carve(void* scratch, int n, int max_prims, int cbins, int max_
   f.lat = reinterpret_cast<float4*>(p); p += align256((size_t)n * max_lat * 64 * sizeof(float4));
   f.geo_list = reinterpret_cast<uint2*>(p); p += align256((size_t)n * geo_items * sizeof(uint2));
   f.solo = reinterpret_cast<uint2*>(p); p += align256((size_t)n * cbins * sizeof(uint2));
+  f.flat = reinterpret_cast<uint2*>(p); p += align256((size_t)n * cbins * sizeof(uint2));
   f.status = nullptr;
   return f;
 }
@@ -845,7 +853,7 @@ size_t render_scratch_bytes(int n, int max_prims, int cbins, int max_pairs, int 
          align256((size_t)n * max_prims * sizeof(PrimRec)) + align256((size_t)max_pairs * sizeof(uint32_t)) +
          align256((size_t)max_pairs * sizeof(BinRec)) +
          align256((size_t)n * max_lat * 64 * sizeof(float4)) + align256((size_t)n * geo_items * sizeof(uint2)) +
-         align256((size_t)n * cbins * sizeof(uint2)) + 256;
+         2 * align256((size_t)n * cbins * sizeof(uint2)) + 256;
 }
 
 // ------------------------------------------------------------------------------------------------ k_frame_setup
@@ -1148,6 +1156,7 @@ k_geometry(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem
 // screen-filling prim costs no more lanes than a sliver): the pair's BinRec.
 constexpr int kBinWarps = 4;
 constexpr int kCountMask = 0xfffff, kGroundInc = 1 << 20;   // a bin's counter: records | ground-quad records << 20
+constexpr int kFlatBin = -0x7fffffff - 1;   // bin_count of a flat bin (k_raster_flat); solo bins hold -(prim + 1) >= -65536
 template <bool kFish>   // true: bins are the LUT's source boxes of the output bins (fused fisheye gather)
 __global__ void __launch_bounds__(kBinWarps * 32)
 k_bin(RenderCfg rc, FrameMem fm, FishTab ft, int max_prims, int max_pairs, int32_t* __restrict__ err) {
@@ -1292,7 +1301,15 @@ k_bin(RenderCfg rc, FrameMem fm, FishTab ft, int max_prims, int max_pairs, int32
   // pass 2: one pair per thread -> its visibility record (the pairs were written by other threads of this CTA: the
   // barrier above orders those writes before these reads)
   const int pair0 = s_base, total = s_total;
-  const bool solo_on = DTS_SOLO && rc.obs_layout == DTS_OBS_HWC && rc.obs_dtype == DTS_OBS_U8 && (W & 3) == 0;
+  const bool lean_fmt = rc.obs_layout == DTS_OBS_HWC && rc.obs_dtype == DTS_OBS_U8 && (W & 3) == 0;   // packed u8 HWC, whole-word rows
+  const bool solo_on = DTS_SOLO && lean_fmt;
+  // start[] is free from here on: per coarse bin, nonzero once a record rules the bin out of k_raster_flat (a mesh
+  // triangle, a tiny triangle, or a solo bin)
+  int* no_flat = start;
+  if (lean_fmt) {
+    for (int b = tid; b < cbins; b += nthr) no_flat[b] = 0;
+    __syncthreads();
+  }
   BinRec* recs = fm.recs;
   for (int i = pair0 + tid; i < pair0 + total; i += nthr) {
     const uint32_t pair = pairs[i];
@@ -1318,8 +1335,27 @@ k_bin(RenderCfg rc, FrameMem fm, FishTab ft, int max_prims, int max_pairs, int32
           fm.bin_count[(size_t)env * cbins + b] = -(p + 1);
           const int slot = atomicAdd(fm.work + 3, 1);
           fm.solo[slot] = make_uint2((unsigned)env, (unsigned)b | ((unsigned)p << 16));
+          atomicOr(&no_flat[b], 1);
         }
       }
+      if (lean_fmt && !(r & 0x200u)) atomicOr(&no_flat[b], 1);
+    }
+  }
+  if (!lean_fmt) return;
+  // flat bins: 1..kStage records, every one a flat road tile or the ground quad, not solo -> k_raster_flat's list, and
+  // k_raster skips them (kFlatBin) unless k_raster_flat hands one back
+  __syncthreads();
+  for (int b0 = wib * 32; b0 < cbins; b0 += nthr) {
+    const int b = b0 + lane, c = b < cbins ? (cnt[b] & kCountMask) : 0;
+    const bool flat = c >= 1 && c <= kStage && !no_flat[b];
+    const unsigned m = __ballot_sync(0xffffffffu, flat);
+    if (!m) continue;
+    int base = 0;
+    if (lane == 0) base = atomicAdd(fm.work + 4, __popc(m));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (flat) {
+      fm.bin_count[(size_t)env * cbins + b] = kFlatBin;
+      fm.flat[base + __popc(m & ((1u << lane) - 1u))] = make_uint2((unsigned)env, (unsigned)b | ((unsigned)c << 16));
     }
   }
 }
@@ -1357,6 +1393,76 @@ constexpr size_t kRasterSmem = (sizeof(BinRec) * 2 * kStage + 16 + 128 * sizeof(
 // order-preserving map of a float onto unsigned (and back): depth keys of the tiny-triangle buffer
 __device__ __forceinline__ unsigned float_key(float f) { const unsigned b = __float_as_uint(f); return b ^ ((b >> 31) ? 0xffffffffu : 0x80000000u); }
 __device__ __forceinline__ float key_float(unsigned k) { return __uint_as_float(k ^ ((k >> 31) ? 0x80000000u : 0xffffffffu)); }
+
+// The MSAA samples of the pixel at (pxc, pyc) (sub-pixels from the coarse bin corner) that record `br` covers, as bits 0-3
+__device__ __forceinline__ int sample_mask(const BinRec& br, int pxc, int pyc) {
+  const int4 E = *reinterpret_cast<const int4*>(br.E0);
+  const int4 A = *reinterpret_cast<const int4*>(br.A);
+  const int4 B = *reinterpret_cast<const int4*>(br.B);
+  const int ec0 = E.x + A.x * pxc + B.x * pyc;
+  const int ec1 = E.y + A.y * pxc + B.y * pyc;
+  const int ec2 = E.z + A.z * pxc + B.z * pyc;
+  int mask = 0;
+  if (br.kind & 1) {
+    const int ec3 = E.w + A.w * pxc + B.w * pyc;
+#pragma unroll
+    for (int s = 0; s < 4; s++) {
+      const int e0 = ec0 + A.x * sample_x(s) + B.x * sample_y(s);
+      const int e1 = ec1 + A.y * sample_x(s) + B.y * sample_y(s);
+      const int e2 = ec2 + A.z * sample_x(s) + B.z * sample_y(s);
+      const int e3 = ec3 + A.w * sample_x(s) + B.w * sample_y(s);
+      if ((e0 | e1 | e2 | e3) >= 0) mask |= 1 << s;
+    }
+  } else {
+#pragma unroll
+    for (int s = 0; s < 4; s++) {
+      const int e0 = ec0 + A.x * sample_x(s) + B.x * sample_y(s);
+      const int e1 = ec1 + A.y * sample_x(s) + B.y * sample_y(s);
+      const int e2 = ec2 + A.z * sample_x(s) + B.z * sample_y(s);
+      if ((e0 | e1 | e2) >= 0) mask |= 1 << s;
+    }
+  }
+  return mask;
+}
+
+// Deferred shading of one pixel of a fine bin whose visibility is resolved (winner prim per MSAA sample, kNoPrim = clear
+// colour): shaded once per distinct winner at the pixel centre (pxa, pya), then the box resolve -> packed u8.  `simple`:
+// the caller knows that every sample of the whole fine bin has the same winner.
+__device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool simple, const float clr[3], const PrimRec* __restrict__ prims,
+                                                  const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa,
+                                                  int pya, int lane, int32_t* __restrict__ err) {
+  (void)lane; (void)err;   // (DTS_STATS counters)
+  const bool same = wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0];
+  const bool all_same = simple || __all_sync(0xffffffffu, same);
+  float c3[3] = {clr[0], clr[1], clr[2]};
+  if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3);   // every lane: its first winner
+  if (all_same) return pack_rgb(c3[0], c3[1], c3[2]);   // four equal samples: the mean is the value itself
+  // edge pixels: the other winners of this pixel (at most three more), summed in the resolve's order
+  float s01[3] = {c3[0], c3[1], c3[2]}, s23[3] = {0.f, 0.f, 0.f};   // 0 + c == c
+  unsigned pend = 0xeu;
+  if (wn[1] == wn[0]) { pend &= ~2u; s01[0] = s01[0] + c3[0]; s01[1] = s01[1] + c3[1]; s01[2] = s01[2] + c3[2]; }
+#pragma unroll
+  for (int t = 2; t < 4; t++)
+    if (wn[t] == wn[0]) { pend &= ~(1u << t); s23[0] = s23[0] + c3[0]; s23[1] = s23[1] + c3[1]; s23[2] = s23[2] + c3[2]; }
+#pragma unroll 1
+  while (__any_sync(0xffffffffu, pend != 0u)) {
+    DTS_COUNT(12, 1);
+    if (pend) {
+      const int s = __ffs(pend) - 1;
+      const unsigned w = s == 1 ? wn[1] : (s == 2 ? wn[2] : wn[3]);
+      float d3[3] = {clr[0], clr[1], clr[2]};
+      if (w != kNoPrim) shade_prim(prims, w, tex_pool, lat_tab, pxa, pya, d3);
+#pragma unroll
+      for (int t = 1; t < 4; t++)
+        if ((pend >> t & 1u) && wn[t] == w) {
+          pend &= ~(1u << t);
+          if (t < 2) { s01[0] = s01[0] + d3[0]; s01[1] = s01[1] + d3[1]; s01[2] = s01[2] + d3[2]; }
+          else { s23[0] = s23[0] + d3[0]; s23[1] = s23[1] + d3[1]; s23[2] = s23[2] + d3[2]; }
+        }
+    }
+  }
+  return pack_rgb((s01[0] + s23[0]) * 0.25f, (s01[1] + s23[1]) * 0.25f, (s01[2] + s23[2]) * 0.25f);
+}
 
 // ------------------------------------------------------------------------------------------------ k_raster
 template <bool kWrapFmt, bool kFish>   // kWrapFmt: a dts_output_format other than packed u8 HWC is written by the resolve;
@@ -1479,7 +1585,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
     issue();
     for (int cbx = 0; cbx < cbins_x; cbx++) {
       const int count = __shfl_sync(0xffffffffu, my_cnt, cbx);
-      if (count < 0) continue;   // drawn by k_raster_solo (a bin inside one prim)
+      if (count < 0) continue;   // drawn by k_raster_solo (a bin inside one prim) or k_raster_flat (kFlatBin)
       const unsigned fvalid = valid8(cbx);
       DTS_COUNT(8, 1);
       if (count == 0) {
@@ -1625,32 +1731,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
                   if ((pflags >> (24 + f)) & 1u) DTS_COUNT(17, 1);
                   int mask = 15;
                   if (!((pflags >> (24 + f)) & 1u)) {
-                    const int4 E = *reinterpret_cast<const int4*>(br.E0);
-                    const int4 A = *reinterpret_cast<const int4*>(br.A);
-                    const int4 B = *reinterpret_cast<const int4*>(br.B);
-                    const int ec0 = E.x + A.x * pxc + B.x * pyc;
-                    const int ec1 = E.y + A.y * pxc + B.y * pyc;
-                    const int ec2 = E.z + A.z * pxc + B.z * pyc;
-                    mask = 0;
-                    if (br.kind & 1) {
-                      const int ec3 = E.w + A.w * pxc + B.w * pyc;
-#pragma unroll
-                      for (int s = 0; s < 4; s++) {
-                        const int e0 = ec0 + A.x * sample_x(s) + B.x * sample_y(s);
-                        const int e1 = ec1 + A.y * sample_x(s) + B.y * sample_y(s);
-                        const int e2 = ec2 + A.z * sample_x(s) + B.z * sample_y(s);
-                        const int e3 = ec3 + A.w * sample_x(s) + B.w * sample_y(s);
-                        if ((e0 | e1 | e2 | e3) >= 0) mask |= 1 << s;
-                      }
-                    } else {
-#pragma unroll
-                      for (int s = 0; s < 4; s++) {
-                        const int e0 = ec0 + A.x * sample_x(s) + B.x * sample_y(s);
-                        const int e1 = ec1 + A.y * sample_x(s) + B.y * sample_y(s);
-                        const int e2 = ec2 + A.z * sample_x(s) + B.z * sample_y(s);
-                        if ((e0 | e1 | e2) >= 0) mask |= 1 << s;
-                      }
-                    }
+                    mask = sample_mask(br, pxc, pyc);
                     if (!mask) continue;
                   }
                   if (coplanar && phase == 0) {
@@ -1762,42 +1843,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
             }
             // ---- deferred shading: once per distinct winner of this pixel, then the box resolve
             DTS_COUNT(11, 1);
-            const int pxa = ox + pxc, pya = oy + pyc;
-            const bool same = wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0];
-            const bool all_same = simple || __all_sync(0xffffffffu, same);
-            unsigned rgb;
-            {
-              float c3[3] = {clr[0], clr[1], clr[2]};
-              if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3);   // every lane: its first winner
-              if (all_same) rgb = pack_rgb(c3[0], c3[1], c3[2]);   // four equal samples: the mean is the value itself
-              else {
-                // edge pixels: the other winners of this pixel (at most three more), summed in the resolve's order
-                float s01[3] = {c3[0], c3[1], c3[2]}, s23[3] = {0.f, 0.f, 0.f};   // 0 + c == c
-                unsigned pend = 0xeu;
-                if (wn[1] == wn[0]) { pend &= ~2u; s01[0] = s01[0] + c3[0]; s01[1] = s01[1] + c3[1]; s01[2] = s01[2] + c3[2]; }
-#pragma unroll
-                for (int t = 2; t < 4; t++)
-                  if (wn[t] == wn[0]) { pend &= ~(1u << t); s23[0] = s23[0] + c3[0]; s23[1] = s23[1] + c3[1]; s23[2] = s23[2] + c3[2]; }
-#pragma unroll 1
-                while (__any_sync(0xffffffffu, pend != 0u)) {
-                  DTS_COUNT(12, 1);
-                  if (pend) {
-                    const int s = __ffs(pend) - 1;
-                    const unsigned w = s == 1 ? wn[1] : (s == 2 ? wn[2] : wn[3]);
-                    float d3[3] = {clr[0], clr[1], clr[2]};
-                    if (w != kNoPrim) shade_prim(prims, w, tex_pool, lat_tab, pxa, pya, d3);
-#pragma unroll
-                    for (int t = 1; t < 4; t++)
-                      if ((pend >> t & 1u) && wn[t] == w) {
-                        pend &= ~(1u << t);
-                        if (t < 2) { s01[0] = s01[0] + d3[0]; s01[1] = s01[1] + d3[1]; s01[2] = s01[2] + d3[2]; }
-                        else { s23[0] = s23[0] + d3[0]; s23[1] = s23[1] + d3[1]; s23[2] = s23[2] + d3[2]; }
-                      }
-                  }
-                }
-                rgb = pack_rgb((s01[0] + s23[0]) * 0.25f, (s01[1] + s23[1]) * 0.25f, (s01[2] + s23[2]) * 0.25f);
-              }
-            }
+            unsigned rgb = shade_resolve(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane, err);
             if (kFish && !px_valid) rgb = 0u;   // cv2.remap BORDER_CONSTANT
             emit(rgb, bx, by);
           }
@@ -1860,6 +1906,130 @@ __global__ void __launch_bounds__(256, DTS_SOLO_MIN_CTAS) k_raster_solo(const DS
         if (bx * kBinW + kBinW <= W) store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
         else store_bin(out, rgb, lane, bx, by, W, H);
       }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ k_raster_flat
+// Coarse bins of at most kStage records that are all flat road tiles or the ground quad (k_bin's flat list: most of the
+// bins neither empty nor solo on a map without objects).  The tiles lie in the plane y = 0 and, up to slivers where two
+// neighbours snapped their shared border differently, do not overlap, so a sample belongs to the one tile that covers it:
+// no depth arithmetic.  The ground quad lies below every tile and takes the samples no tile covers, where its depth
+// passes GL_LESS against the cleared 1.0; samples nothing covers keep the clear colour.  The answer is k_raster's
+// coverage-only (DTS_COPLANAR) path, in a kernel of its own so that it is not held to k_raster's register allocation
+// (depth state, the tiny-triangle buffer, chunk streaming, wrapper layouts, the gather).
+// Hand-back: a sample covered by two tiles (or by two ground records) is not resolved here.  The warp restores the bin's
+// record count and k_raster, launched next on the stream, draws the whole bin depth-tested over what was stored.
+// Packed u8 HWC output with whole-word rows only (k_bin lists no bin otherwise).  Runs after k_raster_solo.
+template <bool kFish>   // true: each lane covers and shades the source pixel the fisheye LUT names for its output pixel
+__global__ void __launch_bounds__(256, DTS_FLAT_MIN_CTAS) k_raster_flat(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
+                                                                        FishTab ft, uint8_t* __restrict__ obs, int max_prims, int max_lat,
+                                                                        int32_t* __restrict__ err) {
+  __shared__ BinRec stages[8][kStage];   // per warp: the records of its bin
+  const int W = rc.width, H = rc.height;
+  const int cbins_x = (W + kCoarseW - 1) / kCoarseW, cbins = cbins_x * ((H + kCoarseH - 1) / kCoarseH);
+  const int lane = threadIdx.x & 31;
+  BinRec* stage = stages[threadIdx.x >> 5];
+  const StoreLane sl = make_store_lane(lane, W);
+  const size_t frame_bytes = (size_t)W * H * 3;
+  const int pxs = (lane & 7) * kSub, pys = (lane >> 3) * kSub;   // this lane's pixel inside a fine bin (sub-pixels)
+  const bool seg = (rc.mode & DTS_RENDER_SEGMENT) != 0;
+  const int n = fm.work[4];
+  const int warps = (gridDim.x * blockDim.x) >> 5;
+  for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+    const uint2 e = fm.flat[i];
+    const int env = (int)e.x, b = (int)(e.y & 0xffffu), count = (int)(e.y >> 16);
+    const int cby = b / cbins_x, cbx = b - cby * cbins_x;
+    DTS_COUNT(24, 1);
+    // ---- stage the records: one per lane, five 128-bit loads
+    uint2 mine = make_uint2(0u, 0u);   // prim_flags, kind
+    __syncwarp();   // every lane is done with the previous bin's records
+    if (lane < count) {
+      const int4* src = reinterpret_cast<const int4*>(fm.recs + fm.bin_start[(size_t)env * cbins + b] + lane);
+      int4* dst = reinterpret_cast<int4*>(stage + lane);
+      int4 v[5];
+#pragma unroll
+      for (int k = 0; k < 5; k++) v[k] = __ldg(src + k);
+#pragma unroll
+      for (int k = 0; k < 5; k++) dst[k] = v[k];
+      mine = make_uint2((unsigned)v[4].z, (unsigned)v[4].w);
+    }
+    __syncwarp();
+    const unsigned ground_bits = __ballot_sync(0xffffffffu, (mine.y & 2u) != 0u);
+    const uint8_t* tex_pool = maps[S.map_id[env]].tex_pool;
+    const PrimRec* prims = fm.prims + (size_t)env * max_prims;
+    const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
+    uint8_t* out = obs + (size_t)env * frame_bytes;
+    const float clr[3] = {seg ? 1.0f : S.rep[env].horizon[0], seg ? 0.0f : S.rep[env].horizon[1], seg ? 1.0f : S.rep[env].horizon[2]};
+    int ox = cbx * kCoarseW * kSub, oy = cby * kCoarseH * kSub;   // coarse bin corner, sub-pixels
+    if (kFish) { const short4 cb = ft.cbox[b]; ox = cb.x * kSub; oy = cb.y * kSub; }   // ... of its source box
+    const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);
+    const int ny = ((cby * kCFY + 1) * kBinH < H) ? 2 : 1;
+#pragma unroll 1
+    for (int f = 0; f < kCFX * kCFY; f++) {
+      if ((f & 3) >= nx || (f >> 2) >= ny) continue;
+      const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);   // fine bin
+      int pxc = pxs + (f & 3) * kBinW * kSub, pyc = pys + (f >> 2) * kBinH * kSub;   // this lane's pixel, coarse-relative
+      bool px_valid = true;
+      if (kFish) {   // (lanes past the image edge read a clamped entry; their pixels are not stored)
+        const int gx = min(bx * kBinW + (lane & 7), W - 1), gy = min(by * kBinH + (lane >> 3), H - 1);
+        const int sxy = __ldg(ft.src_xy + gy * W + gx);
+        const int sx = (int)(short)(sxy & 0xffff), sy = sxy >> 16;
+        px_valid = sx != -32768;
+        pxc = sx * kSub - ox; pyc = sy * kSub - oy;
+      }
+      const bool live = (mine.x >> (16 + f)) & 1u;
+      const unsigned live_mask = __ballot_sync(0xffffffffu, live);
+      const unsigned full_mask = __ballot_sync(0xffffffffu, live && ((mine.x >> (24 + f)) & 1u));
+      const unsigned ground_mask = live_mask & ground_bits, tiles = live_mask & ~ground_mask;
+      // one prim covering every sample of the fine bin (a lone ground record, too: k_raster's simple bin)
+      const unsigned pick = tiles ? tiles : live_mask;
+      const bool simple = pick && !(pick & (pick - 1)) && (pick & full_mask);
+      unsigned wn[4] = {kNoPrim, kNoPrim, kNoPrim, kNoPrim};
+      if (simple) {
+        const unsigned w = stage[__ffs(pick) - 1].prim_flags & 0xffffu;
+        wn[0] = w; wn[1] = w; wn[2] = w; wn[3] = w;
+      } else {
+        int seen = 0, twice = 0;   // samples of this pixel covered so far / covered twice
+        for (unsigned todo = tiles; todo; todo &= todo - 1) {
+          const BinRec& br = stage[__ffs(todo) - 1];
+          const uint32_t pflags = br.prim_flags;
+          const int mask = ((pflags >> (24 + f)) & 1u) ? 15 : sample_mask(br, pxc, pyc);
+          twice |= seen & mask;
+          seen |= mask;
+#pragma unroll
+          for (int s = 0; s < 4; s++)
+            if (mask >> s & 1) wn[s] = pflags & 0xffffu;
+        }
+        // the ground quad on the samples no tile covers (none left anywhere in the fine bin: it is hidden)
+        unsigned todo = __all_sync(0xffffffffu, seen == 15) ? 0u : ground_mask;
+        for (; todo; todo &= todo - 1) {
+          const BinRec& br = stage[__ffs(todo) - 1];
+          const uint32_t pflags = br.prim_flags;
+          const int mask = (((pflags >> (24 + f)) & 1u) ? 15 : sample_mask(br, pxc, pyc)) & ~(seen & 15);
+          if (!mask) continue;
+          twice |= (seen >> 4) & mask;
+          seen |= mask << 4;
+          // GL_LESS against the cleared depth 1.0, the depth plane evaluated exactly as k_raster does
+          const float4 zp = *reinterpret_cast<const float4*>(&br.z0);   // z0 zx zy id
+          const int2 xy0 = *reinterpret_cast<const int2*>(&br.x0);
+          const float cdx = (float)(pxc + 32 - xy0.x) * 0.015625f, cdy = (float)(pyc + 32 - xy0.y) * 0.015625f;
+#pragma unroll
+          for (int s = 0; s < 4; s++) {
+            const float sdx = cdx + (float)(sample_x(s) - 32) * 0.015625f, sdy = cdy + (float)(sample_y(s) - 32) * 0.015625f;
+            if ((mask >> s & 1) && fmaf(zp.z, sdy, fmaf(zp.y, sdx, zp.x)) < 1.0f) wn[s] = pflags & 0xffffu;
+          }
+        }
+        if (__any_sync(0xffffffffu, twice != 0)) {   // rare: k_raster draws the bin, depth-tested
+          DTS_COUNT(25, 1);
+          if (lane == 0) fm.bin_count[(size_t)env * cbins + b] = count;
+          break;
+        }
+      }
+      unsigned rgb = shade_resolve(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane, err);
+      if (kFish && !px_valid) rgb = 0u;   // cv2.remap BORDER_CONSTANT
+      if (bx * kBinW + kBinW <= W) store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
+      else store_bin(out, rgb, lane, bx, by, W, H);
+    }
   }
 }
 
@@ -2125,6 +2295,12 @@ int launch_render(const DState& S, const DMap* maps, const RenderCfg& rc, void* 
     const int solo_ctas = max(1, n_ctas * DTS_SOLO_MIN_CTAS / DTS_RENDER_MIN_CTAS);   // (n_ctas can be 1 for a handful of envs)
     if (fisheye) k_raster_solo<true><<<solo_ctas, 256, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat);
     else k_raster_solo<false><<<solo_ctas, 256, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat);
+    launches++;
+  }
+  if (!wrap && (W & 3) == 0) {   // before k_raster, which draws the bins it hands back
+    const int flat_ctas = max(1, n_ctas * DTS_FLAT_MIN_CTAS / DTS_RENDER_MIN_CTAS);
+    if (fisheye) k_raster_flat<true><<<flat_ctas, 256, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat, err_flag);
+    else k_raster_flat<false><<<flat_ctas, 256, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat, err_flag);
     launches++;
   }
   static bool smem_opt_in = false;
