@@ -27,7 +27,6 @@
 //
 // HBM traffic per env-frame: obs store W*H*3 B (compulsory) + PrimRec slab / BinRec lists / lattice table
 // (tens of KB per env, written by k_geometry / k_bin and read once by k_raster) + texels (shared, L2-resident).
-#include <cstdlib>
 #include <cstddef>
 
 #include "dts_camera.cuh"
@@ -37,21 +36,6 @@ namespace dts {
 
 namespace {
 
-#ifndef DTS_RENDER_THREADS
-#define DTS_RENDER_THREADS 256
-#endif
-#ifndef DTS_RENDER_MIN_CTAS
-#define DTS_RENDER_MIN_CTAS 3
-#endif
-#ifndef DTS_TMA_STAGING
-#define DTS_TMA_STAGING 1   // 0: stage BinRec chunks with per-lane 128-bit loads + shared stores instead of cp.async.bulk (A/B switch)
-#endif
-#ifndef DTS_TINY_PATH
-#define DTS_TINY_PATH 1     // triangles whose pixel box inside a coarse bin is <= 4x4 are rasterised one per lane (A/B switch)
-#endif
-#ifndef DTS_SAMPLE_CULL
-#define DTS_SAMPLE_CULL 1   // triangles of at most 3x3 pixels that cover no sample position are dropped at set-up (A/B switch)
-#endif
 #ifndef DTS_STATS
 #define DTS_STATS 0         // 1: k_raster counts bins / prim visits / shading rounds into the diagnostic counters (tools/raster_stats.py)
 #endif
@@ -60,24 +44,14 @@ namespace {
 #else
 #define DTS_COUNT(slot, n) do { } while (0)
 #endif
-#ifndef DTS_SOLO
-#define DTS_SOLO 1          // coarse bins lying inside ONE prim (besides the ground) are drawn by the lean k_raster_solo (A/B switch)
-#endif
-#ifndef DTS_SOLO_MIN_CTAS
-#define DTS_SOLO_MIN_CTAS 3   // resident CTAs per SM of k_raster_solo (register budget 65536 / (256 * this))
-#endif
-#ifndef DTS_FLAT_MIN_CTAS
-#define DTS_FLAT_MIN_CTAS 4   // resident CTAs per SM of k_raster_flat (register budget 65536 / (256 * this))
-#endif
-#ifndef DTS_COPLANAR
-#define DTS_COPLANAR 1      // fine bins whose prims are all road tiles (coplanar, disjoint) resolve visibility by coverage alone (A/B switch)
-#endif
-#ifndef DTS_COARSE_FAST
-#define DTS_COARSE_FAST 0   // 1: coarse bins lying inside one prim skip visibility and fetch the prim once.  The extra
-                            // code and registers cost more than the skipped flag tests save (k_raster_solo does this
-                            // job instead); kept as an A/B switch only
-#endif
-constexpr int kThreads = DTS_RENDER_THREADS;
+// Occupancy: threads per CTA of the three rasterisers, and the resident CTAs per SM each kernel is compiled for
+// (register budget 65536 / (threads * CTAs)).  Swept on H100 at c2: DESIGN.md §10.
+constexpr int kThreads = 256;
+constexpr int kRasterMinCtas = 3;   // k_raster
+constexpr int kSoloMinCtas = 3;     // k_raster_solo
+constexpr int kFlatMinCtas = 4;     // k_raster_flat
+constexpr int kGeoWarps = 1;        // k_geometry: warps per CTA ...
+constexpr int kGeoMinCtas = 32;     // ... and CTAs per SM
 constexpr int kWarps = kThreads / 32;
 constexpr int kBinW = 8, kBinH = 4;   // fine bin = one warp's pixel block (one pixel per lane)
 constexpr int kCFX = 4, kCFY = 2;     // coarse bin = 4 x 2 fine bins = 32 x 8 px: unit of binning and staging
@@ -91,37 +65,6 @@ __host__ __device__ constexpr int sample_x(int s) { return s == 0 ? 24 : (s == 1
 __host__ __device__ constexpr int sample_y(int s) { return s == 0 ? 8 : (s == 1 ? 24 : (s == 2 ? 40 : 56)); }
 
 struct Vtx { float cx, cy, cz, cw, r, g, b, u, v; };
-
-#ifndef DTS_GEO_X
-#define DTS_GEO_X 0   // code-size experiments of the geometry pass: bit 0 process_triangle_uniform out of line, bit 1 lattice loop rolled, bit 2 mesh vertex loop rolled
-#endif
-#ifndef DTS_GEO_INLINE
-#define DTS_GEO_INLINE 5
-#endif
-// which of the geometry pass's big device functions are inlined: bit 0 shade_vertex, bit 1 setup_and_emit, bit 2 the clipper.
-// With everything inlined setup_and_emit alone is a dozen copies of a large function, more SASS than the instruction cache
-// holds; 5 keeps one out-of-line copy of it.
-#define DTS_GEO_FN_SHADE __forceinline__
-#define DTS_GEO_FN_SETUP __forceinline__
-#define DTS_GEO_FN_CLIP __forceinline__
-#if !(DTS_GEO_INLINE & 1)
-#undef DTS_GEO_FN_SHADE
-#define DTS_GEO_FN_SHADE __noinline__
-#endif
-#if !(DTS_GEO_INLINE & 2)
-#undef DTS_GEO_FN_SETUP
-#define DTS_GEO_FN_SETUP __noinline__
-#endif
-#if !(DTS_GEO_INLINE & 4)
-#undef DTS_GEO_FN_CLIP
-#define DTS_GEO_FN_CLIP __noinline__
-#endif
-#ifndef DTS_GEO_WARPS
-#define DTS_GEO_WARPS 1
-#endif
-#ifndef DTS_GEO_MIN_CTAS
-#define DTS_GEO_MIN_CTAS 32
-#endif
 
 struct __align__(16) PrimRec {   // 128 B in the env's slab, words grouped for 128-bit loads
   int32_t X0, Y0, X1, Y1;        // w0  snapped vertices in cyclic order, orientation normalised (area > 0)
@@ -146,11 +89,15 @@ struct __align__(16) BinRec {    // 80 B per (prim, coarse bin) pair: what visib
   int32_t id;                    // draw id
   int32_t x0, y0;                // anchor vertex relative to the bin corner (sub-pixels)
   uint32_t prim_flags;           // prim index | per fine bin f of the coarse bin: bit 16+f = may touch, bit 24+f = every sample inside
-  int32_t kind;                  // bit 0: quad (4 edges), bit 1: ground quad (draw id < 2), bit 2: tiny triangle — its pixel box
-                                 // inside the coarse bin is at most 4x4 and sits in the unused 4th-edge slots:
-                                 // E0[3] = x0 | y0 << 16, A[3] = x1 | y1 << 16 (pixels from the bin corner, inclusive)
+  int32_t kind;                  // kKind* bits
 };
 static_assert(sizeof(BinRec) == 80, "BinRec layout");
+// BinRec::kind, written by k_bin (build_binrec) and read by the rasterisers
+constexpr int kKindQuad = 1;     // 4 edges
+constexpr int kKindGround = 2;   // the ground quad (draw id < 2)
+constexpr int kKindTiny = 4;     // tiny triangle: its pixel box inside the coarse bin is at most 4x4 and sits in the unused
+                                 // 4th-edge slots: E0[3] = x0 | y0 << 16, A[3] = x1 | y1 << 16 (pixels from the bin corner, inclusive)
+constexpr int kKindFlat = 8;     // road tile of tile mode 1: lies in the plane y = 0
 constexpr unsigned kNoPrim = 0xffffu;   // sample not covered by any prim: clear colour
 
 struct Xform { float MV[12], N[9]; };
@@ -191,8 +138,11 @@ __device__ __forceinline__ void model_view(const double* V, double tx, double ty
   __syncwarp();
 }
 
+// Of the geometry pass's big device functions, shade_vertex and the clipper are inlined and setup_and_emit is not: inlined,
+// setup_and_emit alone is a dozen copies of a large function, more SASS than the instruction cache holds.
+
 // fixed-function transform & lighting of one vertex (float32, operation order = spec)
-__device__ DTS_GEO_FN_SHADE Vtx shade_vertex(const Xform& x, const Shared& sh, float px, float py, float pz, float nx,
+__device__ __forceinline__ Vtx shade_vertex(const Xform& x, const Shared& sh, float px, float py, float pz, float nx,
                                             float ny, float nz, float cr, float cg, float cb, float u, float v) {
   float e[3], ne[3];
 #pragma unroll
@@ -281,8 +231,8 @@ struct EmitCtx {
 // With `d` the prim is the QUAD a,b,c,d (spec tile mode 1: an unclipped road tile): planes of triangle (a,b,c),
 // coverage by four edges.  Returns false — nothing emitted — if the snapped quad is not strictly convex; the
 // caller then draws the two triangles (a,b,c)(a,c,d) instead.
-__device__ DTS_GEO_FN_SETUP bool setup_and_emit(const EmitCtx& ec, const Vtx& a, const Vtx& b, const Vtx& c, int id,
-                                               int tex, int lat, const Vtx* d = nullptr) {
+__device__ __noinline__ bool setup_and_emit(const EmitCtx& ec, const Vtx& a, const Vtx& b, const Vtx& c, int id,
+                                            int tex, int lat, const Vtx* d = nullptr) {
   const Vtx* vs[3] = {&a, &b, &c};
   int X[3], Y[3];
   float zw[3], q[3];
@@ -322,7 +272,6 @@ __device__ DTS_GEO_FN_SETUP bool setup_and_emit(const EmitCtx& ec, const Vtx& a,
   const int px0 = max(minx >> 6, 0), px1 = min(maxx >> 6, ec.W - 1);
   const int py0 = max(miny >> 6, 0), py1 = min(maxy >> 6, ec.H - 1);
   if (px0 > px1 || py0 > py1) return true;   // off screen: emitted nothing, and nothing is what it covers
-#if DTS_SAMPLE_CULL
   if (!d && (maxx >> 6) - (minx >> 6) < 3 && (maxy >> 6) - (miny >> 6) < 3) {   // (the unclamped box: everything below stays small)
     // A small triangle that covers NO sample position draws nothing — half the triangles of a distant mesh at
     // 160x120 — so it needs no record, no bin pair and no visit by the rasteriser.  Same integer edge functions and
@@ -347,7 +296,6 @@ __device__ DTS_GEO_FN_SETUP bool setup_and_emit(const EmitCtx& ec, const Vtx& a,
       }
     if (!any) return true;
   }
-#endif
   PrimRec r;
   r.X0 = x0; r.Y0 = y0; r.X1 = x1; r.Y1 = y1; r.X2 = x2; r.Y2 = y2; r.X3 = x0; r.Y3 = y0;
   const float dx1 = (float)(x1 - x0) * 0.015625f, dy1 = (float)(y1 - y0) * 0.015625f;
@@ -377,7 +325,6 @@ __device__ DTS_GEO_FN_SETUP bool setup_and_emit(const EmitCtx& ec, const Vtx& a,
   r.id = id;
   r.ltq = (lat + 1) | ((tex + 1) << 16);
   r.tex = tex >= 0 ? ec.textures[tex].info : 0u;
-  (void)px0; (void)py0; (void)px1; (void)py1;
   if (d) {   // vertices in cyclic order; planes stay those of triangle (a,b,c) anchored at a
     r.ltq |= 1 << 24;
     r.X1 = qx[1]; r.Y1 = qy[1]; r.X2 = qx[2]; r.Y2 = qy[2]; r.X3 = qx[3]; r.Y3 = qy[3];
@@ -406,7 +353,7 @@ __device__ __forceinline__ Vtx clip_lerp(const Vtx& in, const Vtx& out, float di
 // WHOLE warp for one triangle: lane k owns polygon vertex k, neighbours' plane distances come by shuffle, output
 // slots by ballot prefix sums, so a plane costs a few dozen instructions instead of a serial loop over vertices.
 // Same arithmetic, same vertex order (hence the same fan) as the serial formulation of the spec.
-__device__ DTS_GEO_FN_CLIP void clip_and_emit_warp(const EmitCtx& ec, const Vtx& a, const Vtx& b, const Vtx& c, int id,
+__device__ __forceinline__ void clip_and_emit_warp(const EmitCtx& ec, const Vtx& a, const Vtx& b, const Vtx& c, int id,
                                                    int tex, int lat, int lane) {
   for (int p2 = 0; p2 < 6; p2++) {   // the spec's trivial reject looks at the ORIGINAL triangle, guard planes
     const int cnt = !(plane_dist(a, p2) >= 0.0f) + !(plane_dist(b, p2) >= 0.0f) + !(plane_dist(c, p2) >= 0.0f);
@@ -449,13 +396,8 @@ __device__ DTS_GEO_FN_CLIP void clip_and_emit_warp(const EmitCtx& ec, const Vtx&
 }
 
 // one warp-uniform triangle (ground, analytic tile): classify once, lane 0 emits or the warp clips
-#if DTS_GEO_X & 1
-#define DTS_PTU_FN __noinline__
-#else
-#define DTS_PTU_FN __forceinline__
-#endif
-__device__ DTS_PTU_FN void process_triangle_uniform(const EmitCtx& ec, const Vtx& a, const Vtx& b, const Vtx& c,
-                                                    int id, int tex, int lat, int lane) {
+__device__ __forceinline__ void process_triangle_uniform(const EmitCtx& ec, const Vtx& a, const Vtx& b, const Vtx& c,
+                                                         int id, int tex, int lat, int lane) {
   const int cls = classify(a, b, c);
   if (cls == 2) return;
   if (cls == 0) { if (lane == 0) setup_and_emit(ec, a, b, c, id, tex, lat); }
@@ -512,8 +454,9 @@ __device__ __forceinline__ bool bin_overlaps(const int qx[4], const int qy[4], i
 // trivial-accept bits for each of the bin's 8 fine bins, depth plane, draw id.
 // With `fb` (fused fisheye) the bin's pixels are wherever the LUT sends its output pixels: (ox, oy) is the corner of
 // their source bounding box and fb[f] the source box of fine bin f; the bits then speak about every pixel of that box.
-// Returns the fine bins every sample of which the prim covers (bits 0-7) | ground quad << 8 | (flat road tile or ground
-// quad, and not drawn by the tiny-triangle path) << 9.
+// Returns the fine bins every sample of which the prim covers (bits 0-7) | kRecGround | kRecFlatOk.
+constexpr unsigned kRecGround = 0x100u;   // the ground quad
+constexpr unsigned kRecFlatOk = 0x200u;   // a flat road tile or the ground quad, and not drawn by the tiny-triangle path
 __device__ __forceinline__ unsigned build_binrec(const PrimRec* __restrict__ pr, int p, int ox, int oy, BinRec* __restrict__ out,
                                                  const short4* __restrict__ fb = nullptr) {
   const int4 w0 = __ldg(reinterpret_cast<const int4*>(pr));
@@ -521,7 +464,7 @@ __device__ __forceinline__ unsigned build_binrec(const PrimRec* __restrict__ pr,
   const float4 w2 = __ldg(reinterpret_cast<const float4*>(pr) + 2);
   const int ltq = __ldg(&pr->ltq);
   const int quad = (ltq >> 24) & 1;
-  const int flat = (ltq & 0xffff) ? 8 : 0;   // a road tile of tile mode 1 (it carries a lattice): lies in the plane y = 0
+  const int flat = (ltq & 0xffff) ? kKindFlat : 0;   // a road tile of tile mode 1 (it carries a lattice)
   const int qx[4] = {w0.x, w0.z, w1.x, w1.z}, qy[4] = {w0.y, w0.w, w1.y, w1.w};
   const int nv = quad ? 4 : 3;
   unsigned live = 0xffu, inside = 0xffu;
@@ -570,14 +513,14 @@ __device__ __forceinline__ unsigned build_binrec(const PrimRec* __restrict__ pr,
     }
   }
   int tiny = 0;
-  if (DTS_TINY_PATH && !fb && !quad && live) {
+  if (!fb && !quad && live) {
     // small triangles (a 6 cm duckie is 148 triangles in a dozen pixels) are rasterised one per LANE in k_raster instead
     // of one per warp: they carry their pixel box
     const int minx = min(qx[0], min(qx[1], qx[2])) - ox, maxx = max(qx[0], max(qx[1], qx[2])) - ox;
     const int miny = min(qy[0], min(qy[1], qy[2])) - oy, maxy = max(qy[0], max(qy[1], qy[2])) - oy;
     const int x0 = max(minx >> 6, 0), x1 = min(maxx >> 6, kCoarseW - 1), y0 = max(miny >> 6, 0), y1 = min(maxy >> 6, kCoarseH - 1);
     if (x1 - x0 < 4 && y1 - y0 < 4 && x1 >= x0 && y1 >= y0) {
-      tiny = 4;
+      tiny = kKindTiny;
       E0[3] = x0 | (y0 << 16); A[3] = x1 | (y1 << 16);
     }
   }
@@ -587,8 +530,9 @@ __device__ __forceinline__ unsigned build_binrec(const PrimRec* __restrict__ pr,
   o[1] = make_int4(A[0], A[1], A[2], A[3]);
   o[2] = make_int4(B[0], B[1], B[2], B[3]);
   o[3] = make_int4(__float_as_int(w2.x), __float_as_int(w2.y), __float_as_int(w2.z), id);
-  o[4] = make_int4(qx[0] - ox, qy[0] - oy, (int)((unsigned)p | (live << 16) | ((inside & live) << 24)), quad | (id < 2 ? 2 : 0) | tiny | flat);
-  return (inside & live) | (id < 2 ? 0x100u : 0u) | ((flat || id < 2) && !tiny ? 0x200u : 0u);
+  o[4] = make_int4(qx[0] - ox, qy[0] - oy, (int)((unsigned)p | (live << 16) | ((inside & live) << 24)),
+                   (quad ? kKindQuad : 0) | (id < 2 ? kKindGround : 0) | tiny | flat);
+  return (inside & live) | (id < 2 ? kRecGround : 0u) | ((flat || id < 2) && !tiny ? kRecFlatOk : 0u);
 }
 
 // Fragment colour of prim `w` of the env's slab at the pixel whose centre is (pxa + 32, pya + 32) sub-pixels (spec steps
@@ -806,10 +750,51 @@ __device__ __forceinline__ void store_bin_any(uint8_t* __restrict__ out, int fmt
   if (gx < W && gy < H) store_px_fmt(out, fmt & 3, fmt >> 2, gx, gy, W, H, rgb);
 }
 
+// Packed u8 HWC whose rows are whole 32-bit words: the only output k_raster_solo and k_raster_flat write.  k_bin lists
+// bins for them, and launch_render launches them, under exactly this test; a bin listed but not drawn would stay unwritten.
+__host__ __device__ __forceinline__ bool lean_output(int layout, int dtype, int W) {
+  return layout == DTS_OBS_HWC && dtype == DTS_OBS_U8 && (W & 3) == 0;
+}
+
+// The fine bins of coarse bin (cbx, cby) that lie inside the image, as bits f = column | row << 2: all 8 except on the
+// right / bottom border.  `rows` = fine_rows_in_image(cby, H), which k_raster computes once per row of coarse bins.
+__device__ __forceinline__ unsigned fine_rows_in_image(int cby, int H) { return ((cby * kCFY + 1) * kBinH < H) ? 0xffu : 0x0fu; }
+__device__ __forceinline__ unsigned fine_in_image(int cbx, unsigned rows, int W) {
+  const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);   // fine-bin columns inside the image: 1..4
+  const unsigned cols = (1u << nx) - 1u;
+  return rows & (cols | (cols << 4));
+}
+
+// Fused fisheye: the source pixel the LUT names for this lane's output pixel of fine bin (bx, by), in sub-pixels, and
+// whether there is one (none: cv2.remap BORDER_CONSTANT, black).  Lanes past the image edge read a clamped entry; their
+// pixels are not stored.
+struct FishPx { bool valid; int x, y; };
+__device__ __forceinline__ FishPx fish_source(const FishTab& ft, int bx, int by, int lane, int W, int H) {
+  const int gx = min(bx * kBinW + (lane & 7), W - 1), gy = min(by * kBinH + (lane >> 3), H - 1);
+  const int sxy = __ldg(ft.src_xy + gy * W + gx);
+  const int sx = (int)(short)(sxy & 0xffff), sy = sxy >> 16;
+  return FishPx{sx != -32768, sx * kSub, sy * kSub};
+}
+
+// One fine bin of a lean_output() frame: whole words if the bin lies inside the image, else the general form
+__device__ __forceinline__ void store_bin_lean(uint8_t* __restrict__ out, const StoreLane& sl, unsigned rgb, int lane, int bx, int by,
+                                               int W, int H) {
+  if (bx * kBinW + kBinW <= W) store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
+  else store_bin(out, rgb, lane, bx, by, W, H);
+}
+
+// glClearColor: the env's horizon colour, or on the segment view glClearColor(255, 0, 255) clamped to magenta (S:1752)
+__device__ __forceinline__ void clear_colour(const DState& S, const RenderCfg& rc, int env, float clr[3]) {
+  const bool seg = (rc.mode & DTS_RENDER_SEGMENT) != 0;
+  clr[0] = seg ? 1.0f : S.rep[env].horizon[0];
+  clr[1] = seg ? 0.0f : S.rep[env].horizon[1];
+  clr[2] = seg ? 1.0f : S.rep[env].horizon[2];
+}
+
 }  // namespace
 
 
-int render_ctas_per_sm() { return DTS_RENDER_MIN_CTAS; }
+int render_ctas_per_sm() { return kRasterMinCtas; }
 
 // ------------------------------------------------------------------------------------------------ frame memory
 struct FrameMem {
@@ -823,10 +808,14 @@ struct FrameMem {
   uint2* geo_list;      // [N * items_max] (env, draw item) pairs that passed k_cull
   uint2* solo;          // [N * cbins] (env, coarse bin | prim << 16): coarse bins lying inside one prim (k_bin -> k_raster_solo)
   uint2* flat;          // [N * cbins] (env, coarse bin | record count << 16): flat bins, only road tiles and ground (k_bin -> k_raster_flat)
-  int* work;            // global counters: [0] k_raster work items, [1] pair-pool cursor, [2] geo_list length, [3] solo list length,
-                        // [4] flat list length
+  int* work;            // global counters, zeroed per frame: the kWork* slots
   int32_t* status;      // mapped host word (dts_status): bit 0 = a frame ran out of frame memory
 };
+constexpr int kWorkRaster = 0;     // k_raster's next work item
+constexpr int kWorkPairPool = 1;   // pair-pool cursor (k_bin)
+constexpr int kWorkGeoList = 2;    // geo_list length (k_cull -> k_geometry)
+constexpr int kWorkSoloList = 3;   // solo list length (k_bin -> k_raster_solo)
+constexpr int kWorkFlatList = 4;   // flat list length (k_bin -> k_raster_flat)
 
 __host__ __device__ inline size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
 
@@ -957,7 +946,7 @@ __global__ void __launch_bounds__(256) k_cull(const DState S, const DMap* __rest
   if (!m) return;
   const int lane = threadIdx.x & 31;
   int base = 0;
-  if (lane == __ffs(m) - 1) base = atomicAdd(fm.work + 2, __popc(m));
+  if (lane == __ffs(m) - 1) base = atomicAdd(fm.work + kWorkGeoList, __popc(m));
   base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
   if (vis) fm.geo_list[base + __popc(m & ((1u << lane) - 1u))] = make_uint2((unsigned)env, (unsigned)item);
 }
@@ -965,7 +954,6 @@ __global__ void __launch_bounds__(256) k_cull(const DState S, const DMap* __rest
 // ------------------------------------------------------------------------------------------------ k_geometry
 // One warp per CTA, 64 registers, 32 CTAs per SM: the kernel is latency-bound (short dependent chains), so resident warps
 // matter more than spills.  Each warp draws the (env, item) pairs of k_cull's work list, grid-strided.
-constexpr int kGeoWarps = DTS_GEO_WARPS;
 template <bool kTess>   // true: spec tile mode 0 (DTS_FLAG_TESSELLATE), the literal 98 triangles per road tile
 __device__ __forceinline__ void geometry_item(const DState& S, const DMap* __restrict__ maps, const RenderCfg& rc, const FrameMem& fm,
                                               int max_prims, int max_lat, int32_t* __restrict__ err, int env, int item, int lane,
@@ -1034,11 +1022,7 @@ __device__ __forceinline__ void geometry_item(const DState& S, const DMap* __res
     // the tile's 8x8 lattice, two vertices per lane (tessellated mode: also frustum-culls the whole tile)
     Vtx lv[2];
     int outside[6] = {0, 0, 0, 0, 0, 0};
-#if DTS_GEO_X & 2
-#pragma unroll 1
-#else
 #pragma unroll
-#endif
     for (int h = 0; h < 2; h++) {
       const int vi = lane + 32 * h, a = vi >> 3, b = vi & 7;             // a: u index (x), b: v index (z)
       const float lx = (float)(-ts / 2 + ((double)a / 7.0) * ts), lz = (float)(-ts / 2 + ((double)b / 7.0) * ts);
@@ -1137,12 +1121,12 @@ __device__ __forceinline__ void geometry_item(const DState& S, const DMap* __res
 }
 
 template <bool kTess>
-__global__ void __launch_bounds__(kGeoWarps * 32, DTS_GEO_MIN_CTAS)
+__global__ void __launch_bounds__(kGeoWarps * 32, kGeoMinCtas)
 k_geometry(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, int max_prims, int max_lat,
            int32_t* __restrict__ err) {
   __shared__ GeoWarp gws[kGeoWarps];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const int n_list = fm.work[2];   // written by k_cull
+  const int n_list = fm.work[kWorkGeoList];   // written by k_cull
   for (int wi = blockIdx.x * kGeoWarps + wib; wi < n_list; wi += gridDim.x * kGeoWarps) {
     const uint2 e = fm.geo_list[wi];
     geometry_item<kTess>(S, maps, rc, fm, max_prims, max_lat, err, (int)e.x, (int)e.y, lane, gws[wib]);
@@ -1279,7 +1263,7 @@ k_bin(RenderCfg rc, FrameMem fm, FishTab ft, int max_prims, int max_pairs, int32
           carry += __shfl_sync(0xffffffffu, inc, 31);
         }
         if (lane == 0) {   // this env's run of the batch-wide pair pool
-          const unsigned base = atomicAdd(reinterpret_cast<unsigned*>(fm.work) + 1, (unsigned)carry);
+          const unsigned base = atomicAdd(reinterpret_cast<unsigned*>(fm.work) + kWorkPairPool, (unsigned)carry);
           s_total = carry; s_base = (int)base;
           s_ok = (unsigned long long)base + (unsigned)carry <= (unsigned long long)max_pairs;
         }
@@ -1301,8 +1285,7 @@ k_bin(RenderCfg rc, FrameMem fm, FishTab ft, int max_prims, int max_pairs, int32
   // pass 2: one pair per thread -> its visibility record (the pairs were written by other threads of this CTA: the
   // barrier above orders those writes before these reads)
   const int pair0 = s_base, total = s_total;
-  const bool lean_fmt = rc.obs_layout == DTS_OBS_HWC && rc.obs_dtype == DTS_OBS_U8 && (W & 3) == 0;   // packed u8 HWC, whole-word rows
-  const bool solo_on = DTS_SOLO && lean_fmt;
+  const bool lean_fmt = lean_output(rc.obs_layout, rc.obs_dtype, W);
   // start[] is free from here on: per coarse bin, nonzero once a record rules the bin out of k_raster_flat (a mesh
   // triangle, a tiny triangle, or a solo bin)
   int* no_flat = start;
@@ -1322,23 +1305,20 @@ k_bin(RenderCfg rc, FrameMem fm, FishTab ft, int max_prims, int max_pairs, int32
     } else {
       r = build_binrec(prims + p, p, cbx * kCoarseW * kSub, cby * kCoarseH * kSub, recs + i);
     }
-    {
-      if (solo_on) {
-        // the coarse bin lies inside this prim and holds no other (besides the ground, hidden below it): no visibility
-        // work at all -> the bin goes to k_raster_solo, and k_raster skips it (negative count)
-        const int c = cnt[b];
-        const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);
-        const unsigned cols = (1u << nx) - 1u, valid = (((cby * kCFY + 1) * kBinH < H) ? 0xffu : 0x0fu) & (cols | (cols << 4));
-        // (... or it is the bin's only record: a stretch of bare ground)
-        const bool alone = (r & 0x100u) ? (c & kCountMask) == 1 : (c & kCountMask) - (c >> 20) == 1;
-        if (alone && (r & valid) == valid) {
-          fm.bin_count[(size_t)env * cbins + b] = -(p + 1);
-          const int slot = atomicAdd(fm.work + 3, 1);
-          fm.solo[slot] = make_uint2((unsigned)env, (unsigned)b | ((unsigned)p << 16));
-          atomicOr(&no_flat[b], 1);
-        }
+    if (lean_fmt) {
+      // the coarse bin lies inside this prim and holds no other (besides the ground, hidden below it): no visibility
+      // work at all -> the bin goes to k_raster_solo, and k_raster skips it (negative count)
+      const int c = cnt[b];
+      const unsigned valid = fine_in_image(cbx, fine_rows_in_image(cby, H), W);
+      // (... or it is the bin's only record: a stretch of bare ground)
+      const bool alone = (r & kRecGround) ? (c & kCountMask) == 1 : (c & kCountMask) - (c >> 20) == 1;
+      if (alone && (r & valid) == valid) {
+        fm.bin_count[(size_t)env * cbins + b] = -(p + 1);
+        const int slot = atomicAdd(fm.work + kWorkSoloList, 1);
+        fm.solo[slot] = make_uint2((unsigned)env, (unsigned)b | ((unsigned)p << 16));
+        atomicOr(&no_flat[b], 1);
       }
-      if (lean_fmt && !(r & 0x200u)) atomicOr(&no_flat[b], 1);
+      if (!(r & kRecFlatOk)) atomicOr(&no_flat[b], 1);
     }
   }
   if (!lean_fmt) return;
@@ -1351,7 +1331,7 @@ k_bin(RenderCfg rc, FrameMem fm, FishTab ft, int max_prims, int max_pairs, int32
     const unsigned m = __ballot_sync(0xffffffffu, flat);
     if (!m) continue;
     int base = 0;
-    if (lane == 0) base = atomicAdd(fm.work + 4, __popc(m));
+    if (lane == 0) base = atomicAdd(fm.work + kWorkFlatList, __popc(m));
     base = __shfl_sync(0xffffffffu, base, 0);
     if (flat) {
       fm.bin_count[(size_t)env * cbins + b] = kFlatBin;
@@ -1403,7 +1383,7 @@ __device__ __forceinline__ int sample_mask(const BinRec& br, int pxc, int pyc) {
   const int ec1 = E.y + A.y * pxc + B.y * pyc;
   const int ec2 = E.z + A.z * pxc + B.z * pyc;
   int mask = 0;
-  if (br.kind & 1) {
+  if (br.kind & kKindQuad) {
     const int ec3 = E.w + A.w * pxc + B.w * pyc;
 #pragma unroll
     for (int s = 0; s < 4; s++) {
@@ -1467,7 +1447,7 @@ __device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool sim
 // ------------------------------------------------------------------------------------------------ k_raster
 template <bool kWrapFmt, bool kFish>   // kWrapFmt: a dts_output_format other than packed u8 HWC is written by the resolve;
                                        // kFish: every lane renders the SOURCE pixel the fisheye LUT names for its output pixel
-__global__ void __launch_bounds__(kThreads, DTS_RENDER_MIN_CTAS)
+__global__ void __launch_bounds__(kThreads, kRasterMinCtas)
 k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, FishTab ft, GatherTab gt,
          uint8_t* __restrict__ obs, int max_prims, int max_pairs, int max_lat, int32_t* __restrict__ err) {
   // dynamic shared memory (kRasterSmem bytes): per warp two chunks of records in flight, their mbarriers, and a 128-sample
@@ -1485,7 +1465,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
   const size_t out_elem = (kWrapFmt && rc.obs_dtype == DTS_OBS_F32_UNIT) ? 4 : 1;
   const int pxs = (lane & 7) * kSub, pys = (lane >> 3) * kSub;   // this lane's pixel inside a fine bin (sub-pixels)
   const StoreLane sl = make_store_lane(lane, W);
-  const bool fast_fmt = !kWrapFmt && (W & 3) == 0;   // packed u8 HWC rows of whole words
+  const bool fast_fmt = !kWrapFmt && lean_output(DTS_OBS_HWC, DTS_OBS_U8, W);   // (k_raster<false, *> writes packed u8 HWC)
   const bool planar_u8 = kWrapFmt && rc.obs_dtype == DTS_OBS_U8 &&
                          ((rc.obs_layout == DTS_OBS_CHW && (W & 3) == 0) || (rc.obs_layout == DTS_OBS_CWH && (H & 3) == 0));
   uint64_t* bar = bars[warp];
@@ -1495,11 +1475,11 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
   int cs = 0, ps = 0;    // consumer / producer slot
   const int n_work = rc.n_envs * cbins_y;   // work item = one row of coarse bins of one env
   int work = 0;
-  if (lane == 0) work = atomicAdd(fm.work, 1);
+  if (lane == 0) work = atomicAdd(fm.work + kWorkRaster, 1);
   work = __shfl_sync(0xffffffffu, work, 0);
   while (work < n_work) {
     int next_work = 0;
-    if (lane == 0) next_work = atomicAdd(fm.work, 1);   // consumed after this row: latency hidden
+    if (lane == 0) next_work = atomicAdd(fm.work + kWorkRaster, 1);   // consumed after this row: latency hidden
     const int env = work / cbins_y, cby = work - env * cbins_y;
     const DMap& m = maps[S.map_id[env]];
     const uint8_t* tex_pool = m.tex_pool;
@@ -1527,8 +1507,8 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
         emit_general(out, gt, gather_rows ? 0 : gt.n, env_off, out_fmt, rgb, lane, bx, by, W, H);
       }
     };
-    const bool seg = (rc.mode & DTS_RENDER_SEGMENT) != 0;   // glClearColor(255, 0, 255): clamped to magenta (S:1752)
-    const float clr[3] = {seg ? 1.0f : S.rep[env].horizon[0], seg ? 0.0f : S.rep[env].horizon[1], seg ? 1.0f : S.rep[env].horizon[2]};
+    float clr[3];
+    clear_colour(S, rc, env, clr);
     const unsigned clear_rgb = pack_rgb(clr[0], clr[1], clr[2]);
     // lane l holds the list of coarse bin (cby, l)
     int my_cnt = 0, my_start = 0;
@@ -1537,18 +1517,12 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
       my_start = fm.bin_start[(size_t)env * cbins + cby * cbins_x + lane];
     }
     const unsigned nz = __ballot_sync(0xffffffffu, my_cnt > 0);
-    const unsigned fvalid_y = ((cby * kCFY + 1) * kBinH < H) ? 0xffu : 0x0fu;   // second row of fine bins inside the image?
     // ---- producer: walks the row's chunk sequence one chunk ahead of the consumer.  A list of <= 32 records is
     // ONE chunk shared by the bin's 8 fine bins; a longer list is streamed chunk by chunk for each fine bin in turn
     // (the records are ready-made, re-reading them from L2 costs no arithmetic).
     int pcbx = nz ? __ffs(nz) - 1 : 32, pf = 0, pc = 0;
-    // fine bins of coarse bin `cbx` that lie inside the image, as a bit mask (all 8 except on the right / bottom border)
-    auto valid8 = [&](int cbx) -> unsigned {
-      const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);   // fine-bin columns inside the image: 1..4
-      const unsigned cols = (1u << nx) - 1u;
-      return fvalid_y & (cols | (cols << 4));
-    };
-    auto fine_valid = [&](int cbx, int f) -> bool { return (valid8(cbx) >> f) & 1u; };
+    const unsigned rows_in = fine_rows_in_image(cby, H);
+    auto fine_valid = [&](int cbx, int f) -> bool { return (fine_in_image(cbx, rows_in, W) >> f) & 1u; };
     auto next_bin = [&]() {
       const unsigned rem = nz & ~((2u << pcbx) - 1u);
       pcbx = rem ? __ffs(rem) - 1 : 32;
@@ -1560,19 +1534,10 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
       if (n > kStage) while (pf < kCFX * kCFY && !fine_valid(pcbx, pf)) pf++;   // fine bins outside the image are not visited
       if (n > kStage && pf >= kCFX * kCFY) { next_bin(); return; }               // (cannot happen: fine bin 0 is always inside)
       const int nch = min(kStage, n - pc);
-#if DTS_TMA_STAGING
       if (lane == 0) {
         mbar_expect_tx(&bar[ps], (uint32_t)(nch * sizeof(BinRec)));
         bulk_load(stages[warp][ps], recs + st + pc, (uint32_t)(nch * sizeof(BinRec)), &bar[ps]);
       }
-#else
-      if (lane < nch) {   // A/B baseline: one record per lane through registers
-        const int4* src = reinterpret_cast<const int4*>(recs + st + pc + lane);
-        int4* dst = reinterpret_cast<int4*>(&stages[warp][ps][lane]);
-#pragma unroll
-        for (int k = 0; k < 5; k++) dst[k] = __ldg(src + k);
-      }
-#endif
       ps ^= 1;
       if (n <= kStage) { next_bin(); return; }
       pc += kStage;
@@ -1586,19 +1551,17 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
     for (int cbx = 0; cbx < cbins_x; cbx++) {
       const int count = __shfl_sync(0xffffffffu, my_cnt, cbx);
       if (count < 0) continue;   // drawn by k_raster_solo (a bin inside one prim) or k_raster_flat (kFlatBin)
-      const unsigned fvalid = valid8(cbx);
+      const unsigned fvalid = fine_in_image(cbx, rows_in, W);
       DTS_COUNT(8, 1);
       if (count == 0) {
         DTS_COUNT(9, 1);
 #pragma unroll 1
         for (int f = 0; f < kCFX * kCFY; f++)
           if ((fvalid >> f) & 1u) {
+            const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);
             unsigned rgb = clear_rgb;
-            if (kFish) {
-              const int gx = min((cbx * kCFX + (f & 3)) * kBinW + (lane & 7), W - 1), gy = min((cby * kCFY + (f >> 2)) * kBinH + (lane >> 3), H - 1);
-              if ((short)(__ldg(ft.src_xy + gy * W + gx) & 0xffff) == -32768) rgb = 0u;
-            }
-            emit(rgb, cbx * kCFX + (f & 3), cby * kCFY + (f >> 2));
+            if (kFish && !fish_source(ft, bx, by, lane, W, H).valid) rgb = 0u;
+            emit(rgb, bx, by);
           }
         continue;
       }
@@ -1618,69 +1581,34 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
           // ---- acquire this chunk; the next one starts loading into the other slot meanwhile
           __syncwarp();   // every lane is done with the slot the producer is about to refill
           issue();
-#if DTS_TMA_STAGING
           mbar_wait(&bar[cs], (parity >> cs) & 1u);
           parity ^= 1u << cs;
-#else
-          __syncwarp();
-#endif
           const BinRec* stage = stages[warp][cs];
           cs ^= 1;
           const int nch = min(kStage, count - c0);
           uint2 mine = make_uint2(0u, 0u);
           if (lane < nch) mine = *reinterpret_cast<const uint2*>(&stage[lane].prim_flags);
           const bool first = c0 == 0, last = c0 + kStage >= count;
-          const unsigned ground_bits = __ballot_sync(0xffffffffu, (mine.y & 2u) != 0u);   // the ground quad's records in this chunk
-          const unsigned tiny_bits = kFish ? 0u : __ballot_sync(0xffffffffu, (mine.y & 4u) != 0u);   // one-per-lane triangles
-          const unsigned flat_bits = DTS_COPLANAR ? __ballot_sync(0xffffffffu, (mine.y & 8u) != 0u) : 0u;   // road tiles (plane y = 0)
+          const unsigned ground_bits = __ballot_sync(0xffffffffu, (mine.y & kKindGround) != 0u);   // the ground quad's records in this chunk
+          const unsigned tiny_bits = kFish ? 0u : __ballot_sync(0xffffffffu, (mine.y & kKindTiny) != 0u);   // one-per-lane triangles
+          const unsigned flat_bits = __ballot_sync(0xffffffffu, (mine.y & kKindFlat) != 0u);   // road tiles (plane y = 0)
 #if DTS_STATS
           if (single) {   // census: coarse bins lying inside ONE prim (besides the ground)
-            const unsigned ng_ = __ballot_sync(0xffffffffu, !(mine.y & 2u) && ((mine.x >> 16) & fvalid) != 0u);
-            const unsigned ngfull_ = __ballot_sync(0xffffffffu, !(mine.y & 2u) && ((mine.x >> 24) & fvalid) == fvalid);
+            const unsigned ng_ = __ballot_sync(0xffffffffu, !(mine.y & kKindGround) && ((mine.x >> 16) & fvalid) != 0u);
+            const unsigned ngfull_ = __ballot_sync(0xffffffffu, !(mine.y & kKindGround) && ((mine.x >> 24) & fvalid) == fvalid);
             if (ng_ && !(ng_ & (ng_ - 1)) && (ng_ & ngfull_)) { DTS_COUNT(22, 1); DTS_COUNT(23, __popc(fvalid)); }
           }
 #endif
-          if (DTS_COARSE_FAST && single) {
-            // ---- the whole coarse bin lies inside ONE prim (besides the ground quad, hidden below it): no visibility
-            // work at all, the prim's planes are fetched once for the bin's 256 pixels
-            const unsigned ng = __ballot_sync(0xffffffffu, !(mine.y & 2u) && ((mine.x >> 16) & fvalid) != 0u);
-            const unsigned ngfull = __ballot_sync(0xffffffffu, !(mine.y & 2u) && ((mine.x >> 24) & fvalid) == fvalid);
-            if (ng && !(ng & (ng - 1)) && (ng & ngfull)) {
-              const ShadeIn si = load_shade(prims, stage[__ffs(ng) - 1].prim_flags & 0xffffu);
-#pragma unroll 1
-              for (int f = 0; f < kCFX * kCFY; f++) {
-                if (!((fvalid >> f) & 1u)) continue;
-                const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);
-                int pxa = ox + pxs + (f & 3) * kBinW * kSub, pya = oy + pys + (f >> 2) * kBinH * kSub;
-                bool px_valid = true;
-                if (kFish) {
-                  const int gx = min(bx * kBinW + (lane & 7), W - 1), gy = min(by * kBinH + (lane >> 3), H - 1);
-                  const int sxy = __ldg(ft.src_xy + gy * W + gx);
-                  const int sx = (int)(short)(sxy & 0xffff), sy = sxy >> 16;
-                  px_valid = sx != -32768;
-                  pxa = sx * kSub; pya = sy * kSub;
-                }
-                float c3[3];
-                shade_eval(si, tex_pool, lat_tab, pxa, pya, c3);
-                unsigned rgb = pack_rgb(c3[0], c3[1], c3[2]);
-                if (kFish && !px_valid) rgb = 0u;
-                emit(rgb, bx, by);
-              }
-              continue;
-            }
-          }
 #pragma unroll 1
           for (int f = (single ? 0 : g); f < (single ? kCFX * kCFY : g + 1); f++) {
             if (!((fvalid >> f) & 1u)) continue;
             const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);   // fine bin
             int pxc = pxs + (f & 3) * kBinW * kSub, pyc = pys + (f >> 2) * kBinH * kSub;   // this lane's pixel, coarse-relative
             bool px_valid = true;
-            if (kFish) {   // the source pixel of this lane's output pixel (lanes past the image edge read a clamped entry)
-              const int gx = min(bx * kBinW + (lane & 7), W - 1), gy = min(by * kBinH + (lane >> 3), H - 1);
-              const int sxy = __ldg(ft.src_xy + gy * W + gx);
-              const int sx = (int)(short)(sxy & 0xffff), sy = sxy >> 16;
-              px_valid = sx != -32768;
-              pxc = sx * kSub - ox; pyc = sy * kSub - oy;
+            if (kFish) {
+              const FishPx src = fish_source(ft, bx, by, lane, W, H);
+              px_valid = src.valid;
+              pxc = src.x - ox; pyc = src.y - oy;
             }
             const bool live = (mine.x >> (16 + f)) & 1u;
             const unsigned live_mask = __ballot_sync(0xffffffffu, live);
@@ -1704,7 +1632,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
             // two neighbours snapped their shared border differently) disjoint, so a sample belongs to the one tile that
             // covers it — no depth arithmetic; the ground lies below them and takes what is left.  A sample that turns
             // out to be covered twice sends the whole bin through the depth-tested path (exactly the spec's answer).
-            bool coplanar = DTS_COPLANAR && single && !(live_mask & ~ground_mask & ~flat_bits);
+            bool coplanar = single && !(live_mask & ~ground_mask & ~flat_bits);
             if (coplanar && !simple) DTS_COUNT(20, 1);
             if (!simple) {
               if (first) {
@@ -1865,14 +1793,14 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
 // lean loop gets its own register allocation (the same fast path inside k_raster cost more than it saved).
 // Packed u8 HWC output with whole-word rows only (k_bin marks no bin otherwise).  Runs before k_raster.
 template <bool kFish>   // true: each lane shades the source pixel the fisheye LUT names for its output pixel
-__global__ void __launch_bounds__(256, DTS_SOLO_MIN_CTAS) k_raster_solo(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
+__global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
                                                                         FishTab ft, uint8_t* __restrict__ obs, int max_prims, int max_lat) {
   const int W = rc.width, H = rc.height;
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW;
   const int lane = threadIdx.x & 31;
   const StoreLane sl = make_store_lane(lane, W);
   const size_t frame_bytes = (size_t)W * H * 3;
-  const int n = fm.work[3];
+  const int n = fm.work[kWorkSoloList];
   const int warps = (gridDim.x * blockDim.x) >> 5;
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
     const uint2 e = fm.solo[i];
@@ -1883,29 +1811,27 @@ __global__ void __launch_bounds__(256, DTS_SOLO_MIN_CTAS) k_raster_solo(const DS
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     const ShadeIn si = load_shade(fm.prims + (size_t)env * max_prims, p);
     uint8_t* out = obs + (size_t)env * frame_bytes;
+    // fine bins inside the image as loop bounds rather than fine_in_image(): the mask test costs this loop machine code
     const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);
     const int ny = ((cby * kCFY + 1) * kBinH < H) ? 2 : 1;
 #pragma unroll 1
     for (int fy = 0; fy < ny; fy++)
 #pragma unroll 1
-      for (int fx = 0; fx < nx; fx++) {
-        const int bx = cbx * kCFX + fx, by = cby * kCFY + fy;
-        int pxa = (bx * kBinW + (lane & 7)) * kSub, pya = (by * kBinH + (lane >> 3)) * kSub;
-        bool px_valid = true;
-        if (kFish) {   // (lanes past the image edge read a clamped entry; their pixels are not stored)
-          const int gx = min(bx * kBinW + (lane & 7), W - 1), gy = min(by * kBinH + (lane >> 3), H - 1);
-          const int sxy = __ldg(ft.src_xy + gy * W + gx);
-          const int sx = (int)(short)(sxy & 0xffff), sy = sxy >> 16;
-          px_valid = sx != -32768;
-          pxa = sx * kSub; pya = sy * kSub;
-        }
-        float c3[3];
-        shade_eval(si, tex_pool, lat_tab, pxa, pya, c3);
-        unsigned rgb = pack_rgb(c3[0], c3[1], c3[2]);
-        if (kFish && !px_valid) rgb = 0u;   // cv2.remap BORDER_CONSTANT
-        if (bx * kBinW + kBinW <= W) store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
-        else store_bin(out, rgb, lane, bx, by, W, H);
+    for (int fx = 0; fx < nx; fx++) {
+      const int bx = cbx * kCFX + fx, by = cby * kCFY + fy;
+      int pxa = (bx * kBinW + (lane & 7)) * kSub, pya = (by * kBinH + (lane >> 3)) * kSub;
+      bool px_valid = true;
+      if (kFish) {
+        const FishPx src = fish_source(ft, bx, by, lane, W, H);
+        px_valid = src.valid;
+        pxa = src.x; pya = src.y;
       }
+      float c3[3];
+      shade_eval(si, tex_pool, lat_tab, pxa, pya, c3);
+      unsigned rgb = pack_rgb(c3[0], c3[1], c3[2]);
+      if (kFish && !px_valid) rgb = 0u;
+      store_bin_lean(out, sl, rgb, lane, bx, by, W, H);
+    }
   }
 }
 
@@ -1915,16 +1841,16 @@ __global__ void __launch_bounds__(256, DTS_SOLO_MIN_CTAS) k_raster_solo(const DS
 // neighbours snapped their shared border differently, do not overlap, so a sample belongs to the one tile that covers it:
 // no depth arithmetic.  The ground quad lies below every tile and takes the samples no tile covers, where its depth
 // passes GL_LESS against the cleared 1.0; samples nothing covers keep the clear colour.  The answer is k_raster's
-// coverage-only (DTS_COPLANAR) path, in a kernel of its own so that it is not held to k_raster's register allocation
+// coverage-only path, in a kernel of its own so that it is not held to k_raster's register allocation
 // (depth state, the tiny-triangle buffer, chunk streaming, wrapper layouts, the gather).
 // Hand-back: a sample covered by two tiles (or by two ground records) is not resolved here.  The warp restores the bin's
 // record count and k_raster, launched next on the stream, draws the whole bin depth-tested over what was stored.
 // Packed u8 HWC output with whole-word rows only (k_bin lists no bin otherwise).  Runs after k_raster_solo.
 template <bool kFish>   // true: each lane covers and shades the source pixel the fisheye LUT names for its output pixel
-__global__ void __launch_bounds__(256, DTS_FLAT_MIN_CTAS) k_raster_flat(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
+__global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
                                                                         FishTab ft, uint8_t* __restrict__ obs, int max_prims, int max_lat,
                                                                         int32_t* __restrict__ err) {
-  __shared__ BinRec stages[8][kStage];   // per warp: the records of its bin
+  __shared__ BinRec stages[kWarps][kStage];   // per warp: the records of its bin
   const int W = rc.width, H = rc.height;
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW, cbins = cbins_x * ((H + kCoarseH - 1) / kCoarseH);
   const int lane = threadIdx.x & 31;
@@ -1932,8 +1858,7 @@ __global__ void __launch_bounds__(256, DTS_FLAT_MIN_CTAS) k_raster_flat(const DS
   const StoreLane sl = make_store_lane(lane, W);
   const size_t frame_bytes = (size_t)W * H * 3;
   const int pxs = (lane & 7) * kSub, pys = (lane >> 3) * kSub;   // this lane's pixel inside a fine bin (sub-pixels)
-  const bool seg = (rc.mode & DTS_RENDER_SEGMENT) != 0;
-  const int n = fm.work[4];
+  const int n = fm.work[kWorkFlatList];
   const int warps = (gridDim.x * blockDim.x) >> 5;
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
     const uint2 e = fm.flat[i];
@@ -1954,14 +1879,16 @@ __global__ void __launch_bounds__(256, DTS_FLAT_MIN_CTAS) k_raster_flat(const DS
       mine = make_uint2((unsigned)v[4].z, (unsigned)v[4].w);
     }
     __syncwarp();
-    const unsigned ground_bits = __ballot_sync(0xffffffffu, (mine.y & 2u) != 0u);
+    const unsigned ground_bits = __ballot_sync(0xffffffffu, (mine.y & kKindGround) != 0u);
     const uint8_t* tex_pool = maps[S.map_id[env]].tex_pool;
     const PrimRec* prims = fm.prims + (size_t)env * max_prims;
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     uint8_t* out = obs + (size_t)env * frame_bytes;
-    const float clr[3] = {seg ? 1.0f : S.rep[env].horizon[0], seg ? 0.0f : S.rep[env].horizon[1], seg ? 1.0f : S.rep[env].horizon[2]};
+    float clr[3];
+    clear_colour(S, rc, env, clr);
     int ox = cbx * kCoarseW * kSub, oy = cby * kCoarseH * kSub;   // coarse bin corner, sub-pixels
     if (kFish) { const short4 cb = ft.cbox[b]; ox = cb.x * kSub; oy = cb.y * kSub; }   // ... of its source box
+    // fine bins inside the image as column / row counts rather than fine_in_image(), as in k_raster_solo
     const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);
     const int ny = ((cby * kCFY + 1) * kBinH < H) ? 2 : 1;
 #pragma unroll 1
@@ -1970,12 +1897,10 @@ __global__ void __launch_bounds__(256, DTS_FLAT_MIN_CTAS) k_raster_flat(const DS
       const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);   // fine bin
       int pxc = pxs + (f & 3) * kBinW * kSub, pyc = pys + (f >> 2) * kBinH * kSub;   // this lane's pixel, coarse-relative
       bool px_valid = true;
-      if (kFish) {   // (lanes past the image edge read a clamped entry; their pixels are not stored)
-        const int gx = min(bx * kBinW + (lane & 7), W - 1), gy = min(by * kBinH + (lane >> 3), H - 1);
-        const int sxy = __ldg(ft.src_xy + gy * W + gx);
-        const int sx = (int)(short)(sxy & 0xffff), sy = sxy >> 16;
-        px_valid = sx != -32768;
-        pxc = sx * kSub - ox; pyc = sy * kSub - oy;
+      if (kFish) {
+        const FishPx src = fish_source(ft, bx, by, lane, W, H);
+        px_valid = src.valid;
+        pxc = src.x - ox; pyc = src.y - oy;
       }
       const bool live = (mine.x >> (16 + f)) & 1u;
       const unsigned live_mask = __ballot_sync(0xffffffffu, live);
@@ -2026,9 +1951,8 @@ __global__ void __launch_bounds__(256, DTS_FLAT_MIN_CTAS) k_raster_flat(const DS
         }
       }
       unsigned rgb = shade_resolve(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane, err);
-      if (kFish && !px_valid) rgb = 0u;   // cv2.remap BORDER_CONSTANT
-      if (bx * kBinW + kBinW <= W) store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
-      else store_bin(out, rgb, lane, bx, by, W, H);
+      if (kFish && !px_valid) rgb = 0u;
+      store_bin_lean(out, sl, rgb, lane, bx, by, W, H);
     }
   }
 }
@@ -2228,7 +2152,7 @@ int debug_frame_copy(void* scratch, int n, int max_prims, int cbins, int max_pai
   for (int k = 0; k < 12; k++) V[k] = c.V[k];
   P[0] = c.P00; P[1] = c.P11; P[2] = c.P22; P[3] = c.P23;
   counts[0] = c.n_prims; counts[1] = c.n_lat; counts[2] = c.overflow; counts[3] = 0;
-  cudaMemcpy(&counts[3], fm.work + 1, sizeof(int32_t), cudaMemcpyDeviceToHost);   // (prim, coarse bin) pairs of the whole batch
+  cudaMemcpy(&counts[3], fm.work + kWorkPairPool, sizeof(int32_t), cudaMemcpyDeviceToHost);   // (prim, coarse bin) pairs of the whole batch
   const int np = c.n_prims < max_prims ? c.n_prims : max_prims;
   PrimRec* prims = new PrimRec[np > 0 ? np : 1];
   float4* lat = new float4[(size_t)max_lat * 64];
@@ -2271,15 +2195,14 @@ int launch_render(const DState& S, const DMap* maps, const RenderCfg& rc, void* 
   mark();
   const size_t pairs_total = (size_t)rc.n_envs * items_max;
   k_cull<<<(unsigned)((pairs_total + 255) / 256), 256, 0, st>>>(S, maps, rc, fm, items_max);
-  const int geo_ctas = (n_ctas / DTS_RENDER_MIN_CTAS) * DTS_GEO_MIN_CTAS / kGeoWarps;   // SMs x resident geometry CTAs
+  const int geo_ctas = (n_ctas / kRasterMinCtas) * kGeoMinCtas / kGeoWarps;   // SMs x resident geometry CTAs
   if (rc.tessellate) k_geometry<true><<<geo_ctas, kGeoWarps * 32, 0, st>>>(S, maps, rc, fm, max_prims, max_lat, err_flag);
   else k_geometry<false><<<geo_ctas, kGeoWarps * 32, 0, st>>>(S, maps, rc, fm, max_prims, max_lat, err_flag);
   mark();
   const size_t bin_smem_bytes = (size_t)2 * cbins * sizeof(int);
   const int bin_grid = rc.n_envs;   // CTA per env: one warp where a frame has few bins and prims (160x120: 75 bins — more warps
   // only add barriers and CTA launches), four for large cameras (640x480)
-  static const int bin_warps_env = getenv("DTS_BIN_WARPS") ? atoi(getenv("DTS_BIN_WARPS")) : 0;   // A/B override: 1..4
-  const int bin_threads = bin_warps_env >= 1 && bin_warps_env <= kBinWarps ? bin_warps_env * 32 : (cbins > 128 ? kBinWarps * 32 : 32);
+  const int bin_threads = cbins > 128 ? kBinWarps * 32 : 32;
   if (fisheye) {
     if (bin_smem_bytes > 48 * 1024) cudaFuncSetAttribute(k_bin<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bin_smem_bytes);
     k_bin<true><<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, fish, max_prims, max_pairs, err_flag);
@@ -2291,17 +2214,15 @@ int launch_render(const DState& S, const DMap* maps, const RenderCfg& rc, void* 
   mark();
   const bool wrap = (rc.obs_layout | rc.obs_dtype) != 0;
   int launches = 5;
-  if (DTS_SOLO && !wrap && (W & 3) == 0) {   // (inside the k_raster event bracket: it is rasterisation time)
-    const int solo_ctas = max(1, n_ctas * DTS_SOLO_MIN_CTAS / DTS_RENDER_MIN_CTAS);   // (n_ctas can be 1 for a handful of envs)
-    if (fisheye) k_raster_solo<true><<<solo_ctas, 256, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat);
-    else k_raster_solo<false><<<solo_ctas, 256, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat);
-    launches++;
-  }
-  if (!wrap && (W & 3) == 0) {   // before k_raster, which draws the bins it hands back
-    const int flat_ctas = max(1, n_ctas * DTS_FLAT_MIN_CTAS / DTS_RENDER_MIN_CTAS);
-    if (fisheye) k_raster_flat<true><<<flat_ctas, 256, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat, err_flag);
-    else k_raster_flat<false><<<flat_ctas, 256, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat, err_flag);
-    launches++;
+  if (lean_output(rc.obs_layout, rc.obs_dtype, W)) {   // (inside the k_raster event bracket: it is rasterisation time)
+    // n_ctas can be 1 for a handful of envs
+    const int solo_ctas = max(1, n_ctas * kSoloMinCtas / kRasterMinCtas), flat_ctas = max(1, n_ctas * kFlatMinCtas / kRasterMinCtas);
+    if (fisheye) k_raster_solo<true><<<solo_ctas, kThreads, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat);
+    else k_raster_solo<false><<<solo_ctas, kThreads, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat);
+    // before k_raster, which draws the bins k_raster_flat hands back
+    if (fisheye) k_raster_flat<true><<<flat_ctas, kThreads, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat, err_flag);
+    else k_raster_flat<false><<<flat_ctas, kThreads, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat, err_flag);
+    launches += 2;
   }
   static bool smem_opt_in = false;
   if (!smem_opt_in) {   // > 48 KB of dynamic shared memory per CTA needs the opt-in, once per kernel

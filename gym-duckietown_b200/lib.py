@@ -147,7 +147,7 @@ def load() -> C.CDLL:
         return _lib
     import shutil
     from . import build as _b
-    if os.environ.get("DTS_NO_REBUILD"):     # A/B runs of pre-built variants (tools/ab_all.sh): load what is there
+    if os.environ.get("DTS_NO_REBUILD"):     # runs of a pre-built diagnostic library (tools/run_stats.sh): load what is there
         pass
     elif shutil.which("nvcc"):
         _b.build(force=False)
