@@ -600,11 +600,13 @@ __device__ __forceinline__ void shade_eval(const ShadeIn& si, const uint8_t* __r
     const float tx = u * twf - 0.5f, ty = v * thf - 0.5f;
     const int txi = __float2int_rd(tx), tyi = __float2int_rd(ty);   // floorf(.) as the int the wrap needs; exact back in float
     const float ffx = tx - (float)txi, ffy = ty - (float)tyi;
-    const int ti0 = txi & (tw - 1), ti1 = (ti0 + 1) & (tw - 1);
-    const int tj0 = tyi & (th - 1), tj1 = (tj0 + 1) & (th - 1);
+    // texel indices as unsigned 32-bit values (below 2^30): each address is one wide multiply-add onto the texture base
+    const unsigned ti0 = (unsigned)txi & (tw - 1), ti1 = (ti0 + 1) & (tw - 1);
+    const unsigned tj0 = (unsigned)tyi & (th - 1), tj1 = (tj0 + 1) & (th - 1);
+    const unsigned r0 = tj0 << lw, r1 = tj1 << lw;
     const uchar4* tp = reinterpret_cast<const uchar4*>(tex_pool + ((size_t)(ti & 0xffffffu) << 8));
-    const uchar4 t00 = __ldg(tp + (tj0 << lw) + ti0), t10 = __ldg(tp + (tj0 << lw) + ti1);
-    const uchar4 t01 = __ldg(tp + (tj1 << lw) + ti0), t11 = __ldg(tp + (tj1 << lw) + ti1);
+    const uchar4 t00 = __ldg(tp + (r0 + ti0)), t10 = __ldg(tp + (r0 + ti1));
+    const uchar4 t01 = __ldg(tp + (r1 + ti0)), t11 = __ldg(tp + (r1 + ti1));
     const float a0[3] = {(float)t00.x, (float)t00.y, (float)t00.z}, a1[3] = {(float)t10.x, (float)t10.y, (float)t10.z};
     const float b0[3] = {(float)t01.x, (float)t01.y, (float)t01.z}, b1[3] = {(float)t11.x, (float)t11.y, (float)t11.z};
 #pragma unroll
@@ -1405,19 +1407,16 @@ __device__ __forceinline__ int sample_mask(const BinRec& br, int pxc, int pyc) {
   return mask;
 }
 
-// Deferred shading of one pixel of a fine bin whose visibility is resolved (winner prim per MSAA sample, kNoPrim = clear
-// colour): shaded once per distinct winner at the pixel centre (pxa, pya), then the box resolve -> packed u8.  `simple`:
-// the caller knows that every sample of the whole fine bin has the same winner.
-__device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool simple, const float clr[3], const PrimRec* __restrict__ prims,
-                                                  const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa,
-                                                  int pya, int lane, int32_t* __restrict__ err) {
+// Deferred shading of one pixel whose visibility is resolved (winner prim per MSAA sample, kNoPrim = clear colour): shaded
+// once per distinct winner at the pixel centre (pxa, pya), then the box resolve -> packed u8.
+// resolve_edge is the part after the first winner wn[0] is shaded (colour c3): the pixel's other distinct winners, shaded
+// in rounds of the whole warp (a lane with nothing pending idles), and the box resolve (s01 + s23) * 0.25 into c3, with
+// s01 = c(wn0) + c(wn1), s23 = c(wn2) + c(wn3).  Each shade depends only on (prim, position) and each half has two
+// addends, so neither the lane nor the order in which the winners are shaded changes a bit.  Called by the whole warp.
+__device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], const float clr[3], const PrimRec* __restrict__ prims,
+                                             const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa, int pya,
+                                             int lane, int32_t* __restrict__ err) {
   (void)lane; (void)err;   // (DTS_STATS counters)
-  const bool same = wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0];
-  const bool all_same = simple || __all_sync(0xffffffffu, same);
-  float c3[3] = {clr[0], clr[1], clr[2]};
-  if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3);   // every lane: its first winner
-  if (all_same) return pack_rgb(c3[0], c3[1], c3[2]);   // four equal samples: the mean is the value itself
-  // edge pixels: the other winners of this pixel (at most three more), summed in the resolve's order
   float s01[3] = {c3[0], c3[1], c3[2]}, s23[3] = {0.f, 0.f, 0.f};   // 0 + c == c
   unsigned pend = 0xeu;
   if (wn[1] == wn[0]) { pend &= ~2u; s01[0] = s01[0] + c3[0]; s01[1] = s01[1] + c3[1]; s01[2] = s01[2] + c3[2]; }
@@ -1441,7 +1440,20 @@ __device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool sim
         }
     }
   }
-  return pack_rgb((s01[0] + s23[0]) * 0.25f, (s01[1] + s23[1]) * 0.25f, (s01[2] + s23[2]) * 0.25f);
+#pragma unroll
+  for (int ch = 0; ch < 3; ch++) c3[ch] = (s01[ch] + s23[ch]) * 0.25f;
+}
+// The whole resolve of one fine bin's pixels (k_raster).  `simple`: the caller knows that every sample of the whole fine
+// bin has the same winner.
+__device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool simple, const float clr[3], const PrimRec* __restrict__ prims,
+                                                  const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa,
+                                                  int pya, int lane, int32_t* __restrict__ err) {
+  const bool same = wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0];
+  const bool all_same = simple || __all_sync(0xffffffffu, same);
+  float c3[3] = {clr[0], clr[1], clr[2]};
+  if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3);   // every lane: its first winner
+  if (!all_same) resolve_edge(wn, c3, clr, prims, tex_pool, lat_tab, pxa, pya, lane, err);   // (four equal samples: the mean is the value itself)
+  return pack_rgb(c3[0], c3[1], c3[2]);
 }
 
 // ------------------------------------------------------------------------------------------------ k_raster
@@ -1843,24 +1855,35 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
 // passes GL_LESS against the cleared 1.0; samples nothing covers keep the clear colour.  The answer is k_raster's
 // coverage-only path, in a kernel of its own so that it is not held to k_raster's register allocation
 // (depth state, the tiny-triangle buffer, chunk streaming, wrapper layouts, the gather).
-// Hand-back: a sample covered by two tiles (or by two ground records) is not resolved here.  The warp restores the bin's
-// record count and k_raster, launched next on the stream, draws the whole bin depth-tested over what was stored.
+// Edge pixels are shaded across the whole coarse bin: each fine bin shades every pixel's first winner, and a pixel with
+// more than one distinct winner (about a quarter of a general fine bin's lanes) joins a per-warp queue instead of keeping
+// the warp for a round at a quarter of its lanes.  Whenever 32 pixels are queued, and after the bin's last fine bin, each
+// lane takes one and shades its other winners (resolve_edge: the same bits whichever lane shades them).  The bin's
+// colours collect in shared memory and are stored once the bin is done.
+// Hand-back: a sample covered by two tiles (or by two ground records) is not resolved here.  The warp drops the bin's
+// queue and colours, restores its record count, and k_raster, launched next on the stream, draws the whole bin
+// depth-tested.
 // Packed u8 HWC output with whole-word rows only (k_bin lists no bin otherwise).  Runs after k_raster_solo.
+constexpr int kEdgeQ = 64;   // queue ring: flushed at 32 entries, so at most 31 + 32 wait at once
 template <bool kFish>   // true: each lane covers and shades the source pixel the fisheye LUT names for its output pixel
 __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
                                                                         FishTab ft, uint8_t* __restrict__ obs, int max_prims, int max_lat,
                                                                         int32_t* __restrict__ err) {
   __shared__ BinRec stages[kWarps][kStage];   // per warp: the records of its bin
+  __shared__ unsigned bin_rgb[kWarps][kCFX * kCFY * 32];   // per warp: packed colour of pixel `lane` of fine bin f at f * 32 + lane
+  // per warp: the edge-pixel queue, an entry in two words: (pixel slot, pxa, pya, wn0 | wn1 << 16), (wn2 | wn3 << 16, first colour)
+  __shared__ uint4 edge_q[kWarps][2][kEdgeQ];
   const int W = rc.width, H = rc.height;
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW, cbins = cbins_x * ((H + kCoarseH - 1) / kCoarseH);
   const int lane = threadIdx.x & 31;
   BinRec* stage = stages[threadIdx.x >> 5];
-  const StoreLane sl = make_store_lane(lane, W);
+  unsigned* rgb_buf = bin_rgb[threadIdx.x >> 5];
+  uint4 (*q)[kEdgeQ] = edge_q[threadIdx.x >> 5];
   const size_t frame_bytes = (size_t)W * H * 3;
   const int pxs = (lane & 7) * kSub, pys = (lane >> 3) * kSub;   // this lane's pixel inside a fine bin (sub-pixels)
-  const int n = fm.work[kWorkFlatList];
   const int warps = (gridDim.x * blockDim.x) >> 5;
-  for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+  // (the list length is read per bin, from L1: held across the bin it would take a register)
+  for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < __ldg(fm.work + kWorkFlatList); i += warps) {
     const uint2 e = fm.flat[i];
     const int env = (int)e.x, b = (int)(e.y & 0xffffu), count = (int)(e.y >> 16);
     const int cby = b / cbins_x, cbx = b - cby * cbins_x;
@@ -1891,8 +1914,10 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
     // fine bins inside the image as column / row counts rather than fine_in_image(), as in k_raster_solo
     const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);
     const int ny = ((cby * kCFY + 1) * kBinH < H) ? 2 : 1;
+    unsigned qs = 0;   // edge-pixel queue: entries head = qs >> 16 .. tail - 1 = (qs & 0xffff) - 1, modulo kEdgeQ (one register)
+    int f = 0;
 #pragma unroll 1
-    for (int f = 0; f < kCFX * kCFY; f++) {
+    for (; f < kCFX * kCFY; f++) {
       if ((f & 3) >= nx || (f >> 2) >= ny) continue;
       const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);   // fine bin
       int pxc = pxs + (f & 3) * kBinW * kSub, pyc = pys + (f >> 2) * kBinH * kSub;   // this lane's pixel, coarse-relative
@@ -1950,9 +1975,52 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
           break;
         }
       }
-      unsigned rgb = shade_resolve(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane, err);
-      if (kFish && !px_valid) rgb = 0u;
-      store_bin_lean(out, sl, rgb, lane, bx, by, W, H);
+      // ---- every lane: its first winner.  One winner: the pixel is done.  More: it waits in the queue.  (A pixel the
+      // fisheye LUT gives no source is black either way.)
+      float c3[3] = {clr[0], clr[1], clr[2]};
+      if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, ox + pxc, oy + pyc, c3);
+      const bool edge = px_valid && !(wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0]);
+      const unsigned edges = __ballot_sync(0xffffffffu, edge);
+      const unsigned slot = f * 32 + lane;
+      if (edge) {
+        const int e = (qs + __popc(edges & ((1u << lane) - 1u))) & (kEdgeQ - 1);
+        q[0][e] = make_uint4(slot, (unsigned)(ox + pxc), (unsigned)(oy + pyc), wn[0] | (wn[1] << 16));
+        q[1][e] = make_uint4(wn[2] | (wn[3] << 16), __float_as_uint(c3[0]), __float_as_uint(c3[1]), __float_as_uint(c3[2]));
+      } else {
+        rgb_buf[slot] = (kFish && !px_valid) ? 0u : pack_rgb(c3[0], c3[1], c3[2]);
+      }
+      qs += __popc(edges);
+      DTS_COUNT(26, __popc(edges));
+      // ---- the queued pixels' other winners, one pixel per lane: 32 at a time, and what is left after the last fine bin
+#pragma unroll 1
+      for (int nq = (qs & 0xffffu) - (qs >> 16); nq >= 32 || (nq > 0 && f == (ny - 1) * kCFX + nx - 1); nq = (qs & 0xffffu) - (qs >> 16)) {
+        DTS_COUNT(27, 1);
+        const int take = min(nq, 32);
+        __syncwarp();   // the entries were written by other lanes
+        unsigned qw[4] = {0u, 0u, 0u, 0u};   // (lanes without an entry: one winner, nothing to shade)
+        float q3[3] = {0.f, 0.f, 0.f};
+        unsigned qslot = 0u;
+        int qx = 0, qy = 0;
+        if (lane < take) {
+          const int e = ((qs >> 16) + lane) & (kEdgeQ - 1);
+          const uint4 a = q[0][e], c = q[1][e];
+          qslot = a.x; qx = (int)a.y; qy = (int)a.z;
+          qw[0] = a.w & 0xffffu; qw[1] = a.w >> 16; qw[2] = c.x & 0xffffu; qw[3] = c.x >> 16;
+          q3[0] = __uint_as_float(c.y); q3[1] = __uint_as_float(c.z); q3[2] = __uint_as_float(c.w);
+        }
+        resolve_edge(qw, q3, clr, prims, tex_pool, lat_tab, qx, qy, lane, err);
+        if (lane < take) rgb_buf[qslot] = pack_rgb(q3[0], q3[1], q3[2]);
+        qs += (unsigned)take << 16;
+        __syncwarp();   // read before the next fine bin's entries overwrite the ring
+      }
+    }
+    if (f < kCFX * kCFY) continue;   // handed back
+    __syncwarp();   // queued pixels' colours were written by other lanes
+    const StoreLane sl = make_store_lane(lane, W);   // (made here: held across the bin it would cost registers)
+#pragma unroll 1
+    for (int f = 0; f < kCFX * kCFY; f++) {
+      if ((f & 3) >= nx || (f >> 2) >= ny) continue;
+      store_bin_lean(out, sl, rgb_buf[f * 32 + lane], lane, cbx * kCFX + (f & 3), cby * kCFY + (f >> 2), W, H);
     }
   }
 }
