@@ -1,9 +1,7 @@
 // dts_api.cu — the C ABI of libdtsim.so (include/dtsim.h): handle management, host->device
 // staging of maps and episode parameters, and stream-ordered launches of the kernels.
-#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <dlfcn.h>
 #include <string>
@@ -34,10 +32,7 @@ struct dts_sim {
   // reset staging (device) sized num_envs
   struct { int32_t* map_id; double *pos_x, *pos_z, *angle, *wheel_dist, *trim; float *f1[3]; float *f3[5];
            float* light_pos; int32_t* light_stale; uint32_t* hidden; } stage{};
-  // render
-  void* render_scratch = nullptr;
-  int render_ctas = 0, max_prims = 0, bin_cap = 0, max_lat = 0, items_max = 0;
-  FishTab fish{};   // fused fisheye tables (dts_set_fisheye_lut)
+  Renderer* render = nullptr;           // frame memory and fisheye tables
   int32_t* d_err = nullptr;
   int32_t* h_status = nullptr;          // mapped pinned host word: bit 0 = a frame overflowed its frame memory
   int32_t* d_status = nullptr;          // its device address
@@ -188,6 +183,7 @@ int dts_create(const dts_config* cfg, dts_sim** out) {
   bad |= sim->dalloc(&st.light_pos, 4 * (size_t)n);
   bad |= sim->dalloc(&st.light_stale, n);
   bad |= sim->dalloc(&st.hidden, 8 * (size_t)n);
+  sim->render = renderer_create(*cfg);
   if (bad) { g_create_error = sim->err; dts_destroy(sim); return 1; }
   sim->h_maps.assign(cfg->max_maps, DMap{});
   sim->map_allocs.resize(cfg->max_maps);
@@ -201,9 +197,8 @@ void dts_destroy(dts_sim* sim) {
   cudaDeviceSynchronize();
   for (void* p : sim->allocs) cudaFree(p);
   for (auto& v : sim->map_allocs) for (void* p : v) cudaFree(p);
-  void* extra[] = {sim->render_scratch, (void*)sim->fish.src_xy, (void*)sim->fish.cbox, (void*)sim->fish.fbox, (void*)sim->fish.rbox,
-                   (void*)sim->fish.cell_start, (void*)sim->fish.cell_bins, (void*)sim->fish.home_start, (void*)sim->fish.home_ent,
-                   sim->q_in, sim->q_outd, sim->q_outi, sim->q_hidden};
+  renderer_destroy(sim->render);
+  void* extra[] = {sim->q_in, sim->q_outd, sim->q_outi, sim->q_hidden};
   for (void* p : extra) if (p) cudaFree(p);
   for (int p = 0; p < sim->gather_world; p++)
     if (sim->gather_peer[p] && sim->gather_peer[p] != sim->gather_buf) cudaIpcCloseMemHandle(sim->gather_peer[p]);
@@ -413,7 +408,7 @@ int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
     return 1;
   }
   m.valid = 1;
-  if (sim->render_scratch) { cudaFree(sim->render_scratch); sim->render_scratch = nullptr; }   // re-sized for the new scene on the next render
+  renderer_release_frame(*sim->render);
   sim->h_maps[map_id] = m;
   DTS_CUDA(cudaMemcpy(sim->d_maps + map_id, &m, sizeof(DMap), cudaMemcpyHostToDevice));
   return 0;
@@ -425,100 +420,9 @@ int dts_set_fisheye_lut(dts_sim* sim, const float* rmapx, const float* rmapy, in
   if (width != sim->cfg.cam_width || height != sim->cfg.cam_height)
     return sim->fail("fisheye LUT is %dx%d but the camera is %dx%d", width, height, sim->cfg.cam_width, sim->cfg.cam_height);
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  // distortion.py:118 gathers img[rint(rmapy), rint(rmapx)].  The rasteriser renders those source pixels directly
-  // (FishTab): per output pixel the source position, per 8x4 fine / 32x8 coarse output bin / row of coarse bins the
-  // bounding box of its source pixels (the bins prims are sorted into).
-  const int W = width, H = height;
-  const int cbx_n = (W + 31) / 32, cby_n = (H + 7) / 8, cbins = cbx_n * cby_n;
-  std::vector<int32_t> src((size_t)W * H);
-  const short4 empty = make_short4(32767, 32767, -32768, -32768);
-  std::vector<short4> cbox(cbins, empty), fbox((size_t)cbins * 8, empty), rbox(cby_n, empty);
-  auto grow = [](short4& b, int x, int y) {
-    b.x = (short)(x < b.x ? x : b.x); b.y = (short)(y < b.y ? y : b.y);
-    b.z = (short)(x > b.z ? x : b.z); b.w = (short)(y > b.w ? y : b.w);
-  };
-  for (int y = 0; y < H; y++)
-    for (int x = 0; x < W; x++) {
-      const float fx = rmapx[(size_t)y * W + x], fy = rmapy[(size_t)y * W + x];
-      const int sx = (int)rintf(fx), sy = (int)rintf(fy);   // round-half-even like the kernel's rintf
-      const bool ok = fx == fx && fy == fy && sx >= 0 && sx < W && sy >= 0 && sy < H;
-      src[(size_t)y * W + x] = ok ? (int32_t)((uint32_t)(sx & 0xffff) | ((uint32_t)sy << 16)) : (int32_t)0x80008000u;
-      if (!ok) continue;
-      const int cb = (y / 8) * cbx_n + x / 32, f = ((y & 7) >> 2) * 4 + ((x & 31) >> 3);
-      grow(cbox[cb], sx, sy); grow(fbox[(size_t)cb * 8 + f], sx, sy); grow(rbox[y / 8], sx, sy);
-    }
-  // int32 edge functions inside a coarse bin need |A x + B y| < 2^30 over its source box: |A| <= 5*64*H, |B| <= 5*64*W
-  // (4x guard band), x <= 64*w, y <= 64*h  ->  H*w + W*h < 2^30 / (5*64*64)
-  for (int b = 0; b < cbins; b++) {
-    if (cbox[b].z < cbox[b].x) continue;
-    const long long w = cbox[b].z - cbox[b].x + 2, h = cbox[b].w - cbox[b].y + 2;
-    if ((long long)H * w + (long long)W * h >= (1LL << 30) / (5 * 64 * 64))
-      return sim->fail("fisheye LUT sends output bin %d to a %lldx%lld px source region: too wide for the rasteriser's int32 edge functions", b, w, h);
-  }
-  // inverse index: source cell (same 32x8 grid, over the source image) -> output bins whose source box meets it
-  std::vector<int32_t> cell_start(cbins + 1, 0);
-  std::vector<uint16_t> cell_bins;
-  {
-    std::vector<std::vector<uint16_t>> lists(cbins);
-    for (int b = 0; b < cbins; b++) {
-      if (cbox[b].z < cbox[b].x) continue;
-      for (int cy = cbox[b].y / 8; cy <= cbox[b].w / 8; cy++)
-        for (int cx = cbox[b].x / 32; cx <= cbox[b].z / 32; cx++) lists[cy * cbx_n + cx].push_back((uint16_t)b);
-    }
-    for (int c = 0; c < cbins; c++) {
-      cell_start[c] = (int32_t)cell_bins.size();
-      cell_bins.insert(cell_bins.end(), lists[c].begin(), lists[c].end());
-    }
-    cell_start[cbins] = (int32_t)cell_bins.size();
-    if (cell_bins.empty()) cell_bins.push_back(0);
-  }
-  // ... and the index by HOME cell (the cell of the box's top-left corner): each bin once, with its box
-  std::vector<int32_t> home_start(cbins + 1, 0);
-  std::vector<int4> home_ent;
-  int ext_x = 0, ext_y = 0;
-  {
-    std::vector<std::vector<int>> lists(cbins);
-    for (int b = 0; b < cbins; b++) {
-      if (cbox[b].z < cbox[b].x) continue;
-      lists[(cbox[b].y / 8) * cbx_n + cbox[b].x / 32].push_back(b);
-      ext_x = std::max(ext_x, cbox[b].z / 32 - cbox[b].x / 32);
-      ext_y = std::max(ext_y, cbox[b].w / 8 - cbox[b].y / 8);
-    }
-    for (int c = 0; c < cbins; c++) {
-      home_start[c] = (int32_t)home_ent.size();
-      for (int b : lists[c])
-        home_ent.push_back(make_int4((int)((uint32_t)(uint16_t)cbox[b].x | ((uint32_t)(uint16_t)cbox[b].y << 16)),
-                                     (int)((uint32_t)(uint16_t)cbox[b].z | ((uint32_t)(uint16_t)cbox[b].w << 16)), b, 0));
-    }
-    home_start[cbins] = (int32_t)home_ent.size();
-    if (home_ent.empty()) home_ent.push_back(make_int4(0, 0, 0, 0));
-  }
-  void* old[] = {(void*)sim->fish.src_xy, (void*)sim->fish.cbox, (void*)sim->fish.fbox, (void*)sim->fish.rbox,
-                 (void*)sim->fish.cell_start, (void*)sim->fish.cell_bins, (void*)sim->fish.home_start, (void*)sim->fish.home_ent};
   DTS_CUDA(cudaDeviceSynchronize());
-  for (void* p : old) if (p) cudaFree(p);
-  sim->fish = FishTab{};
-  int32_t* d_src = nullptr; short4 *d_c = nullptr, *d_f = nullptr, *d_r = nullptr;
-  DTS_CUDA(cudaMalloc(&d_src, src.size() * sizeof(int32_t)));
-  DTS_CUDA(cudaMalloc(&d_c, cbox.size() * sizeof(short4)));
-  DTS_CUDA(cudaMalloc(&d_f, fbox.size() * sizeof(short4)));
-  DTS_CUDA(cudaMalloc(&d_r, rbox.size() * sizeof(short4)));
-  DTS_CUDA(cudaMemcpy(d_src, src.data(), src.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-  DTS_CUDA(cudaMemcpy(d_c, cbox.data(), cbox.size() * sizeof(short4), cudaMemcpyHostToDevice));
-  DTS_CUDA(cudaMemcpy(d_f, fbox.data(), fbox.size() * sizeof(short4), cudaMemcpyHostToDevice));
-  DTS_CUDA(cudaMemcpy(d_r, rbox.data(), rbox.size() * sizeof(short4), cudaMemcpyHostToDevice));
-  int32_t* d_cs = nullptr; uint16_t* d_cb = nullptr;
-  DTS_CUDA(cudaMalloc(&d_cs, cell_start.size() * sizeof(int32_t)));
-  DTS_CUDA(cudaMalloc(&d_cb, cell_bins.size() * sizeof(uint16_t)));
-  DTS_CUDA(cudaMemcpy(d_cs, cell_start.data(), cell_start.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-  DTS_CUDA(cudaMemcpy(d_cb, cell_bins.data(), cell_bins.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-  int32_t* d_hs = nullptr; int4* d_he = nullptr;
-  DTS_CUDA(cudaMalloc(&d_hs, home_start.size() * sizeof(int32_t)));
-  DTS_CUDA(cudaMalloc(&d_he, home_ent.size() * sizeof(int4)));
-  DTS_CUDA(cudaMemcpy(d_hs, home_start.data(), home_start.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-  DTS_CUDA(cudaMemcpy(d_he, home_ent.data(), home_ent.size() * sizeof(int4), cudaMemcpyHostToDevice));
-  sim->fish = FishTab{d_src, d_c, d_f, d_r, d_cs, d_cb, d_hs, d_he, ext_x, ext_y};
-  return 0;
+  const std::string e = renderer_set_fisheye(*sim->render, rmapx, rmapy);
+  return e.empty() ? 0 : sim->fail("%s", e.c_str());
 }
 
 // > 0: round-robin over that many slots; < 0: uniform draw over -n slots; 0: the env keeps its map
@@ -592,57 +496,13 @@ int dts_reset_random(dts_sim* sim, const uint8_t* mask_dev, void* stream) {
   return 0;
 }
 
-static int ensure_render(dts_sim* sim) {
-  if (sim->render_scratch) return 0;
-  int sms = 132;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, sim->cfg.device);
-  const bool tess = (sim->cfg.flags & DTS_FLAG_TESSELLATE) != 0;
-  int max_tris = 2, max_lat = 1, items_max = 1;
-  for (const DMap& m : sim->h_maps) {
-    if (!m.valid) continue;
-    int t = 2 + (tess ? 98 : 6) * m.n_tiles + m.agent.tri_count;   // a clipped tile quad fans into a few triangles
-    std::vector<DObject> objs(m.n_objects);
-    if (m.n_objects) cudaMemcpy(objs.data(), m.objects, sizeof(DObject) * m.n_objects, cudaMemcpyDeviceToHost);
-    for (const DObject& o : objs) t += o.tri_count;
-    max_tris = t > max_tris ? t : max_tris;
-    max_lat = m.n_tiles > max_lat ? m.n_tiles : max_lat;
-    const int items = 1 + m.n_tiles + m.n_objects + 1;   // + the agent's own mesh (top-down views)
-    items_max = items > items_max ? items : items_max;
-  }
-  sim->render_ctas = sms * render_ctas_per_sm();
-  sim->max_prims = max_tris + max_tris / 4 + 64;  // clipping can add fan triangles
-  if (items_max > 65535) return sim->fail("scene too large: %d draw items per frame (limit 65535)", items_max);
-  if (sim->max_prims > 65535) return sim->fail("scene too large: %d triangles per frame (limit 65535)", sim->max_prims);
-  sim->max_lat = max_lat;
-  sim->items_max = items_max;
-  const int cbins = ((sim->cfg.cam_width + 31) / 32) * ((sim->cfg.cam_height + 7) / 8);
-  // (prim, coarse bin) pairs.  Upper bound per env: the ground fan (<= 8 x cbins), a few screen-filling tiles and one
-  // screen-filling prop; under the fused fisheye the bins are overlapping source boxes (x ~4).  The batch shares ONE
-  // pool, each env taking exactly what its frame needs: capacity = that bound x num_envs, capped at DTS_PAIR_POOL_GB
-  // (default 16) of records — a typical frame uses a small fraction of its bound.
-  const long long per_env = (3LL * sim->max_prims + 24LL * cbins + 256) * ((sim->cfg.flags & DTS_FLAG_DISTORTION) ? 4 : 1);
-  double pool_gb = 16.0;
-  if (const char* e = getenv("DTS_PAIR_POOL_GB")) pool_gb = atof(e) > 0 ? atof(e) : pool_gb;
-  long long pool = per_env * sim->cfg.num_envs;
-  const long long cap = (long long)(pool_gb * 1073741824.0 / 84.0);
-  if (pool > cap) pool = cap;
-  if (pool > 2000000000LL) pool = 2000000000LL;
-  if (pool < per_env) pool = per_env;
-  sim->bin_cap = (int)pool;
-  const size_t frame = (size_t)sim->items_max;   // (env, item) work-list entries per env
-  const size_t bytes = render_scratch_bytes(sim->cfg.num_envs, sim->max_prims, cbins, sim->bin_cap, sim->max_lat, frame);
-  cudaError_t e = cudaMalloc(&sim->render_scratch, bytes);
-  if (e != cudaSuccess) return sim->fail("render scratch cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
-  return 0;
-}
-
 int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
   if (!sim) return 1;
   if (!obs_dev) return sim->fail("obs_dev is NULL");
   if (check_maps(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  if (ensure_render(sim)) return 1;
-  if ((sim->cfg.flags & DTS_FLAG_DISTORTION) && !sim->fish.src_xy) return sim->fail("distortion enabled but no fisheye LUT set");
+  const std::string e = renderer_prepare(*sim->render, sim->h_maps.data(), (int)sim->h_maps.size());
+  if (!e.empty()) return sim->fail("%s", e.c_str());
   RenderCfg rc{sim->cfg.cam_width, sim->cfg.cam_height, sim->cfg.flags, sim->cfg.num_envs,
                (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->render_mode};
   if (*(volatile int32_t*)sim->h_status & 1)
@@ -669,9 +529,8 @@ int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
       gt.base[p] = reinterpret_cast<uint8_t*>(sim->gather_peer[p]) + (uint64_t)sim->gather_rank * sim->gather_bytes;
     sim->gather_next = false;
   }
-  int k = launch_render(sim->S, sim->d_maps, rc, target, sim->render_scratch, sim->render_ctas, sim->max_prims,
-                        sim->bin_cap, sim->max_lat, sim->items_max, sim->fish, gt, sim->d_err,
-                        sim->d_status, marks, mark_level, (cudaStream_t)stream);
+  int k = launch_render(*sim->render, sim->S, sim->d_maps, rc, target, gt, sim->d_err, sim->d_status, marks, mark_level,
+                        (cudaStream_t)stream);
   if (sim->resize_w) {
     launch_resize(sim->resize_src, sim->cfg.cam_width, sim->cfg.cam_height, sim->resize_w, sim->resize_h, sim->cfg.num_envs,
                   sim->resize_xtab, sim->resize_ytab, obs_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->resize_band, sim->resize_cap,
@@ -798,20 +657,7 @@ int dts_set_resize(dts_sim* sim, int out_w, int out_h) {
   DTS_CUDA(cudaMemcpy(sim->resize_xtab, xt.data(), xt.size() * 2, cudaMemcpyHostToDevice));
   DTS_CUDA(cudaMemcpy(sim->resize_ytab, yt.data(), yt.size() * 2, cudaMemcpyHostToDevice));
   sim->resize_w = out_w; sim->resize_h = out_h;
-  // band height of the tiled kernel: the tallest band (<= 16 output rows) whose source rows + horizontal sums fit in 40 KB
-  // of shared memory (several CTAs per SM); 0 = no band fits even in the opt-in maximum, use the untiled kernel
-  sim->resize_band = sim->resize_cap = 0;
-  const char* untiled = getenv("DTS_RESIZE_UNTILED");   // A/B switch
-  const size_t budget = (size_t)(getenv("DTS_RESIZE_SMEM_KB") ? atoi(getenv("DTS_RESIZE_SMEM_KB")) : 40) * 1024;   // A/B: shared memory per band
-  for (int R = 16; R >= 1 && !(untiled && untiled[0] == '1'); R--) {
-    int cap = 0;
-    for (int r0 = 0; r0 < out_h; r0 += R) {
-      const int r1 = std::min(r0 + R, out_h);
-      cap = std::max(cap, (int)yt[(size_t)8 * (r1 - 1) + 3] - (int)yt[(size_t)8 * r0] + 1);
-    }
-    const size_t smem = resize_band_smem(sim->cfg.cam_width, out_w, cap);
-    if (smem <= budget || (R == 1 && smem <= 200 * 1024)) { sim->resize_band = R; sim->resize_cap = cap; break; }
-  }
+  plan_resize_bands(sim->cfg.cam_width, out_w, out_h, yt.data(), &sim->resize_band, &sim->resize_cap);
   return 0;
 }
 
@@ -964,16 +810,10 @@ int dts_debug_episode(dts_sim* sim, int env, void* out144) {
 int dts_debug_frame(dts_sim* sim, int env, double V[12], float P[4], int32_t counts[4], float* lattice_by_cell, int n_cells) {
   if (!sim) return 1;
   if (env < 0 || env >= sim->cfg.num_envs) return sim->fail("env out of range");
-  if (!sim->render_scratch) return sim->fail("nothing rendered yet");
-  if (sim->cfg.flags & DTS_FLAG_TESSELLATE) return sim->fail("dts_debug_frame reads the analytic-tile lattice (tile mode 1)");
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   DTS_CUDA(cudaDeviceSynchronize());
-  const int cbins = ((sim->cfg.cam_width + 31) / 32) * ((sim->cfg.cam_height + 7) / 8);
-  const size_t frame = (size_t)sim->items_max;
-  if (debug_frame_copy(sim->render_scratch, sim->cfg.num_envs, sim->max_prims, cbins, sim->bin_cap, sim->max_lat, frame, env, V, P,
-                       counts, lattice_by_cell, n_cells, 2))
-    return sim->fail("debug_frame_copy failed");
-  return 0;
+  const std::string e = debug_frame_copy(*sim->render, env, V, P, counts, lattice_by_cell, n_cells);
+  return e.empty() ? 0 : sim->fail("%s", e.c_str());
 }
 
 /* debug: copy the 32 int32 diagnostic counters (word 0 = overflow flag; 8.. = DTS_STATS counters) */

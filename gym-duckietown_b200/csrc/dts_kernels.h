@@ -1,5 +1,7 @@
 // dts_kernels.h — host-callable launchers of the dtsim kernels.
 #pragma once
+#include <string>
+
 #include "dts_common.cuh"
 
 namespace dts {
@@ -34,26 +36,6 @@ void launch_assign_maps(const DState& S, const DMap* maps, const uint8_t* mask, 
 void launch_query(const DMap* maps, int map_id, int dyn_env, int n_envs, int n, const double* q, const uint32_t* hidden,
                   double* outd, int32_t* outi, cudaStream_t st);
 
-// Fused fisheye gather (distortion.py:118, obs[y, x] = undistorted[rint(rmapy), rint(rmapx)]): the rasteriser renders
-// each OUTPUT pixel at the source position the LUT names, so no undistorted frame is ever written.  Prims are binned
-// against the source-pixel bounding boxes of the output bins.  All device pointers, built by dts_set_fisheye_lut.
-struct FishTab {
-  const int32_t* src_xy;   // [H][W]  sx | sy << 16 (int16 each); sx = -32768: source outside the image -> 0
-  const short4* cbox;      // [cbins]    source bounding box (x0, y0, x1, y1) of a 32x8 coarse output bin; x1 < x0: empty
-  const short4* fbox;      // [cbins][8] the same for each of its 8x4 fine bins
-  const short4* rbox;      // [cbins_y]  and for each row of coarse bins
-  // inverse index for binning small prims: the output coarse bins whose source box meets cell c of a 32x8-px grid laid
-  // over the SOURCE image (CSR: cell_bins[cell_start[c] .. cell_start[c + 1]))
-  const int32_t* cell_start;   // [cbins + 1]
-  const uint16_t* cell_bins;
-  // second inverse index for prims spanning many cells: every output bin listed ONCE, under the source cell holding the
-  // top-left corner of its box (CSR); an entry is (x0 | y0 << 16, x1 | y1 << 16, bin, 0).  ext_x / ext_y: how many
-  // cells a box reaches to the right of / below its home cell at most
-  const int32_t* home_start;   // [cbins + 1]
-  const int4* home_ent;
-  int ext_x, ext_y;
-};
-
 // Fused end-of-rollout observation gather (SURVEY 8e): on the rollout's last step the rasteriser's resolve stores every
 // frame, besides the caller's tensor, straight into the gather buffers of all GPUs of the box — peer memory mapped with
 // cudaIpc, written over NVLink while the frame is being rasterised — instead of a separate all-gather pass afterwards.
@@ -64,24 +46,33 @@ struct GatherTab {
   uint8_t* base[DTS_MAX_PEERS];
 };
 
-// render (dts_render.cu)
-int render_ctas_per_sm();
-// scratch for `n` envs: FrameCtx, PrimRec slabs, the batch's pair / record pool (max_pairs entries), lattice tables and
-// the (env, item) work list of the geometry pass
-size_t render_scratch_bytes(int n, int max_prims, int cbins, int max_pairs, int max_lat, size_t geo_items);
+// render (dts_render.cu).  The renderer of one handle: the launch sizes, the frame memory, sized from the uploaded maps,
+// and the fisheye tables.  Functions that can fail return the error text, empty on success.
+struct Renderer;
+Renderer* renderer_create(const dts_config& cfg);   // on cfg.device, which must be current
+void renderer_destroy(Renderer* r);
+void renderer_release_frame(Renderer& r);   // the maps changed: the next render re-sizes frame memory for them
+// Before every render: reserves frame memory for the valid maps of maps[0 .. n_maps) unless it is reserved, and checks
+// that a fisheye LUT is set if the camera needs one.
+std::string renderer_prepare(Renderer& r, const DMap* maps, int n_maps);
+// The fused fisheye's tables for a LUT of the camera's size (obs[y, x] = frame[rint(rmapy), rint(rmapx)]); they replace
+// the previous ones, so no render may be in flight.  A LUT the rasteriser cannot take leaves the previous tables.
+std::string renderer_set_fisheye(Renderer& r, const float* rmapx, const float* rmapy);
 // `marks`: NULL or kProfMarks events recorded on `st` before k_frame_setup and after each of k_frame_setup, k_geometry,
 // k_bin, k_raster and the post passes (dts_profile_*).  `status_dev`: device address of the mapped host status word.
 constexpr int kProfMarks = 6;
-int launch_render(const DState& S, const DMap* maps, const RenderCfg& rc, void* obs, void* scratch, int n_ctas,
-                  int max_prims, int max_pairs, int max_lat, int items_max, const FishTab& fish, const GatherTab& gather,
+int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, void* obs, const GatherTab& gather,
                   int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level, cudaStream_t st);
+// What the last render left in frame memory for one env (dts_debug_frame), after the device has synchronised
+std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, int32_t* counts, float* lattice_by_cell,
+                             int n_cells);
 
 // ResizeWrapper on the device: src u8[N][H][W][3] -> dst [N] x (ow x oh) in `layout` / `dtype` (dts_set_resize)
 void launch_resize(const uint8_t* src, int W, int H, int ow, int oh, int n_envs, const int16_t* xtab, const int16_t* ytab,
                    void* dst, int layout, int dtype, int band_rows, int band_cap, cudaStream_t st);
-size_t resize_band_smem(int W, int ow, int cap);   // dynamic shared memory of k_resize_band for a band spanning `cap` source rows
+// Output rows per CTA of k_resize_band and the largest source-row span of a band, for the row tap table `ytab`
+// ([oh][8]); both 0: the untiled k_resize
+void plan_resize_bands(int W, int ow, int oh, const int16_t* ytab, int* band_rows, int* band_cap);
 void launch_blend4(const uint8_t* const f[4], const double w[4], double* out, size_t n, cudaStream_t st);
-int debug_frame_copy(void* scratch, int n, int max_prims, int cbins, int max_pairs, int max_lat, size_t geo_items,
-                     int env, double* V, float* P, int32_t* counts, float* lattice_by_cell, int n_cells, int tris_per_tile);
 
 }  // namespace dts

@@ -27,12 +27,35 @@
 //
 // HBM traffic per env-frame: obs store W*H*3 B (compulsory) + PrimRec slab / BinRec lists / lattice table
 // (tens of KB per env, written by k_geometry / k_bin and read once by k_raster) + texels (shared, L2-resident).
+#include <algorithm>
 #include <cstddef>
+#include <cstdlib>
+#include <type_traits>
+#include <vector>
 
 #include "dts_camera.cuh"
 #include "dts_kernels.h"
 
 namespace dts {
+
+// Fused fisheye gather (distortion.py:118, obs[y, x] = undistorted[rint(rmapy), rint(rmapx)]): the rasteriser renders
+// each OUTPUT pixel at the source position the LUT names, so no undistorted frame is ever written.  Prims are binned
+// against the source-pixel bounding boxes of the output bins.  All device pointers, built by renderer_set_fisheye.
+struct FishTab {
+  const int32_t* src_xy;   // [H][W]  sx | sy << 16 (int16 each); sx = -32768: source outside the image -> 0
+  const short4* cbox;      // [cbins]    source bounding box (x0, y0, x1, y1) of a 32x8 coarse output bin; x1 < x0: empty
+  const short4* fbox;      // [cbins][8] the same for each of its 8x4 fine bins
+  // inverse index for binning small prims: the output coarse bins whose source box meets cell c of a 32x8-px grid laid
+  // over the SOURCE image (CSR: cell_bins[cell_start[c] .. cell_start[c + 1]))
+  const int32_t* cell_start;   // [cbins + 1]
+  const uint16_t* cell_bins;
+  // second inverse index for prims spanning many cells: every output bin listed ONCE, under the source cell holding the
+  // top-left corner of its box (CSR); an entry is (x0 | y0 << 16, x1 | y1 << 16, bin, 0).  ext_x / ext_y: how many
+  // cells a box reaches to the right of / below its home cell at most
+  const int32_t* home_start;   // [cbins + 1]
+  const int4* home_ent;
+  int ext_x, ext_y;
+};
 
 namespace {
 
@@ -59,6 +82,11 @@ constexpr int kCoarseW = kBinW * kCFX, kCoarseH = kBinH * kCFY;
 constexpr int kStage = 32;        // prims staged per pass and warp
 constexpr float kGuard = 4.0f;
 constexpr int kSub = 64;          // sub-pixel units per pixel
+constexpr int kTessTris = 98;     // spec tile mode 0: a road tile is its literal 7x7 quads, two triangles each
+// Draw ids of one road tile: its triangles in tile mode 0; in tile mode 1 its quad, or the two triangles it splits into
+__host__ __device__ constexpr int tile_draw_ids(bool tess) { return tess ? kTessTris : 2; }
+// Draw items of a frame: the ground (item 0), the tiles, the placed objects, and last the agent's own mesh
+__host__ __device__ constexpr int agent_item(int n_tiles, int n_objects) { return 1 + n_tiles + n_objects; }
 // MSAA sample offsets in 1/64 px, (.375,.125)(.875,.375)(.125,.625)(.625,.875); constexpr so that the
 // unrolled sample loops fold them into immediates
 __host__ __device__ constexpr int sample_x(int s) { return s == 0 ? 24 : (s == 1 ? 56 : (s == 2 ? 8 : 40)); }
@@ -795,9 +823,6 @@ __device__ __forceinline__ void clear_colour(const DState& S, const RenderCfg& r
 
 }  // namespace
 
-
-int render_ctas_per_sm() { return kRasterMinCtas; }
-
 // ------------------------------------------------------------------------------------------------ frame memory
 struct FrameMem {
   FrameCtx* ctx;        // [N]
@@ -821,30 +846,39 @@ constexpr int kWorkFlatList = 4;   // flat list length (k_bin -> k_raster_flat)
 
 __host__ __device__ inline size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
 
-__host__ FrameMem carve(void* scratch, int n, int max_prims, int cbins, int max_pairs, int max_lat, size_t geo_items) {
-  uint8_t* p = reinterpret_cast<uint8_t*>(scratch);
-  FrameMem f;
-  f.work = reinterpret_cast<int*>(p); p += 256;
-  f.ctx = reinterpret_cast<FrameCtx*>(p); p += align256((size_t)n * sizeof(FrameCtx));
-  f.bin_count = reinterpret_cast<int*>(p); p += align256((size_t)n * cbins * sizeof(int));
-  f.bin_start = reinterpret_cast<int*>(p); p += align256((size_t)n * cbins * sizeof(int));
-  f.prims = reinterpret_cast<PrimRec*>(p); p += align256((size_t)n * max_prims * sizeof(PrimRec));
-  f.pairs = reinterpret_cast<uint32_t*>(p); p += align256((size_t)max_pairs * sizeof(uint32_t));   // max_pairs = pool entries
-  f.recs = reinterpret_cast<BinRec*>(p); p += align256((size_t)max_pairs * sizeof(BinRec));
-  f.lat = reinterpret_cast<float4*>(p); p += align256((size_t)n * max_lat * 64 * sizeof(float4));
-  f.geo_list = reinterpret_cast<uint2*>(p); p += align256((size_t)n * geo_items * sizeof(uint2));
-  f.solo = reinterpret_cast<uint2*>(p); p += align256((size_t)n * cbins * sizeof(uint2));
-  f.flat = reinterpret_cast<uint2*>(p); p += align256((size_t)n * cbins * sizeof(uint2));
-  f.status = nullptr;
-  return f;
-}
+struct Renderer {
+  int n, W, H, flags;        // envs, camera and DTS_FLAG_* of the handle
+  int sms;                   // launch sizes are SMs x resident CTAs per SM of each kernel
+  int cbins;                 // coarse bins per frame
+  // frame sizes, set with the frame memory from the uploaded maps: PrimRec slab and lattice slots per env, draw items
+  // per env, and entries of the batch's pair pool
+  int max_prims = 0, max_lat = 0, items_max = 0, pool = 0;
+  void* frame = nullptr;     // frame memory (null: not reserved since the last map upload)
+  FrameMem fm{};             // ... carved
+  FishTab fish{};            // fused fisheye tables (null until a LUT is set)
+};
 
-size_t render_scratch_bytes(int n, int max_prims, int cbins, int max_pairs, int max_lat, size_t geo_items) {
-  return 256 + align256((size_t)n * sizeof(FrameCtx)) + 2 * align256((size_t)n * cbins * sizeof(int)) +
-         align256((size_t)n * max_prims * sizeof(PrimRec)) + align256((size_t)max_pairs * sizeof(uint32_t)) +
-         align256((size_t)max_pairs * sizeof(BinRec)) +
-         align256((size_t)n * max_lat * 64 * sizeof(float4)) + align256((size_t)n * geo_items * sizeof(uint2)) +
-         2 * align256((size_t)n * cbins * sizeof(uint2)) + 256;
+// The one statement of the frame-memory layout: points `f` into the allocation at `base` and returns its size, so
+// carving from base 0 sizes it.
+__host__ size_t carve(const Renderer& r, uintptr_t base, FrameMem& f) {
+  const size_t n = r.n;
+  size_t o = 0;
+  auto take = [&](auto*& p, size_t count) {
+    p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(base + o);
+    o += align256(count * sizeof(*p));
+  };
+  take(f.work, 64);
+  take(f.ctx, n);
+  take(f.bin_count, n * r.cbins);
+  take(f.bin_start, n * r.cbins);
+  take(f.prims, n * r.max_prims);
+  take(f.pairs, r.pool);
+  take(f.recs, r.pool);
+  take(f.lat, n * r.max_lat * 64);
+  take(f.geo_list, n * r.items_max);
+  take(f.solo, n * r.cbins);
+  take(f.flat, n * r.cbins);
+  return o + 256;   // (+ 256 B of slack past the last list)
 }
 
 // ------------------------------------------------------------------------------------------------ k_frame_setup
@@ -895,8 +929,8 @@ __device__ __forceinline__ bool item_visible(const DState& S, const DMap& m, con
                                              int item, ItemPose& ip) {
   const int n_tiles = m.grid_w * m.grid_h;
   ip.dyn_kind = 0; ip.opx = 0.f; ip.opz = 0.f; ip.orot = 0.f;
-  ip.agent_item = item == 1 + n_tiles + m.n_objects;   // top-down views draw the agent's own mesh last (S:1923-1929)
-  if (item > 1 + n_tiles + m.n_objects) return false;
+  ip.agent_item = item == agent_item(n_tiles, m.n_objects);   // top-down views draw the agent's own mesh last (S:1923-1929)
+  if (item > agent_item(n_tiles, m.n_objects)) return false;
   if (ip.agent_item && (!(rc.mode & DTS_RENDER_TOP_DOWN) || m.agent.tri_count == 0)) return false;
   if (item >= 1 && item <= n_tiles) {
     const int t = item - 1, ti = t / m.grid_h, tj = t - ti * m.grid_h;
@@ -978,7 +1012,7 @@ __device__ __forceinline__ void geometry_item(const DState& S, const DMap* __res
   __syncwarp();
   EmitCtx ec{m.textures, &sh, &ctx, fm.prims + (size_t)env * max_prims, max_prims, W, H};
   float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
-  const int tris_per_tile = kTess ? 98 : 2;
+  const int tris_per_tile = tile_draw_ids(kTess);
   Xform& x = sh.x;
   if (item == 0) {
     // ground quad S:1805-1812: glScalef(50,0.01,50) applied to (+-1,-0.8,+-1), world-space +y normal
@@ -1067,10 +1101,10 @@ __device__ __forceinline__ void geometry_item(const DState& S, const DMap* __res
       }
       } else {
       // literal vertex list S:407-433 (spec tile mode 0): 7x7 quads, (0,1,2)(0,2,3) split, 3 shades / triangle
-      for (int k0 = 0; k0 < 98; k0 += 32) {
+      for (int k0 = 0; k0 < kTessTris; k0 += 32) {
         const int k = k0 + lane;
         Vtx v[3];
-        if (k < 98) {
+        if (k < kTessTris) {
           const int quad = k >> 1, half = k & 1, a = quad / 7, b = quad - 7 * a;
 #pragma unroll
           for (int j = 0; j < 3; j++) {
@@ -1081,7 +1115,7 @@ __device__ __forceinline__ void geometry_item(const DState& S, const DMap* __res
                                 (float)(1.0 - (double)bb / 7.0));
           }
         }
-        process_triangle_lanes(ec, k < 98, v[0], v[1], v[2], base_id + k, tex, -1, lane);
+        process_triangle_lanes(ec, k < kTessTris, v[0], v[1], v[2], base_id + k, tex, -1, lane);
           }
     }
   } else {
@@ -2189,13 +2223,33 @@ __global__ void __launch_bounds__(256) k_resize_band(const uint8_t* __restrict__
   }
 }
 
-size_t resize_band_smem(int W, int ow, int cap) {
+// dynamic shared memory of k_resize_band for a band spanning `cap` source rows
+static size_t resize_band_smem(int W, int ow, int cap) {
   return (size_t)ow * 16 + (((size_t)cap * W * 3 + 15) & ~(size_t)15) + (size_t)cap * ow * 3 * 4 + 16;   // (+16: word loads may run past the last row)
+}
+
+constexpr size_t kResizeBandSmem = 40 * 1024;   // shared memory a band may take and still leave room for several CTAs per SM
+
+void plan_resize_bands(int W, int ow, int oh, const int16_t* ytab, int* band_rows, int* band_cap) {
+  // the tallest band (<= 16 output rows) whose source rows + horizontal sums fit in kResizeBandSmem, or single rows in
+  // up to 200 KB (the opt-in maximum); otherwise, and under DTS_RESIZE_UNTILED=1, the untiled kernel
+  *band_rows = *band_cap = 0;
+  const char* untiled = getenv("DTS_RESIZE_UNTILED");
+  if (untiled && untiled[0] == '1') return;
+  for (int R = 16; R >= 1; R--) {
+    int cap = 0;
+    for (int r0 = 0; r0 < oh; r0 += R) {
+      const int r1 = std::min(r0 + R, oh);
+      cap = std::max(cap, (int)ytab[(size_t)8 * (r1 - 1) + 3] - (int)ytab[(size_t)8 * r0] + 1);
+    }
+    const size_t smem = resize_band_smem(W, ow, cap);
+    if (smem <= kResizeBandSmem || (R == 1 && smem <= 200 * 1024)) { *band_rows = R; *band_cap = cap; return; }
+  }
 }
 
 void launch_resize(const uint8_t* src, int W, int H, int ow, int oh, int n_envs, const int16_t* xtab, const int16_t* ytab,
                    void* dst, int layout, int dtype, int band_rows, int band_cap, cudaStream_t st) {
-  if (band_rows > 0) {   // tiled form (dts_set_resize found a band height whose rows fit in shared memory)
+  if (band_rows > 0) {   // tiled form (plan_resize_bands found a band height whose rows fit in shared memory)
     const size_t smem = resize_band_smem(W, ow, band_cap);
     static size_t opted = 0;
     if (smem > 48 * 1024 && smem > opted) { cudaFuncSetAttribute(k_resize_band, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); opted = smem; }
@@ -2209,24 +2263,175 @@ void launch_resize(const uint8_t* src, int W, int H, int ow, int oh, int n_envs,
   k_resize<<<blocks, 256, 0, st>>>(src, W, H, ow, oh, n_envs, xtab, ytab, dst, layout, dtype);
 }
 
+// ------------------------------------------------------------------------------------------------ the renderer
+static void free_fish(FishTab& f) {
+  const void* p[] = {f.src_xy, f.cbox, f.fbox, f.cell_start, f.cell_bins, f.home_start, f.home_ent};
+  for (const void* q : p) cudaFree(const_cast<void*>(q));
+  f = FishTab{};
+}
+
+Renderer* renderer_create(const dts_config& cfg) {
+  Renderer* r = new Renderer();
+  r->n = cfg.num_envs; r->W = cfg.cam_width; r->H = cfg.cam_height; r->flags = cfg.flags;
+  r->sms = 132;
+  cudaDeviceGetAttribute(&r->sms, cudaDevAttrMultiProcessorCount, cfg.device);
+  r->cbins = ((r->W + kCoarseW - 1) / kCoarseW) * ((r->H + kCoarseH - 1) / kCoarseH);
+  return r;
+}
+
+void renderer_release_frame(Renderer& r) {
+  cudaFree(r.frame);
+  r.frame = nullptr;
+}
+
+void renderer_destroy(Renderer* r) {
+  if (r) { renderer_release_frame(*r); free_fish(r->fish); }
+  delete r;
+}
+
+std::string renderer_prepare(Renderer& r, const DMap* maps, int n_maps) {
+  if (!r.frame) {
+    // prims k_geometry emits per road tile: the literal triangles of tile mode 0, or the quad of tile mode 1, which a
+    // clip splits into two triangles and fans into a few more
+    const int tile_prims = (r.flags & DTS_FLAG_TESSELLATE) ? kTessTris : 6;
+    int max_tris = 2, max_lat = 1, items_max = 1;
+    for (int i = 0; i < n_maps; i++) {
+      const DMap& m = maps[i];
+      if (!m.valid) continue;
+      int t = 2 + tile_prims * m.n_tiles + m.agent.tri_count;   // the ground quad's two triangles, the tiles, the meshes
+      std::vector<DObject> objs(m.n_objects);
+      if (m.n_objects) cudaMemcpy(objs.data(), m.objects, sizeof(DObject) * m.n_objects, cudaMemcpyDeviceToHost);
+      for (const DObject& o : objs) t += o.tri_count;
+      max_tris = std::max(max_tris, t);
+      max_lat = std::max(max_lat, m.n_tiles);
+      items_max = std::max(items_max, agent_item(m.n_tiles, m.n_objects) + 1);
+    }
+    const int max_prims = max_tris + max_tris / 4 + 64;   // clipping can add fan triangles
+    if (items_max > 65535) return "scene too large: " + std::to_string(items_max) + " draw items per frame (limit 65535)";
+    if (max_prims > 65535) return "scene too large: " + std::to_string(max_prims) + " triangles per frame (limit 65535)";
+    // (prim, coarse bin) pairs k_bin emits per env at most: the ground fan (<= 8 x cbins), a few screen-filling tiles
+    // and one screen-filling prop; under the fused fisheye the bins are overlapping source boxes (x ~4).  The batch
+    // shares ONE pool, each env taking exactly what its frame needs: capacity = that bound x num_envs, capped at
+    // DTS_PAIR_POOL_GB (default 16) of pairs and records — a typical frame uses a small fraction of its bound.
+    const long long per_env = (3LL * max_prims + 24LL * r.cbins + 256) * ((r.flags & DTS_FLAG_DISTORTION) ? 4 : 1);
+    double pool_gb = 16.0;
+    if (const char* e = getenv("DTS_PAIR_POOL_GB")) pool_gb = atof(e) > 0 ? atof(e) : pool_gb;
+    const long long cap = (long long)(pool_gb * 1073741824.0 / (double)(sizeof(uint32_t) + sizeof(BinRec)));
+    const long long pool = std::max(std::min({per_env * r.n, cap, 2000000000LL}), per_env);
+    r.max_prims = max_prims; r.max_lat = max_lat; r.items_max = items_max; r.pool = (int)pool;
+    const size_t bytes = carve(r, 0, r.fm);
+    const cudaError_t e = cudaMalloc(&r.frame, bytes);
+    if (e != cudaSuccess) {
+      r.frame = nullptr;
+      return "render scratch cudaMalloc(" + std::to_string(bytes) + ") failed: " + cudaGetErrorString(e);
+    }
+    carve(r, reinterpret_cast<uintptr_t>(r.frame), r.fm);
+  }
+  if ((r.flags & DTS_FLAG_DISTORTION) && !r.fish.src_xy) return "distortion enabled but no fisheye LUT set";
+  return "";
+}
+
+std::string renderer_set_fisheye(Renderer& r, const float* rmapx, const float* rmapy) {
+  // distortion.py:118 gathers img[rint(rmapy), rint(rmapx)].  The rasteriser renders those source pixels directly: per
+  // output pixel the source position, per fine / coarse output bin the bounding box of its source pixels (the bins
+  // prims are sorted into).
+  const int W = r.W, H = r.H, cbx_n = (W + kCoarseW - 1) / kCoarseW, cbins = r.cbins;
+  std::vector<int32_t> src((size_t)W * H);
+  const short4 empty = make_short4(32767, 32767, -32768, -32768);
+  std::vector<short4> cbox(cbins, empty), fbox((size_t)cbins * kCFX * kCFY, empty);
+  auto grow = [](short4& b, int x, int y) {
+    b.x = (short)(x < b.x ? x : b.x); b.y = (short)(y < b.y ? y : b.y);
+    b.z = (short)(x > b.z ? x : b.z); b.w = (short)(y > b.w ? y : b.w);
+  };
+  for (int y = 0; y < H; y++)
+    for (int x = 0; x < W; x++) {
+      const float fx = rmapx[(size_t)y * W + x], fy = rmapy[(size_t)y * W + x];
+      const int sx = (int)rintf(fx), sy = (int)rintf(fy);   // round-half-even like the kernel's rintf
+      const bool ok = fx == fx && fy == fy && sx >= 0 && sx < W && sy >= 0 && sy < H;
+      src[(size_t)y * W + x] = ok ? (int32_t)((uint32_t)(sx & 0xffff) | ((uint32_t)sy << 16)) : (int32_t)0x80008000u;
+      if (!ok) continue;
+      const int cb = (y / kCoarseH) * cbx_n + x / kCoarseW, f = (y % kCoarseH / kBinH) * kCFX + x % kCoarseW / kBinW;
+      grow(cbox[cb], sx, sy); grow(fbox[(size_t)cb * kCFX * kCFY + f], sx, sy);
+    }
+  // int32 edge functions inside a coarse bin need |A x + B y| < 2^30 over its source box, where (guard band) |A| <=
+  // kEdge * H, |B| <= kEdge * W, x <= kSub * w, y <= kSub * h  ->  H * w + W * h < 2^30 / (kEdge * kSub)
+  constexpr long long kEdge = (long long)(kGuard + 1) * kSub;
+  for (int b = 0; b < cbins; b++) {
+    if (cbox[b].z < cbox[b].x) continue;
+    const long long w = cbox[b].z - cbox[b].x + 2, h = cbox[b].w - cbox[b].y + 2;
+    if ((long long)H * w + (long long)W * h >= (1LL << 30) / (kEdge * kSub))
+      return "fisheye LUT sends output bin " + std::to_string(b) + " to a " + std::to_string(w) + "x" + std::to_string(h) +
+             " px source region: too wide for the rasteriser's int32 edge functions";
+  }
+  // two inverse indices over source cells (the coarse grid laid over the source image): per cell, the output bins whose
+  // source box meets it, and the output bins whose box has its top-left corner there, each bin under one HOME cell
+  std::vector<std::vector<int>> meets(cbins), homes(cbins);
+  int ext_x = 0, ext_y = 0;
+  for (int b = 0; b < cbins; b++) {
+    const short4 q = cbox[b];
+    if (q.z < q.x) continue;
+    const int cx0 = q.x / kCoarseW, cy0 = q.y / kCoarseH, cx1 = q.z / kCoarseW, cy1 = q.w / kCoarseH;
+    for (int cy = cy0; cy <= cy1; cy++)
+      for (int cx = cx0; cx <= cx1; cx++) meets[cy * cbx_n + cx].push_back(b);
+    homes[cy0 * cbx_n + cx0].push_back(b);
+    ext_x = std::max(ext_x, cx1 - cx0);
+    ext_y = std::max(ext_y, cy1 - cy0);
+  }
+  std::vector<int32_t> cell_start, home_start;
+  std::vector<uint16_t> cell_bins;
+  std::vector<int4> home_ent;   // with the box
+  for (int c = 0; c < cbins; c++) {
+    cell_start.push_back((int32_t)cell_bins.size());
+    home_start.push_back((int32_t)home_ent.size());
+    for (int b : meets[c]) cell_bins.push_back((uint16_t)b);
+    for (int b : homes[c])
+      home_ent.push_back(make_int4((int)((uint32_t)(uint16_t)cbox[b].x | ((uint32_t)(uint16_t)cbox[b].y << 16)),
+                                   (int)((uint32_t)(uint16_t)cbox[b].z | ((uint32_t)(uint16_t)cbox[b].w << 16)), b, 0));
+  }
+  cell_start.push_back((int32_t)cell_bins.size());
+  home_start.push_back((int32_t)home_ent.size());
+  if (cell_bins.empty()) cell_bins.push_back(0);
+  if (home_ent.empty()) home_ent.push_back(make_int4(0, 0, 0, 0));
+  free_fish(r.fish);
+  FishTab t{};
+  cudaError_t e = cudaSuccess;
+  auto upload = [&](auto& dst, const auto& v) {
+    void* d = nullptr;
+    if (e == cudaSuccess) e = cudaMalloc(&d, v.size() * sizeof(v[0]));
+    if (e != cudaSuccess) return;
+    dst = reinterpret_cast<std::remove_reference_t<decltype(dst)>>(d);
+    e = cudaMemcpy(d, v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice);
+  };
+  upload(t.src_xy, src); upload(t.cbox, cbox); upload(t.fbox, fbox);
+  upload(t.cell_start, cell_start); upload(t.cell_bins, cell_bins);
+  upload(t.home_start, home_start); upload(t.home_ent, home_ent);
+  if (e != cudaSuccess) { free_fish(t); return std::string("fisheye table upload failed: ") + cudaGetErrorString(e); }
+  t.ext_x = ext_x; t.ext_y = ext_y;
+  r.fish = t;
+  return "";
+}
+
 // Test hook (dts_debug_frame): what k_frame_setup / k_geometry left in frame memory for one env of the last render —
 // the camera model-view and projection, the prim / lattice counts, and the lit 8x8 lattice of every road tile that
 // was emitted, re-ordered by grid cell (i * grid_h + j; cells that were culled stay NaN).
-int debug_frame_copy(void* scratch, int n, int max_prims, int cbins, int max_pairs, int max_lat, size_t geo_items,
-                     int env, double* V, float* P, int32_t* counts, float* lattice_by_cell, int n_cells, int tris_per_tile) {
-  const FrameMem fm = carve(scratch, n, max_prims, cbins, max_pairs, max_lat, geo_items);
+std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, int32_t* counts, float* lattice_by_cell,
+                             int n_cells) {
+  if (!r.frame) return "nothing rendered yet";
+  if (r.flags & DTS_FLAG_TESSELLATE) return "dts_debug_frame reads the analytic-tile lattice (tile mode 1)";
+  const FrameMem& fm = r.fm;
+  const int max_prims = r.max_prims, max_lat = r.max_lat, tris_per_tile = tile_draw_ids(false);
   FrameCtx c;
-  if (cudaMemcpy(&c, fm.ctx + env, sizeof c, cudaMemcpyDeviceToHost) != cudaSuccess) return 1;
+  if (cudaMemcpy(&c, fm.ctx + env, sizeof c, cudaMemcpyDeviceToHost) != cudaSuccess) return "debug_frame_copy failed";
   for (int k = 0; k < 12; k++) V[k] = c.V[k];
   P[0] = c.P00; P[1] = c.P11; P[2] = c.P22; P[3] = c.P23;
   counts[0] = c.n_prims; counts[1] = c.n_lat; counts[2] = c.overflow; counts[3] = 0;
   cudaMemcpy(&counts[3], fm.work + kWorkPairPool, sizeof(int32_t), cudaMemcpyDeviceToHost);   // (prim, coarse bin) pairs of the whole batch
   const int np = c.n_prims < max_prims ? c.n_prims : max_prims;
-  PrimRec* prims = new PrimRec[np > 0 ? np : 1];
-  float4* lat = new float4[(size_t)max_lat * 64];
+  std::vector<PrimRec> prims(np > 0 ? np : 1);
+  std::vector<float4> lat((size_t)max_lat * 64);
   int rc = 0;
-  if (np && cudaMemcpy(prims, fm.prims + (size_t)env * max_prims, (size_t)np * sizeof(PrimRec), cudaMemcpyDeviceToHost) != cudaSuccess) rc = 1;
-  if (cudaMemcpy(lat, fm.lat + (size_t)env * max_lat * 64, (size_t)max_lat * 64 * sizeof(float4), cudaMemcpyDeviceToHost) != cudaSuccess) rc = 1;
+  if (np && cudaMemcpy(prims.data(), fm.prims + (size_t)env * max_prims, (size_t)np * sizeof(PrimRec), cudaMemcpyDeviceToHost) != cudaSuccess) rc = 1;
+  if (cudaMemcpy(lat.data(), fm.lat + (size_t)env * max_lat * 64, (size_t)max_lat * 64 * sizeof(float4), cudaMemcpyDeviceToHost) != cudaSuccess) rc = 1;
   for (int k = 0; k < n_cells * 64 * 3; k++) lattice_by_cell[k] = nanf("");
   for (int p = 0; p < np && !rc; p++) {
     const int slot = (prims[p].ltq & 0xffff) - 1;
@@ -2239,19 +2444,14 @@ int debug_frame_copy(void* scratch, int n, int max_prims, int cbins, int max_pai
       lattice_by_cell[(cell * 64 + v) * 3 + 2] = lat[slot * 64 + v].z;
     }
   }
-  delete[] prims;
-  delete[] lat;
-  return rc;
+  return rc ? "debug_frame_copy failed" : "";
 }
 
-int launch_render(const DState& S, const DMap* maps, const RenderCfg& rc, void* obs_any, void* scratch, int n_ctas,
-                  int max_prims, int max_pairs, int max_lat, int items_max, const FishTab& fish, const GatherTab& gather,
+int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, void* obs_any, const GatherTab& gather,
                   int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level, cudaStream_t st) {
-  const int W = rc.width, H = rc.height;
   uint8_t* obs = reinterpret_cast<uint8_t*>(obs_any);
-  const int cbins = ((W + kCoarseW - 1) / kCoarseW) * ((H + kCoarseH - 1) / kCoarseH);
   const bool fisheye = (rc.flags & DTS_FLAG_DISTORTION) != 0;
-  FrameMem fm = carve(scratch, rc.n_envs, max_prims, cbins, max_pairs, max_lat, (size_t)items_max);
+  FrameMem fm = r.fm;
   fm.status = status_dev;
   int mk = 0;
   // level 2: an event at every kernel boundary; level 1: only the two around k_raster (marks 3 and 4), so that the
@@ -2261,35 +2461,28 @@ int launch_render(const DState& S, const DMap* maps, const RenderCfg& rc, void* 
   mark();
   k_frame_setup<<<(rc.n_envs + 127) / 128, 128, 0, st>>>(S, maps, rc, fm);
   mark();
-  const size_t pairs_total = (size_t)rc.n_envs * items_max;
-  k_cull<<<(unsigned)((pairs_total + 255) / 256), 256, 0, st>>>(S, maps, rc, fm, items_max);
-  const int geo_ctas = (n_ctas / kRasterMinCtas) * kGeoMinCtas / kGeoWarps;   // SMs x resident geometry CTAs
-  if (rc.tessellate) k_geometry<true><<<geo_ctas, kGeoWarps * 32, 0, st>>>(S, maps, rc, fm, max_prims, max_lat, err_flag);
-  else k_geometry<false><<<geo_ctas, kGeoWarps * 32, 0, st>>>(S, maps, rc, fm, max_prims, max_lat, err_flag);
+  const size_t pairs_total = (size_t)rc.n_envs * r.items_max;
+  k_cull<<<(unsigned)((pairs_total + 255) / 256), 256, 0, st>>>(S, maps, rc, fm, r.items_max);
+  const auto geometry = rc.tessellate ? k_geometry<true> : k_geometry<false>;
+  geometry<<<r.sms * kGeoMinCtas / kGeoWarps, kGeoWarps * 32, 0, st>>>(S, maps, rc, fm, r.max_prims, r.max_lat, err_flag);
   mark();
-  const size_t bin_smem_bytes = (size_t)2 * cbins * sizeof(int);
+  const size_t bin_smem_bytes = (size_t)2 * r.cbins * sizeof(int);
   const int bin_grid = rc.n_envs;   // CTA per env: one warp where a frame has few bins and prims (160x120: 75 bins — more warps
   // only add barriers and CTA launches), four for large cameras (640x480)
-  const int bin_threads = cbins > 128 ? kBinWarps * 32 : 32;
-  if (fisheye) {
-    if (bin_smem_bytes > 48 * 1024) cudaFuncSetAttribute(k_bin<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bin_smem_bytes);
-    k_bin<true><<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, fish, max_prims, max_pairs, err_flag);
-  } else {
-    if (bin_smem_bytes > 48 * 1024)   // cameras beyond ~640x480 (cbins > 1536): opt in to large dynamic shared memory
-      cudaFuncSetAttribute(k_bin<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bin_smem_bytes);
-    k_bin<false><<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, fish, max_prims, max_pairs, err_flag);
-  }
+  const int bin_threads = r.cbins > 128 ? kBinWarps * 32 : 32;
+  const auto bin = fisheye ? k_bin<true> : k_bin<false>;
+  if (bin_smem_bytes > 48 * 1024)   // cameras beyond ~640x480 (cbins > 1536): opt in to large dynamic shared memory
+    cudaFuncSetAttribute(bin, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bin_smem_bytes);
+  bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, r.fish, r.max_prims, r.pool, err_flag);
   mark();
   const bool wrap = (rc.obs_layout | rc.obs_dtype) != 0;
   int launches = 5;
-  if (lean_output(rc.obs_layout, rc.obs_dtype, W)) {   // (inside the k_raster event bracket: it is rasterisation time)
-    // n_ctas can be 1 for a handful of envs
-    const int solo_ctas = max(1, n_ctas * kSoloMinCtas / kRasterMinCtas), flat_ctas = max(1, n_ctas * kFlatMinCtas / kRasterMinCtas);
-    if (fisheye) k_raster_solo<true><<<solo_ctas, kThreads, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat);
-    else k_raster_solo<false><<<solo_ctas, kThreads, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat);
+  if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
+    const auto solo = fisheye ? k_raster_solo<true> : k_raster_solo<false>;
+    const auto flat = fisheye ? k_raster_flat<true> : k_raster_flat<false>;
+    solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, r.fish, obs, r.max_prims, r.max_lat);
     // before k_raster, which draws the bins k_raster_flat hands back
-    if (fisheye) k_raster_flat<true><<<flat_ctas, kThreads, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat, err_flag);
-    else k_raster_flat<false><<<flat_ctas, kThreads, 0, st>>>(S, maps, rc, fm, fish, obs, max_prims, max_lat, err_flag);
+    flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, r.fish, obs, r.max_prims, r.max_lat, err_flag);
     launches += 2;
   }
   static bool smem_opt_in = false;
@@ -2300,13 +2493,8 @@ int launch_render(const DState& S, const DMap* maps, const RenderCfg& rc, void* 
     cudaFuncSetAttribute(k_raster<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
     smem_opt_in = true;
   }
-  if (fisheye) {
-    if (wrap) k_raster<true, true><<<n_ctas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, fish, gather, obs, max_prims, max_pairs, max_lat, err_flag);
-    else k_raster<false, true><<<n_ctas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, fish, gather, obs, max_prims, max_pairs, max_lat, err_flag);
-  } else {
-    if (wrap) k_raster<true, false><<<n_ctas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, fish, gather, obs, max_prims, max_pairs, max_lat, err_flag);
-    else k_raster<false, false><<<n_ctas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, fish, gather, obs, max_prims, max_pairs, max_lat, err_flag);
-  }
+  const auto raster = fisheye ? (wrap ? k_raster<true, true> : k_raster<false, true>) : (wrap ? k_raster<true, false> : k_raster<false, false>);
+  raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, r.fish, gather, obs, r.max_prims, r.pool, r.max_lat, err_flag);
   mark();
   mark();   // (post passes: none yet)
   return launches;

@@ -1,4 +1,4 @@
-"""Device-only step time with the device ResizeWrapper under the current DTS_RESIZE_* switches (A/B of k_resize_band)."""
+"""Device-only step time with the device ResizeWrapper: k_resize_band, or the untiled k_resize under DTS_RESIZE_UNTILED=1."""
 import os, sys, time, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from gym_duckietown_b200.batched_env import BatchedDuckietownEnv
