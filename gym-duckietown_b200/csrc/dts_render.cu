@@ -2346,8 +2346,11 @@ std::string renderer_set_fisheye(Renderer& r, const float* rmapx, const float* r
   for (int y = 0; y < H; y++)
     for (int x = 0; x < W; x++) {
       const float fx = rmapx[(size_t)y * W + x], fy = rmapy[(size_t)y * W + x];
-      const int sx = (int)rintf(fx), sy = (int)rintf(fy);   // round-half-even like the kernel's rintf
-      const bool ok = fx == fx && fy == fy && sx >= 0 && sx < W && sy >= 0 && sy < H;
+      // round half to even (numpy's rint); NaN, inf and huge entries are out of range before any float -> int conversion,
+      // which would be undefined for them
+      const bool finite = fabsf(fx) < 1073741824.0f && fabsf(fy) < 1073741824.0f;
+      const int sx = finite ? (int)rintf(fx) : -1, sy = finite ? (int)rintf(fy) : -1;
+      const bool ok = sx >= 0 && sx < W && sy >= 0 && sy < H;
       src[(size_t)y * W + x] = ok ? (int32_t)((uint32_t)(sx & 0xffff) | ((uint32_t)sy << 16)) : (int32_t)0x80008000u;
       if (!ok) continue;
       const int cb = (y / kCoarseH) * cbx_n + x / kCoarseW, f = (y % kCoarseH / kBinH) * kCFX + x % kCoarseW / kBinW;

@@ -340,6 +340,8 @@ class Sim:
 
     def set_fisheye_lut(self, rmapx: np.ndarray, rmapy: np.ndarray):
         rx, ry = np.ascontiguousarray(rmapx, np.float32), np.ascontiguousarray(rmapy, np.float32)
+        if rx.ndim != 2 or rx.shape != ry.shape:   # the library reads camera_height x camera_width floats from each
+            raise ValueError(f"fisheye LUT: rmapx {rx.shape} and rmapy {ry.shape} must be two 2-D arrays of one shape")
         self._check(self.lib.dts_set_fisheye_lut(self.h, _ptr(rx), _ptr(ry), rx.shape[1], rx.shape[0]),
                     "dts_set_fisheye_lut")
 

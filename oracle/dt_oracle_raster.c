@@ -556,8 +556,11 @@ void orr_render(const orr_scene* sc, double px, double pz, double angle, const o
     for (int xx = 0; xx < W; xx++) {
       int sx = xx, sy = y, valid = 1;
       if (lut_x) {
-        sx = (int)rintf(lut_x[(size_t)y * W + xx]);
-        sy = (int)rintf(lut_y[(size_t)y * W + xx]);
+        const float fx = lut_x[(size_t)y * W + xx], fy = lut_y[(size_t)y * W + xx];
+        /* range-check before converting: (int) of NaN, inf or |v| >= 2^31 is undefined */
+        const int finite = fabsf(fx) < 1073741824.0f && fabsf(fy) < 1073741824.0f;
+        sx = finite ? (int)rintf(fx) : -1;
+        sy = finite ? (int)rintf(fy) : -1;
         valid = sx >= 0 && sx < W && sy >= 0 && sy < H;  /* cv2.remap BORDER_CONSTANT -> 0 */
       }
       for (int ch = 0; ch < 3; ch++) {

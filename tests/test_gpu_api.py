@@ -1,5 +1,5 @@
 """The reference's own smoke script (run_tests.py:10-52) replayed against the drop-in classes, plus
-fisheye / MultiMap / auto-reset behaviour through the public API."""
+MultiMap / auto-reset behaviour through the public API (the fisheye is in test_gpu_fisheye.py)."""
 import numpy as np
 import pytest
 
@@ -79,35 +79,6 @@ def test_full_transparency_info_and_helpers(torch_cuda):
     with pytest.raises(NotInLane):
         env.get_lane_pos2(np.array([0.1, 0, 0.1]), 0.0)   # grass tile
     assert env._valid_pose(env.cur_pos, env.cur_angle)
-    env.close()
-
-
-def test_fisheye_fused_gather_vs_oracle(torch_cuda):
-    """config 4 shape: 640x480 + distortion (+ domain_rand): the fused gather equals rendering the
-    undistorted frame with the oracle and applying the reference LUT."""
-    torch = torch_cuda
-    import oracle as orc
-    from gym_duckietown_b200 import maps
-    from gym_duckietown_b200.batched_env import BatchedDuckietownEnv
-    from test_gpu_render import oracle_episode
-
-    N, W, H = 6, 640, 480
-    env = BatchedDuckietownEnv(N, "udem1", camera_width=W, camera_height=H, domain_rand=True, distortion=True, seed=50)
-    captured = {}
-    orig = env.sim.reset
-    env.sim.reset = lambda mask, params, stream=0: (captured.update(params), orig(mask, params, stream))[1]
-    obs = env.reset()
-    torch.cuda.synchronize()
-    st = {k: v.cpu().numpy() for k, v in env.state.items()}
-    sc = orc.OracleScene(maps.load_map("udem1"))
-    lut = (env.camera_model.rmapx, env.camera_model.rmapy)
-    gpu = obs.cpu().numpy()
-    for k in range(N):
-        cpu = sc.render(st["pos_x"][k], st["pos_z"][k], st["angle"][k], oracle_episode(orc, captured, k), W, H, True, lut)
-        undist = sc.render(st["pos_x"][k], st["pos_z"][k], st["angle"][k], oracle_episode(orc, captured, k), W, H, True)
-        assert np.array_equal(env.camera_model.distort(undist), cpu)   # oracle gather == product's numpy gather
-        d = np.abs(gpu[k].astype(int) - cpu.astype(int))
-        assert d.max() <= 1, (k, d.max(), int((d > 1).sum()))
     env.close()
 
 
