@@ -82,6 +82,7 @@ class BatchedDuckietownEnv:
         self.map_ids = np.zeros(num_envs, np.int32)
         self._first_reset = True
         self.resize = None
+        self.resize_method = None
         self.output_format = dict(obs_layout="hwc", obs_dtype="uint8", reward="raw", discrete_actions=False,
                                   action_vel_scale=1.0)
         self.seed(seed)
@@ -119,11 +120,19 @@ class BatchedDuckietownEnv:
             self.obs = torch.zeros((self.num_envs,) + shape, device=self.device,
                                    dtype=torch.uint8 if f["obs_dtype"] == "uint8" else torch.float32)
 
-    def set_resize(self, resize_w: Optional[int], resize_h: Optional[int]):
-        """ResizeWrapper (wrappers.py:111-141) on the device: render at the camera size, emit `resize_w` x `resize_h`
-        observations (cv2.INTER_CUBIC's 8-bit fixed-point arithmetic) in the current layout / dtype.  None switches off."""
-        self.resize = (int(resize_w), int(resize_h)) if resize_w else None
-        self.sim.set_resize(*(self.resize or (0, 0)))
+    RESIZE_METHODS = {"cv2_cubic": L.RESIZE_CV2_CUBIC, "pil_bilinear": L.RESIZE_PIL_BILINEAR}
+
+    def set_resize(self, resize_w: Optional[int], resize_h: Optional[int], method: str = "cv2_cubic"):
+        """A resize wrapper on the device: render at the camera size, emit `resize_w` x `resize_h` observations in the
+        current layout / dtype.  method 'cv2_cubic': src/gym_duckietown/wrappers.py:111-141's ResizeWrapper
+        (cv2.INTER_CUBIC's 8-bit fixed-point arithmetic); 'pil_bilinear': learning/utils/wrappers.py:39-54's
+        (scipy.misc.imresize = Pillow's bilinear, bit-exact; targets of at least 1/32 of the camera per axis).  None
+        switches off.  A target the device refuses raises and leaves the previous setting in effect."""
+        if method not in self.RESIZE_METHODS:
+            raise ValueError(f"resize method must be one of {sorted(self.RESIZE_METHODS)}, not {method!r}")
+        resize = (int(resize_w), int(resize_h)) if resize_w else None
+        self.sim.set_resize(*(resize or (0, 0)), filter=self.RESIZE_METHODS[method])
+        self.resize, self.resize_method = resize, method if resize else None
         self._alloc_obs()
         return self
 

@@ -46,6 +46,7 @@ struct dts_sim {
   // fused ResizeWrapper (dts_set_resize): full-size render target + tap tables
   int resize_w = 0, resize_h = 0;
   int resize_band = 0, resize_cap = 0;   // k_resize_band: output rows per CTA and the largest source-row span of a band (0: untiled kernel)
+  int resize_filter = DTS_RESIZE_CV2_CUBIC;   // dts_set_resize_filter; the Pillow filter's tables are the renderer's
   uint8_t* resize_src = nullptr;
   int16_t *resize_xtab = nullptr, *resize_ytab = nullptr;
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
@@ -496,6 +497,16 @@ int dts_reset_random(dts_sim* sim, const uint8_t* mask_dev, void* stream) {
   return 0;
 }
 
+// the resize pass dts_set_resize_filter selected: full-size u8 HWC frames -> the caller's tensor
+static void launch_selected_resize(dts_sim* sim, const uint8_t* src, void* dst, cudaStream_t st) {
+  if (sim->resize_filter == DTS_RESIZE_PIL_BILINEAR) {
+    launch_pil_resize(*sim->render, src, dst, sim->fmt.obs_layout, sim->fmt.obs_dtype, st);
+    return;
+  }
+  launch_resize(src, sim->cfg.cam_width, sim->cfg.cam_height, sim->resize_w, sim->resize_h, sim->cfg.num_envs,
+                sim->resize_xtab, sim->resize_ytab, dst, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->resize_band, sim->resize_cap, st);
+}
+
 int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
   if (!sim) return 1;
   if (!obs_dev) return sim->fail("obs_dev is NULL");
@@ -532,9 +543,7 @@ int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
   int k = launch_render(*sim->render, sim->S, sim->d_maps, rc, target, gt, sim->d_err, sim->d_status, marks, mark_level,
                         (cudaStream_t)stream);
   if (sim->resize_w) {
-    launch_resize(sim->resize_src, sim->cfg.cam_width, sim->cfg.cam_height, sim->resize_w, sim->resize_h, sim->cfg.num_envs,
-                  sim->resize_xtab, sim->resize_ytab, obs_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->resize_band, sim->resize_cap,
-                  (cudaStream_t)stream);
+    launch_selected_resize(sim, sim->resize_src, obs_dev, (cudaStream_t)stream);
     k++;
   }
   if (marks && mark_level >= 2) cudaEventRecord(marks[kProfMarks - 1], (cudaStream_t)stream);   // closes the "post" interval
@@ -637,17 +646,31 @@ static void cubic_axis_table(int src, int dst, std::vector<int16_t>& tab) {
   }
 }
 
-int dts_set_resize(dts_sim* sim, int out_w, int out_h) {
+int dts_set_resize(dts_sim* sim, int out_w, int out_h) { return dts_set_resize_filter(sim, out_w, out_h, DTS_RESIZE_CV2_CUBIC); }
+
+int dts_set_resize_filter(dts_sim* sim, int out_w, int out_h, int filter) {
   if (!sim) return 1;
+  if (filter != DTS_RESIZE_CV2_CUBIC && filter != DTS_RESIZE_PIL_BILINEAR) return sim->fail("bad resize filter %d", filter);
   if (out_w < 0 || out_h < 0 || (out_w == 0) != (out_h == 0)) return sim->fail("bad resize target %dx%d", out_w, out_h);
   if (out_w > 4096 || out_h > 4096) return sim->fail("resize target %dx%d too large", out_w, out_h);
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   DTS_CUDA(cudaDeviceSynchronize());
+  // the Pillow tables first: a target that pass refuses leaves the previous setting in effect
+  const std::string e = renderer_set_pil_resize(*sim->render, filter == DTS_RESIZE_PIL_BILINEAR ? out_w : 0,
+                                                filter == DTS_RESIZE_PIL_BILINEAR ? out_h : 0);
+  if (!e.empty()) return sim->fail("%s", e.c_str());
   void* old[] = {sim->resize_src, sim->resize_xtab, sim->resize_ytab};
   for (void* p : old) if (p) cudaFree(p);
   sim->resize_src = nullptr; sim->resize_xtab = sim->resize_ytab = nullptr;
   sim->resize_w = sim->resize_h = 0;
+  sim->resize_filter = DTS_RESIZE_CV2_CUBIC;
   if (!out_w) return 0;
+  if (filter == DTS_RESIZE_PIL_BILINEAR) {
+    DTS_CUDA(cudaMalloc(&sim->resize_src, (size_t)sim->cfg.num_envs * sim->cfg.cam_width * sim->cfg.cam_height * 3));
+    sim->resize_w = out_w; sim->resize_h = out_h;
+    sim->resize_filter = filter;
+    return 0;
+  }
   std::vector<int16_t> xt, yt;
   cubic_axis_table(sim->cfg.cam_width, out_w, xt);
   cubic_axis_table(sim->cfg.cam_height, out_h, yt);
@@ -737,9 +760,7 @@ int dts_resize_frames(dts_sim* sim, const uint8_t* src_dev, void* dst_dev, void*
   if (!sim->resize_w) return sim->fail("dts_set_resize first");
   if (!src_dev || !dst_dev) return sim->fail("NULL frame pointer");
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  launch_resize(src_dev, sim->cfg.cam_width, sim->cfg.cam_height, sim->resize_w, sim->resize_h, sim->cfg.num_envs,
-                sim->resize_xtab, sim->resize_ytab, dst_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->resize_band, sim->resize_cap,
-                (cudaStream_t)stream);
+  launch_selected_resize(sim, src_dev, dst_dev, (cudaStream_t)stream);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   return 0;

@@ -73,6 +73,12 @@ void launch_resize(const uint8_t* src, int W, int H, int ow, int oh, int n_envs,
 // Output rows per CTA of k_resize_band and the largest source-row span of a band, for the row tap table `ytab`
 // ([oh][8]); both 0: the untiled k_resize
 void plan_resize_bands(int W, int ow, int oh, const int16_t* ytab, int* band_rows, int* band_cap);
+// learning/utils/wrappers.py's ResizeWrapper (Pillow BILINEAR) on the device: builds the tap tables and band plan of
+// the camera -> ow x oh resize (0 x 0: frees them).  A target the pass cannot take (more than 65 taps per output pixel
+// on an axis, i.e. less than 1/32 of the camera size) is refused and leaves the previous tables.
+std::string renderer_set_pil_resize(Renderer& r, int ow, int oh);
+// src u8[N][H][W][3] -> dst [N] x (ow x oh) in `layout` / `dtype`, with the tables renderer_set_pil_resize built
+void launch_pil_resize(const Renderer& r, const uint8_t* src, void* dst, int layout, int dtype, cudaStream_t st);
 void launch_blend4(const uint8_t* const f[4], const double w[4], double* out, size_t n, cudaStream_t st);
 
 }  // namespace dts

@@ -57,6 +57,16 @@ struct FishTab {
   int ext_x, ext_y;
 };
 
+// Pillow's bilinear resize (k_resize_pil): both axes' fixed-point tap tables and the band plan
+struct PilTab {
+  int W, H, ow, oh;   // camera and target size
+  int tx, ty;         // taps per output column / row: the most any one has; the others are padded with zero taps
+  int band, cap;      // output rows per CTA, source rows a band spans at most
+  int pitch, ow3p;    // shared-memory row pitch of the staged source (32-bit words) and of the horizontal result (bytes)
+  size_t smem;        // dynamic shared memory per CTA
+  int32_t* tab;       // device: xs[ow] (first source column), xw[ow][tx] (22-bit weights), ys[oh], yw[oh][ty]; null: off
+};
+
 namespace {
 
 #ifndef DTS_STATS
@@ -856,6 +866,7 @@ struct Renderer {
   void* frame = nullptr;     // frame memory (null: not reserved since the last map upload)
   FrameMem fm{};             // ... carved
   FishTab fish{};            // fused fisheye tables (null until a LUT is set)
+  PilTab pil{};              // Pillow bilinear resize tables (null unless that filter is selected)
 };
 
 // The one statement of the frame-memory layout: points `f` into the allocation at `base` and returns its size, so
@@ -2263,6 +2274,233 @@ void launch_resize(const uint8_t* src, int W, int H, int ow, int oh, int n_envs,
   k_resize<<<blocks, 256, 0, st>>>(src, W, H, ow, oh, n_envs, xtab, ytab, dst, layout, dtype);
 }
 
+// ------------------------------------------------------------------------------------------------ k_resize_pil
+// learning/utils/wrappers.py:39-54's ResizeWrapper: scipy.misc.imresize(obs, shape), which for a uint8 RGB frame is
+// PIL.Image.resize((w, h), BILINEAR), in Pillow's 8-bit arithmetic (Resample.c): per axis a triangle filter widened by
+// the scale factor when it shrinks (7 taps per output pixel at 640 -> 160), weights normalised in double and rounded
+// to 22-bit fixed point (tables: renderer_set_pil_resize); the horizontal pass first, acc = 2^21 + sum px * w in
+// int32, clipped to u8, then the vertical pass on those bytes.
+// A CTA per (band of `band` output rows, env).  The band's source rows pass through shared memory kPilChunk at a time,
+// one pixel per 32-bit word; a warp takes one output column of those rows, a lane per row, its two half-warps the even
+// and odd taps (row pitch = 2 mod 32 words, so the 32 lanes read 32 different banks).  The horizontal results, u8 like
+// Pillow's intermediate image, stay in shared memory for the whole band (480 B per source row at 160 wide); the
+// vertical pass reads them a word (four bytes of an output row) per lane.
+constexpr int kPilChunk = 16;                   // source rows staged at a time: one per lane of a half-warp
+constexpr size_t kPilSmem = 74 * 1024;          // a band plan that fits keeps three CTAs per SM
+constexpr size_t kPilSmemMax = 200 * 1024;      // otherwise the smallest plan, up to this
+constexpr int kPilMaxTaps = 65;                 // Pillow's ksize at a 32x reduction
+
+__device__ __forceinline__ unsigned pil_clip8(int acc) { return (unsigned)min(max(acc >> 22, 0), 255); }
+
+__global__ void __launch_bounds__(256) k_resize_pil(const uint8_t* __restrict__ src, const PilTab t, void* __restrict__ dst,
+                                                    int layout, int dtype) {
+  extern __shared__ __align__(16) unsigned char pil_smem[];
+  const int W = t.W, H = t.H, ow = t.ow, oh = t.oh, ow3 = ow * 3, pitch = t.pitch, ow3p = t.ow3p;
+  const int bands = (oh + t.band - 1) / t.band;
+  const int env = blockIdx.x / bands, r0 = (blockIdx.x - env * bands) * t.band, r1 = min(r0 + t.band, oh);
+  const int32_t* __restrict__ xs = t.tab;
+  const int32_t* __restrict__ xw = xs + ow;
+  const int32_t* __restrict__ ys = xw + (size_t)ow * t.tx;
+  const int32_t* __restrict__ yw = ys + oh;
+  const int lo = __ldg(ys + r0), hi = __ldg(ys + r1 - 1) + t.ty;   // the band's source rows [lo, hi)
+  uint32_t* stage = reinterpret_cast<uint32_t*>(pil_smem);         // [kPilChunk][pitch] source pixels, RGBX
+  uint8_t* inter = pil_smem + (size_t)kPilChunk * pitch * 4;       // [cap][ow3p] horizontal result, u8 RGB
+  const uint8_t* frame = src + (size_t)env * W * H * 3;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  const int hr = lane & 15, half = lane >> 4;
+  // four pixels = three aligned words when rows are whole groups of four and the frame is word-aligned
+  const bool words_in = (W & 3) == 0 && (reinterpret_cast<uintptr_t>(frame) & 3) == 0;
+  for (int c0 = lo; c0 < hi; c0 += kPilChunk) {
+    const int nr = min(kPilChunk, hi - c0);
+    if (words_in) {
+      const int groups = W >> 2, items = nr * groups;
+      const uint32_t* rows = reinterpret_cast<const uint32_t*>(frame + (size_t)c0 * W * 3);
+      for (int i0 = threadIdx.x; i0 < items; i0 += 4 * blockDim.x) {
+        uint32_t v[4][3];
+#pragma unroll
+        for (int q = 0; q < 4; q++) {   // all loads first: 48 B per thread in flight
+          const int i = i0 + q * blockDim.x;
+          if (i < items) { v[q][0] = __ldg(rows + 3 * i); v[q][1] = __ldg(rows + 3 * i + 1); v[q][2] = __ldg(rows + 3 * i + 2); }
+        }
+#pragma unroll
+        for (int q = 0; q < 4; q++) {
+          const int i = i0 + q * blockDim.x;
+          if (i >= items) break;
+          const int r = i / groups, g = i - r * groups;
+          uint2* d = reinterpret_cast<uint2*>(stage + r * pitch + 4 * g);   // (pitch even: 8-byte aligned)
+          d[0] = make_uint2(v[q][0], __byte_perm(v[q][0], v[q][1], 0x0543));
+          d[1] = make_uint2(__byte_perm(v[q][1], v[q][2], 0x0432), v[q][2] >> 8);
+        }
+      }
+    } else {
+      for (int i = threadIdx.x; i < nr * W; i += blockDim.x) {
+        const int r = i / W, x = i - r * W;
+        const uint8_t* p = frame + ((size_t)(c0 + r) * W + x) * 3;
+        stage[r * pitch + x] = (uint32_t)__ldg(p) | ((uint32_t)__ldg(p + 1) << 8) | ((uint32_t)__ldg(p + 2) << 16);
+      }
+    }
+    __syncthreads();
+    // horizontal pass: a warp per output column, lane hr = staged row, half = even / odd taps
+    for (int x = warp; x < ow; x += nwarps) {
+      const uint32_t* sp = stage + hr * pitch + __ldg(xs + x);
+      const int32_t* wx = xw + (size_t)x * t.tx;
+      int a0 = 0, a1 = 0, a2 = 0;
+      for (int k = half; k < t.tx; k += 2) {
+        const int w = __ldg(wx + k);
+        const uint32_t v = sp[k];
+        a0 += (int)(v & 255u) * w;
+        a1 += (int)__byte_perm(v, 0, 0x4441) * w;
+        a2 += (int)__byte_perm(v, 0, 0x4442) * w;
+      }
+      a0 += __shfl_xor_sync(0xffffffffu, a0, 16);
+      a1 += __shfl_xor_sync(0xffffffffu, a1, 16);
+      a2 += __shfl_xor_sync(0xffffffffu, a2, 16);
+      if (half == 0 && hr < nr) {
+        uint8_t* o = inter + (size_t)(c0 - lo + hr) * ow3p + 3 * x;
+        o[0] = (uint8_t)pil_clip8(a0 + (1 << 21));
+        o[1] = (uint8_t)pil_clip8(a1 + (1 << 21));
+        o[2] = (uint8_t)pil_clip8(a2 + (1 << 21));
+      }
+    }
+    __syncthreads();
+  }
+  // vertical pass: a warp per output row, a lane per word of four bytes of it
+  const size_t out_elem = dtype == DTS_OBS_F32_UNIT ? 4 : 1;
+  uint8_t* out = reinterpret_cast<uint8_t*>(dst) + (size_t)env * ow3 * oh * out_elem;
+  const bool words_out = layout == DTS_OBS_HWC && dtype == DTS_OBS_U8 && (ow3 & 3) == 0 && (reinterpret_cast<uintptr_t>(dst) & 3) == 0;
+  const int wpr = (ow3 + 3) >> 2, ipw = ow3p >> 2;
+  for (int y = r0 + warp; y < r1; y += nwarps) {
+    const uint32_t* col = reinterpret_cast<const uint32_t*>(inter + (size_t)(__ldg(ys + y) - lo) * ow3p);
+    const int32_t* wy = yw + (size_t)y * t.ty;
+    for (int j = lane; j < wpr; j += 32) {
+      int a[4] = {1 << 21, 1 << 21, 1 << 21, 1 << 21};
+      for (int k = 0; k < t.ty; k++) {
+        const int w = __ldg(wy + k);
+        const uint32_t v = col[k * ipw + j];
+        a[0] += (int)(v & 255u) * w;
+        a[1] += (int)__byte_perm(v, 0, 0x4441) * w;
+        a[2] += (int)__byte_perm(v, 0, 0x4442) * w;
+        a[3] += (int)(v >> 24) * w;
+      }
+      const int e = 4 * j;
+      if (words_out) {
+        *reinterpret_cast<uint32_t*>(out + (size_t)y * ow3 + e) =
+            pil_clip8(a[0]) | (pil_clip8(a[1]) << 8) | (pil_clip8(a[2]) << 16) | (pil_clip8(a[3]) << 24);
+        continue;
+      }
+#pragma unroll
+      for (int q = 0; q < 4; q++) {
+        if (e + q >= ow3) break;
+        const int x = (e + q) / 3, ch = e + q - 3 * x;
+        const unsigned v = pil_clip8(a[q]);
+        const size_t oi = fmt_index(layout, x, y, ch, ow, oh);
+        if (dtype == DTS_OBS_F32_UNIT) reinterpret_cast<float*>(out)[oi] = (float)v / 255.0f;   // NormalizeWrapper LW:66-70
+        else out[oi] = (uint8_t)v;
+      }
+    }
+  }
+}
+
+// Pillow's precompute_coeffs (Resample.c) for one axis, bilinear filter, then normalize_coeffs_8bpc: per output index
+// the first source index and `taps` weights, the window moved left where it would run past the last source pixel
+// (its extra taps are zero).  Returns Pillow's ksize for the scale.
+static int pil_axis(int in, int out, std::vector<int32_t>& start, std::vector<int32_t>& w, int& taps) {
+  const double scale = (double)in / out, fs = scale < 1.0 ? 1.0 : scale, support = fs, ss = 1.0 / fs;
+  const int ksize = (int)ceil(support) * 2 + 1;
+  if (ksize > kPilMaxTaps) return ksize;
+  std::vector<int> lo(out), n(out);
+  std::vector<int32_t> kk((size_t)out * ksize, 0);
+  taps = 1;
+  for (int i = 0; i < out; i++) {
+    const double center = (i + 0.5) * scale;
+    int xmin = (int)(center - support + 0.5), xmax = (int)(center + support + 0.5);
+    if (xmin < 0) xmin = 0;
+    if (xmax > in) xmax = in;
+    const int cnt = std::min(xmax - xmin, ksize);
+    double k[kPilMaxTaps], ww = 0.0;
+    for (int x = 0; x < cnt; x++) {
+      double u = (x + xmin - center + 0.5) * ss;
+      if (u < 0.0) u = -u;
+      k[x] = u < 1.0 ? 1.0 - u : 0.0;
+      ww += k[x];
+    }
+    for (int x = 0; x < cnt; x++) {
+      if (ww != 0.0) k[x] /= ww;
+      kk[(size_t)i * ksize + x] = (int32_t)(0.5 + k[x] * (1 << 22));   // the weights are >= 0
+    }
+    lo[i] = xmin; n[i] = cnt;
+    taps = std::max(taps, cnt);
+  }
+  start.assign(out, 0);
+  w.assign((size_t)out * taps, 0);
+  for (int i = 0; i < out; i++) {
+    const int s = std::min(lo[i], in - taps);
+    start[i] = s;
+    for (int x = 0; x < n[i]; x++) w[(size_t)i * taps + lo[i] - s + x] = kk[(size_t)i * ksize + x];
+  }
+  return ksize;
+}
+
+static void free_pil(PilTab& p) {
+  cudaFree(p.tab);
+  p = PilTab{};
+}
+
+std::string renderer_set_pil_resize(Renderer& r, int ow, int oh) {
+  if (!ow || !oh) { free_pil(r.pil); return ""; }
+  PilTab t{};
+  t.W = r.W; t.H = r.H; t.ow = ow; t.oh = oh;
+  std::vector<int32_t> xs, xw, ys, yw;
+  const int kx = pil_axis(r.W, ow, xs, xw, t.tx), ky = pil_axis(r.H, oh, ys, yw, t.ty);
+  if (kx > kPilMaxTaps || ky > kPilMaxTaps)
+    return "Pillow bilinear resize " + std::to_string(r.W) + "x" + std::to_string(r.H) + " -> " + std::to_string(ow) + "x" +
+           std::to_string(oh) + " needs " + std::to_string(std::max(kx, ky)) + " taps per output pixel; the device pass takes " +
+           "at most " + std::to_string(kPilMaxTaps) + " (targets of at least 1/32 of the camera size per axis)";
+  t.pitch = r.W + ((2 - r.W) & 31);                 // = 2 mod 32: the 16 rows x 2 tap parities of a warp hit 32 banks
+  t.ow3p = (ow * 3 + 3) & ~3;
+  if (((t.ow3p >> 2) & 1) == 0) t.ow3p += 4;        // an odd word pitch: a column's 16 rows are stored to 16 banks
+  // band height: the least staged rows (whole chunks) over the frame, within kPilSmem if any plan is, else the least
+  // shared memory; ties go to taller bands (fewer CTAs)
+  const size_t stage = (size_t)kPilChunk * t.pitch * 4;
+  long long best_rows = -1;
+  size_t best_smem = 0;
+  for (int R = 1; R <= std::min(oh, 64); R++) {
+    int cap = 0;
+    long long rows = 0;
+    for (int r0 = 0; r0 < oh; r0 += R) {
+      const int r1 = std::min(r0 + R, oh), span = ys[r1 - 1] + t.ty - ys[r0];
+      cap = std::max(cap, span);
+      rows += (span + kPilChunk - 1) / kPilChunk * kPilChunk;
+    }
+    const size_t smem = stage + (size_t)cap * t.ow3p;
+    if (smem > kPilSmemMax) continue;
+    const bool fits = smem <= kPilSmem, best_fits = best_rows >= 0 && best_smem <= kPilSmem;
+    const bool better = best_rows < 0 || (fits && !best_fits) ||
+                        (fits == best_fits && (fits ? rows <= best_rows : smem < best_smem));
+    if (better) { best_rows = rows; best_smem = smem; t.band = R; t.cap = cap; }
+  }
+  if (best_rows < 0)
+    return "Pillow bilinear resize to " + std::to_string(ow) + "x" + std::to_string(oh) + ": a single output row needs more " +
+           "than " + std::to_string(kPilSmemMax / 1024) + " KB of shared memory";
+  t.smem = best_smem;
+  std::vector<int32_t> tab;
+  for (const auto* v : {&xs, &xw, &ys, &yw}) tab.insert(tab.end(), v->begin(), v->end());
+  cudaError_t e = cudaMalloc(&t.tab, tab.size() * sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaMemcpy(t.tab, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && t.smem > 48 * 1024)
+    e = cudaFuncSetAttribute(k_resize_pil, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPilSmemMax);
+  if (e != cudaSuccess) { free_pil(t); return std::string("Pillow resize table upload failed: ") + cudaGetErrorString(e); }
+  free_pil(r.pil);
+  r.pil = t;
+  return "";
+}
+
+void launch_pil_resize(const Renderer& r, const uint8_t* src, void* dst, int layout, int dtype, cudaStream_t st) {
+  const PilTab& t = r.pil;
+  const unsigned grid = (unsigned)(((t.oh + t.band - 1) / t.band) * (size_t)r.n);
+  k_resize_pil<<<grid, 256, t.smem, st>>>(src, t, dst, layout, dtype);
+}
+
 // ------------------------------------------------------------------------------------------------ the renderer
 static void free_fish(FishTab& f) {
   const void* p[] = {f.src_xy, f.cbox, f.fbox, f.cell_start, f.cell_bins, f.home_start, f.home_ent};
@@ -2285,7 +2523,7 @@ void renderer_release_frame(Renderer& r) {
 }
 
 void renderer_destroy(Renderer* r) {
-  if (r) { renderer_release_frame(*r); free_fish(r->fish); }
+  if (r) { renderer_release_frame(*r); free_fish(r->fish); free_pil(r->pil); }
   delete r;
 }
 

@@ -80,6 +80,7 @@ OBS_HWC, OBS_CHW, OBS_CWH = 0, 1, 2
 OBS_U8, OBS_F32_UNIT = 0, 1
 REWARD_RAW, REWARD_DT = 0, 1
 ACTIONS_CONTINUOUS, ACTIONS_DISCRETE3 = 0, 1
+RESIZE_CV2_CUBIC, RESIZE_PIL_BILINEAR = 0, 1   # dts_set_resize_filter
 
 
 class OutputFormat(C.Structure):
@@ -173,6 +174,7 @@ def load() -> C.CDLL:
     lib.dts_query_poses.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp]
     lib.dts_assign_maps.argtypes = [vp, vp, vp, vp]
     lib.dts_set_resize.argtypes = [vp, i, i]
+    lib.dts_set_resize_filter.argtypes = [vp, i, i, i]
     lib.dts_set_render_mode.argtypes = [vp, i]
     lib.dts_resize_frames.argtypes = [vp, vp, vp, vp]
     lib.dts_blend4.argtypes = [vp, vp, vp, vp, C.c_uint64, vp]
@@ -203,7 +205,7 @@ def load() -> C.CDLL:
 
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
-           "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_render_mode", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
+           "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame", "dts_last_error", "dts_destroy"]
 
 
@@ -416,8 +418,12 @@ class Sim:
         self._check(self.lib.dts_set_render_mode(self.h, (RENDER_SEGMENT if segment else 0) | (RENDER_TOP_DOWN if top_down else 0)),
                     "dts_set_render_mode")
 
-    def set_resize(self, out_w: int, out_h: int):
-        self._check(self.lib.dts_set_resize(self.h, int(out_w), int(out_h)), "dts_set_resize")
+    def set_resize(self, out_w: int, out_h: int, filter: int = 0):
+        """filter RESIZE_CV2_CUBIC (dts_set_resize) or RESIZE_PIL_BILINEAR (dts_set_resize_filter)."""
+        if filter == RESIZE_CV2_CUBIC:
+            self._check(self.lib.dts_set_resize(self.h, int(out_w), int(out_h)), "dts_set_resize")
+        else:
+            self._check(self.lib.dts_set_resize_filter(self.h, int(out_w), int(out_h), int(filter)), "dts_set_resize_filter")
 
     def resize_frames(self, src_ptr: int, dst_ptr: int, stream: int = 0):
         self._check(self.lib.dts_resize_frames(self.h, src_ptr, dst_ptr, stream), "dts_resize_frames")

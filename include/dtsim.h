@@ -274,6 +274,14 @@ int dts_set_output_format(dts_sim* sim, const dts_output_format* fmt);
  * num_envs x 3 x out_h x out_w elements in the selected layout / dtype (OpenCV's 8-bit fixed-point bicubic; matches cv2
  * within 1 LSB).  out_w = out_h = 0 switches it off. */
 int dts_set_resize(dts_sim* sim, int out_w, int out_h);
+/* The same resize slot with a choice of filter.  DTS_RESIZE_CV2_CUBIC is dts_set_resize.  DTS_RESIZE_PIL_BILINEAR is
+ * learning/utils/wrappers.py:39-54's ResizeWrapper: scipy.misc.imresize(obs, (out_h, out_w, 3)), which for a uint8 RGB
+ * frame is PIL.Image.resize((out_w, out_h), BILINEAR) — Pillow's 8-bit fixed-point triangle filter, widened by the
+ * scale factor when it shrinks; bit-exact.  That filter takes targets of at least 1/32 of the camera size per axis
+ * (at most 65 taps per output pixel): a smaller one is refused and the previous setting stays in effect.
+ * out_w = out_h = 0 switches resizing off whatever the filter. */
+enum { DTS_RESIZE_CV2_CUBIC = 0, DTS_RESIZE_PIL_BILINEAR = 1 };
+int dts_set_resize_filter(dts_sim* sim, int out_w, int out_h, int filter);
 /* MotionBlurWrapper (learning/utils/wrappers.py:8-54): out f64[n] = np.average of four u8 frame batches with `weights`
  * (numpy's evaluation order), and the knobs that wrapper turns on the wrapped env: delta_time / frame_skip (it divides
  * env.delta_time by 3 and drives update_physics itself, LW:13-14) and the action convention (wheel commands). */
