@@ -83,6 +83,8 @@ class BatchedDuckietownEnv:
         self._first_reset = True
         self.resize = None
         self.resize_method = None
+        self._undistort = False      # Simulator.undistort: no fisheye on any render
+        self.rectification = None    # (mapx, mapy) UndistortWrapper installed for reset / step observations
         self.output_format = dict(obs_layout="hwc", obs_dtype="uint8", reward="raw", discrete_actions=False,
                                   action_vel_scale=1.0)
         self.seed(seed)
@@ -143,6 +145,32 @@ class BatchedDuckietownEnv:
         frames = frames.to(self.device).contiguous()
         self.sim.resize_frames(frames.data_ptr(), self.obs.data_ptr(), self._stream())
         return self.obs
+
+    @property
+    def undistort(self) -> bool:
+        """Simulator.undistort (S:361), which UndistortWrapper sets: True skips the fisheye gather of a `distortion` env
+        (S:1969-1970), so every render is the pinhole frame, and reset / step observations go through the installed
+        rectification if there is one.  On an env without distortion it changes nothing."""
+        return self._undistort
+
+    @undistort.setter
+    def undistort(self, value: bool):
+        self._undistort = bool(value)
+        self.sim.set_render_mode(**self._base_mode())
+
+    def set_rectification(self, mapx: Optional[np.ndarray], mapy: Optional[np.ndarray]):
+        """UndistortWrapper's `cv2.remap(obs, mapx, mapy, INTER_NEAREST)` of reset / step observations, fused into the
+        render (dts_set_rectify_lut): each output pixel is rendered at the source pixel the map names.  Applies while
+        `undistort` is True; needs an env built with distortion=True.  None, None removes it.  A map the device refuses
+        raises and leaves the previous one in effect."""
+        self.sim.set_rectify_lut(mapx, mapy)
+        self.rectification = None if mapx is None and mapy is None else (mapx, mapy)
+        self.sim.set_render_mode(**self._base_mode())
+        return self
+
+    def _base_mode(self) -> dict:
+        """The render mode of reset / step observations."""
+        return dict(pinhole=self._undistort, rectify=self._undistort and self.rectification is not None)
 
     # ------------------------------------------------------------------ gym-like surface
     def seed(self, seed=None):
@@ -210,14 +238,17 @@ class BatchedDuckietownEnv:
         return obs, reward, done.view(torch.bool), self.state
 
     def render_obs(self, segment: bool = False, top_down: bool = False, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """render_obs(segment) (S:1953-1972) of the current state; `top_down` gives _render_img(top_down=True)'s camera."""
+        """render_obs(segment) (S:1953-1972) of the current state; `top_down` gives _render_img(top_down=True)'s camera.
+        Under `undistort` this is the pinhole frame: UndistortWrapper rectifies only reset / step observations."""
         tgt = self.obs if out is None else out
-        if segment or top_down:
-            self.sim.set_render_mode(segment, top_down)
+        base = self._base_mode()
+        mode = dict(segment=segment, top_down=top_down, pinhole=self._undistort, rectify=False)
+        if segment or top_down or base["rectify"]:
+            self.sim.set_render_mode(**mode)
             try:
                 self.sim.render(tgt.data_ptr(), self._stream())
             finally:
-                self.sim.set_render_mode(False, False)
+                self.sim.set_render_mode(**base)
         else:
             self.sim.render(tgt.data_ptr(), self._stream())
         return tgt

@@ -422,7 +422,20 @@ int dts_set_fisheye_lut(dts_sim* sim, const float* rmapx, const float* rmapy, in
     return sim->fail("fisheye LUT is %dx%d but the camera is %dx%d", width, height, sim->cfg.cam_width, sim->cfg.cam_height);
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   DTS_CUDA(cudaDeviceSynchronize());
-  const std::string e = renderer_set_fisheye(*sim->render, rmapx, rmapy);
+  const std::string e = renderer_set_lut(*sim->render, false, rmapx, rmapy);
+  return e.empty() ? 0 : sim->fail("%s", e.c_str());
+}
+
+int dts_set_rectify_lut(dts_sim* sim, const float* mapx, const float* mapy, int width, int height) {
+  if (!sim) return 1;
+  // a gather's bins are overlapping source boxes: only a DTS_FLAG_DISTORTION handle sizes its pair pool for them
+  if (!(sim->cfg.flags & DTS_FLAG_DISTORTION)) return sim->fail("rectification LUT on a handle created without DTS_FLAG_DISTORTION");
+  if (!mapx != !mapy) return sim->fail("rectification LUT: one of mapx / mapy is NULL");
+  if (mapx && (width != sim->cfg.cam_width || height != sim->cfg.cam_height))
+    return sim->fail("rectification LUT is %dx%d but the camera is %dx%d", width, height, sim->cfg.cam_width, sim->cfg.cam_height);
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  DTS_CUDA(cudaDeviceSynchronize());
+  const std::string e = renderer_set_lut(*sim->render, true, mapx, mapy);
   return e.empty() ? 0 : sim->fail("%s", e.c_str());
 }
 
@@ -512,7 +525,7 @@ int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
   if (!obs_dev) return sim->fail("obs_dev is NULL");
   if (check_maps(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  const std::string e = renderer_prepare(*sim->render, sim->h_maps.data(), (int)sim->h_maps.size());
+  const std::string e = renderer_prepare(*sim->render, sim->h_maps.data(), (int)sim->h_maps.size(), sim->render_mode);
   if (!e.empty()) return sim->fail("%s", e.c_str());
   RenderCfg rc{sim->cfg.cam_width, sim->cfg.cam_height, sim->cfg.flags, sim->cfg.num_envs,
                (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->render_mode};
@@ -750,7 +763,8 @@ int dts_set_timing(dts_sim* sim, double delta_time, int frame_skip, int action_m
 
 int dts_set_render_mode(dts_sim* sim, int mode) {
   if (!sim) return 1;
-  if (mode & ~(DTS_RENDER_SEGMENT | DTS_RENDER_TOP_DOWN)) return sim->fail("bad render mode %d", mode);
+  if (mode & ~(DTS_RENDER_SEGMENT | DTS_RENDER_TOP_DOWN | DTS_RENDER_PINHOLE | DTS_RENDER_RECTIFY))
+    return sim->fail("bad render mode %d", mode);
   sim->render_mode = mode;
   return 0;
 }

@@ -23,7 +23,7 @@ struct RenderCfg {
   int32_t n_envs;
   int32_t tessellate;         // 1: literal 98 triangles per road tile (spec tile mode 0)
   int32_t obs_layout, obs_dtype;   // DTS_OBS_* (dts_output_format)
-  int32_t mode;               // DTS_RENDER_SEGMENT | DTS_RENDER_TOP_DOWN (dts_set_render_mode)
+  int32_t mode;               // DTS_RENDER_* (dts_set_render_mode)
 };
 
 void launch_step_logic(const DState& S, const DMap* maps, const StepCfg& c, int n_maps_cycle, const float* actions,
@@ -53,11 +53,12 @@ Renderer* renderer_create(const dts_config& cfg);   // on cfg.device, which must
 void renderer_destroy(Renderer* r);
 void renderer_release_frame(Renderer& r);   // the maps changed: the next render re-sizes frame memory for them
 // Before every render: reserves frame memory for the valid maps of maps[0 .. n_maps) unless it is reserved, and checks
-// that a fisheye LUT is set if the camera needs one.
-std::string renderer_prepare(Renderer& r, const DMap* maps, int n_maps);
-// The fused fisheye's tables for a LUT of the camera's size (obs[y, x] = frame[rint(rmapy), rint(rmapx)]); they replace
-// the previous ones, so no render may be in flight.  A LUT the rasteriser cannot take leaves the previous tables.
-std::string renderer_set_fisheye(Renderer& r, const float* rmapx, const float* rmapy);
+// that a fisheye LUT is set if the camera needs one and a rectification LUT if render `mode` asks for it.
+std::string renderer_prepare(Renderer& r, const DMap* maps, int n_maps, int mode);
+// The fused gather's tables for a LUT of the camera's size (obs[y, x] = frame[rint(rmapy), rint(rmapx)]), in the fisheye
+// slot or (`rectify`) the rectification slot; they replace that slot's previous ones, so no render may be in flight.  A
+// LUT the rasteriser cannot take leaves the previous tables; NULL maps free the slot.
+std::string renderer_set_lut(Renderer& r, bool rectify, const float* rmapx, const float* rmapy);
 // `marks`: NULL or kProfMarks events recorded on `st` before k_frame_setup and after each of k_frame_setup, k_geometry,
 // k_bin, k_raster and the post passes (dts_profile_*).  `status_dev`: device address of the mapped host status word.
 constexpr int kProfMarks = 6;

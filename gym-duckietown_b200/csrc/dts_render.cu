@@ -40,7 +40,8 @@ namespace dts {
 
 // Fused fisheye gather (distortion.py:118, obs[y, x] = undistorted[rint(rmapy), rint(rmapx)]): the rasteriser renders
 // each OUTPUT pixel at the source position the LUT names, so no undistorted frame is ever written.  Prims are binned
-// against the source-pixel bounding boxes of the output bins.  All device pointers, built by renderer_set_fisheye.
+// against the source-pixel bounding boxes of the output bins.  All device pointers, built by renderer_set_lut, for the
+// fisheye LUT or UndistortWrapper's rectification map alike.
 struct FishTab {
   const int32_t* src_xy;   // [H][W]  sx | sy << 16 (int16 each); sx = -32768: source outside the image -> 0
   const short4* cbox;      // [cbins]    source bounding box (x0, y0, x1, y1) of a 32x8 coarse output bin; x1 < x0: empty
@@ -866,6 +867,7 @@ struct Renderer {
   void* frame = nullptr;     // frame memory (null: not reserved since the last map upload)
   FrameMem fm{};             // ... carved
   FishTab fish{};            // fused fisheye tables (null until a LUT is set)
+  FishTab rect{};            // UndistortWrapper's rectification, gathered the same way (null unless set)
   PilTab pil{};              // Pillow bilinear resize tables (null unless that filter is selected)
 };
 
@@ -2523,11 +2525,11 @@ void renderer_release_frame(Renderer& r) {
 }
 
 void renderer_destroy(Renderer* r) {
-  if (r) { renderer_release_frame(*r); free_fish(r->fish); free_pil(r->pil); }
+  if (r) { renderer_release_frame(*r); free_fish(r->fish); free_fish(r->rect); free_pil(r->pil); }
   delete r;
 }
 
-std::string renderer_prepare(Renderer& r, const DMap* maps, int n_maps) {
+std::string renderer_prepare(Renderer& r, const DMap* maps, int n_maps, int mode) {
   if (!r.frame) {
     // prims k_geometry emits per road tile: the literal triangles of tile mode 0, or the quad of tile mode 1, which a
     // clip splits into two triangles and fans into a few more
@@ -2566,13 +2568,20 @@ std::string renderer_prepare(Renderer& r, const DMap* maps, int n_maps) {
     carve(r, reinterpret_cast<uintptr_t>(r.frame), r.fm);
   }
   if ((r.flags & DTS_FLAG_DISTORTION) && !r.fish.src_xy) return "distortion enabled but no fisheye LUT set";
+  if ((mode & DTS_RENDER_RECTIFY) && !r.rect.src_xy) return "DTS_RENDER_RECTIFY but no rectification LUT set";
   return "";
 }
 
-std::string renderer_set_fisheye(Renderer& r, const float* rmapx, const float* rmapy) {
-  // distortion.py:118 gathers img[rint(rmapy), rint(rmapx)].  The rasteriser renders those source pixels directly: per
-  // output pixel the source position, per fine / coarse output bin the bounding box of its source pixels (the bins
-  // prims are sorted into).
+std::string renderer_set_lut(Renderer& r, bool rectify, const float* rmapx, const float* rmapy) {
+  // distortion.py:118 gathers img[rint(rmapy), rint(rmapx)], UndistortWrapper (wrappers.py:227) the same with its own
+  // map.  The rasteriser renders those source pixels directly: per output pixel the source position, per fine / coarse
+  // output bin the bounding box of its source pixels (the bins prims are sorted into).
+  FishTab& slot = rectify ? r.rect : r.fish;
+  const char* what = rectify ? "rectification LUT" : "fisheye LUT";
+  if (!rmapx || !rmapy) {
+    free_fish(slot);
+    return "";
+  }
   const int W = r.W, H = r.H, cbx_n = (W + kCoarseW - 1) / kCoarseW, cbins = r.cbins;
   std::vector<int32_t> src((size_t)W * H);
   const short4 empty = make_short4(32767, 32767, -32768, -32768);
@@ -2601,7 +2610,7 @@ std::string renderer_set_fisheye(Renderer& r, const float* rmapx, const float* r
     if (cbox[b].z < cbox[b].x) continue;
     const long long w = cbox[b].z - cbox[b].x + 2, h = cbox[b].w - cbox[b].y + 2;
     if ((long long)H * w + (long long)W * h >= (1LL << 30) / (kEdge * kSub))
-      return "fisheye LUT sends output bin " + std::to_string(b) + " to a " + std::to_string(w) + "x" + std::to_string(h) +
+      return std::string(what) + " sends output bin " + std::to_string(b) + " to a " + std::to_string(w) + "x" + std::to_string(h) +
              " px source region: too wide for the rasteriser's int32 edge functions";
   }
   // two inverse indices over source cells (the coarse grid laid over the source image): per cell, the output bins whose
@@ -2633,7 +2642,6 @@ std::string renderer_set_fisheye(Renderer& r, const float* rmapx, const float* r
   home_start.push_back((int32_t)home_ent.size());
   if (cell_bins.empty()) cell_bins.push_back(0);
   if (home_ent.empty()) home_ent.push_back(make_int4(0, 0, 0, 0));
-  free_fish(r.fish);
   FishTab t{};
   cudaError_t e = cudaSuccess;
   auto upload = [&](auto& dst, const auto& v) {
@@ -2646,9 +2654,10 @@ std::string renderer_set_fisheye(Renderer& r, const float* rmapx, const float* r
   upload(t.src_xy, src); upload(t.cbox, cbox); upload(t.fbox, fbox);
   upload(t.cell_start, cell_start); upload(t.cell_bins, cell_bins);
   upload(t.home_start, home_start); upload(t.home_ent, home_ent);
-  if (e != cudaSuccess) { free_fish(t); return std::string("fisheye table upload failed: ") + cudaGetErrorString(e); }
+  if (e != cudaSuccess) { free_fish(t); return std::string(what) + " table upload failed: " + cudaGetErrorString(e); }
   t.ext_x = ext_x; t.ext_y = ext_y;
-  r.fish = t;
+  free_fish(slot);
+  slot = t;
   return "";
 }
 
@@ -2691,7 +2700,12 @@ std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, in
 int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, void* obs_any, const GatherTab& gather,
                   int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level, cudaStream_t st) {
   uint8_t* obs = reinterpret_cast<uint8_t*>(obs_any);
-  const bool fisheye = (rc.flags & DTS_FLAG_DISTORTION) != 0;
+  // the gather the frame goes through, if any: the rectification (DTS_RENDER_RECTIFY), none (DTS_RENDER_PINHOLE or no
+  // DTS_FLAG_DISTORTION) or the fisheye.  Both tables run the same kFish kernels.
+  const FishTab* lut = (rc.mode & DTS_RENDER_RECTIFY) ? &r.rect
+                     : ((rc.flags & DTS_FLAG_DISTORTION) && !(rc.mode & DTS_RENDER_PINHOLE)) ? &r.fish : nullptr;
+  const bool fisheye = lut != nullptr;
+  const FishTab ft = fisheye ? *lut : FishTab{};
   FrameMem fm = r.fm;
   fm.status = status_dev;
   int mk = 0;
@@ -2714,16 +2728,16 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   const auto bin = fisheye ? k_bin<true> : k_bin<false>;
   if (bin_smem_bytes > 48 * 1024)   // cameras beyond ~640x480 (cbins > 1536): opt in to large dynamic shared memory
     cudaFuncSetAttribute(bin, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bin_smem_bytes);
-  bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, r.fish, r.max_prims, r.pool, err_flag);
+  bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, ft, r.max_prims, r.pool, err_flag);
   mark();
   const bool wrap = (rc.obs_layout | rc.obs_dtype) != 0;
   int launches = 5;
   if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
     const auto solo = fisheye ? k_raster_solo<true> : k_raster_solo<false>;
     const auto flat = fisheye ? k_raster_flat<true> : k_raster_flat<false>;
-    solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, r.fish, obs, r.max_prims, r.max_lat);
+    solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat);
     // before k_raster, which draws the bins k_raster_flat hands back
-    flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, r.fish, obs, r.max_prims, r.max_lat, err_flag);
+    flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, err_flag);
     launches += 2;
   }
   static bool smem_opt_in = false;
@@ -2735,7 +2749,7 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
     smem_opt_in = true;
   }
   const auto raster = fisheye ? (wrap ? k_raster<true, true> : k_raster<false, true>) : (wrap ? k_raster<true, false> : k_raster<false, false>);
-  raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, r.fish, gather, obs, r.max_prims, r.pool, r.max_lat, err_flag);
+  raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, ft, gather, obs, r.max_prims, r.pool, r.max_lat, err_flag);
   mark();
   mark();   // (post passes: none yet)
   return launches;

@@ -17,7 +17,18 @@ import numpy as np
 CAMERA_MATRIX = np.reshape([305.5718893575089, 0, 303.0797142544728, 0, 308.8338858195428, 231.8845403702499,
                             0, 0, 1], (3, 3))
 DISTORTION_COEFS = np.reshape([-0.2, 0.0305, 0.0005859930422629722, -0.0006697840226199427, 0], (1, 5))
+# P of the rectified image UndistortWrapper emits — wrappers.py:184-198
+RECTIFIED_PROJECTION = np.reshape([220.2460277141687, 0, 301.8668918355899, 0, 0, 238.6758484095299, 227.0880056118307,
+                                   0, 0, 0, 1, 0], (3, 4))
 _SPLAT = [(-1, -1, 7), (-1, 0, 10), (-1, 1, 7), (0, -1, 10), (0, 0, 20), (0, 1, 10), (1, -1, 7), (1, 0, 10), (1, 1, 7)]
+
+
+def rectify_maps(width: int, height: int):
+    """UndistortWrapper's (mapx, mapy), float32 [height][width] each (wrappers.py:210-225): the map it builds at the
+    observation's size, with K and D of the raw camera, R = I and its own P.  The wrapper's observation is
+    `cv2.remap(pinhole_frame, mapx, mapy, INTER_NEAREST)`: frame[rint(mapy), rint(mapx)], 0 outside the frame."""
+    return cv2.initUndistortRectifyMap(CAMERA_MATRIX, DISTORTION_COEFS, np.eye(3), RECTIFIED_PROJECTION,
+                                       (int(width), int(height)), cv2.CV_32FC1)
 
 
 def invert_map(mapx: np.ndarray, mapy: np.ndarray):
@@ -95,5 +106,7 @@ class Distortion:
         return out
 
     def undistort(self, observation: np.ndarray) -> np.ndarray:
-        """UndistortWrapper's inverse step (distortion.py:127-136)."""
+        """Distortion._undistort (distortion.py:127-136): remaps with this camera model's maps, whose new camera
+        matrix comes from getOptimalNewCameraMatrix.  Not UndistortWrapper's map, which uses the wrapper's own P
+        (rectify_maps); at 640x480 the two differ by up to 18 px."""
         return cv2.remap(observation, self.mapx, self.mapy, cv2.INTER_NEAREST)

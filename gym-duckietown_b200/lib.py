@@ -92,7 +92,7 @@ class Mesh(C.Structure):
     _fields_ = [("tri_offset", C.c_int32), ("tri_count", C.c_int32), ("seg_flat_tex", C.c_int32), ("reserved", C.c_int32)]
 
 
-RENDER_SEGMENT, RENDER_TOP_DOWN = 1, 2
+RENDER_SEGMENT, RENDER_TOP_DOWN, RENDER_PINHOLE, RENDER_RECTIFY = 1, 2, 4, 8
 
 
 class MapBlob(C.Structure):
@@ -165,6 +165,7 @@ def load() -> C.CDLL:
     lib.dts_create.argtypes = [C.POINTER(Config), C.POINTER(vp)]
     lib.dts_upload_map.argtypes = [vp, i, C.POINTER(MapBlob)]
     lib.dts_set_fisheye_lut.argtypes = [vp, vp, vp, i, i]
+    lib.dts_set_rectify_lut.argtypes = [vp, vp, vp, i, i]
     lib.dts_reset.argtypes = [vp, vp, C.POINTER(EpisodeParams), vp]
     lib.dts_reset_random.argtypes = [vp, vp, vp]
     lib.dts_seed_streams.argtypes = [vp, vp, vp]
@@ -204,7 +205,7 @@ def load() -> C.CDLL:
     return lib
 
 
-EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
+EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
            "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame", "dts_last_error", "dts_destroy"]
 
@@ -340,12 +341,26 @@ class Sim:
         holder = MapBlobHolder(md, user_tile_start)
         self._check(self.lib.dts_upload_map(self.h, map_id, C.byref(holder.blob)), "dts_upload_map")
 
-    def set_fisheye_lut(self, rmapx: np.ndarray, rmapy: np.ndarray):
-        rx, ry = np.ascontiguousarray(rmapx, np.float32), np.ascontiguousarray(rmapy, np.float32)
+    @staticmethod
+    def _lut(what: str, mx: np.ndarray, my: np.ndarray):
+        rx, ry = np.ascontiguousarray(mx, np.float32), np.ascontiguousarray(my, np.float32)
         if rx.ndim != 2 or rx.shape != ry.shape:   # the library reads camera_height x camera_width floats from each
-            raise ValueError(f"fisheye LUT: rmapx {rx.shape} and rmapy {ry.shape} must be two 2-D arrays of one shape")
+            raise ValueError(f"{what}: {rx.shape} and {ry.shape} must be two 2-D arrays of one shape")
+        return rx, ry
+
+    def set_fisheye_lut(self, rmapx: np.ndarray, rmapy: np.ndarray):
+        rx, ry = self._lut("fisheye LUT", rmapx, rmapy)
         self._check(self.lib.dts_set_fisheye_lut(self.h, _ptr(rx), _ptr(ry), rx.shape[1], rx.shape[0]),
                     "dts_set_fisheye_lut")
+
+    def set_rectify_lut(self, mapx: Optional[np.ndarray], mapy: Optional[np.ndarray]):
+        """UndistortWrapper's map for DTS_RENDER_RECTIFY; None, None clears it."""
+        if mapx is None and mapy is None:
+            self._check(self.lib.dts_set_rectify_lut(self.h, None, None, 0, 0), "dts_set_rectify_lut")
+            return
+        rx, ry = self._lut("rectification LUT", mapx, mapy)
+        self._check(self.lib.dts_set_rectify_lut(self.h, _ptr(rx), _ptr(ry), rx.shape[1], rx.shape[0]),
+                    "dts_set_rectify_lut")
 
     def reset(self, mask_ptr: Optional[int], params: dict, stream: int = 0):
         n = self.cfg.num_envs
@@ -414,9 +429,10 @@ class Sim:
             raise ValueError("map_ids must have one entry per env")
         self._check(self.lib.dts_assign_maps(self.h, mask_ptr, _ptr(ids), stream), "dts_assign_maps")
 
-    def set_render_mode(self, segment: bool = False, top_down: bool = False):
-        self._check(self.lib.dts_set_render_mode(self.h, (RENDER_SEGMENT if segment else 0) | (RENDER_TOP_DOWN if top_down else 0)),
-                    "dts_set_render_mode")
+    def set_render_mode(self, segment: bool = False, top_down: bool = False, pinhole: bool = False, rectify: bool = False):
+        mode = (RENDER_SEGMENT if segment else 0) | (RENDER_TOP_DOWN if top_down else 0) | \
+               (RENDER_PINHOLE if pinhole else 0) | (RENDER_RECTIFY if rectify else 0)
+        self._check(self.lib.dts_set_render_mode(self.h, mode), "dts_set_render_mode")
 
     def set_resize(self, out_w: int, out_h: int, filter: int = 0):
         """filter RESIZE_CV2_CUBIC (dts_set_resize) or RESIZE_PIL_BILINEAR (dts_set_resize_filter)."""

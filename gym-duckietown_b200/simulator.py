@@ -80,7 +80,7 @@ class Simulator(Env):
         self.frame_rate, self.delta_time, self.frame_skip = frame_rate, 1.0 / frame_rate, frame_skip
         self.camera_width, self.camera_height, self.robot_speed = camera_width, camera_height, robot_speed
         self.accept_start_angle_deg = accept_start_angle_deg
-        self.distortion, self.undistort, self.dynamics_rand = distortion, False, dynamics_rand
+        self.distortion, self.dynamics_rand = distortion, dynamics_rand
         self.seed_value = seed
         self.randomize_maps_on_reset = randomize_maps_on_reset
         map_arg = map_name
@@ -197,6 +197,16 @@ class Simulator(Env):
 
     def _scalars(self):
         return {k: v[0].item() for k, v in self._b.state.items()}
+
+    @property
+    def undistort(self) -> bool:
+        """S:361, set by the reference's UndistortWrapper: True returns pinhole frames instead of fisheye ones (S:1969-1970),
+        which that wrapper then remaps on the host.  Kept by the batched env (BatchedDuckietownEnv.undistort)."""
+        return self._b.undistort
+
+    @undistort.setter
+    def undistort(self, value: bool):
+        self._b.undistort = value
 
     @property
     def cur_pos(self):

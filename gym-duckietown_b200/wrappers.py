@@ -13,6 +13,8 @@ same constructor arguments, same resulting observation_space as the reference cl
 
 `ResizeWrapper` runs cv2.INTER_CUBIC's 8-bit arithmetic in a device pass right after the render
 (`dts_set_resize`), so the resized batch — not the full frames — is what a host-facing pipeline copies out.
+`UndistortWrapper`'s rectification is a second table of the render's fused gather (`dts_set_rectify_lut`): the
+rectified frame is rendered directly, with no extra pass.
 """
 from __future__ import annotations
 
@@ -60,6 +62,13 @@ class _FusedWrapper:
 
     def reset(self, *a, **kw):
         return self.env.reset(*a, **kw)
+
+    def _wrapped(self):
+        """The fused wrappers below this one, outermost first."""
+        e = self.env
+        while isinstance(e, _FusedWrapper):
+            yield e
+            e = e.env
 
 
 class ImgWrapper(_FusedWrapper):
@@ -142,6 +151,35 @@ class ResizeWrapper(_FusedWrapper):
         self.batched.set_resize(resize_w, resize_h)
 
 
+class UndistortWrapper(_FusedWrapper):
+    """W:145-227 — the env renders without its fisheye (`unwrapped.undistort = True`) and every reset / step observation
+    is `cv2.remap(obs, mapx, mapy, cv2.INTER_NEAREST)` with the map `cv2.initUndistortRectifyMap(K, D, I, P, (W, H),
+    CV_32FC1)` at the observation's size (distortion.rectify_maps).  Here that gather runs inside the render through a
+    second table of the fused fisheye kernels (BatchedDuckietownEnv.set_rectification): the rectified frame is rendered
+    directly.  `render_obs()` stays the pinhole frame, as in the reference.
+
+    Stacking: resize, layout and dtype wrappers may go above this one (the resize pass reads the rectified render; a
+    nearest gather commutes with /255 and with the transposes).  Below it they are refused — the reference would then
+    build the map at the resized or transposed shape — and so is MotionBlurWrapper in either order."""
+
+    def __init__(self, env=None):
+        super().__init__(env)
+        assert self.unwrapped.distortion, "Distortion is false, no need for this wrapper"
+        b = self.batched
+        if b.resize is not None:
+            raise ValueError(f"the env already resizes its observations to {b.resize[0]}x{b.resize[1]}: put "
+                             "UndistortWrapper below the resize wrapper, whose pass then reads the rectified frames")
+        if b.output_format["obs_layout"] != "hwc":
+            raise ValueError(f"the env emits {b.output_format['obs_layout'].upper()} observations: put UndistortWrapper "
+                             "below the layout wrapper, so that its map is built for H x W x 3 frames")
+        if any(isinstance(w, MotionBlurWrapper) for w in self._wrapped()):
+            raise ValueError("UndistortWrapper does not go on top of MotionBlurWrapper")
+        from .distortion import rectify_maps
+        self.mapx, self.mapy = rectify_maps(b.camera_width, b.camera_height)
+        b.set_rectification(self.mapx, self.mapy)
+        self.unwrapped.undistort = True                                      # W:159
+
+
 class MotionBlurWrapper(_FusedWrapper):
     """LW:8-54 — the reference class sets `frame_skip = 3`, divides the wrapped env's delta_time by it and, per step,
     renders before each of three `update_physics(action)` calls and once after, returning
@@ -157,6 +195,8 @@ class MotionBlurWrapper(_FusedWrapper):
         b = self.batched
         if b.auto_reset:
             raise ValueError("MotionBlurWrapper steps the physics three times per step: build the env without auto_reset")
+        if b.undistort:
+            raise ValueError("MotionBlurWrapper does not go on top of UndistortWrapper or an env with undistort set")
         self.frame_skip = 3
         b.delta_time = b.delta_time / self.frame_skip                       # LW:14
         from . import lib as L

@@ -243,6 +243,13 @@ int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* blob);
  * undistorted frame is materialised and no second pass runs.  Fails if the LUT scatters one 32x8 output bin over a
  * source region too wide for the rasteriser's int32 edge functions. */
 int dts_set_fisheye_lut(dts_sim* sim, const float* rmapx, const float* rmapy, int width, int height);
+/* UndistortWrapper's rectification (wrappers.py:206-227: cv2.remap(frame, mapx, mapy, INTER_NEAREST) of the pinhole
+ * frame, with mapx/mapy from cv2.initUndistortRectifyMap(K, D, I, P, (W, H), CV_32FC1)): a second LUT [H][W] each (HOST
+ * pointers), gathered by the same fused kernels as the fisheye's under DTS_RENDER_RECTIFY, so the rectified frame
+ * costs no extra pass.  Validated like dts_set_fisheye_lut (camera-sized only; non-finite or huge entries name no
+ * source; a LUT too wide for the edge functions is refused and the previous one stays in effect).  Only on a handle
+ * created with DTS_FLAG_DISTORTION, whose pair pool is sized for gathers.  NULL, NULL clears it. */
+int dts_set_rectify_lut(dts_sim* sim, const float* mapx, const float* mapy, int width, int height);
 /* Simulator.reset() (simulator.py:528-763) with host-drawn episode parameters.
  * mask_dev: device u8[num_envs] (NULL = all). */
 int dts_reset(dts_sim* sim, const uint8_t* mask_dev, const dts_episode_params* params, void* stream);
@@ -263,8 +270,12 @@ int dts_render(dts_sim* sim, void* obs_dev, void* stream);
  *   DTS_RENDER_SEGMENT   segment=True: lighting off (S:1730-1733), magenta clear + ground (S:1752, 1808), no distractors
  *                        (S:1814), segmentation textures / flat per-class mesh colours
  *   DTS_RENDER_TOP_DOWN  top_down=True: camera above the map centre looking down (S:1786-1798), the agent's own mesh drawn
- *                        at cur_pos (S:1923-1929) */
-enum { DTS_RENDER_SEGMENT = 1, DTS_RENDER_TOP_DOWN = 2 };
+ *                        at cur_pos (S:1923-1929)
+ *   DTS_RENDER_PINHOLE   Simulator.undistort = True: the fisheye gather of DTS_FLAG_DISTORTION is skipped (S:1969-1970,
+ *                        2001-2002), the pinhole frame is emitted
+ *   DTS_RENDER_RECTIFY   UndistortWrapper's observation (wrappers.py:206-227): the pinhole frame gathered through the
+ *                        dts_set_rectify_lut table; implies PINHOLE.  dts_render fails while no such table is set. */
+enum { DTS_RENDER_SEGMENT = 1, DTS_RENDER_TOP_DOWN = 2, DTS_RENDER_PINHOLE = 4, DTS_RENDER_RECTIFY = 8 };
 int dts_set_render_mode(dts_sim* sim, int mode);
 /* Select the fused wrapper behaviour for subsequent dts_step / dts_render calls (default: all zero, scale 1).
  * obs_dev then holds num_envs * 3 * H * W elements of uint8 or float32 in the chosen layout. */
