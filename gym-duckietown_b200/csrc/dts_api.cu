@@ -36,6 +36,8 @@ struct dts_sim {
   int32_t* d_err = nullptr;
   int32_t* h_status = nullptr;          // mapped pinned host word: bit 0 = a frame overflowed its frame memory
   int32_t* d_status = nullptr;          // its device address
+  int32_t* ended = nullptr;             // dts_step_terminal: [N] the envs whose episode ended this step, *n_ended of them
+  int32_t* n_ended = nullptr;
   // fused end-of-rollout gather over peer memory (dts_gather_*)
   uint8_t* gather_buf = nullptr;        // [world][bytes_per_rank], this rank's copy of everybody's observations
   uint64_t gather_bytes = 0;
@@ -169,6 +171,8 @@ int dts_create(const dts_config* cfg, dts_sim** out) {
   bad |= sim->dalloc(&S.rep, n);
   bad |= sim->dalloc(&sim->d_maps, cfg->max_maps);
   bad |= sim->dalloc(&sim->d_err, 32);
+  bad |= sim->dalloc(&sim->ended, n);
+  bad |= sim->dalloc(&sim->n_ended, 1);
   if (cudaHostAlloc((void**)&sim->h_status, 64, cudaHostAllocMapped) != cudaSuccess ||
       cudaHostGetDevicePointer((void**)&sim->d_status, sim->h_status, 0) != cudaSuccess) {
     sim->fail("cudaHostAlloc(mapped status word) failed"); bad = 1;
@@ -510,36 +514,40 @@ int dts_reset_random(dts_sim* sim, const uint8_t* mask_dev, void* stream) {
   return 0;
 }
 
-// the resize pass dts_set_resize_filter selected: full-size u8 HWC frames -> the caller's tensor
-static void launch_selected_resize(dts_sim* sim, const uint8_t* src, void* dst, cudaStream_t st) {
+// the resize pass dts_set_resize_filter selected: full-size u8 HWC frames -> the caller's tensor (the listed envs only,
+// given a device env list)
+static void launch_selected_resize(dts_sim* sim, const uint8_t* src, void* dst, cudaStream_t st,
+                                   const int32_t* env_list = nullptr, const int32_t* env_count = nullptr) {
   if (sim->resize_filter == DTS_RESIZE_PIL_BILINEAR) {
-    launch_pil_resize(*sim->render, src, dst, sim->fmt.obs_layout, sim->fmt.obs_dtype, st);
+    launch_pil_resize(*sim->render, src, dst, sim->fmt.obs_layout, sim->fmt.obs_dtype, env_list, env_count, st);
     return;
   }
   launch_resize(src, sim->cfg.cam_width, sim->cfg.cam_height, sim->resize_w, sim->resize_h, sim->cfg.num_envs,
-                sim->resize_xtab, sim->resize_ytab, dst, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->resize_band, sim->resize_cap, st);
+                sim->resize_xtab, sim->resize_ytab, dst, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->resize_band, sim->resize_cap,
+                env_list, env_count, st);
 }
 
-int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
-  if (!sim) return 1;
+// dts_render of every env, or of the envs on a device list (dts_step_terminal's second pass; not profiled)
+static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t* env_list, const int32_t* env_count) {
   if (!obs_dev) return sim->fail("obs_dev is NULL");
   if (check_maps(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   const std::string e = renderer_prepare(*sim->render, sim->h_maps.data(), (int)sim->h_maps.size(), sim->render_mode);
   if (!e.empty()) return sim->fail("%s", e.c_str());
   RenderCfg rc{sim->cfg.cam_width, sim->cfg.cam_height, sim->cfg.flags, sim->cfg.num_envs,
-               (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->render_mode};
+               (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->render_mode,
+               env_list, env_count};
   if (*(volatile int32_t*)sim->h_status & 1)
     return sim->fail("an earlier frame overflowed its render frame memory (prim slab / bin lists) and was left incomplete");
   cudaEvent_t* marks = nullptr;
-  if (sim->profiling) {
+  if (sim->profiling && !env_list) {
     const size_t base = sim->prof_events.size();
     sim->prof_events.resize(base + kProfMarks);
     for (int k = 0; k < kProfMarks; k++) DTS_CUDA(cudaEventCreate(&sim->prof_events[base + k]));
     marks = sim->prof_events.data() + base;
     sim->prof_frames++;
   }
-  const int mark_level = sim->profiling;
+  const int mark_level = marks ? sim->profiling : 0;
   void* target = obs_dev;
   if (sim->resize_w) {   // render full size, packed u8 HWC, into the library's buffer; k_resize writes the caller's tensor
     rc.obs_layout = DTS_OBS_HWC; rc.obs_dtype = DTS_OBS_U8;
@@ -556,13 +564,53 @@ int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
   int k = launch_render(*sim->render, sim->S, sim->d_maps, rc, target, gt, sim->d_err, sim->d_status, marks, mark_level,
                         (cudaStream_t)stream);
   if (sim->resize_w) {
-    launch_selected_resize(sim, sim->resize_src, obs_dev, (cudaStream_t)stream);
+    launch_selected_resize(sim, sim->resize_src, obs_dev, (cudaStream_t)stream, env_list, env_count);
     k++;
   }
   if (marks && mark_level >= 2) cudaEventRecord(marks[kProfMarks - 1], (cudaStream_t)stream);   // closes the "post" interval
   sim->launches += k;
   DTS_CUDA(cudaGetLastError());
   return 0;
+}
+
+int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
+  if (!sim) return 1;
+  return render_pass(sim, obs_dev, stream, nullptr, nullptr);
+}
+
+int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, void* terminal_obs_dev, float* reward_dev,
+                      uint8_t* done_dev, void* stream) {
+  if (!sim) return 1;
+  if (!actions_dev) return sim->fail("actions_dev is NULL");
+  if (!(sim->cfg.flags & DTS_FLAG_AUTO_RESET)) return sim->fail("dts_step_terminal needs a handle created with DTS_FLAG_AUTO_RESET");
+  if (obs_dev && !terminal_obs_dev) return sim->fail("terminal_obs_dev is NULL");
+  if (obs_dev && terminal_obs_dev == obs_dev) return sim->fail("terminal_obs_dev must be a buffer of its own, not obs_dev");
+  if (sim->gather_next) return sim->fail("a fused gather is armed (dts_gather_next): dts_step_terminal does not write it");
+  if (check_maps(sim)) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  if (!sim->seeded) return sim->fail("auto-reset needs seeded streams: call dts_seed_streams first");
+  cudaStream_t st = (cudaStream_t)stream;
+  // 1. the step with the respawn held back: k_step_logic's only use of DTS_FLAG_AUTO_RESET is that respawn
+  StepCfg deferred = sim->step_cfg;
+  deferred.flags &= ~DTS_FLAG_AUTO_RESET;
+  launch_step_logic(sim->S, sim->d_maps, deferred, map_select(sim), actions_dev, reward_dev, done_dev, st);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  // 2. every env's frame of the state the step left: the terminal frame where the episode ended
+  if (obs_dev && render_pass(sim, obs_dev, stream, nullptr, nullptr)) return 1;
+  // 3. the ended envs respawn, in the same order of draws as inside k_step_logic, and are listed
+  DTS_CUDA(cudaMemsetAsync(sim->n_ended, 0, sizeof(int32_t), st));
+  launch_respawn_ended(sim->S, sim->d_maps, sim->step_cfg, map_select(sim), sim->ended, sim->n_ended, st);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  if (!obs_dev) return 0;
+  // 4. their terminal frames -> terminal_obs_dev; 5. their first frames -> obs_dev
+  const size_t px = sim->resize_w ? (size_t)sim->resize_w * sim->resize_h : (size_t)sim->cfg.cam_width * sim->cfg.cam_height;
+  const size_t row_bytes = px * 3 * (sim->fmt.obs_dtype == DTS_OBS_F32_UNIT ? 4 : 1);
+  launch_copy_rows(obs_dev, terminal_obs_dev, row_bytes, sim->ended, sim->n_ended, sim->cfg.num_envs, st);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  return render_pass(sim, obs_dev, stream, sim->ended, sim->n_ended);
 }
 
 int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* reward_dev, uint8_t* done_dev,

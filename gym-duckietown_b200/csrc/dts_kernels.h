@@ -24,6 +24,11 @@ struct RenderCfg {
   int32_t tessellate;         // 1: literal 98 triangles per road tile (spec tile mode 0)
   int32_t obs_layout, obs_dtype;   // DTS_OBS_* (dts_output_format)
   int32_t mode;               // DTS_RENDER_* (dts_set_render_mode)
+  // Optional device list of the envs to draw: env_list[0 .. *env_count).  NULL: all n_envs.  The host never reads the
+  // count: grids stay sized for n_envs and slots at or past the count exit.  Frame memory stays indexed by env id, so
+  // the envs left out keep what the previous pass put there.  (n_envs stays the SoA stride of the per-env state.)
+  const int32_t* env_list;
+  const int32_t* env_count;
 };
 
 void launch_step_logic(const DState& S, const DMap* maps, const StepCfg& c, int n_maps_cycle, const float* actions,
@@ -33,6 +38,10 @@ void launch_reset_random(const DState& S, const DMap* maps, const StepCfg& c, in
 void launch_reset_params(const DState& S, const DMap* maps, const StepCfg& c, const uint8_t* mask,
                          const ResetStaging& p, cudaStream_t st);
 void launch_assign_maps(const DState& S, const DMap* maps, const uint8_t* mask, const int32_t* map_id, cudaStream_t st);
+// The auto-reset k_step_logic does in place, deferred (dts_step_terminal): every env whose episode ended re-spawns, and
+// is appended to ended[0 .. *n_ended), which the caller zeroes first.  The list's order is not deterministic.
+void launch_respawn_ended(const DState& S, const DMap* maps, const StepCfg& c, int n_maps_cycle, int32_t* ended,
+                          int32_t* n_ended, cudaStream_t st);
 void launch_query(const DMap* maps, int map_id, int dyn_env, int n_envs, int n, const double* q, const uint32_t* hidden,
                   double* outd, int32_t* outi, cudaStream_t st);
 
@@ -68,9 +77,11 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
 std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, int32_t* counts, float* lattice_by_cell,
                              int n_cells);
 
-// ResizeWrapper on the device: src u8[N][H][W][3] -> dst [N] x (ow x oh) in `layout` / `dtype` (dts_set_resize)
+// ResizeWrapper on the device: src u8[N][H][W][3] -> dst [N] x (ow x oh) in `layout` / `dtype` (dts_set_resize).  The
+// resize passes take an optional device env list like RenderCfg's (NULL, NULL: every env).
 void launch_resize(const uint8_t* src, int W, int H, int ow, int oh, int n_envs, const int16_t* xtab, const int16_t* ytab,
-                   void* dst, int layout, int dtype, int band_rows, int band_cap, cudaStream_t st);
+                   void* dst, int layout, int dtype, int band_rows, int band_cap, const int32_t* env_list,
+                   const int32_t* env_count, cudaStream_t st);
 // Output rows per CTA of k_resize_band and the largest source-row span of a band, for the row tap table `ytab`
 // ([oh][8]); both 0: the untiled k_resize
 void plan_resize_bands(int W, int ow, int oh, const int16_t* ytab, int* band_rows, int* band_cap);
@@ -79,7 +90,11 @@ void plan_resize_bands(int W, int ow, int oh, const int16_t* ytab, int* band_row
 // on an axis, i.e. less than 1/32 of the camera size) is refused and leaves the previous tables.
 std::string renderer_set_pil_resize(Renderer& r, int ow, int oh);
 // src u8[N][H][W][3] -> dst [N] x (ow x oh) in `layout` / `dtype`, with the tables renderer_set_pil_resize built
-void launch_pil_resize(const Renderer& r, const uint8_t* src, void* dst, int layout, int dtype, cudaStream_t st);
+void launch_pil_resize(const Renderer& r, const uint8_t* src, void* dst, int layout, int dtype, const int32_t* env_list,
+                       const int32_t* env_count, cudaStream_t st);
+// dst row e = src row e (row_bytes each) for every env e of list[0 .. *count), count <= n_envs
+void launch_copy_rows(const void* src, void* dst, size_t row_bytes, const int32_t* list, const int32_t* count, int n_envs,
+                      cudaStream_t st);
 void launch_blend4(const uint8_t* const f[4], const double w[4], double* out, size_t n, cudaStream_t st);
 
 }  // namespace dts

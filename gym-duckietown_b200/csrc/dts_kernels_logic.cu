@@ -250,6 +250,24 @@ __global__ void __launch_bounds__(128) k_reset_random(DState S, const DMap* __re
   evaluate_pose(S, m, c, e, S.pos_x[e], S.pos_z[e], S.angle[e], 0, nullptr, nullptr);
 }
 
+// dts_step_terminal's auto-reset, run after the terminal frames are rendered: k_step_logic ran with
+// DTS_FLAG_AUTO_RESET cleared, so this is the same respawn() on the same state, and the env's PCG64 stream continues
+// where the step's dyn_rand draws left it.  The envs that respawn are appended to `ended` (warp-aggregated).
+__global__ void __launch_bounds__(128) k_respawn_ended(DState S, const DMap* __restrict__ maps, StepCfg c, int n_maps_cycle,
+                                                       int32_t* __restrict__ ended, int32_t* __restrict__ n_ended) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool end = e < S.n && S.done_code[e] != DTS_IN_PROGRESS;
+  const unsigned m = __ballot_sync(0xffffffffu, end);
+  if (!m) return;
+  const int lane = threadIdx.x & 31;
+  int base = 0;
+  if (lane == __ffs(m) - 1) base = atomicAdd(n_ended, __popc(m));
+  base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
+  if (!end) return;
+  ended[base + __popc(m & ((1u << lane) - 1u))] = e;
+  respawn(S, maps, c, n_maps_cycle, e);
+}
+
 // dts_reset with host-drawn parameters (already copied to device staging arrays in `p`)
 __global__ void __launch_bounds__(128) k_reset_params(DState S, const DMap* __restrict__ maps, StepCfg c,
                                                       const uint8_t* __restrict__ mask, ResetStaging p) {
@@ -336,6 +354,10 @@ void launch_step_logic(const DState& S, const DMap* maps, const StepCfg& c, int 
 void launch_reset_random(const DState& S, const DMap* maps, const StepCfg& c, int n_maps_cycle, const uint8_t* mask,
                          cudaStream_t st) {
   k_reset_random<<<(S.n + 127) / 128, 128, 0, st>>>(S, maps, c, n_maps_cycle, mask);
+}
+void launch_respawn_ended(const DState& S, const DMap* maps, const StepCfg& c, int n_maps_cycle, int32_t* ended,
+                          int32_t* n_ended, cudaStream_t st) {
+  k_respawn_ended<<<(S.n + 127) / 128, 128, 0, st>>>(S, maps, c, n_maps_cycle, ended, n_ended);
 }
 void launch_reset_params(const DState& S, const DMap* maps, const StepCfg& c, const uint8_t* mask,
                          const ResetStaging& p, cudaStream_t st) {

@@ -832,6 +832,10 @@ __device__ __forceinline__ void clear_colour(const DState& S, const RenderCfg& r
   clr[2] = seg ? 1.0f : S.rep[env].horizon[2];
 }
 
+// A pass over a device env list (RenderCfg::env_list): the number of slots drawn, and the env of slot s < that number
+__device__ __forceinline__ int n_listed(const int32_t* list, const int32_t* count, int n_envs) { return list ? __ldg(count) : n_envs; }
+__device__ __forceinline__ int listed_env(const int32_t* list, int slot) { return list ? __ldg(list + slot) : slot; }
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ frame memory
@@ -896,8 +900,9 @@ __host__ size_t carve(const Renderer& r, uintptr_t base, FrameMem& f) {
 
 // ------------------------------------------------------------------------------------------------ k_frame_setup
 __global__ void __launch_bounds__(128) k_frame_setup(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm) {
-  const int env = blockIdx.x * blockDim.x + threadIdx.x;
-  if (env >= rc.n_envs) return;
+  const int slot = blockIdx.x * blockDim.x + threadIdx.x;
+  if (slot >= n_listed(rc.env_list, rc.env_count, rc.n_envs)) return;
+  const int env = listed_env(rc.env_list, slot);
   FrameCtx& c = fm.ctx[env];
   const RenderEp ep = S.rep[env];
   double V[12];
@@ -985,9 +990,11 @@ __device__ __forceinline__ bool item_visible(const DState& S, const DMap& m, con
 // aggregated atomic append), so that k_geometry spends warps only on items that will emit something.
 __global__ void __launch_bounds__(256) k_cull(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, int items_max) {
   const size_t g = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  const int item = (int)(g / rc.n_envs), env = (int)(g - (size_t)item * rc.n_envs);
+  const int item = (int)(g / rc.n_envs), slot = (int)(g - (size_t)item * rc.n_envs);
   bool vis = false;
-  if (item < items_max) {
+  int env = 0;
+  if (item < items_max && slot < n_listed(rc.env_list, rc.env_count, rc.n_envs)) {
+    env = listed_env(rc.env_list, slot);
     ItemPose ip;
     vis = item_visible(S, maps[S.map_id[env]], rc, fm.ctx[env], env, item, ip);
   }
@@ -1190,13 +1197,16 @@ k_geometry(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem
 constexpr int kBinWarps = 4;
 constexpr int kCountMask = 0xfffff, kGroundInc = 1 << 20;   // a bin's counter: records | ground-quad records << 20
 constexpr int kFlatBin = -0x7fffffff - 1;   // bin_count of a flat bin (k_raster_flat); solo bins hold -(prim + 1) >= -65536
-template <bool kFish>   // true: bins are the LUT's source boxes of the output bins (fused fisheye gather)
+// kListed: the frame draws the envs of rc.env_list.  (Its own instance: an env id loaded from the list stays live across
+// the kernel, where blockIdx.x is re-read for free, and would cost the fisheye instance registers and spills.)
+template <bool kFish, bool kListed>   // kFish: bins are the LUT's source boxes of the output bins (fused fisheye gather)
 __global__ void __launch_bounds__(kBinWarps * 32)
 k_bin(RenderCfg rc, FrameMem fm, FishTab ft, int max_prims, int max_pairs, int32_t* __restrict__ err) {
   extern __shared__ int bin_smem[];
   __shared__ int s_total, s_base, s_ok;
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, tid = threadIdx.x;
-  const int env = blockIdx.x, nthr = blockDim.x;   // 1 warp per env for small cameras, 4 for large ones (launch_render)
+  if (kListed && (int)blockIdx.x >= __ldg(rc.env_count)) return;   // (the whole CTA)
+  const int env = kListed ? __ldg(rc.env_list + blockIdx.x) : (int)blockIdx.x, nthr = blockDim.x;   // 1 warp per env for small cameras, 4 for large ones (launch_render)
   const int W = rc.width, H = rc.height;
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW, cbins_y = (H + kCoarseH - 1) / kCoarseH, cbins = cbins_x * cbins_y;
   int* cnt = bin_smem;
@@ -1532,14 +1542,15 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
   __syncwarp();
   uint32_t parity = 0;   // bit s: the phase the next wait on slot s completes
   int cs = 0, ps = 0;    // consumer / producer slot
-  const int n_work = rc.n_envs * cbins_y;   // work item = one row of coarse bins of one env
+  const int n_work = n_listed(rc.env_list, rc.env_count, rc.n_envs) * cbins_y;   // work item = one row of coarse bins of one env
   int work = 0;
   if (lane == 0) work = atomicAdd(fm.work + kWorkRaster, 1);
   work = __shfl_sync(0xffffffffu, work, 0);
   while (work < n_work) {
     int next_work = 0;
     if (lane == 0) next_work = atomicAdd(fm.work + kWorkRaster, 1);   // consumed after this row: latency hidden
-    const int env = work / cbins_y, cby = work - env * cbins_y;
+    const int slot = work / cbins_y, cby = work - slot * cbins_y;
+    const int env = listed_env(rc.env_list, slot);
     const DMap& m = maps[S.map_id[env]];
     const uint8_t* tex_pool = m.tex_pool;
     const PrimRec* prims = fm.prims + (size_t)env * max_prims;
@@ -2082,11 +2093,11 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
 __global__ void __launch_bounds__(256) k_resize(const uint8_t* __restrict__ src, int W, int H, int ow, int oh, int n_envs,
                                                 const int16_t* __restrict__ xtab /*[ow][8]: 4 indices, 4 taps*/,
                                                 const int16_t* __restrict__ ytab /*[oh][8]*/, void* __restrict__ dst, int layout,
-                                                int dtype) {
-  const size_t total = (size_t)n_envs * ow * oh;
+                                                int dtype, const int32_t* __restrict__ env_list, const int32_t* __restrict__ env_count) {
+  const size_t total = (size_t)n_listed(env_list, env_count, n_envs) * ow * oh;
   for (size_t g = blockIdx.x * (size_t)blockDim.x + threadIdx.x; g < total; g += (size_t)gridDim.x * blockDim.x) {
     const int x = (int)(g % ow), y = (int)((g / ow) % oh);
-    const size_t env = g / ((size_t)ow * oh);
+    const size_t env = (size_t)listed_env(env_list, (int)(g / ((size_t)ow * oh)));
     const int4 xa = __ldg(reinterpret_cast<const int4*>(xtab + 8 * x)), ya = __ldg(reinterpret_cast<const int4*>(ytab + 8 * y));
     const int xi[4] = {(short)(xa.x & 0xffff), xa.x >> 16, (short)(xa.y & 0xffff), xa.y >> 16};
     const int xw[4] = {(short)(xa.z & 0xffff), xa.z >> 16, (short)(xa.w & 0xffff), xa.w >> 16};
@@ -2145,6 +2156,32 @@ void launch_blend4(const uint8_t* const f[4], const double w[4], double* out, si
   k_blend4<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, st>>>(f[0], f[1], f[2], f[3], w[0], w[1], w[2], w[3], scl, out, n);
 }
 
+// ------------------------------------------------------------------------------------------------ k_copy_rows
+// dts_step_terminal's terminal frames: the observation rows of the envs that ended -> the same rows of the terminal
+// buffer, a CTA per listed env (grid-strided over the list), 16-byte vectors when both rows and the row size allow them.
+__global__ void __launch_bounds__(256) k_copy_rows(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, size_t row_bytes,
+                                                   const int32_t* __restrict__ list, const int32_t* __restrict__ count) {
+  const int n = __ldg(count);
+  for (int s = blockIdx.x; s < n; s += gridDim.x) {
+    const size_t off = (size_t)__ldg(list + s) * row_bytes;
+    const uint8_t* a = src + off;
+    uint8_t* b = dst + off;
+    if (((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | row_bytes) & 15) == 0) {
+      for (size_t i = threadIdx.x; i < row_bytes / 16; i += blockDim.x)
+        reinterpret_cast<int4*>(b)[i] = __ldg(reinterpret_cast<const int4*>(a) + i);
+    } else {
+      for (size_t i = threadIdx.x; i < row_bytes; i += blockDim.x) b[i] = __ldg(a + i);
+    }
+  }
+}
+
+void launch_copy_rows(const void* src, void* dst, size_t row_bytes, const int32_t* list, const int32_t* count, int n_envs,
+                      cudaStream_t st) {
+  const size_t cap = device_sms() * 8, blocks = (size_t)n_envs < cap ? (size_t)n_envs : cap;
+  k_copy_rows<<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const uint8_t*>(src), reinterpret_cast<uint8_t*>(dst), row_bytes,
+                                                list, count);
+}
+
 // The same resize, tiled: a CTA per (band of `R` output rows, env).  The band's source rows (contiguous bytes of the
 // render) are copied to shared memory with 16-byte loads, the horizontal pass runs once per source row into an int32
 // buffer in shared memory, the vertical pass reads it and writes four output bytes per thread as one word — instead
@@ -2153,10 +2190,13 @@ void launch_blend4(const uint8_t* const f[4], const double w[4], double* out, si
 // (computed on the host from the same tap table).
 __global__ void __launch_bounds__(256) k_resize_band(const uint8_t* __restrict__ src, int W, int H, int ow, int oh,
                                                      const int16_t* __restrict__ xtab, const int16_t* __restrict__ ytab,
-                                                     void* __restrict__ dst, int layout, int dtype, int R, int cap) {
+                                                     void* __restrict__ dst, int layout, int dtype, int R, int cap,
+                                                     const int32_t* __restrict__ env_list, const int32_t* __restrict__ env_count) {
   extern __shared__ __align__(16) unsigned char rs_smem[];
   const int bands = (oh + R - 1) / R;
-  const int env = blockIdx.x / bands, r0 = (blockIdx.x - env * bands) * R, r1 = min(r0 + R, oh);
+  const int slot = blockIdx.x / bands, r0 = (blockIdx.x - slot * bands) * R, r1 = min(r0 + R, oh);
+  if (env_list && slot >= __ldg(env_count)) return;   // (the whole CTA)
+  const int env = listed_env(env_list, slot);
   const int s_lo = ytab[8 * r0], s_hi = ytab[8 * (r1 - 1) + 3], nrows = min(s_hi - s_lo + 1, cap);
   const int rowb = W * 3, ow3 = ow * 3;
   int4* xt = reinterpret_cast<int4*>(rs_smem);                                      // [ow] tap table
@@ -2261,19 +2301,20 @@ void plan_resize_bands(int W, int ow, int oh, const int16_t* ytab, int* band_row
 }
 
 void launch_resize(const uint8_t* src, int W, int H, int ow, int oh, int n_envs, const int16_t* xtab, const int16_t* ytab,
-                   void* dst, int layout, int dtype, int band_rows, int band_cap, cudaStream_t st) {
+                   void* dst, int layout, int dtype, int band_rows, int band_cap, const int32_t* env_list,
+                   const int32_t* env_count, cudaStream_t st) {
   if (band_rows > 0) {   // tiled form (plan_resize_bands found a band height whose rows fit in shared memory)
     const size_t smem = resize_band_smem(W, ow, band_cap);
     static size_t opted = 0;
     if (smem > 48 * 1024 && smem > opted) { cudaFuncSetAttribute(k_resize_band, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); opted = smem; }
     k_resize_band<<<(unsigned)(((oh + band_rows - 1) / band_rows) * (size_t)n_envs), 256, smem, st>>>(src, W, H, ow, oh, xtab, ytab, dst, layout, dtype,
-                                                                                      band_rows, band_cap);
+                                                                                      band_rows, band_cap, env_list, env_count);
     return;
   }
   const size_t total = (size_t)n_envs * ow * oh;
   const size_t cap = device_sms() * 16;
   const int blocks = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
-  k_resize<<<blocks, 256, 0, st>>>(src, W, H, ow, oh, n_envs, xtab, ytab, dst, layout, dtype);
+  k_resize<<<blocks, 256, 0, st>>>(src, W, H, ow, oh, n_envs, xtab, ytab, dst, layout, dtype, env_list, env_count);
 }
 
 // ------------------------------------------------------------------------------------------------ k_resize_pil
@@ -2295,11 +2336,14 @@ constexpr int kPilMaxTaps = 65;                 // Pillow's ksize at a 32x reduc
 __device__ __forceinline__ unsigned pil_clip8(int acc) { return (unsigned)min(max(acc >> 22, 0), 255); }
 
 __global__ void __launch_bounds__(256) k_resize_pil(const uint8_t* __restrict__ src, const PilTab t, void* __restrict__ dst,
-                                                    int layout, int dtype) {
+                                                    int layout, int dtype, const int32_t* __restrict__ env_list,
+                                                    const int32_t* __restrict__ env_count) {
   extern __shared__ __align__(16) unsigned char pil_smem[];
   const int W = t.W, H = t.H, ow = t.ow, oh = t.oh, ow3 = ow * 3, pitch = t.pitch, ow3p = t.ow3p;
   const int bands = (oh + t.band - 1) / t.band;
-  const int env = blockIdx.x / bands, r0 = (blockIdx.x - env * bands) * t.band, r1 = min(r0 + t.band, oh);
+  const int slot = blockIdx.x / bands, r0 = (blockIdx.x - slot * bands) * t.band, r1 = min(r0 + t.band, oh);
+  if (env_list && slot >= __ldg(env_count)) return;   // (the whole CTA)
+  const int env = listed_env(env_list, slot);
   const int32_t* __restrict__ xs = t.tab;
   const int32_t* __restrict__ xw = xs + ow;
   const int32_t* __restrict__ ys = xw + (size_t)ow * t.tx;
@@ -2497,10 +2541,11 @@ std::string renderer_set_pil_resize(Renderer& r, int ow, int oh) {
   return "";
 }
 
-void launch_pil_resize(const Renderer& r, const uint8_t* src, void* dst, int layout, int dtype, cudaStream_t st) {
+void launch_pil_resize(const Renderer& r, const uint8_t* src, void* dst, int layout, int dtype, const int32_t* env_list,
+                       const int32_t* env_count, cudaStream_t st) {
   const PilTab& t = r.pil;
   const unsigned grid = (unsigned)(((t.oh + t.band - 1) / t.band) * (size_t)r.n);
-  k_resize_pil<<<grid, 256, t.smem, st>>>(src, t, dst, layout, dtype);
+  k_resize_pil<<<grid, 256, t.smem, st>>>(src, t, dst, layout, dtype, env_list, env_count);
 }
 
 // ------------------------------------------------------------------------------------------------ the renderer
@@ -2725,7 +2770,7 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   const int bin_grid = rc.n_envs;   // CTA per env: one warp where a frame has few bins and prims (160x120: 75 bins — more warps
   // only add barriers and CTA launches), four for large cameras (640x480)
   const int bin_threads = r.cbins > 128 ? kBinWarps * 32 : 32;
-  const auto bin = fisheye ? k_bin<true> : k_bin<false>;
+  const auto bin = rc.env_list ? (fisheye ? k_bin<true, true> : k_bin<false, true>) : (fisheye ? k_bin<true, false> : k_bin<false, false>);
   if (bin_smem_bytes > 48 * 1024)   // cameras beyond ~640x480 (cbins > 1536): opt in to large dynamic shared memory
     cudaFuncSetAttribute(bin, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bin_smem_bytes);
   bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, ft, r.max_prims, r.pool, err_flag);

@@ -170,6 +170,7 @@ def load() -> C.CDLL:
     lib.dts_reset_random.argtypes = [vp, vp, vp]
     lib.dts_seed_streams.argtypes = [vp, vp, vp]
     lib.dts_step.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.dts_step_terminal.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.dts_render.argtypes = [vp, vp, vp]
     lib.dts_get_state.argtypes = [vp, C.POINTER(StateView)]
     lib.dts_query_poses.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp]
@@ -206,7 +207,7 @@ def load() -> C.CDLL:
 
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
-           "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
+           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame", "dts_last_error", "dts_destroy"]
 
 
@@ -396,6 +397,12 @@ class Sim:
 
     def step(self, actions_ptr: int, obs_ptr: Optional[int], reward_ptr: int, done_ptr: int, stream: int = 0):
         self._check(self.lib.dts_step(self.h, actions_ptr, obs_ptr, reward_ptr, done_ptr, stream), "dts_step")
+
+    def step_terminal(self, actions_ptr: int, obs_ptr: Optional[int], terminal_obs_ptr: Optional[int], reward_ptr: int,
+                      done_ptr: int, stream: int = 0):
+        """dts_step that also writes the terminal frame of every env that ended into its row of terminal_obs."""
+        self._check(self.lib.dts_step_terminal(self.h, actions_ptr, obs_ptr, terminal_obs_ptr, reward_ptr, done_ptr, stream),
+                    "dts_step_terminal")
 
     def render(self, obs_ptr: int, stream: int = 0):
         self._check(self.lib.dts_render(self.h, obs_ptr, stream), "dts_render")

@@ -29,7 +29,7 @@ enum { DTS_IN_PROGRESS = 0, DTS_INVALID_POSE = 1, DTS_MAX_STEPS = 2 };
 enum { DTS_ACTION_PWM = 0,      /* Simulator.step(action=[u_left,u_right])        simulator.py:1669 */
        DTS_ACTION_VEL_STEER = 1 /* DuckietownEnv.step(action=[vel, steering])  envs/duckietown_env.py:36-59 */ };
 /* flags */
-enum { DTS_FLAG_AUTO_RESET = 1,   /* done envs are re-spawned on device inside dts_step */
+enum { DTS_FLAG_AUTO_RESET = 1,   /* done envs are re-spawned on device inside dts_step / dts_step_terminal */
        DTS_FLAG_DOMAIN_RAND = 2,  /* simulator.py:213  (camera noise S:1768, DR sampling in device resets) */
        DTS_FLAG_DISTORTION = 4,   /* simulator.py:223  fisheye gather fused into the render (distortion.py:118) */
        DTS_FLAG_DYNAMICS_RAND = 8,/* simulator.py:224  per-env trim on the motor gains (S:746-748) */
@@ -264,6 +264,19 @@ int dts_reset_random(dts_sim* sim, const uint8_t* mask_dev, void* stream);
  * (NULL = skip rendering), reward f32[N], done u8[N]. All DEVICE pointers. */
 int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* reward_dev, uint8_t* done_dev,
              void* stream);
+/* dts_step that also returns the TERMINAL frames, on a DTS_FLAG_AUTO_RESET handle: for every env whose episode ended
+ * (done = 1), terminal_obs_dev's row gets what the reference's step() returns there (render_obs() S:1677, before the
+ * caller's reset()), and obs_dev's row the first frame of the next episode, as from dts_step.  Rows of envs that did
+ * not end keep what terminal_obs_dev held.  terminal_obs_dev has obs_dev's size (layout, dtype, resize) and must not
+ * be obs_dev.  Stream order: k_step_logic without the respawn, the render of all envs into obs_dev, k_respawn_ended
+ * (the respawn, state and draws bit for bit those of dts_step, and a device list of the ended envs), k_copy_rows (their
+ * rows -> terminal_obs_dev) and a second render into obs_dev over the listed envs only, whose kernels exit at once when
+ * nothing ended.  Launches: 2 R + 3, R being dts_render's (5, or 7 when the rasteriser writes packed u8 HWC of a width divisible by 4, +1
+ * with a resize), plus a 4-byte memset; obs_dev = NULL (no render): 2.  Fails without DTS_FLAG_AUTO_RESET, with
+ * terminal_obs_dev == obs_dev, and while a fused gather is armed (dts_gather_next), which it does not write.  The
+ * second pass is not timed by dts_profile_*.  Never synchronises. */
+int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, void* terminal_obs_dev, float* reward_dev,
+                      uint8_t* done_dev, void* stream);
 /* Simulator.render_obs() (simulator.py:1953-1972) of the current state. */
 int dts_render(dts_sim* sim, void* obs_dev, void* stream);
 /* Render variants of _render_img (S:1707-1951) for subsequent dts_render / dts_step calls (0 = the agent camera):
