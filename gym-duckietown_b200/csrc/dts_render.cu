@@ -5,11 +5,13 @@
 // the lean rasterisers of coarse bins lying inside one prim / holding only road tiles and ground, are described at their
 // definitions):
 //   k_frame_setup  thread per env: camera matrices (f64), gluPerspective, counters -> FrameCtx[env]
-//   k_geometry     warp per (env, draw item) over the whole GPU: ground / map tile / placed mesh.  Model-view
-//                  f64->f32, fixed-function per-vertex lighting, frustum cull, near + guard-band clip, snap to
-//                  1/64 px, triangle setup -> 128-byte PrimRec appended to the env's slab.  A road tile is ONE quad:
-//                  its 8x8 lit lattice goes to the env's table and the Gouraud interpolant is evaluated per pixel
-//                  (render spec tile mode 1); RenderCfg.tessellate switches to the literal 98 triangles (mode 0).
+//   k_tiles        warp per env, lane per road tile (tile mode 1): the ground and the map's tiles.  A road tile is ONE
+//                  quad: its 8x8 lit lattice goes to the env's table and the Gouraud interpolant is evaluated per
+//                  pixel (render spec tile mode 1); RenderCfg.tessellate switches to the literal 98 triangles (mode 0),
+//                  which k_geometry draws like meshes.
+//   k_geometry     warp per (env, draw item) over the whole GPU: placed meshes (and in tile mode 0 the ground and the
+//                  tiles).  Model-view f64->f32, fixed-function per-vertex lighting, frustum cull, near + guard-band
+//                  clip, snap to 1/64 px, triangle setup -> 128-byte PrimRec appended to the env's slab.
 //   k_bin          warp per env: exact (prim, 32x8-px coarse bin) pairs — count, warp scan, scatter — then, dense
 //                  over the pairs (one pair per lane), the 80-byte BinRec each pair needs for visibility: edge
 //                  functions re-based to the bin corner (exact in 64 bits, then int32), per-fine-bin reject /
@@ -86,6 +88,9 @@ constexpr int kSoloMinCtas = 3;     // k_raster_solo
 constexpr int kFlatMinCtas = 4;     // k_raster_flat
 constexpr int kGeoWarps = 1;        // k_geometry: warps per CTA ...
 constexpr int kGeoMinCtas = 32;     // ... and CTAs per SM
+constexpr int kTileWarps = 4;       // k_tiles: warps (envs) per CTA ...
+constexpr int kTileMinCtas = 4;     // ... and CTAs per SM (35 KB of shared memory each; 119 registers, no spills: at 6
+                                    // or 5 CTAs, 80 or 96 registers, the lane phase spills)
 constexpr int kWarps = kThreads / 32;
 constexpr int kBinW = 8, kBinH = 4;   // fine bin = one warp's pixel block (one pixel per lane)
 constexpr int kCFX = 4, kCFY = 2;     // coarse bin = 4 x 2 fine bins = 32 x 8 px: unit of binning and staging
@@ -158,22 +163,24 @@ struct __align__(16) GeoWarp {    // per warp of k_geometry, shared memory
 };
 using Shared = GeoWarp;           // shade_vertex reads ep and P from it
 
-// MV = V * T(t) * S(sc) * Ry(c,s), N = rot(V) * Ry / sc — float64 then rounded (spec).  Lanes 0..11 each produce
-// one entry of the 3x4 matrix (and of N for the rotation part) into the warp's shared Xform.
+// MV = V * T(t) * S(sc) * Ry(c,s), N = rot(V) * Ry / sc — float64 then rounded (spec).  Entry (r, k) of the 3x4
+// matrix, and of N for the rotation part (k < 3).
+__device__ __forceinline__ void model_view_entry(const double* V, double tx, double ty, double tz, double sc, double c,
+                                                 double s, int r, int k, Xform& x) {
+  if (k < 3) {
+    const double R0 = k == 0 ? c : (k == 1 ? 0.0 : s), R1 = k == 1 ? 1.0 : 0.0, R2 = k == 0 ? -s : (k == 1 ? 0.0 : c);
+    const double a = V[4 * r + 0] * R0 + V[4 * r + 1] * R1 + V[4 * r + 2] * R2;
+    x.MV[4 * r + k] = (float)(a * sc);
+    x.N[3 * r + k] = (float)(sc == 1.0 ? a : a / sc);   // x / 1.0 == x exactly
+  } else {
+    x.MV[4 * r + 3] = (float)(V[4 * r + 0] * tx + V[4 * r + 1] * ty + V[4 * r + 2] * tz + V[4 * r + 3]);
+  }
+}
+// Warp form: lanes 0..11 each produce one entry into the warp's shared Xform.
 __device__ __forceinline__ void model_view(const double* V, double tx, double ty, double tz, double sc, double c,
                                            double s, Xform& x, int lane) {
   __syncwarp();
-  if (lane < 12) {
-    const int r = lane >> 2, k = lane & 3;
-    if (k < 3) {
-      const double R0 = k == 0 ? c : (k == 1 ? 0.0 : s), R1 = k == 1 ? 1.0 : 0.0, R2 = k == 0 ? -s : (k == 1 ? 0.0 : c);
-      const double a = V[4 * r + 0] * R0 + V[4 * r + 1] * R1 + V[4 * r + 2] * R2;
-      x.MV[4 * r + k] = (float)(a * sc);
-      x.N[3 * r + k] = (float)(sc == 1.0 ? a : a / sc);   // x / 1.0 == x exactly
-    } else {
-      x.MV[4 * r + 3] = (float)(V[4 * r + 0] * tx + V[4 * r + 1] * ty + V[4 * r + 2] * tz + V[4 * r + 3]);
-    }
-  }
+  if (lane < 12) model_view_entry(V, tx, ty, tz, sc, c, s, lane >> 2, lane & 3, x);
   __syncwarp();
 }
 
@@ -227,6 +234,20 @@ __device__ __forceinline__ Vtx shade_vertex(const Xform& x, const Shared& sh, fl
   o.cz = sh.P22 * e[2] + sh.P23;
   o.cw = -e[2];
   return o;
+}
+
+// Road tile S:1852-1884: its lattice vertex (a, b) of the 8x8 grid (a: u index along x, b: v index along z), lit white
+__device__ __forceinline__ Vtx tile_vertex(const Xform& x, const Shared& sh, double ts, int a, int b) {
+  const float lx = (float)(-ts / 2 + ((double)a / 7.0) * ts), lz = (float)(-ts / 2 + ((double)b / 7.0) * ts);
+  return shade_vertex(x, sh, lx, 0.0f, lz, 0.f, 1.f, 0.f, 1.f, 1.f, 1.f, (float)((double)a / 7.0), (float)(1.0 - (double)b / 7.0));
+}
+// ... and its placement: glTranslatef((i + 0.5) * TS, 0, (j + 0.5) * TS) S:1870 (GLfloat arguments), glRotatef(angle*90+180) S:1873
+struct TilePose { double tx, tz, cs, sn; };
+__device__ __forceinline__ TilePose tile_pose(const DMap& m, int ti, int tj) {
+  const int quarter = (m.tile_angle[tj * m.grid_w + ti] + 2) & 3;
+  const double ts = m.tile_size;
+  return TilePose{(double)(float)((ti + 0.5) * ts), (double)(float)((tj + 0.5) * ts),
+                  quarter == 0 ? 1.0 : (quarter == 2 ? -1.0 : 0.0), quarter == 1 ? 1.0 : (quarter == 3 ? -1.0 : 0.0)};
 }
 
 __device__ __forceinline__ float plane_dist(const Vtx& a, int pl) {
@@ -368,7 +389,12 @@ __device__ __noinline__ bool setup_and_emit(const EmitCtx& ec, const Vtx& a, con
     r.ltq |= 1 << 24;
     r.X1 = qx[1]; r.Y1 = qy[1]; r.X2 = qx[2]; r.Y2 = qy[2]; r.X3 = qx[3]; r.Y3 = qy[3];
   }
-  const int slot = atomicAdd(&ec.ctx->n_prims, 1);
+  // the slab slot: one atomic for all the lanes emitting together (a warp draws one env at a time, so they share ctx)
+  const unsigned act = __activemask();
+  const int lane = threadIdx.x & 31, leader = __ffs(act) - 1;
+  int slot = 0;
+  if (lane == leader) slot = atomicAdd(&ec.ctx->n_prims, __popc(act));
+  slot = __shfl_sync(act, slot, leader) + __popc(act & ((1u << lane) - 1u));
   if (slot >= ec.max_prims) { ec.ctx->overflow = 1; return true; }
   const int4* src = reinterpret_cast<const int4*>(&r);
   int4* dst = reinterpret_cast<int4*>(ec.prims + slot);
@@ -987,20 +1013,24 @@ __device__ __forceinline__ bool item_visible(const DState& S, const DMap& m, con
 
 // ------------------------------------------------------------------------------------------------ k_cull
 // thread per (env, draw item), item-major: the pairs that survive item_visible() go to a compact work list (warp-
-// aggregated atomic append), so that k_geometry spends warps only on items that will emit something.
-__global__ void __launch_bounds__(256) k_cull(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, int items_max) {
+// aggregated atomic append), so that k_geometry spends warps only on items that will emit something.  In tile mode 1
+// the ground and the road tiles are k_tiles' work, so only the placed meshes and the agent's own are listed.
+__global__ void __launch_bounds__(256) k_cull(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, int items_max,
+                                              int32_t* __restrict__ err) {
   const size_t g = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   const int item = (int)(g / rc.n_envs), slot = (int)(g - (size_t)item * rc.n_envs);
   bool vis = false;
   int env = 0;
   if (item < items_max && slot < n_listed(rc.env_list, rc.env_count, rc.n_envs)) {
     env = listed_env(rc.env_list, slot);
+    const DMap& m = maps[S.map_id[env]];
     ItemPose ip;
-    vis = item_visible(S, maps[S.map_id[env]], rc, fm.ctx[env], env, item, ip);
+    vis = (rc.tessellate || item > m.grid_w * m.grid_h) && item_visible(S, m, rc, fm.ctx[env], env, item, ip);
   }
   const unsigned m = __ballot_sync(0xffffffffu, vis);
   if (!m) return;
   const int lane = threadIdx.x & 31;
+  DTS_COUNT(28, __popc(m));
   int base = 0;
   if (lane == __ffs(m) - 1) base = atomicAdd(fm.work + kWorkGeoList, __popc(m));
   base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
@@ -1008,12 +1038,37 @@ __global__ void __launch_bounds__(256) k_cull(const DState S, const DMap* __rest
 }
 
 // ------------------------------------------------------------------------------------------------ k_geometry
+// The per-env state a geometry warp reads from shared memory: light and material (RenderEp), camera, projection, the
+// unlit flag.  `sh` must be free: the caller has synchronised the warp since its last use.
+__device__ __forceinline__ void load_geo_warp(GeoWarp& sh, const DState& S, const FrameCtx& ctx, int env, bool seg, int lane) {
+  for (int k = lane; k < (int)(sizeof(RenderEp) / 4); k += 32)
+    reinterpret_cast<uint32_t*>(&sh.ep)[k] = reinterpret_cast<const uint32_t*>(&S.rep[env])[k];
+  if (lane < 12) sh.V[lane] = ctx.V[lane];
+  if (lane == 12) { sh.P00 = ctx.P00; sh.P11 = ctx.P11; sh.P22 = ctx.P22; sh.P23 = ctx.P23; sh.unlit = seg ? 1 : 0; }
+  __syncwarp();
+}
+
+// ground quad S:1805-1812 (draw ids 0, 1): glScalef(50,0.01,50) applied to (+-1,-0.8,+-1), world-space +y normal
+__device__ __forceinline__ void draw_ground(const EmitCtx& ec, GeoWarp& sh, bool seg, int lane) {
+  model_view(sh.V, 0.0, 0.0, 0.0, 1.0, 1.0, 0.0, sh.x, lane);
+  const float gy = (float)(-0.8 * 0.01);
+  const float P[4][3] = {{-50.f, gy, 50.f}, {-50.f, gy, -50.f}, {50.f, gy, -50.f}, {50.f, gy, 50.f}};
+  const float magenta[3] = {255.f, 0.f, 255.f};   // glColor3f(255, 0, 255) S:1808: clamped to (1, 0, 1) as a vertex colour
+  const float* g = seg ? magenta : sh.ep.ground;
+  const int pl_ = lane & 3;   // lanes 0..3 light the four corners, the two triangles (0,1,2)(0,2,3) are then warp-uniform
+  const Vtx mine = shade_vertex(sh.x, sh, P[pl_][0], P[pl_][1], P[pl_][2], 0.f, 1.f, 0.f, g[0], g[1], g[2], 0.f, 0.f);
+  if (lane < 4) sh.corners[lane] = mine;
+  __syncwarp();
+  process_triangle_uniform(ec, sh.corners[0], sh.corners[1], sh.corners[2], 0, -1, -1, lane);
+  process_triangle_uniform(ec, sh.corners[0], sh.corners[2], sh.corners[3], 1, -1, -1, lane);
+}
+
 // One warp per CTA, 64 registers, 32 CTAs per SM: the kernel is latency-bound (short dependent chains), so resident warps
-// matter more than spills.  Each warp draws the (env, item) pairs of k_cull's work list, grid-strided.
+// matter more than spills.  Each warp draws the (env, item) pairs of k_cull's work list, grid-strided: in tile mode 1 the
+// placed meshes only (k_tiles draws the ground and the road tiles), in tile mode 0 every item.
 template <bool kTess>   // true: spec tile mode 0 (DTS_FLAG_TESSELLATE), the literal 98 triangles per road tile
 __device__ __forceinline__ void geometry_item(const DState& S, const DMap* __restrict__ maps, const RenderCfg& rc, const FrameMem& fm,
-                                              int max_prims, int max_lat, int32_t* __restrict__ err, int env, int item, int lane,
-                                              GeoWarp& sh) {
+                                              int max_prims, int32_t* __restrict__ err, int env, int item, int lane, GeoWarp& sh) {
   const DMap& m = maps[S.map_id[env]];
   const int n_tiles = m.grid_w * m.grid_h;
   const bool seg = (rc.mode & DTS_RENDER_SEGMENT) != 0;
@@ -1025,118 +1080,53 @@ __device__ __forceinline__ void geometry_item(const DState& S, const DMap* __res
   const int dyn_kind = ip.dyn_kind;
   const float opx = ip.opx, opz = ip.opz, orot = ip.orot;
   __syncwarp();   // the previous item of this warp is done with the shared GeoWarp
-  for (int k = lane; k < (int)(sizeof(RenderEp) / 4); k += 32)
-    reinterpret_cast<uint32_t*>(&sh.ep)[k] = reinterpret_cast<const uint32_t*>(&S.rep[env])[k];
-  if (lane < 12) sh.V[lane] = ctx.V[lane];
-  if (lane == 12) { sh.P00 = ctx.P00; sh.P11 = ctx.P11; sh.P22 = ctx.P22; sh.P23 = ctx.P23; sh.unlit = seg ? 1 : 0; }
-  __syncwarp();
+  load_geo_warp(sh, S, ctx, env, seg, lane);
   EmitCtx ec{m.textures, &sh, &ctx, fm.prims + (size_t)env * max_prims, max_prims, W, H};
-  float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
   const int tris_per_tile = tile_draw_ids(kTess);
   Xform& x = sh.x;
-  if (item == 0) {
-    // ground quad S:1805-1812: glScalef(50,0.01,50) applied to (+-1,-0.8,+-1), world-space +y normal
-    model_view(sh.V, 0.0, 0.0, 0.0, 1.0, 1.0, 0.0, x, lane);
-    const float gy = (float)(-0.8 * 0.01);
-    const float P[4][3] = {{-50.f, gy, 50.f}, {-50.f, gy, -50.f}, {50.f, gy, -50.f}, {50.f, gy, 50.f}};
-    const float magenta[3] = {255.f, 0.f, 255.f};   // glColor3f(255, 0, 255) S:1808: clamped to (1, 0, 1) as a vertex colour
-    const float* g = seg ? magenta : sh.ep.ground;
-    const int pl_ = lane & 3;   // lanes 0..3 light the four corners, the two triangles (0,1,2)(0,2,3) are then warp-uniform
-    const Vtx mine = shade_vertex(x, sh, P[pl_][0], P[pl_][1], P[pl_][2], 0.f, 1.f, 0.f, g[0], g[1], g[2], 0.f, 0.f);
-    if (lane < 4) sh.corners[lane] = mine;
-    __syncwarp();
-    process_triangle_uniform(ec, sh.corners[0], sh.corners[1], sh.corners[2], 0, -1, -1, lane);
-    process_triangle_uniform(ec, sh.corners[0], sh.corners[2], sh.corners[3], 1, -1, -1, lane);
-  } else if (item <= n_tiles) {
-    // road tile S:1852-1884: draw order i outer, j inner
-    const int t = item - 1, ti = t / m.grid_h, tj = t - ti * m.grid_h;
-    const int idx = tj * m.grid_w + ti;
-    const int quarter = (m.tile_angle[idx] + 2) & 3;                     // glRotatef(angle*90+180) S:1873
-    const double cs = quarter == 0 ? 1.0 : (quarter == 2 ? -1.0 : 0.0), sn = quarter == 1 ? 1.0 : (quarter == 3 ? -1.0 : 0.0);
-    const double ts = m.tile_size;
-    // glTranslatef((i + 0.5) * TS, 0, (j + 0.5) * TS) S:1870 takes GLfloat arguments
-    model_view(sh.V, (double)(float)((ti + 0.5) * ts), 0.0, (double)(float)((tj + 0.5) * ts), 1.0, cs, sn, x, lane);
-    int tex = m.tile_tex[idx];
-    if (seg && tex >= 0) tex = m.tex_segment[tex];   // Texture.bind(segment=True) G:52-56
-    const int base_id = 2 + tris_per_tile * t;
-    if (!kTess) {
-      // analytic tile: the prim is the quad of the 4 corners — cull on those before lighting the lattice
-      const int ca = (lane == 1 || lane == 2) ? 7 : 0, cb = (lane >= 2) ? 7 : 0;   // lanes 0..3: (0,0) (7,0) (7,7) (0,7)
-      const float lx = (float)(-ts / 2 + ((double)ca / 7.0) * ts), lz = (float)(-ts / 2 + ((double)cb / 7.0) * ts);
-      const Vtx v = shade_vertex(x, sh, lx, 0.0f, lz, 0.f, 1.f, 0.f, 1.f, 1.f, 1.f, (float)((double)ca / 7.0),
-                                 (float)(1.0 - (double)cb / 7.0));
-      const unsigned four = 0xFu;
-      bool culled4 = false;
-      culled4 |= (__ballot_sync(0xffffffffu, !(v.cz + v.cw >= 0.0f)) & four) == four;
-      culled4 |= (__ballot_sync(0xffffffffu, !(v.cw - v.cz >= 0.0f)) & four) == four;
-      culled4 |= (__ballot_sync(0xffffffffu, v.cx < -v.cw) & four) == four;
-      culled4 |= (__ballot_sync(0xffffffffu, v.cx > v.cw) & four) == four;
-      culled4 |= (__ballot_sync(0xffffffffu, v.cy < -v.cw) & four) == four;
-      culled4 |= (__ballot_sync(0xffffffffu, v.cy > v.cw) & four) == four;
-      if (culled4) return;
-    }
-    // the tile's 8x8 lattice, two vertices per lane (tessellated mode: also frustum-culls the whole tile)
-    Vtx lv[2];
-    int outside[6] = {0, 0, 0, 0, 0, 0};
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-      const int vi = lane + 32 * h, a = vi >> 3, b = vi & 7;             // a: u index (x), b: v index (z)
-      const float lx = (float)(-ts / 2 + ((double)a / 7.0) * ts), lz = (float)(-ts / 2 + ((double)b / 7.0) * ts);
-      lv[h] = shade_vertex(x, sh, lx, 0.0f, lz, 0.f, 1.f, 0.f, 1.f, 1.f, 1.f, (float)((double)a / 7.0),
-                           (float)(1.0 - (double)b / 7.0));
-      const Vtx& v = lv[h];
-      outside[0] += !(v.cz + v.cw >= 0.0f); outside[1] += !(v.cw - v.cz >= 0.0f);
-      outside[2] += v.cx < -v.cw; outside[3] += v.cx > v.cw; outside[4] += v.cy < -v.cw; outside[5] += v.cy > v.cw;
-    }
-    if (kTess) {
-      bool culled = false;
-#pragma unroll
-      for (int p = 0; p < 6; p++) culled |= __all_sync(0xffffffffu, outside[p] == 2);
-      if (culled) return;
-    }
-    if (!kTess) {
-      // analytic tile (spec tile mode 1): lattice colours -> table, one quad (0,1,2)(0,2,3) of the corners
-      int slot = 0;
-      if (lane == 0) slot = atomicAdd(&ctx.n_lat, 1);
-      slot = __shfl_sync(0xffffffffu, slot, 0);
-      if (slot >= max_lat) { if (lane == 0) ctx.overflow = 1; return; }
-#pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int vi = lane + 32 * h;
-        lat_tab[slot * 64 + vi] = make_float4(lv[h].r, lv[h].g, lv[h].b, 0.0f);
-        int corner = -1;
-        if (vi == 0) corner = 0; else if (vi == 56) corner = 1; else if (vi == 63) corner = 2; else if (vi == 7) corner = 3;
-        if (corner >= 0) { Vtx c = lv[h]; c.r = 0.f; c.g = 0.f; c.b = 0.f; sh.corners[corner] = c; }
-      }
-      __syncwarp();
-      // a tile that needs no clipping is ONE quad prim (its diagonal then splits no bin); otherwise two triangles
-      bool as_quad = false;
-      if (classify(sh.corners[0], sh.corners[1], sh.corners[2]) == 0 && classify(sh.corners[0], sh.corners[2], sh.corners[3]) == 0) {
-        if (lane == 0) as_quad = setup_and_emit(ec, sh.corners[0], sh.corners[1], sh.corners[2], base_id, tex, slot, &sh.corners[3]);
-        as_quad = __shfl_sync(0xffffffffu, (int)as_quad, 0) != 0;
-      }
-      if (!as_quad) {
-        process_triangle_uniform(ec, sh.corners[0], sh.corners[1], sh.corners[2], base_id, tex, slot, lane);
-        process_triangle_uniform(ec, sh.corners[0], sh.corners[2], sh.corners[3], base_id + 1, tex, slot, lane);
-      }
+  if (item <= n_tiles) {
+    if constexpr (kTess) {
+      if (item == 0) {
+        draw_ground(ec, sh, seg, lane);
       } else {
-      // literal vertex list S:407-433 (spec tile mode 0): 7x7 quads, (0,1,2)(0,2,3) split, 3 shades / triangle
-      for (int k0 = 0; k0 < kTessTris; k0 += 32) {
-        const int k = k0 + lane;
-        Vtx v[3];
-        if (k < kTessTris) {
-          const int quad = k >> 1, half = k & 1, a = quad / 7, b = quad - 7 * a;
+        // road tile S:1852-1884: draw order i outer, j inner
+        const int t = item - 1, ti = t / m.grid_h, tj = t - ti * m.grid_h;
+        const int idx = tj * m.grid_w + ti;
+        const TilePose tp = tile_pose(m, ti, tj);
+        const double ts = m.tile_size;
+        model_view(sh.V, tp.tx, 0.0, tp.tz, 1.0, tp.cs, tp.sn, x, lane);
+        int tex = m.tile_tex[idx];
+        if (seg && tex >= 0) tex = m.tex_segment[tex];   // Texture.bind(segment=True) G:52-56
+        const int base_id = 2 + tris_per_tile * t;
+        // frustum-cull the whole tile on its 8x8 lattice, two vertices per lane
+        int outside[6] = {0, 0, 0, 0, 0, 0};
 #pragma unroll
-          for (int j = 0; j < 3; j++) {
-            const int aa = j == 0 ? a : (j == 1 ? a + 1 : (half == 0 ? a + 1 : a));
-            const int bb = j == 0 ? b : (j == 1 ? (half == 0 ? b : b + 1) : b + 1);
-            const float lx = (float)(-ts / 2 + ((double)aa / 7.0) * ts), lz = (float)(-ts / 2 + ((double)bb / 7.0) * ts);
-            v[j] = shade_vertex(x, sh, lx, 0.0f, lz, 0.f, 1.f, 0.f, 1.f, 1.f, 1.f, (float)((double)aa / 7.0),
-                                (float)(1.0 - (double)bb / 7.0));
-          }
+        for (int h = 0; h < 2; h++) {
+          const int vi = lane + 32 * h;
+          const Vtx v = tile_vertex(x, sh, ts, vi >> 3, vi & 7);
+          outside[0] += !(v.cz + v.cw >= 0.0f); outside[1] += !(v.cw - v.cz >= 0.0f);
+          outside[2] += v.cx < -v.cw; outside[3] += v.cx > v.cw; outside[4] += v.cy < -v.cw; outside[5] += v.cy > v.cw;
         }
-        process_triangle_lanes(ec, k < kTessTris, v[0], v[1], v[2], base_id + k, tex, -1, lane);
+        bool culled = false;
+#pragma unroll
+        for (int p = 0; p < 6; p++) culled |= __all_sync(0xffffffffu, outside[p] == 2);
+        if (culled) return;
+        // literal vertex list S:407-433 (spec tile mode 0): 7x7 quads, (0,1,2)(0,2,3) split, 3 shades / triangle
+        for (int k0 = 0; k0 < kTessTris; k0 += 32) {
+          const int k = k0 + lane;
+          Vtx v[3];
+          if (k < kTessTris) {
+            const int quad = k >> 1, half = k & 1, a = quad / 7, b = quad - 7 * a;
+#pragma unroll
+            for (int j = 0; j < 3; j++) {
+              const int aa = j == 0 ? a : (j == 1 ? a + 1 : (half == 0 ? a + 1 : a));
+              const int bb = j == 0 ? b : (j == 1 ? (half == 0 ? b : b + 1) : b + 1);
+              v[j] = tile_vertex(x, sh, ts, aa, bb);
+            }
           }
+          process_triangle_lanes(ec, k < kTessTris, v[0], v[1], v[2], base_id + k, tex, -1, lane);
+        }
+      }
     }
   } else {
     // placed mesh S:1905-1907, O:123-148: T(pos) S(scale) Ry(y_rot)
@@ -1178,15 +1168,119 @@ __device__ __forceinline__ void geometry_item(const DState& S, const DMap* __res
 
 template <bool kTess>
 __global__ void __launch_bounds__(kGeoWarps * 32, kGeoMinCtas)
-k_geometry(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, int max_prims, int max_lat,
-           int32_t* __restrict__ err) {
+k_geometry(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, int max_prims, int32_t* __restrict__ err) {
   __shared__ GeoWarp gws[kGeoWarps];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const int n_list = fm.work[kWorkGeoList];   // written by k_cull
   for (int wi = blockIdx.x * kGeoWarps + wib; wi < n_list; wi += gridDim.x * kGeoWarps) {
     const uint2 e = fm.geo_list[wi];
-    geometry_item<kTess>(S, maps, rc, fm, max_prims, max_lat, err, (int)e.x, (int)e.y, lane, gws[wib]);
+    geometry_item<kTess>(S, maps, rc, fm, max_prims, err, (int)e.x, (int)e.y, lane, gws[wib]);
   }
+}
+
+// ------------------------------------------------------------------------------------------------ k_tiles
+// Tile mode 1: the ground and every road tile of one env (one listed slot) per warp.  The lanes take the map's grid cells
+// 32 at a time, a tile per lane: bounding-sphere test, model-view (the f64 entries of model_view_entry), the four corners
+// lit and culled against the frustum, and — where no clipping is needed — the quad set up and emitted, all 32 tiles at
+// once.  Lattice and prim slots come from one atomic per warp.  Then the whole warp lights the 64 lattice vertices of
+// each surviving tile, two per lane, from the transform its lane left in shared memory; tiles that need the clipper, and
+// quads that are not strictly convex after snapping, go one at a time through the warp-wide triangle path, as does the
+// ground quad.  Same expressions as a tile drawn by one warp, so the prims and lattices are bit-identical; only their
+// slots in the env's slab come in another order.
+struct TileLanes {
+  Xform x[32];      // the transform of lane k's tile
+  Vtx c[32][4];     // its corners (0,0) (7,0) (7,7) (0,7), uncoloured: the quad's vertices
+};
+__global__ void __launch_bounds__(kTileWarps * 32, kTileMinCtas)
+k_tiles(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, int max_prims, int max_lat, int32_t* __restrict__ err) {
+  __shared__ GeoWarp gws[kTileWarps];
+  __shared__ TileLanes tls[kTileWarps];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  const int slot = blockIdx.x * kTileWarps + wib;
+  if (slot >= n_listed(rc.env_list, rc.env_count, rc.n_envs)) return;   // (the whole warp)
+  const int env = listed_env(rc.env_list, slot);
+  GeoWarp& sh = gws[wib];
+  TileLanes& tl = tls[wib];
+  const DMap& m = maps[S.map_id[env]];
+  FrameCtx& ctx = fm.ctx[env];
+  const bool seg = (rc.mode & DTS_RENDER_SEGMENT) != 0;
+  load_geo_warp(sh, S, ctx, env, seg, lane);
+  const EmitCtx ec{m.textures, &sh, &ctx, fm.prims + (size_t)env * max_prims, max_prims, rc.width, rc.height};
+  float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
+  const int n_tiles = m.grid_w * m.grid_h;
+  const double ts = m.tile_size;
+  for (int t0 = 0; t0 < n_tiles; t0 += 32) {
+    // lane phase: tile t (draw order i outer, j inner, S:1852-1884)
+    const int t = t0 + lane, ti = t / m.grid_h, tj = t - ti * m.grid_h, idx = tj * m.grid_w + ti;
+    bool live = false;
+    if (t < n_tiles && m.tile_kind[idx] >= 0) {
+      float ex, ey, ez;   // (item_visible's test of the tile)
+      eye_point(sh.V, (ti + 0.5) * ts, 0.0, (tj + 0.5) * ts, ex, ey, ez);
+      live = !sphere_outside(sh.P00, sh.P11, ex, ey, ez, (float)(ts * 0.7071067811865476) * 1.001f + 1e-4f);
+    }
+#if DTS_STATS
+    const unsigned in_sphere = __ballot_sync(0xffffffffu, live);   // (the whole warp: DTS_COUNT is lane 0 alone)
+    DTS_COUNT(29, __popc(in_sphere));
+#endif
+    Vtx* cn = tl.c[lane];
+    if (live) {
+      const TilePose tp = tile_pose(m, ti, tj);
+      Xform x;
+#pragma unroll
+      for (int e = 0; e < 12; e++) model_view_entry(sh.V, tp.tx, 0.0, tp.tz, 1.0, tp.cs, tp.sn, e >> 2, e & 3, x);
+      tl.x[lane] = x;
+      // the prim is the quad of the 4 corners: cull on those before lighting the lattice
+      int out[6] = {0, 0, 0, 0, 0, 0};
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        Vtx v = tile_vertex(x, sh, ts, (k == 1 || k == 2) ? 7 : 0, k >= 2 ? 7 : 0);
+        out[0] += !(v.cz + v.cw >= 0.0f); out[1] += !(v.cw - v.cz >= 0.0f);
+        out[2] += v.cx < -v.cw; out[3] += v.cx > v.cw; out[4] += v.cy < -v.cw; out[5] += v.cy > v.cw;
+        v.r = 0.f; v.g = 0.f; v.b = 0.f;
+        cn[k] = v;
+      }
+#pragma unroll
+      for (int p = 0; p < 6; p++) live &= out[p] != 4;
+    }
+    const unsigned lit = __ballot_sync(0xffffffffu, live);
+    if (!lit) continue;
+    int lat = 0;
+    if (lane == 0) lat = atomicAdd(&ctx.n_lat, __popc(lit));
+    lat = __shfl_sync(0xffffffffu, lat, 0) + __popc(lit & ((1u << lane) - 1u));
+    if (live && lat >= max_lat) { ctx.overflow = 1; live = false; }
+    int tex = -1;
+    bool clip = false;   // drawn by the warp-wide path
+    if (live) {
+      tex = m.tile_tex[idx];
+      if (seg && tex >= 0) tex = m.tex_segment[tex];   // Texture.bind(segment=True) G:52-56
+      // a tile that needs no clipping is ONE quad prim (its diagonal then splits no bin); otherwise two triangles
+      clip = !(classify(cn[0], cn[1], cn[2]) == 0 && classify(cn[0], cn[2], cn[3]) == 0 &&
+               setup_and_emit(ec, cn[0], cn[1], cn[2], 2 + 2 * t, tex, lat, &cn[3]));
+    }
+    __syncwarp();
+    // warp phase: the lattice colours of each surviving tile -> table
+    for (unsigned todo = __ballot_sync(0xffffffffu, live); todo; todo &= todo - 1) {
+      const int src = __ffs(todo) - 1, s = __shfl_sync(0xffffffffu, lat, src);
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int vi = lane + 32 * h;
+        const Vtx v = tile_vertex(tl.x[src], sh, ts, vi >> 3, vi & 7);
+        lat_tab[s * 64 + vi] = make_float4(v.r, v.g, v.b, 0.0f);
+      }
+    }
+    // ... and the tiles the lanes could not emit as one quad: triangles (0,1,2)(0,2,3), clipped where needed
+    for (unsigned todo = __ballot_sync(0xffffffffu, clip); todo; todo &= todo - 1) {
+      const int src = __ffs(todo) - 1, id = 2 + 2 * (t0 + src);
+      const int stex = __shfl_sync(0xffffffffu, tex, src), slat = __shfl_sync(0xffffffffu, lat, src);
+      const Vtx* c = tl.c[src];
+      process_triangle_uniform(ec, c[0], c[1], c[2], id, stex, slat, lane);
+      process_triangle_uniform(ec, c[0], c[2], c[3], id + 1, stex, slat, lane);
+    }
+    __syncwarp();   // before the next chunk's lanes overwrite their TileLanes entries
+  }
+  draw_ground(ec, sh, seg, lane);
+  __syncwarp();
+  if (lane == 0 && ctx.overflow) { atomicOr(err, 1); *reinterpret_cast<volatile int32_t*>(fm.status) = 1; }
 }
 
 // ------------------------------------------------------------------------------------------------ k_bin
@@ -2762,9 +2856,14 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   k_frame_setup<<<(rc.n_envs + 127) / 128, 128, 0, st>>>(S, maps, rc, fm);
   mark();
   const size_t pairs_total = (size_t)rc.n_envs * r.items_max;
-  k_cull<<<(unsigned)((pairs_total + 255) / 256), 256, 0, st>>>(S, maps, rc, fm, r.items_max);
+  k_cull<<<(unsigned)((pairs_total + 255) / 256), 256, 0, st>>>(S, maps, rc, fm, r.items_max, err_flag);
+  int launches = 5;
+  if (!rc.tessellate) {   // (inside the k_geometry event bracket: it is geometry time)
+    k_tiles<<<(rc.n_envs + kTileWarps - 1) / kTileWarps, kTileWarps * 32, 0, st>>>(S, maps, rc, fm, r.max_prims, r.max_lat, err_flag);
+    launches++;
+  }
   const auto geometry = rc.tessellate ? k_geometry<true> : k_geometry<false>;
-  geometry<<<r.sms * kGeoMinCtas / kGeoWarps, kGeoWarps * 32, 0, st>>>(S, maps, rc, fm, r.max_prims, r.max_lat, err_flag);
+  geometry<<<r.sms * kGeoMinCtas / kGeoWarps, kGeoWarps * 32, 0, st>>>(S, maps, rc, fm, r.max_prims, err_flag);
   mark();
   const size_t bin_smem_bytes = (size_t)2 * r.cbins * sizeof(int);
   const int bin_grid = rc.n_envs;   // CTA per env: one warp where a frame has few bins and prims (160x120: 75 bins — more warps
@@ -2776,7 +2875,6 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, ft, r.max_prims, r.pool, err_flag);
   mark();
   const bool wrap = (rc.obs_layout | rc.obs_dtype) != 0;
-  int launches = 5;
   if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
     const auto solo = fisheye ? k_raster_solo<true> : k_raster_solo<false>;
     const auto flat = fisheye ? k_raster_flat<true> : k_raster_flat<false>;

@@ -16,6 +16,7 @@ names = {8: "coarse bins", 9: "  empty (cleared)", 10: "sum of list lengths (rec
          11: "fine bins shaded", 13: "  simple (one covering prim, no visibility pass)", 12: "extra shading rounds (2nd..4th winner of edge pixels)",
          26: "  k_raster_flat: edge pixels queued for their other winners", 27: "  k_raster_flat: batches of queued pixels (32, or a bin's rest)",
          16: "warp-wide prim visits", 17: "  trivially accepted (no edge tests)", 20: "general bins holding only road tiles (coverage-only visibility)", 21: "  of those redone with depth (a sample covered twice)", 22: "coarse bins inside one prim (solo)", 23: "  their fine bins",
-         24: "flat coarse bins (k_raster_flat: road tiles and ground only)", 25: "  handed back to k_raster (a sample covered twice)", 18: "tiny-triangle passes (fine bins)", 19: "  tiny triangles in them"}
+         24: "flat coarse bins (k_raster_flat: road tiles and ground only)", 25: "  handed back to k_raster (a sample covered twice)", 18: "tiny-triangle passes (fine bins)", 19: "  tiny triangles in them",
+         28: "k_cull's list: (env, mesh) items for k_geometry", 29: "k_tiles: road tiles inside the bounding-sphere test"}
 for k, v in names.items():
     print(f"{v:60s} {c[k]:12d}  per env {c[k]/4096:10.1f}")
