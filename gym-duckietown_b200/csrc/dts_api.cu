@@ -33,6 +33,7 @@ struct dts_sim {
   struct { int32_t* map_id; double *pos_x, *pos_z, *angle, *wheel_dist, *trim; float *f1[3]; float *f3[5];
            float* light_pos; int32_t* light_stale; uint32_t* hidden; } stage{};
   Renderer* render = nullptr;           // frame memory and fisheye tables
+  Resizer* resize = nullptr;            // the post-render ResizeWrapper (dts_set_resize_filter)
   int32_t* d_err = nullptr;
   int32_t* h_status = nullptr;          // mapped pinned host word: bit 0 = a frame overflowed its frame memory
   int32_t* d_status = nullptr;          // its device address
@@ -45,12 +46,6 @@ struct dts_sim {
   void* gather_peer[DTS_MAX_PEERS] = {};   // peers' buffers opened with cudaIpcOpenMemHandle (own entry = gather_buf)
   bool gather_next = false;
   int render_mode = 0;                  // dts_set_render_mode             // the next dts_render also stores into the gather buffers
-  // fused ResizeWrapper (dts_set_resize): full-size render target + tap tables
-  int resize_w = 0, resize_h = 0;
-  int resize_band = 0, resize_cap = 0;   // k_resize_band: output rows per CTA and the largest source-row span of a band (0: untiled kernel)
-  int resize_filter = DTS_RESIZE_CV2_CUBIC;   // dts_set_resize_filter; the Pillow filter's tables are the renderer's
-  uint8_t* resize_src = nullptr;
-  int16_t *resize_xtab = nullptr, *resize_ytab = nullptr;
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
   int profiling = 0;                    // 0 off, 1 events around k_raster only, 2 around every render kernel
   std::vector<cudaEvent_t> prof_events; // kProfMarks events per profiled frame
@@ -189,6 +184,7 @@ int dts_create(const dts_config* cfg, dts_sim** out) {
   bad |= sim->dalloc(&st.light_stale, n);
   bad |= sim->dalloc(&st.hidden, 8 * (size_t)n);
   sim->render = renderer_create(*cfg);
+  sim->resize = resizer_create(*cfg);
   if (bad) { g_create_error = sim->err; dts_destroy(sim); return 1; }
   sim->h_maps.assign(cfg->max_maps, DMap{});
   sim->map_allocs.resize(cfg->max_maps);
@@ -203,13 +199,12 @@ void dts_destroy(dts_sim* sim) {
   for (void* p : sim->allocs) cudaFree(p);
   for (auto& v : sim->map_allocs) for (void* p : v) cudaFree(p);
   renderer_destroy(sim->render);
+  resizer_destroy(sim->resize);
   void* extra[] = {sim->q_in, sim->q_outd, sim->q_outi, sim->q_hidden};
   for (void* p : extra) if (p) cudaFree(p);
   for (int p = 0; p < sim->gather_world; p++)
     if (sim->gather_peer[p] && sim->gather_peer[p] != sim->gather_buf) cudaIpcCloseMemHandle(sim->gather_peer[p]);
   if (sim->gather_buf) cudaFree(sim->gather_buf);
-  void* rz[] = {sim->resize_src, sim->resize_xtab, sim->resize_ytab};
-  for (void* p : rz) if (p) cudaFree(p);
   if (sim->h_status) cudaFreeHost(sim->h_status);
   for (cudaEvent_t e : sim->prof_events) cudaEventDestroy(e);
   delete sim;
@@ -514,19 +509,6 @@ int dts_reset_random(dts_sim* sim, const uint8_t* mask_dev, void* stream) {
   return 0;
 }
 
-// the resize pass dts_set_resize_filter selected: full-size u8 HWC frames -> the caller's tensor (the listed envs only,
-// given a device env list)
-static void launch_selected_resize(dts_sim* sim, const uint8_t* src, void* dst, cudaStream_t st,
-                                   const int32_t* env_list = nullptr, const int32_t* env_count = nullptr) {
-  if (sim->resize_filter == DTS_RESIZE_PIL_BILINEAR) {
-    launch_pil_resize(*sim->render, src, dst, sim->fmt.obs_layout, sim->fmt.obs_dtype, env_list, env_count, st);
-    return;
-  }
-  launch_resize(src, sim->cfg.cam_width, sim->cfg.cam_height, sim->resize_w, sim->resize_h, sim->cfg.num_envs,
-                sim->resize_xtab, sim->resize_ytab, dst, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->resize_band, sim->resize_cap,
-                env_list, env_count, st);
-}
-
 // dts_render of every env, or of the envs on a device list (dts_step_terminal's second pass; not profiled)
 static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t* env_list, const int32_t* env_count) {
   if (!obs_dev) return sim->fail("obs_dev is NULL");
@@ -549,13 +531,14 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
   }
   const int mark_level = marks ? sim->profiling : 0;
   void* target = obs_dev;
-  if (sim->resize_w) {   // render full size, packed u8 HWC, into the library's buffer; k_resize writes the caller's tensor
+  const ResizeTarget rz = resizer_target(*sim->resize);
+  if (rz.ow) {   // render full size, packed u8 HWC, into the resizer's buffer; the resize writes the caller's tensor
     rc.obs_layout = DTS_OBS_HWC; rc.obs_dtype = DTS_OBS_U8;
-    target = sim->resize_src;
+    target = rz.staging;
   }
   GatherTab gt{};
   if (sim->gather_next) {
-    if (sim->resize_w) return sim->fail("the fused gather writes the rasteriser's own output: not combined with dts_set_resize");
+    if (rz.ow) return sim->fail("the fused gather writes the rasteriser's own output: not combined with dts_set_resize");
     gt.n = sim->gather_world;
     for (int p = 0; p < sim->gather_world; p++)
       gt.base[p] = reinterpret_cast<uint8_t*>(sim->gather_peer[p]) + (uint64_t)sim->gather_rank * sim->gather_bytes;
@@ -563,8 +546,9 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
   }
   int k = launch_render(*sim->render, sim->S, sim->d_maps, rc, target, gt, sim->d_err, sim->d_status, marks, mark_level,
                         (cudaStream_t)stream);
-  if (sim->resize_w) {
-    launch_selected_resize(sim, sim->resize_src, obs_dev, (cudaStream_t)stream, env_list, env_count);
+  if (rz.ow) {
+    launch_resize(*sim->resize, rz.staging, obs_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, env_list, env_count,
+                  (cudaStream_t)stream);
     k++;
   }
   if (marks && mark_level >= 2) cudaEventRecord(marks[kProfMarks - 1], (cudaStream_t)stream);   // closes the "post" interval
@@ -605,7 +589,8 @@ int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, voi
   DTS_CUDA(cudaGetLastError());
   if (!obs_dev) return 0;
   // 4. their terminal frames -> terminal_obs_dev; 5. their first frames -> obs_dev
-  const size_t px = sim->resize_w ? (size_t)sim->resize_w * sim->resize_h : (size_t)sim->cfg.cam_width * sim->cfg.cam_height;
+  const ResizeTarget rz = resizer_target(*sim->resize);
+  const size_t px = rz.ow ? (size_t)rz.ow * rz.oh : (size_t)sim->cfg.cam_width * sim->cfg.cam_height;
   const size_t row_bytes = px * 3 * (sim->fmt.obs_dtype == DTS_OBS_F32_UNIT ? 4 : 1);
   launch_copy_rows(obs_dev, terminal_obs_dev, row_bytes, sim->ended, sim->n_ended, sim->cfg.num_envs, st);
   sim->launches++;
@@ -683,30 +668,6 @@ int dts_assign_maps(dts_sim* sim, const uint8_t* mask_dev, const int32_t* map_id
   return 0;
 }
 
-// cv2.resize INTER_CUBIC tap table of one axis (OpenCV resize(): fx = (float)((d + 0.5) * scale - 0.5), interpolateCubic
-// with A = -0.75 in float32, taps = saturate_cast<short>(w * 2048), indices clamped to the image)
-static void cubic_axis_table(int src, int dst, std::vector<int16_t>& tab) {
-  tab.assign((size_t)dst * 8, 0);
-  const double inv = (double)dst / (double)src, scale = 1.0 / inv;
-  for (int d = 0; d < dst; d++) {
-    float fx = (float)((d + 0.5) * scale - 0.5);
-    const int sx = (int)floorf(fx);
-    fx -= (float)sx;
-    const float A = -0.75f, x = fx;
-    float c[4];
-    c[0] = ((A * (x + 1) - 5 * A) * (x + 1) + 8 * A) * (x + 1) - 4 * A;
-    c[1] = ((A + 2) * x - (A + 3)) * x * x + 1;
-    c[2] = ((A + 2) * (1 - x) - (A + 3)) * (1 - x) * (1 - x) + 1;
-    c[3] = 1.f - c[0] - c[1] - c[2];
-    for (int k = 0; k < 4; k++) {
-      int idx = sx - 1 + k;
-      idx = idx < 0 ? 0 : (idx > src - 1 ? src - 1 : idx);
-      tab[(size_t)d * 8 + k] = (int16_t)idx;
-      tab[(size_t)d * 8 + 4 + k] = (int16_t)lrintf(c[k] * 2048.0f);
-    }
-  }
-}
-
 int dts_set_resize(dts_sim* sim, int out_w, int out_h) { return dts_set_resize_filter(sim, out_w, out_h, DTS_RESIZE_CV2_CUBIC); }
 
 int dts_set_resize_filter(dts_sim* sim, int out_w, int out_h, int filter) {
@@ -716,33 +677,8 @@ int dts_set_resize_filter(dts_sim* sim, int out_w, int out_h, int filter) {
   if (out_w > 4096 || out_h > 4096) return sim->fail("resize target %dx%d too large", out_w, out_h);
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   DTS_CUDA(cudaDeviceSynchronize());
-  // the Pillow tables first: a target that pass refuses leaves the previous setting in effect
-  const std::string e = renderer_set_pil_resize(*sim->render, filter == DTS_RESIZE_PIL_BILINEAR ? out_w : 0,
-                                                filter == DTS_RESIZE_PIL_BILINEAR ? out_h : 0);
-  if (!e.empty()) return sim->fail("%s", e.c_str());
-  void* old[] = {sim->resize_src, sim->resize_xtab, sim->resize_ytab};
-  for (void* p : old) if (p) cudaFree(p);
-  sim->resize_src = nullptr; sim->resize_xtab = sim->resize_ytab = nullptr;
-  sim->resize_w = sim->resize_h = 0;
-  sim->resize_filter = DTS_RESIZE_CV2_CUBIC;
-  if (!out_w) return 0;
-  if (filter == DTS_RESIZE_PIL_BILINEAR) {
-    DTS_CUDA(cudaMalloc(&sim->resize_src, (size_t)sim->cfg.num_envs * sim->cfg.cam_width * sim->cfg.cam_height * 3));
-    sim->resize_w = out_w; sim->resize_h = out_h;
-    sim->resize_filter = filter;
-    return 0;
-  }
-  std::vector<int16_t> xt, yt;
-  cubic_axis_table(sim->cfg.cam_width, out_w, xt);
-  cubic_axis_table(sim->cfg.cam_height, out_h, yt);
-  DTS_CUDA(cudaMalloc(&sim->resize_src, (size_t)sim->cfg.num_envs * sim->cfg.cam_width * sim->cfg.cam_height * 3));
-  DTS_CUDA(cudaMalloc(&sim->resize_xtab, xt.size() * 2));
-  DTS_CUDA(cudaMalloc(&sim->resize_ytab, yt.size() * 2));
-  DTS_CUDA(cudaMemcpy(sim->resize_xtab, xt.data(), xt.size() * 2, cudaMemcpyHostToDevice));
-  DTS_CUDA(cudaMemcpy(sim->resize_ytab, yt.data(), yt.size() * 2, cudaMemcpyHostToDevice));
-  sim->resize_w = out_w; sim->resize_h = out_h;
-  plan_resize_bands(sim->cfg.cam_width, out_w, out_h, yt.data(), &sim->resize_band, &sim->resize_cap);
-  return 0;
+  const std::string e = resizer_set(*sim->resize, filter, out_w, out_h);
+  return e.empty() ? 0 : sim->fail("%s", e.c_str());
 }
 
 // ---- fused end-of-rollout gather: peer buffers over cudaIpc, written by the rasteriser itself --------------------
@@ -819,10 +755,10 @@ int dts_set_render_mode(dts_sim* sim, int mode) {
 
 int dts_resize_frames(dts_sim* sim, const uint8_t* src_dev, void* dst_dev, void* stream) {
   if (!sim) return 1;
-  if (!sim->resize_w) return sim->fail("dts_set_resize first");
+  if (!resizer_target(*sim->resize).ow) return sim->fail("dts_set_resize first");
   if (!src_dev || !dst_dev) return sim->fail("NULL frame pointer");
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  launch_selected_resize(sim, src_dev, dst_dev, (cudaStream_t)stream);
+  launch_resize(*sim->resize, src_dev, dst_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, nullptr, nullptr, (cudaStream_t)stream);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   return 0;

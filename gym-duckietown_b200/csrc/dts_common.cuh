@@ -143,4 +143,25 @@ struct StepCfg {
   dts_dr_op dr_ops[DTS_MAX_DR_OPS];
 };
 
+// One pixel in a wrapper layout / dtype (dts_output_format): element index of channel c at (x, y)
+__device__ __forceinline__ size_t fmt_index(int layout, int x, int y, int c, int W, int H) {
+  return layout == DTS_OBS_CHW ? ((size_t)c * H + y) * W + x
+       : layout == DTS_OBS_CWH ? ((size_t)c * W + x) * H + y
+                               : ((size_t)y * W + x) * 3 + c;
+}
+// Channel c of it, value v (0..255): u8, or float32 v / 255
+__device__ __forceinline__ void store_elem_fmt(void* frame, int layout, int dtype, int x, int y, int c, int W, int H, unsigned v) {
+  const size_t i = fmt_index(layout, x, y, c, W, H);
+  if (dtype == DTS_OBS_F32_UNIT) reinterpret_cast<float*>(frame)[i] = (float)v / 255.0f;   // NormalizeWrapper LW:66-70
+  else reinterpret_cast<uint8_t*>(frame)[i] = (uint8_t)v;
+}
+__device__ __forceinline__ void store_px_fmt(void* frame, int layout, int dtype, int x, int y, int W, int H, unsigned rgb) {
+#pragma unroll
+  for (int c = 0; c < 3; c++) store_elem_fmt(frame, layout, dtype, x, y, c, W, H, (rgb >> (8 * c)) & 255u);
+}
+
+// A pass over a device env list (RenderCfg::env_list): the number of slots drawn, and the env of slot s < that number
+__device__ __forceinline__ int n_listed(const int32_t* list, const int32_t* count, int n_envs) { return list ? __ldg(count) : n_envs; }
+__device__ __forceinline__ int listed_env(const int32_t* list, int slot) { return list ? __ldg(list + slot) : slot; }
+
 }  // namespace dts

@@ -1,7 +1,7 @@
 """src/gym_duckietown/wrappers.py's ResizeWrapper (cv2.resize, INTER_CUBIC): the numpy restatement in
 oracle/cv2_cubic.py, which the GPU tests hold the device pass to at 0 LSB, pinned against what the reference class
 returned (tests/golden/wrappers.npz), against OpenCV itself where it imports, and against a float64 convolution.
-Also the host arithmetic of the device's band plan (plan_resize_bands in dts_render.cu), so that the GPU sweep below
+Also the host arithmetic of the device's band plan (plan_resize_bands in dts_post.cu), so that the GPU sweep below
 keeps reaching every branch of k_resize_band / k_resize."""
 import os
 
