@@ -138,6 +138,16 @@ int dts_create(const dts_config* cfg, dts_sim** out) {
       if (op.type < DTS_DR_INT || op.type > DTS_DR_NORMAL || op.size < 0 || op.target < DTS_DR_NONE || op.target > DTS_DR_TRIM) {
         g_create_error = "bad dts_dr_op"; delete sim; return 1;
       }
+      // Generator.integers raises ValueError("low >= high") on an empty range; the device would draw garbage.  The
+      // device takes int64 bounds, so a high of 2^63 or more is refused too.
+      for (int j = 0; op.type == DTS_DR_INT && j < (op.size < 3 ? op.size : 3); j++) {
+        if (!(op.a[j] < op.b[j]) || !(op.a[j] >= -9223372036854775808.0) || !(op.b[j] < 9223372036854775808.0)) {
+          char buf[160];
+          snprintf(buf, sizeof buf, "dts_dr_op %d: int draw needs low < high within int64, got low %.17g high %.17g",
+                   k, op.a[j], op.b[j]);
+          g_create_error = buf; delete sim; return 1;
+        }
+      }
     }
   } else {   // randomization/config/default_dr.json, keys sorted (randomizer.py:33)
     const dts_dr_op def[7] = {
@@ -840,6 +850,43 @@ int dts_debug_counters(dts_sim* sim, int32_t out[32]) {
   if (!sim) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   DTS_CUDA(cudaMemcpy(out, sim->d_err, 32 * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+/* debug: every env's stream as [N][6] (dts_seed_streams' layout); synchronises */
+int dts_debug_streams(dts_sim* sim, uint64_t* out_host) {
+  if (!sim) return 1;
+  if (!out_host) return sim->fail("out_host is NULL");
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  DTS_CUDA(cudaDeviceSynchronize());
+  const size_t n = sim->cfg.num_envs;
+  std::vector<uint64_t> soa(6 * n);
+  DTS_CUDA(cudaMemcpy(soa.data(), sim->S.rng, 6 * n * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+  for (size_t e = 0; e < n; e++)
+    for (int k = 0; k < 6; k++) out_host[6 * e + k] = soa[k * n + e];
+  return 0;
+}
+
+/* debug: a program of NpStream draws from every env's stream (see dtsim.h) */
+int dts_debug_draw(dts_sim* sim, const dts_draw_op* ops, int n_ops, uint64_t* out_dev, void* stream) {
+  if (!sim) return 1;
+  if (!ops || !out_dev || n_ops <= 0) return sim->fail("dts_debug_draw needs ops, n_ops > 0 and out_dev");
+  int64_t total = 0;
+  for (int k = 0; k < n_ops; k++) {
+    const dts_draw_op& op = ops[k];
+    if (op.kind < DTS_DRAW_NEXT64 || op.kind > DTS_DRAW_NORMAL || op.count < 0) return sim->fail("bad dts_draw_op %d", k);
+    if (op.kind == DTS_DRAW_INTEGERS && !(op.lo < op.hi)) return sim->fail("dts_draw_op %d: integers needs lo < hi", k);
+    total += op.count;
+  }
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  dts_draw_op* d_ops = nullptr;
+  DTS_CUDA(cudaMallocAsync((void**)&d_ops, n_ops * sizeof(dts_draw_op), st));
+  DTS_CUDA(cudaMemcpyAsync(d_ops, ops, n_ops * sizeof(dts_draw_op), cudaMemcpyHostToDevice, st));
+  launch_debug_draw(sim->S, d_ops, n_ops, total, out_dev, st);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  DTS_CUDA(cudaFreeAsync(d_ops, st));
   return 0;
 }
 

@@ -44,6 +44,8 @@ void launch_respawn_ended(const DState& S, const DMap* maps, const StepCfg& c, i
                           int32_t* n_ended, cudaStream_t st);
 void launch_query(const DMap* maps, int map_id, int dyn_env, int n_envs, int n, const double* q, const uint32_t* hidden,
                   double* outd, int32_t* outi, cudaStream_t st);
+// dts_debug_draw: every env runs ops[0 .. n_ops) (device copy) from its stream; out[env][0 .. total)
+void launch_debug_draw(const DState& S, const dts_draw_op* ops, int n_ops, int64_t total, uint64_t* out, cudaStream_t st);
 
 // Fused end-of-rollout observation gather (SURVEY 8e): on the rollout's last step the rasteriser's resolve stores every
 // frame, besides the caller's tensor, straight into the gather buffers of all GPUs of the box — peer memory mapped with

@@ -346,6 +346,31 @@ __global__ void __launch_bounds__(128) k_query(const DMap* __restrict__ maps, in
   outi[8 * t + 7] = idx >= 0 && m.tile_drivable[idx];
 }
 
+// dts_debug_draw: the env's stream runs a program of NpStream calls; draw i -> out[e * total + i]
+__global__ void __launch_bounds__(128) k_debug_draw(DState S, const dts_draw_op* __restrict__ ops, int n_ops, int64_t total,
+                                                    uint64_t* __restrict__ out) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= S.n) return;
+  NpStream rs;
+  load_stream(S, e, rs);
+  uint64_t* o = out + (size_t)e * total;
+  for (int k = 0; k < n_ops; k++) {
+    const dts_draw_op op = ops[k];
+    for (int i = 0; i < op.count; i++) {
+      uint64_t v;
+      switch (op.kind) {
+        case DTS_DRAW_NEXT64: v = rs.next64(); break;
+        case DTS_DRAW_NEXT32: v = rs.next32(); break;
+        case DTS_DRAW_UNIFORM: v = (uint64_t)__double_as_longlong(rs.uniform(op.a, op.b)); break;
+        case DTS_DRAW_INTEGERS: v = (uint64_t)rs.integers(op.lo, op.hi); break;
+        default: v = (uint64_t)__double_as_longlong(rs.normal(op.a, op.b)); break;
+      }
+      *o++ = v;
+    }
+  }
+  store_stream(S, e, rs);
+}
+
 // ------------------------------------------------------------------ launchers
 void launch_step_logic(const DState& S, const DMap* maps, const StepCfg& c, int n_maps_cycle, const float* actions,
                        float* reward, uint8_t* done, cudaStream_t st) {
@@ -369,6 +394,9 @@ void launch_assign_maps(const DState& S, const DMap* maps, const uint8_t* mask, 
 void launch_query(const DMap* maps, int map_id, int dyn_env, int n_envs, int n, const double* q, const uint32_t* hidden,
                   double* outd, int32_t* outi, cudaStream_t st) {
   k_query<<<(n + 127) / 128, 128, 0, st>>>(maps, map_id, dyn_env, n_envs, n, q, hidden, outd, outi);
+}
+void launch_debug_draw(const DState& S, const dts_draw_op* ops, int n_ops, int64_t total, uint64_t* out, cudaStream_t st) {
+  k_debug_draw<<<(S.n + 127) / 128, 128, 0, st>>>(S, ops, n_ops, total, out);
 }
 
 }  // namespace dts

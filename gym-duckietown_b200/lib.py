@@ -94,6 +94,13 @@ class Mesh(C.Structure):
 
 RENDER_SEGMENT, RENDER_TOP_DOWN, RENDER_PINHOLE, RENDER_RECTIFY = 1, 2, 4, 8
 
+DRAW_NEXT64, DRAW_NEXT32, DRAW_UNIFORM, DRAW_INTEGERS, DRAW_NORMAL = 0, 1, 2, 3, 4   # dts_debug_draw
+
+
+class DrawOp(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("count", C.c_int32), ("a", C.c_double), ("b", C.c_double),
+                ("lo", C.c_int64), ("hi", C.c_int64)]
+
 
 class MapBlob(C.Structure):
     _fields_ = [
@@ -197,6 +204,8 @@ def load() -> C.CDLL:
     lib.dts_debug_counters.argtypes = [vp, vp]
     lib.dts_debug_episode.argtypes = [vp, i, vp]
     lib.dts_debug_frame.argtypes = [vp, i, vp, vp, vp, vp, i]
+    lib.dts_debug_streams.argtypes = [vp, vp]
+    lib.dts_debug_draw.argtypes = [vp, C.POINTER(DrawOp), i, vp, vp]
     lib.dts_launch_count.restype = C.c_uint64
     lib.dts_last_error.argtypes = [vp]
     lib.dts_last_error.restype = C.c_char_p
@@ -208,7 +217,8 @@ def load() -> C.CDLL:
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
            "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
-           "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame", "dts_last_error", "dts_destroy"]
+           "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
+           "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
 
 
 def _ptr(a: Optional[np.ndarray]):
@@ -499,6 +509,28 @@ class Sim:
         lat = np.zeros((n_cells, 64, 3), np.float32)
         self._check(self.lib.dts_debug_frame(self.h, env, _ptr(V), _ptr(P), _ptr(cnt), _ptr(lat), n_cells), "dts_debug_frame")
         return dict(V=V, P=P, n_prims=int(cnt[0]), n_lat=int(cnt[1]), overflow=int(cnt[2]), batch_pairs=int(cnt[3]), lattice=lat)
+
+    def debug_streams(self) -> List[dict]:
+        """Every env's device stream as a numpy `PCG64.state` dict (what `Generator.bit_generator.state` returns);
+        synchronises."""
+        raw = np.zeros((self.cfg.num_envs, 6), np.uint64)
+        self._check(self.lib.dts_debug_streams(self.h, _ptr(raw)), "dts_debug_streams")
+        return [{"bit_generator": "PCG64", "state": {"state": int(r[0]) << 64 | int(r[1]), "inc": int(r[2]) << 64 | int(r[3])},
+                 "has_uint32": int(r[4]), "uinteger": int(r[5])} for r in raw]
+
+    def debug_draw(self, ops, out_ptr: int, stream: int = 0) -> int:
+        """Every env runs the program `ops` = [(DRAW_*, count, a, b)] from its own stream (dts_debug_draw): integers take
+        int bounds a <= x < b, uniform / normal float ones.  Writes u64[num_envs][total] at device `out_ptr`; returns
+        total, the draws per env."""
+        arr = (DrawOp * len(ops))()
+        for k, (kind, count, a, b) in enumerate(ops):
+            arr[k].kind, arr[k].count = int(kind), int(count)
+            if kind == DRAW_INTEGERS:
+                arr[k].lo, arr[k].hi = int(a), int(b)
+            else:
+                arr[k].a, arr[k].b = float(a), float(b)
+        self._check(self.lib.dts_debug_draw(self.h, arr, len(ops), out_ptr, stream), "dts_debug_draw")
+        return sum(int(op[1]) for op in ops)
 
     def debug_counters(self) -> np.ndarray:
         out = np.zeros(32, np.int32)

@@ -372,6 +372,24 @@ int dts_debug_episode(dts_sim* sim, int env, void* out144);
 int dts_debug_frame(dts_sim* sim, int env, double V[12], float P[4], int32_t counts[4], float* lattice_by_cell, int n_cells);
 /* 32 diagnostic counters: [0] != 0 -> a render scratch buffer overflowed (frame incomplete). */
 int dts_debug_counters(dts_sim* sim, int32_t out[32]);
+/* debug (tests/test_gpu_np_streams.py): every env's numpy PCG64 stream as out_host[N][6] = state_hi, state_lo, inc_hi,
+ * inc_lo, has_uint32, uinteger — the layout dts_seed_streams takes.  Synchronises. */
+int dts_debug_streams(dts_sim* sim, uint64_t* out_host);
+/* debug: one short program of draws, run by every env from its own stream through the NpStream methods the device
+ * resets call.  Op k draws `count` values of `kind`; draw i of the program goes to out_dev[env][i] (u64[N][total]):
+ * integers as int64, doubles as their bit patterns, next32 zero-extended.  The env's stream advances as the draws
+ * did.  Device output, stream-ordered; integers need lo < hi, as numpy does. */
+enum { DTS_DRAW_NEXT64 = 0,   /* bit_generator.random_raw() */
+       DTS_DRAW_NEXT32 = 1,   /* integers(0, 2**32, dtype=np.uint32) */
+       DTS_DRAW_UNIFORM = 2,  /* uniform(a, b) */
+       DTS_DRAW_INTEGERS = 3, /* integers(lo, hi) */
+       DTS_DRAW_NORMAL = 4    /* normal(a, b) */ };
+typedef struct {
+  int32_t kind, count;
+  double a, b;              /* uniform / normal */
+  int64_t lo, hi;           /* integers */
+} dts_draw_op;
+int dts_debug_draw(dts_sim* sim, const dts_draw_op* ops, int n_ops, uint64_t* out_dev, void* stream);
 const char* dts_last_error(dts_sim* sim); /* sim may be NULL: error of the last failed dts_create */
 void dts_destroy(dts_sim* sim);
 
