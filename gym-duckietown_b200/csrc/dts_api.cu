@@ -1,5 +1,5 @@
 // dts_api.cu — the C ABI of libdtsim.so (include/dtsim.h): handle management, host->device
-// staging of maps and episode parameters, and stream-ordered launches of the kernels.
+// staging of episode parameters, and stream-ordered launches of the kernels.
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -26,12 +26,10 @@ struct dts_sim {
   StepCfg step_cfg;
   DState S;
   std::vector<void*> allocs;           // freed in dts_destroy
-  std::vector<std::vector<void*>> map_allocs;
-  std::vector<DMap> h_maps;
-  DMap* d_maps = nullptr;
   // reset staging (device) sized num_envs
   struct { int32_t* map_id; double *pos_x, *pos_z, *angle, *wheel_dist, *trim; float *f1[3]; float *f3[5];
            float* light_pos; int32_t* light_stale; uint32_t* hidden; } stage{};
+  MapSlots* maps = nullptr;             // the uploaded maps (dts_upload_map)
   Renderer* render = nullptr;           // frame memory and fisheye tables
   Resizer* resize = nullptr;            // the post-render ResizeWrapper (dts_set_resize_filter)
   int32_t* d_err = nullptr;
@@ -68,23 +66,13 @@ struct dts_sim {
     err = buf;
     return 1;
   }
-  template <typename T> int dalloc(T** p, size_t count, std::vector<void*>* owner = nullptr) {
+  template <typename T> int dalloc(T** p, size_t count) {
     void* q = nullptr;
     cudaError_t e = cudaMalloc(&q, count * sizeof(T) + 16);
     if (e != cudaSuccess) return fail("cudaMalloc(%zu B) failed: %s", count * sizeof(T), cudaGetErrorString(e));
     cudaMemset(q, 0, count * sizeof(T) + 16);
-    (owner ? *owner : allocs).push_back(q);
+    allocs.push_back(q);
     *p = (T*)q;
-    return 0;
-  }
-  template <typename T> int upload(const T** dst, const T* src, size_t count, std::vector<void*>* owner) {
-    T* d = nullptr;
-    if (dalloc(&d, count ? count : 1, owner)) return 1;
-    if (count && src) {
-      cudaError_t e = cudaMemcpy(d, src, count * sizeof(T), cudaMemcpyHostToDevice);
-      if (e != cudaSuccess) return fail("cudaMemcpy H2D failed: %s", cudaGetErrorString(e));
-    }
-    *dst = d;
     return 0;
   }
 };
@@ -174,7 +162,7 @@ int dts_create(const dts_config* cfg, dts_sim** out) {
   for (auto p : u8) bad |= sim->dalloc(p, n);
   bad |= sim->dalloc(&S.rng, 6 * (size_t)n);
   bad |= sim->dalloc(&S.rep, n);
-  bad |= sim->dalloc(&sim->d_maps, cfg->max_maps);
+  if (!(sim->maps = maps_create(*cfg))) bad |= sim->fail("cudaMalloc(map table of %d slots) failed", cfg->max_maps);
   bad |= sim->dalloc(&sim->d_err, 32);
   bad |= sim->dalloc(&sim->ended, n);
   bad |= sim->dalloc(&sim->n_ended, 1);
@@ -196,8 +184,6 @@ int dts_create(const dts_config* cfg, dts_sim** out) {
   sim->render = renderer_create(*cfg);
   sim->resize = resizer_create(*cfg);
   if (bad) { g_create_error = sim->err; dts_destroy(sim); return 1; }
-  sim->h_maps.assign(cfg->max_maps, DMap{});
-  sim->map_allocs.resize(cfg->max_maps);
   *out = sim;
   return 0;
 }
@@ -207,7 +193,7 @@ void dts_destroy(dts_sim* sim) {
   cudaSetDevice(sim->cfg.device);
   cudaDeviceSynchronize();
   for (void* p : sim->allocs) cudaFree(p);
-  for (auto& v : sim->map_allocs) for (void* p : v) cudaFree(p);
+  maps_destroy(sim->maps);
   renderer_destroy(sim->render);
   resizer_destroy(sim->resize);
   void* extra[] = {sim->q_in, sim->q_outd, sim->q_outi, sim->q_hidden};
@@ -222,205 +208,10 @@ void dts_destroy(dts_sim* sim) {
 
 int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
   if (!sim) return 1;
-  if (!b || map_id < 0 || map_id >= sim->cfg.max_maps) return sim->fail("bad map_id %d", map_id);
-  if (b->n_objects > DTS_MAX_OBJECTS) return sim->fail("map has %d objects, limit %d", b->n_objects, DTS_MAX_OBJECTS);
-  if (b->grid_w <= 0 || b->grid_h <= 0 || !(b->tile_size > 0)) return sim->fail("invalid tile grid");
-  if (b->n_dyn < 0 || b->n_dyn > DTS_MAX_DYN) return sim->fail("map has %d dynamic obstacles, limit %d", b->n_dyn, DTS_MAX_DYN);
-  // validate the whole blob BEFORE the slot's previous allocations are released: a rejected upload leaves the
-  // old map intact
-  for (int o = 0; o < b->n_objects; o++) {
-    const dts_object& s = b->objects[o];
-    if (s.mesh_id < 0 || s.mesh_id >= b->n_meshes) return sim->fail("object %d: bad mesh_id", o);
-    if (s.alt_tex_to >= b->n_textures || s.alt_tex_from >= b->n_textures) return sim->fail("object %d: alt texture out of range", o);
-    if (s.dyn_slot >= b->n_dyn) return sim->fail("object %d: dyn_slot %d out of range", o, s.dyn_slot);
-  }
-  for (int t = 0; t < b->n_textures; t++) {
-    const dts_texture& s = b->textures[t];
-    if (s.width <= 0 || s.height <= 0 || (s.width & (s.width - 1)) || (s.height & (s.height - 1)))
-      return sim->fail("texture %d: %dx%d is not a power of two", t, s.width, s.height);
-  }
-  for (int s = 0; s < b->n_dyn; s++) {
-    const dts_dyn_object& q = b->dyn[s];
-    if (q.kind != DTS_DYN_DUCKIE && q.kind != DTS_DYN_DUCKIEBOT && q.kind != DTS_DYN_TRAFFICLIGHT) return sim->fail("dyn %d: bad kind %d", s, q.kind);
-    if (q.object_index < 0 || q.object_index >= b->n_objects || b->objects[q.object_index].dyn_slot != s)
-      return sim->fail("dyn %d: object_index %d does not point back to this slot", s, q.object_index);
-  }
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  DTS_CUDA(cudaDeviceSynchronize());
-  auto& own = sim->map_allocs[map_id];
-  for (void* p : own) cudaFree(p);
-  own.clear();
-  sim->h_maps[map_id].valid = 0;   // until the new map is complete, the slot holds nothing (a failed cudaMalloc below leaves it empty)
-  DMap m{};
-  const size_t T = (size_t)b->grid_w * b->grid_h;
-  m.tile_size = b->tile_size; m.grid_w = b->grid_w; m.grid_h = b->grid_h; m.n_tiles = (int)T;
-  int bad = 0;
-  bad |= sim->upload(&m.tile_kind, b->tile_kind, T, &own);
-  bad |= sim->upload(&m.tile_angle, b->tile_angle, T, &own);
-  bad |= sim->upload(&m.tile_drivable, b->tile_drivable, T, &own);
-  bad |= sim->upload(&m.tile_tex, b->tile_tex, T, &own);
-  bad |= sim->upload(&m.tile_curve_off, b->tile_curve_off, T, &own);
-  bad |= sim->upload(&m.tile_curve_cnt, b->tile_curve_cnt, T, &own);
-  bad |= sim->upload(&m.curves, b->curves, (size_t)b->n_curves * 12, &own);
-  m.n_coll = b->n_coll;
-  bad |= sim->upload(&m.coll_corners, b->coll_corners, (size_t)b->n_coll * 8, &own);
-  bad |= sim->upload(&m.coll_norms, b->coll_norms, (size_t)b->n_coll * 4, &own);
-  bad |= sim->upload(&m.coll_centers, b->coll_centers, (size_t)b->n_coll * 3, &own);
-  bad |= sim->upload(&m.coll_radii, b->coll_radii, (size_t)b->n_coll, &own);
-  std::vector<int32_t> drv;
-  for (int j = 0; j < b->grid_h; j++)       // reference scan order S:810-860
-    for (int i = 0; i < b->grid_w; i++)
-      if (b->tile_kind[j * b->grid_w + i] >= 0 && b->tile_drivable[j * b->grid_w + i]) { drv.push_back(i); drv.push_back(j); }
-  m.start_i = b->start_tile[0]; m.start_j = b->start_tile[1];
-  if (m.start_i < 0 || m.start_j < 0 || m.start_i >= b->grid_w || m.start_j >= b->grid_h) { m.start_i = -1; m.start_j = -1; }
-  m.has_start_pose = b->has_start_pose != 0;
-  for (int k = 0; k < 3; k++) m.start_pose[k] = b->start_pose[k];
-  m.n_drivable = (int)drv.size() / 2;
-  bad |= sim->upload(&m.drivable_ij, drv.data(), drv.size(), &own);
-  // objects: add spawn radius (S:1467) and a bounding sphere per placed mesh
-  std::vector<DObject> objs(b->n_objects);
-  for (int o = 0; o < b->n_objects; o++) {
-    const dts_object& s = b->objects[o];
-    if (s.mesh_id < 0 || s.mesh_id >= b->n_meshes) return sim->fail("object %d: bad mesh_id", o);
-    const dts_mesh& me = b->meshes[s.mesh_id];
-    DObject& d = objs[o];
-    for (int k = 0; k < 3; k++) { d.pos[k] = (float)s.pos[k]; d.dpos[k] = s.pos[k]; }   // glTranslatef takes floats
-    d.dyn_slot = s.dyn_slot;
-    d.alt_from = s.alt_tex_from; d.alt_to = s.alt_tex_to;
-    if (s.alt_tex_to >= b->n_textures || s.alt_tex_from >= b->n_textures) return sim->fail("object %d: alt texture out of range", o);
-    if (s.dyn_slot >= b->n_dyn) return sim->fail("object %d: dyn_slot %d out of range", o, s.dyn_slot);
-    d.scale = s.scale; d.y_rot_deg = s.y_rot_deg; d.mesh_id = s.mesh_id; d.optional = s.optional;
-    d.tri_offset = me.tri_offset; d.tri_count = me.tri_count;
-    d.seg_tex = (me.seg_flat_tex >= 0 && me.seg_flat_tex < b->n_textures) ? me.seg_flat_tex : -1; d.pad_ = 0;
-    float lo[3] = {1e30f, 1e30f, 1e30f}, hi[3] = {-1e30f, -1e30f, -1e30f};
-    for (int t = 0; t < me.tri_count * 3; t++)
-      for (int k = 0; k < 3; k++) {
-        const float v = b->tri_pos[((size_t)me.tri_offset * 3 + t) * 3 + k];
-        lo[k] = v < lo[k] ? v : lo[k];
-        hi[k] = v > hi[k] ? v : hi[k];
-      }
-    float mx = hi[0] > hi[1] ? hi[0] : hi[1];
-    mx = mx > hi[2] ? mx : hi[2];
-    d.spawn_rad = mx * 0.5f * s.scale + 0.25f;     // MIN_SPAWN_OBJ_DIST S:156
-    float r2 = 0.f;
-    for (int k = 0; k < 3; k++) { d.centre[k] = 0.5f * (lo[k] + hi[k]); const float h = 0.5f * (hi[k] - lo[k]); r2 += h * h; }
-    d.bound_rad = sqrtf(r2);
-  }
-  m.n_objects = b->n_objects;
-  bad |= sim->upload(&m.objects, objs.data(), objs.size(), &own);
-  m.n_tris = b->n_tris;
-  bad |= sim->upload(&m.tri_pos, b->tri_pos, (size_t)b->n_tris * 9, &own);
-  bad |= sim->upload(&m.tri_nrm, b->tri_nrm, (size_t)b->n_tris * 9, &own);
-  bad |= sim->upload(&m.tri_uv, b->tri_uv, (size_t)b->n_tris * 6, &own);
-  bad |= sim->upload(&m.tri_col, b->tri_col, (size_t)b->n_tris * 9, &own);
-  bad |= sim->upload(&m.tri_tex, b->tri_tex, (size_t)b->n_tris, &own);
-  std::vector<DTexture> tex(b->n_textures);
-  {
-    size_t pool_bytes = 0;
-    std::vector<size_t> off(b->n_textures);
-    for (int t = 0; t < b->n_textures; t++) {
-      const dts_texture& s = b->textures[t];
-      off[t] = pool_bytes;
-      pool_bytes += ((size_t)s.width * s.height * 4 + 255) & ~size_t(255);
-    }
-    if (pool_bytes >= (size_t(1) << 32)) return sim->fail("textures exceed 4 GB");
-    std::vector<uint8_t> pool(pool_bytes ? pool_bytes : 256, 0);
-    for (int t = 0; t < b->n_textures; t++) {
-      const dts_texture& s = b->textures[t];
-      memcpy(pool.data() + off[t], s.rgba, (size_t)s.width * s.height * 4);
-    }
-    bad |= sim->upload(&m.tex_pool, pool.data(), pool.size(), &own);
-    for (int t = 0; t < b->n_textures && !bad; t++) {
-      const dts_texture& s = b->textures[t];
-      int lw = 0, lh = 0;
-      while ((1 << lw) < s.width) lw++;
-      while ((1 << lh) < s.height) lh++;
-      if (lw > 15 || lh > 15) return sim->fail("texture %d: %dx%d too large", t, s.width, s.height);
-      tex[t].w = s.width; tex[t].h = s.height; tex[t].rgba = m.tex_pool + off[t];
-      tex[t].info = (uint32_t)(off[t] >> 8) | ((uint32_t)lw << 24) | ((uint32_t)lh << 28);
-      tex[t].pad = 0;
-    }
-  }
-  m.n_textures = b->n_textures;
-  bad |= sim->upload(&m.textures, tex.data(), tex.size(), &own);
-  {
-    std::vector<int16_t> seg(b->n_textures > 0 ? b->n_textures : 1);
-    for (int t = 0; t < b->n_textures; t++) {
-      const int v = b->tex_segment ? b->tex_segment[t] : -1;
-      seg[t] = (int16_t)((v >= 0 && v < b->n_textures) ? v : t);
-    }
-    bad |= sim->upload(&m.tex_segment, seg.data(), seg.size(), &own);
-    DObject ag{};
-    if (b->agent_mesh >= 0 && b->agent_mesh < b->n_meshes) {   // self.mesh, drawn by top-down views at cur_pos (S:1923-1929)
-      const dts_mesh& me = b->meshes[b->agent_mesh];
-      ag.scale = 1.0f; ag.mesh_id = b->agent_mesh; ag.tri_offset = me.tri_offset; ag.tri_count = me.tri_count;
-      ag.dyn_slot = -1; ag.alt_from = ag.alt_to = -1;
-      ag.seg_tex = (me.seg_flat_tex >= 0 && me.seg_flat_tex < b->n_textures) ? me.seg_flat_tex : -1;
-      float lo[3] = {1e30f, 1e30f, 1e30f}, hi[3] = {-1e30f, -1e30f, -1e30f};
-      for (int t = 0; t < me.tri_count * 3; t++)
-        for (int k = 0; k < 3; k++) {
-          const float v = b->tri_pos[((size_t)me.tri_offset * 3 + t) * 3 + k];
-          lo[k] = v < lo[k] ? v : lo[k];
-          hi[k] = v > hi[k] ? v : hi[k];
-        }
-      float r2 = 0.f;
-      for (int k = 0; k < 3; k++) { ag.centre[k] = 0.5f * (lo[k] + hi[k]); const float h = 0.5f * (hi[k] - lo[k]); r2 += h * h; }
-      ag.bound_rad = sqrtf(r2);
-    }
-    m.agent = ag;
-  }
-  // dynamic obstacles: constants + every env's copy of the load-time state ([field][slot][env])
-  m.n_dyn = b->n_dyn;
-  {
-    const size_t N = sim->cfg.num_envs, D = b->n_dyn;
-    std::vector<DDyn> par(D);
-    std::vector<double> st((size_t)DTS_DYN_FIELDS * D * N);
-    for (size_t s = 0; s < D; s++) {
-      const dts_dyn_object& q = b->dyn[s];
-      if (q.kind != DTS_DYN_DUCKIE && q.kind != DTS_DYN_DUCKIEBOT && q.kind != DTS_DYN_TRAFFICLIGHT) return sim->fail("dyn %zu: bad kind %d", s, q.kind);
-      if (q.object_index < 0 || q.object_index >= b->n_objects || b->objects[q.object_index].dyn_slot != (int)s)
-        return sim->fail("dyn %zu: object_index %d does not point back to this slot", s, q.object_index);
-      DDyn& p = par[s];
-      p.kind = q.kind; p.object_index = q.object_index; p.pos_y = q.pos[1];
-      for (int k = 0; k < 4; k++) p.norms[k] = q.norms[k / 2][k % 2];
-      p.safety_radius = q.safety_radius; p.walk_distance = q.walk_distance; p.wiggle = q.wiggle; p.angle0 = q.angle;
-      p.follow_dist = q.follow_dist; p.velocity = q.velocity; p.gain = q.gain; p.trim = q.trim; p.radius = q.radius;
-      p.k = q.k; p.limit = q.limit; p.wheel_dist = q.wheel_dist; p.robot_width = q.robot_width; p.robot_length = q.robot_length;
-      double f[DTS_DYN_FIELDS] = {};
-      f[DTS_DYN_PX] = q.pos[0]; f[DTS_DYN_PZ] = q.pos[2]; f[DTS_DYN_ANGLE] = q.angle;
-      f[DTS_DYN_YROT] = q.angle * (180.0 / 3.14159265358979323846);       // np.rad2deg O:57
-      for (int k = 0; k < 4; k++) { f[DTS_DYN_CORNERS + 2 * k] = q.corners[k][0]; f[DTS_DYN_CORNERS + 2 * k + 1] = q.corners[k][1]; }
-      f[DTS_DYN_START_X] = q.pos[0]; f[DTS_DYN_START_Z] = q.pos[2];
-      f[DTS_DYN_WAIT] = q.wait_time; f[DTS_DYN_VEL] = q.vel; f[DTS_DYN_TIME] = 0.0; f[DTS_DYN_ACTIVE] = 0.0;
-      p.freq = q.freq; p.tl_first = -1; p.pad = 0;
-      if (q.kind == DTS_DYN_TRAFFICLIGHT) f[DTS_DYN_PATTERN] = q.pattern ? 1.0 : 0.0;
-      for (int k = 0; k < DTS_DYN_FIELDS; k++)
-        for (size_t e = 0; e < N; e++) st[((size_t)k * D + s) * N + e] = f[k];
-    }
-    int tl_first = -1, tl_last = -1;
-    for (size_t s = 0; s < D; s++)
-      if (par[s].kind == DTS_DYN_TRAFFICLIGHT) { if (tl_first < 0) tl_first = (int)s; tl_last = (int)s; }
-    for (size_t s = 0; s < D; s++) par[s].tl_first = tl_first;
-    if (tl_first >= 0)   // every constructor assigns the shared mesh's card (O:453): the last light's pattern shows
-      for (size_t e = 0; e < N; e++) st[((size_t)DTS_DYN_SHOWN * D + tl_first) * N + e] = b->dyn[tl_last].pattern ? 1.0 : 0.0;
-    bad |= sim->upload(&m.dyn, par.data(), par.size(), &own);
-    const double* dst = nullptr;
-    bad |= sim->upload(&dst, st.data(), st.size(), &own);
-    m.dyn_state = const_cast<double*>(dst);
-    std::vector<double> init((size_t)DTS_DYN_FIELDS * D);
-    for (int k = 0; k < DTS_DYN_FIELDS; k++)
-      for (size_t s = 0; s < D; s++) init[(size_t)k * D + s] = N ? st[((size_t)k * D + s) * N] : 0.0;
-    bad |= sim->upload(&m.dyn_init, init.data(), init.size(), &own);
-  }
-  if (bad) {
-    DMap empty{};
-    cudaMemcpy(sim->d_maps + map_id, &empty, sizeof(DMap), cudaMemcpyHostToDevice);
-    return 1;
-  }
-  m.valid = 1;
+  const std::string e = maps_upload(*sim->maps, map_id, b);
+  if (!e.empty()) return sim->fail("%s", e.c_str());
   renderer_release_frame(*sim->render);
-  sim->h_maps[map_id] = m;
-  DTS_CUDA(cudaMemcpy(sim->d_maps + map_id, &m, sizeof(DMap), cudaMemcpyHostToDevice));
   return 0;
 }
 
@@ -452,10 +243,10 @@ int dts_set_rectify_lut(dts_sim* sim, const float* mapx, const float* mapy, int 
 static int map_select(const dts_sim* sim) { return sim->cfg.random_maps > 0 ? -sim->cfg.random_maps : sim->cfg.cycle_maps; }
 
 static int check_maps(dts_sim* sim) {
-  if (!sim->h_maps[0].valid) return sim->fail("no map uploaded in slot 0");
+  if (!maps_get(*sim->maps, 0)) return sim->fail("no map uploaded in slot 0");
   const int cyc = sim->cfg.cycle_maps > sim->cfg.random_maps ? sim->cfg.cycle_maps : sim->cfg.random_maps;
   for (int k = 0; k < cyc; k++)
-    if (k >= sim->cfg.max_maps || !sim->h_maps[k].valid) return sim->fail("cycle_maps / random_maps = %d but slot %d is empty", cyc, k);
+    if (!maps_get(*sim->maps, k)) return sim->fail("cycle_maps / random_maps = %d but slot %d is empty", cyc, k);
   return 0;
 }
 
@@ -471,7 +262,7 @@ int dts_reset(dts_sim* sim, const uint8_t* mask_dev, const dts_episode_params* p
   if (!p) p = &z;
   if (p->map_id) {
     for (size_t e = 0; e < n; e++)
-      if (p->map_id[e] < 0 || p->map_id[e] >= sim->cfg.max_maps || !sim->h_maps[p->map_id[e]].valid)
+      if (!maps_get(*sim->maps, p->map_id[e]))
         return sim->fail("episode map_id[%zu]=%d has no uploaded map", e, p->map_id[e]);
   }
 #define STAGE(field, dst, cnt)                                                                         \
@@ -484,7 +275,7 @@ int dts_reset(dts_sim* sim, const uint8_t* mask_dev, const dts_episode_params* p
   STAGE(light_diffuse, sg.f3[3], 3 * n) STAGE(ground_color, sg.f3[4], 3 * n)
   STAGE(light_pos, sg.light_pos, 4 * n) STAGE(light_stale, sg.light_stale, n) STAGE(obj_hidden, sg.hidden, 8 * n)
 #undef STAGE
-  launch_reset_params(sim->S, sim->d_maps, sim->step_cfg, mask_dev, rs, st);
+  launch_reset_params(sim->S, maps_table(*sim->maps), sim->step_cfg, mask_dev, rs, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   // the staging buffers are pageable-host copies: make them safe to reuse before returning
@@ -513,7 +304,7 @@ int dts_reset_random(dts_sim* sim, const uint8_t* mask_dev, void* stream) {
   if (check_maps(sim)) return 1;
   if (!sim->seeded) return sim->fail("dts_seed_streams must be called before a device-side reset");
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  launch_reset_random(sim->S, sim->d_maps, sim->step_cfg, map_select(sim), mask_dev, (cudaStream_t)stream);
+  launch_reset_random(sim->S, maps_table(*sim->maps), sim->step_cfg, map_select(sim), mask_dev, (cudaStream_t)stream);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   return 0;
@@ -524,7 +315,7 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
   if (!obs_dev) return sim->fail("obs_dev is NULL");
   if (check_maps(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  const std::string e = renderer_prepare(*sim->render, sim->h_maps.data(), (int)sim->h_maps.size(), sim->render_mode);
+  const std::string e = renderer_prepare(*sim->render, maps_counts(*sim->maps), sim->render_mode);
   if (!e.empty()) return sim->fail("%s", e.c_str());
   RenderCfg rc{sim->cfg.cam_width, sim->cfg.cam_height, sim->cfg.flags, sim->cfg.num_envs,
                (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->render_mode,
@@ -554,7 +345,7 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
       gt.base[p] = reinterpret_cast<uint8_t*>(sim->gather_peer[p]) + (uint64_t)sim->gather_rank * sim->gather_bytes;
     sim->gather_next = false;
   }
-  int k = launch_render(*sim->render, sim->S, sim->d_maps, rc, target, gt, sim->d_err, sim->d_status, marks, mark_level,
+  int k = launch_render(*sim->render, sim->S, maps_table(*sim->maps), rc, target, gt, sim->d_err, sim->d_status, marks, mark_level,
                         (cudaStream_t)stream);
   if (rz.ow) {
     launch_resize(*sim->resize, rz.staging, obs_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, env_list, env_count,
@@ -587,14 +378,14 @@ int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, voi
   // 1. the step with the respawn held back: k_step_logic's only use of DTS_FLAG_AUTO_RESET is that respawn
   StepCfg deferred = sim->step_cfg;
   deferred.flags &= ~DTS_FLAG_AUTO_RESET;
-  launch_step_logic(sim->S, sim->d_maps, deferred, map_select(sim), actions_dev, reward_dev, done_dev, st);
+  launch_step_logic(sim->S, maps_table(*sim->maps), deferred, map_select(sim), actions_dev, reward_dev, done_dev, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   // 2. every env's frame of the state the step left: the terminal frame where the episode ended
   if (obs_dev && render_pass(sim, obs_dev, stream, nullptr, nullptr)) return 1;
   // 3. the ended envs respawn, in the same order of draws as inside k_step_logic, and are listed
   DTS_CUDA(cudaMemsetAsync(sim->n_ended, 0, sizeof(int32_t), st));
-  launch_respawn_ended(sim->S, sim->d_maps, sim->step_cfg, map_select(sim), sim->ended, sim->n_ended, st);
+  launch_respawn_ended(sim->S, maps_table(*sim->maps), sim->step_cfg, map_select(sim), sim->ended, sim->n_ended, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   if (!obs_dev) return 0;
@@ -616,7 +407,7 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   if ((sim->cfg.flags & DTS_FLAG_AUTO_RESET) && !sim->seeded)
     return sim->fail("auto-reset needs seeded streams: call dts_seed_streams first");
-  launch_step_logic(sim->S, sim->d_maps, sim->step_cfg, map_select(sim), actions_dev, reward_dev, done_dev,
+  launch_step_logic(sim->S, maps_table(*sim->maps), sim->step_cfg, map_select(sim), actions_dev, reward_dev, done_dev,
                     (cudaStream_t)stream);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
@@ -637,7 +428,7 @@ int dts_query_poses(dts_sim* sim, int map_id, int dyn_env, int n, const double* 
                     double* out_f64, int32_t* out_i32, void* stream) {
   cudaStream_t qs = (cudaStream_t)stream;   // ordered after the caller's in-flight steps (they move the dynamic obstacles)
   if (!sim) return 1;
-  if (map_id < 0 || map_id >= sim->cfg.max_maps || !sim->h_maps[map_id].valid) return sim->fail("bad map_id %d", map_id);
+  if (!maps_get(*sim->maps, map_id)) return sim->fail("bad map_id %d", map_id);
   if (dyn_env >= sim->cfg.num_envs) return sim->fail("dyn_env %d out of range", dyn_env);
   if (n <= 0) return 0;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
@@ -652,7 +443,7 @@ int dts_query_poses(dts_sim* sim, int map_id, int dyn_env, int n, const double* 
   }
   DTS_CUDA(cudaMemcpyAsync(sim->q_in, query, (size_t)n * 32, cudaMemcpyHostToDevice, qs));
   if (hidden) DTS_CUDA(cudaMemcpyAsync(sim->q_hidden, hidden, (size_t)n * 32, cudaMemcpyHostToDevice, qs));
-  launch_query(sim->d_maps, map_id, dyn_env < 0 ? -1 : dyn_env, sim->cfg.num_envs, n, sim->q_in, hidden ? sim->q_hidden : nullptr, sim->q_outd, sim->q_outi, qs);
+  launch_query(maps_table(*sim->maps), map_id, dyn_env < 0 ? -1 : dyn_env, sim->cfg.num_envs, n, sim->q_in, hidden ? sim->q_hidden : nullptr, sim->q_outd, sim->q_outi, qs);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   DTS_CUDA(cudaMemcpyAsync(out_f64, sim->q_outd, (size_t)n * 32, cudaMemcpyDeviceToHost, qs));
@@ -666,12 +457,12 @@ int dts_assign_maps(dts_sim* sim, const uint8_t* mask_dev, const int32_t* map_id
   if (!map_id_host) return sim->fail("map_id_host is NULL");
   const size_t n = sim->cfg.num_envs;
   for (size_t e = 0; e < n; e++)
-    if (map_id_host[e] < 0 || map_id_host[e] >= sim->cfg.max_maps || !sim->h_maps[map_id_host[e]].valid)
+    if (!maps_get(*sim->maps, map_id_host[e]))
       return sim->fail("dts_assign_maps: map_id[%zu]=%d has no uploaded map", e, map_id_host[e]);
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   DTS_CUDA(cudaMemcpyAsync(sim->stage.map_id, map_id_host, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  launch_assign_maps(sim->S, sim->d_maps, mask_dev, sim->stage.map_id, st);
+  launch_assign_maps(sim->S, maps_table(*sim->maps), mask_dev, sim->stage.map_id, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   DTS_CUDA(cudaStreamSynchronize(st));   // pageable host source
@@ -819,9 +610,10 @@ int dts_set_output_format(dts_sim* sim, const dts_output_format* f) {
 
 int dts_get_dyn_state(dts_sim* sim, int map_id, double** state_dev, int32_t* n_dyn) {
   if (!sim) return 1;
-  if (map_id < 0 || map_id >= sim->cfg.max_maps || !sim->h_maps[map_id].valid) return sim->fail("bad map_id %d", map_id);
-  if (state_dev) *state_dev = sim->h_maps[map_id].n_dyn ? sim->h_maps[map_id].dyn_state : nullptr;
-  if (n_dyn) *n_dyn = sim->h_maps[map_id].n_dyn;
+  const DMap* m = maps_get(*sim->maps, map_id);
+  if (!m) return sim->fail("bad map_id %d", map_id);
+  if (state_dev) *state_dev = m->n_dyn ? m->dyn_state : nullptr;
+  if (n_dyn) *n_dyn = m->n_dyn;
   return 0;
 }
 

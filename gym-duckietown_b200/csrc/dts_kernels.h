@@ -1,6 +1,7 @@
 // dts_kernels.h — host-callable launchers of the dtsim kernels.
 #pragma once
 #include <string>
+#include <vector>
 
 #include "dts_common.cuh"
 
@@ -57,15 +58,31 @@ struct GatherTab {
   uint8_t* base[DTS_MAX_PEERS];
 };
 
+// maps (dts_maps.cu).  The map slots of one handle (dts_upload_map): each slot's DMap, on the host and in the device
+// table the kernels index by S.map_id, and the device memory behind it.
+struct MapSlots;
+// What frame memory is sized from: road tiles, placed objects, and the triangles of the placed meshes and the agent's
+// mesh (all zero: an empty slot)
+struct MapCounts { int n_tiles, n_objects; long long n_tris; };
+MapSlots* maps_create(const dts_config& cfg);   // cfg.max_maps empty slots on the current device; null if out of memory
+void maps_destroy(MapSlots* m);
+// The blob `b` into `slot`, synchronising the device.  Returns the error text, empty on success.  The whole blob is
+// checked and the new map's device memory filled before the slot changes: a refusal or a failed allocation leaves the
+// slot, on the host and on the device, as it was.
+std::string maps_upload(MapSlots& m, int slot, const dts_map_blob* b);
+const DMap* maps_table(const MapSlots& m);           // device [max_maps]
+const DMap* maps_get(const MapSlots& m, int slot);   // the slot's host record; null if out of range or empty
+const std::vector<MapCounts>& maps_counts(const MapSlots& m);   // [max_maps]
+
 // render (dts_render.cu).  The renderer of one handle: the launch sizes, the frame memory, sized from the uploaded maps,
 // and the fisheye tables.  Functions that can fail return the error text, empty on success.
 struct Renderer;
 Renderer* renderer_create(const dts_config& cfg);   // on cfg.device, which must be current
 void renderer_destroy(Renderer* r);
 void renderer_release_frame(Renderer& r);   // the maps changed: the next render re-sizes frame memory for them
-// Before every render: reserves frame memory for the valid maps of maps[0 .. n_maps) unless it is reserved, and checks
-// that a fisheye LUT is set if the camera needs one and a rectification LUT if render `mode` asks for it.
-std::string renderer_prepare(Renderer& r, const DMap* maps, int n_maps, int mode);
+// Before every render: reserves frame memory for the maps of `counts` unless it is reserved, and checks that a fisheye
+// LUT is set if the camera needs one and a rectification LUT if render `mode` asks for it.
+std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode);
 // The fused gather's tables for a LUT of the camera's size (obs[y, x] = frame[rint(rmapy), rint(rmapx)]), in the fisheye
 // slot or (`rectify`) the rectification slot; they replace that slot's previous ones, so no render may be in flight.  A
 // LUT the rasteriser cannot take leaves the previous tables; NULL maps free the slot.

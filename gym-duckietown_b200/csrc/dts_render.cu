@@ -2165,24 +2165,21 @@ void renderer_destroy(Renderer* r) {
   delete r;
 }
 
-std::string renderer_prepare(Renderer& r, const DMap* maps, int n_maps, int mode) {
+std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode) {
   if (!r.frame) {
     // prims k_geometry emits per road tile: the literal triangles of tile mode 0, or the quad of tile mode 1, which a
     // clip splits into two triangles and fans into a few more
     const int tile_prims = (r.flags & DTS_FLAG_TESSELLATE) ? kTessTris : 6;
-    int max_tris = 2, max_lat = 1, items_max = 1;
-    for (int i = 0; i < n_maps; i++) {
-      const DMap& m = maps[i];
-      if (!m.valid) continue;
-      int t = 2 + tile_prims * m.n_tiles + m.agent.tri_count;   // the ground quad's two triangles, the tiles, the meshes
-      std::vector<DObject> objs(m.n_objects);
-      if (m.n_objects) cudaMemcpy(objs.data(), m.objects, sizeof(DObject) * m.n_objects, cudaMemcpyDeviceToHost);
-      for (const DObject& o : objs) t += o.tri_count;
+    long long max_tris = 2;
+    int max_lat = 1, items_max = 1;
+    for (const MapCounts& m : counts) {
+      if (!m.n_tiles) continue;   // an empty slot
+      const long long t = 2 + (long long)tile_prims * m.n_tiles + m.n_tris;   // the ground quad's two triangles, the tiles, the meshes
       max_tris = std::max(max_tris, t);
       max_lat = std::max(max_lat, m.n_tiles);
       items_max = std::max(items_max, agent_item(m.n_tiles, m.n_objects) + 1);
     }
-    const int max_prims = max_tris + max_tris / 4 + 64;   // clipping can add fan triangles
+    const long long max_prims = max_tris + max_tris / 4 + 64;   // clipping can add fan triangles
     if (items_max > 65535) return "scene too large: " + std::to_string(items_max) + " draw items per frame (limit 65535)";
     if (max_prims > 65535) return "scene too large: " + std::to_string(max_prims) + " triangles per frame (limit 65535)";
     // (prim, coarse bin) pairs k_bin emits per env at most: the ground fan (<= 8 x cbins), a few screen-filling tiles
@@ -2194,7 +2191,7 @@ std::string renderer_prepare(Renderer& r, const DMap* maps, int n_maps, int mode
     if (const char* e = getenv("DTS_PAIR_POOL_GB")) pool_gb = atof(e) > 0 ? atof(e) : pool_gb;
     const long long cap = (long long)(pool_gb * 1073741824.0 / (double)(sizeof(uint32_t) + sizeof(BinRec)));
     const long long pool = std::max(std::min({per_env * r.n, cap, 2000000000LL}), per_env);
-    r.max_prims = max_prims; r.max_lat = max_lat; r.items_max = items_max; r.pool = (int)pool;
+    r.max_prims = (int)max_prims; r.max_lat = max_lat; r.items_max = items_max; r.pool = (int)pool;
     const size_t bytes = carve(r, 0, r.fm);
     const cudaError_t e = cudaMalloc(&r.frame, bytes);
     if (e != cudaSuccess) {

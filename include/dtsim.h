@@ -235,7 +235,11 @@ typedef struct {
 
 /* Simulator.__init__ (simulator.py:207-384) minus map loading. */
 int dts_create(const dts_config* cfg, dts_sim** out);
-/* Simulator._load_map/_interpret_map/_load_objects (simulator.py:765-931) : device copy of one map. */
+/* Simulator._load_map/_interpret_map/_load_objects (simulator.py:765-931) : device copy of one map into slot map_id
+ * (< max_maps), in place of the slot's previous map; synchronises the device.  The whole blob is checked, and the new
+ * map's device memory allocated and filled, before the slot changes: a refused blob or a failed allocation returns
+ * nonzero and leaves the slot as it was, its previous map (or none) still in effect.  A successful upload re-creates
+ * the map's dynamic obstacles for every env, and the next render re-sizes frame memory for the new set of maps. */
 int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* blob);
 /* Distortion.rmapx/rmapy (distortion.py:85-125): LUT of the fused fisheye gather, [H][W] each (HOST pointers).  The
  * rasteriser renders every output pixel AT the source position rint(rmap) names — obs[y,x] = undistorted[rint(rmapy),

@@ -391,6 +391,72 @@ def test_upload_map_resizes_frame_memory(torch_cuda):
     env.close()
 
 
+def _texture(h, w, hgt, backed):
+    """Texture 0 of the blob becomes w x hgt; `backed`: over a zeroed buffer of that size, else over the old texels."""
+    from gym_duckietown_b200 import lib as L
+    texs = h.keep["texs"]
+    if backed:
+        h.keep["big"] = np.zeros((hgt, w, 4), np.uint8)
+    texs[0] = L.Texture(w, hgt, h.keep["big"].ctypes.data if backed else texs[0].rgba)
+
+
+def _set(arr, i, **kw):
+    for k, v in kw.items():
+        setattr(arr[i], k, v)
+
+
+# Every refusal of dts_upload_map, on a fresh blob of loop_pedestrians (6 objects, the first 4 of them the pedestrians
+# of dyn slots 0-3; 2 meshes of 148 and 72 triangles; 8 textures): (slot, corruption, the error it gets)
+REFUSED_UPLOADS = {
+    "map_id": (2, lambda h: None, "bad map_id 2"),
+    "too_many_objects": (0, lambda h: setattr(h.blob, "n_objects", 257), "map has 257 objects, limit 256"),
+    "bad_grid": (0, lambda h: setattr(h.blob, "grid_w", 0), "invalid tile grid"),
+    "n_dyn": (0, lambda h: setattr(h.blob, "n_dyn", 33), "map has 33 dynamic obstacles, limit 32"),
+    "mesh_id": (0, lambda h: _set(h.keep["objs"], 5, mesh_id=2), "object 5: bad mesh_id"),
+    "alt_texture": (0, lambda h: _set(h.keep["objs"], 5, alt_tex_to=h.blob.n_textures), "object 5: alt texture out of range"),
+    "dyn_slot": (0, lambda h: _set(h.keep["objs"], 4, dyn_slot=4), "object 4: dyn_slot 4 out of range"),
+    "not_power_of_two": (0, lambda h: _texture(h, 255, 256, False), "texture 0: 255x256 is not a power of two"),
+    "side_over_2^15": (0, lambda h: _texture(h, 65536, 1, True), "texture 0: 65536x1 too large"),
+    "pool_over_4GB": (0, lambda h: _texture(h, 32768, 32768, False), "textures exceed 4 GB"),
+    "mesh_past_n_tris": (0, lambda h: _set(h.keep["meshes"], 1, tri_count=73), "mesh 1: triangles 148 .. 221 past n_tris 220"),
+    "dyn_kind": (0, lambda h: _set(h.keep["dyn"], 0, kind=9), "dyn 0: bad kind 9"),
+    "dyn_back_pointer": (0, lambda h: _set(h.keep["dyn"], 0, object_index=4),
+                         "dyn 0: object_index 4 does not point back to this slot"),
+}
+
+
+@pytest.mark.parametrize("case", list(REFUSED_UPLOADS))
+def test_refused_upload_leaves_the_slot_as_it_was(case, torch_cuda):
+    """A blob dts_upload_map refuses changes nothing: slot 0 keeps its map on the host and the device, the next frames
+    are the frames before it, bit for bit and equal to the oracle's, and the batch still steps."""
+    import ctypes as C
+    torch = torch_cuda
+    import oracle as orc
+    from gym_duckietown_b200 import lib as L, maps
+    md = maps.load_map("loop_pedestrians")
+    n = 128
+    P = poses_for(md, np.random.default_rng(17), n)
+    env = make_env(["loop_pedestrians", "loop_pedestrians"], n)
+    place(env, np.zeros(n, np.int32), P[:, 0].copy(), P[:, 1].copy(), P[:, 2].copy())
+    before = env.render_obs().clone()
+    slot, corrupt, message = REFUSED_UPLOADS[case]
+    holder = L.MapBlobHolder(md)
+    corrupt(holder)
+    sim = env.sim
+    assert sim.lib.dts_upload_map(sim.h, slot, C.byref(holder.blob)) != 0
+    assert sim.lib.dts_last_error(sim.h).decode() == message
+    after = env.render_obs()
+    torch.cuda.synchronize()
+    assert torch.equal(after, before), f"{case}: the frames changed"
+    want = oracle_scene(md).render_batch(P[:, 0], P[:, 1], P[:, 2], [orc.default_episode() for _ in range(n)], 160, 120,
+                                         threads=THREADS)
+    assert_exact(after.cpu().numpy(), want, f"refused_{case}")
+    env.check()
+    env.step(torch.zeros(n, 2, device=env.device))
+    env.check()
+    env.close()
+
+
 # -------------------------------------------------------------------------------------- 5. step logic, mixed
 def test_mixed_batch_trajectory_vs_oracle(golden_dir, torch_cuda):
     """test_trajectory_vs_oracle with env k on map k % 5, static and dynamic maps, auto-reset off."""
