@@ -274,6 +274,105 @@ class BatchedDuckietownEnv:
             self.sim.render(tgt.data_ptr(), self._stream())
         return tgt
 
+    # snapshots ----------------------------------------------------------------------------------
+    @property
+    def state_fingerprint(self) -> int:
+        """Identifies the record layout and the maps this env's records refer to (dts_state_info); a map upload
+        changes it."""
+        return self.sim.state_info()[1]
+
+    def save_state(self, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Every env's complete simulator state as one record per env: uint8 [num_envs, record_bytes] on the env's
+        device, written on the current stream without synchronising (dts_save_state).  The tensor's `fingerprint`
+        attribute is `state_fingerprint` at save time; `load_state` checks it."""
+        rb, fp = self.sim.state_info()
+        if out is None:
+            out = torch.empty((self.num_envs, rb), dtype=torch.uint8, device=self.device)
+        else:
+            self._check_records(out, "out")
+        self.sim.save_state(out.data_ptr(), self._stream())
+        out.fingerprint = fp
+        return out
+
+    def _check_records(self, records: torch.Tensor, what: str):
+        rb = self.sim.state_info()[0]
+        if not isinstance(records, torch.Tensor) or records.device != self.device or records.dtype != torch.uint8 \
+                or tuple(records.shape) != (self.num_envs, rb) or not records.is_contiguous():
+            raise ValueError(f"{what} must be a contiguous uint8 tensor [num_envs, {rb}] on {self.device}")
+
+    def load_state(self, records: torch.Tensor, mask: Optional[torch.Tensor] = None, fingerprint: Optional[int] = None):
+        """Env e (every env, or those where `mask` is true) takes record e of `records` as its complete state
+        (dts_load_state), on the current stream without synchronising.  `fingerprint` defaults to the one `save_state`
+        attached to `records`; one that is not this env's `state_fingerprint` (other maps, a map re-uploaded since)
+        raises and changes nothing.  `render_obs()` then draws the loaded state; `self.obs` is left as it was.  Only
+        the device state is loaded: `load_state_dict` / `copy_envs` also carry the host-side reset state."""
+        self._check_records(records, "records")
+        if fingerprint is None:
+            fingerprint = getattr(records, "fingerprint", None)
+            if fingerprint is None:
+                raise ValueError("records carry no fingerprint: pass the fingerprint of the env that saved them")
+        mask_ptr = None
+        if mask is not None:
+            if tuple(mask.shape) != (self.num_envs,):
+                raise ValueError("mask must have one entry per env")
+            mask = mask.to(device=self.device, dtype=torch.uint8).contiguous()
+            mask_ptr = mask.data_ptr()
+        self.sim.load_state(mask_ptr, records.data_ptr(), int(fingerprint), self._stream())
+
+    def _host_state(self) -> dict:
+        """The host-side per-env reset state: what host resets draw from (sampler streams, last horizon, reset count)
+        and the map ids host resets assign."""
+        s = self.sampler
+        return dict(rngs=[g.bit_generator.state for g in s.rngs], last_horizon=[np.array(h, float) for h in s.last_horizon],
+                    episodes=s.episodes.copy(), map_ids=self.map_ids.copy())
+
+    def _set_host_state(self, h: dict, envs, src):
+        s = self.sampler
+        for e, k in zip(envs, src):
+            s.rngs[e].bit_generator.state = h["rngs"][k]
+            s.last_horizon[e] = np.array(h["last_horizon"][k], float)
+            s.episodes[e] = h["episodes"][k]
+            self.map_ids[e] = h["map_ids"][k]
+
+    def copy_envs(self, src) -> None:
+        """Env e becomes a copy of env src[e] as it was before the call; src[e] = -1 keeps env e.  `src` is int64
+        [num_envs].  On the device this is `load_state(save_state()[src], src >= 0)`; the host-side reset state is
+        copied too, so envs under host resets branch correctly."""
+        src = torch.as_tensor(src, dtype=torch.int64)
+        if tuple(src.shape) != (self.num_envs,):
+            raise ValueError("src must have one entry per env")
+        src_h = src.cpu().numpy()
+        if ((src_h < -1) | (src_h >= self.num_envs)).any():
+            raise ValueError("src entries must be -1 or an env index")
+        src_d = src.to(self.device)
+        recs = self.save_state()
+        gathered = recs[src_d.clamp(min=0)]
+        self.load_state(gathered, mask=src_d >= 0, fingerprint=recs.fingerprint)
+        envs = np.flatnonzero(src_h >= 0)
+        self._set_host_state(self._host_state(), envs, src_h[envs])
+
+    def state_dict(self) -> dict:
+        """Everything needed to continue this batch elsewhere: every env's record (on the CPU), its fingerprint and the
+        host-side reset state, in types `torch.save` / `torch.load` round-trip.  Synchronises.  Load it into an env
+        built with the same keywords (`load_state_dict`)."""
+        h = self._host_state()
+        recs = self.save_state()
+        return {"records": recs.cpu(), "fingerprint": int(recs.fingerprint), "rngs": h["rngs"],
+                "last_horizon": torch.from_numpy(np.stack(h["last_horizon"])),
+                "episodes": torch.from_numpy(h["episodes"]), "map_ids": torch.from_numpy(h["map_ids"]),
+                "first_reset": bool(self._first_reset)}
+
+    def load_state_dict(self, d: dict) -> None:
+        """Continue from `state_dict()`: every env's device and host state.  A fingerprint from other maps raises and
+        changes nothing."""
+        recs = d["records"].to(self.device).contiguous()
+        self.load_state(recs, fingerprint=int(d["fingerprint"]))
+        h = dict(rngs=d["rngs"], last_horizon=list(d["last_horizon"].numpy()), episodes=d["episodes"].numpy(),
+                 map_ids=d["map_ids"].numpy())
+        envs = np.arange(self.num_envs)
+        self._set_host_state(h, envs, envs)
+        self._first_reset = bool(d["first_reset"])
+
     # convenience views --------------------------------------------------------------------------
     @property
     def cur_pos(self) -> torch.Tensor:

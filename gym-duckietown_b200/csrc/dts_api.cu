@@ -32,8 +32,10 @@ struct dts_sim {
   MapSlots* maps = nullptr;             // the uploaded maps (dts_upload_map)
   Renderer* render = nullptr;           // frame memory and fisheye tables
   Resizer* resize = nullptr;            // the post-render ResizeWrapper (dts_set_resize_filter)
+  StateRecords* state = nullptr;        // the snapshot record layout (dts_save_state / dts_load_state)
   int32_t* d_err = nullptr;
-  int32_t* h_status = nullptr;          // mapped pinned host word: bit 0 = a frame overflowed its frame memory
+  int32_t* h_status = nullptr;          // mapped pinned host words: [0] a frame overflowed its frame memory,
+                                        // [1] dts_load_state met a record naming no uploaded map
   int32_t* d_status = nullptr;          // its device address
   int32_t* ended = nullptr;             // dts_step_terminal: [N] the envs whose episode ended this step, *n_ended of them
   int32_t* n_ended = nullptr;
@@ -183,6 +185,11 @@ int dts_create(const dts_config* cfg, dts_sim** out) {
   bad |= sim->dalloc(&st.hidden, 8 * (size_t)n);
   sim->render = renderer_create(*cfg);
   sim->resize = resizer_create(*cfg);
+  if (!(sim->state = state_create(*cfg))) bad |= sim->fail("cudaMalloc(state record layout) failed");
+  else if (!bad) {
+    const std::string e = state_layout(*sim->state, S, *sim->maps);
+    if (!e.empty()) bad |= sim->fail("%s", e.c_str());
+  }
   if (bad) { g_create_error = sim->err; dts_destroy(sim); return 1; }
   *out = sim;
   return 0;
@@ -196,6 +203,7 @@ void dts_destroy(dts_sim* sim) {
   maps_destroy(sim->maps);
   renderer_destroy(sim->render);
   resizer_destroy(sim->resize);
+  state_destroy(sim->state);
   void* extra[] = {sim->q_in, sim->q_outd, sim->q_outi, sim->q_hidden};
   for (void* p : extra) if (p) cudaFree(p);
   for (int p = 0; p < sim->gather_world; p++)
@@ -212,7 +220,9 @@ int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
   const std::string e = maps_upload(*sim->maps, map_id, b);
   if (!e.empty()) return sim->fail("%s", e.c_str());
   renderer_release_frame(*sim->render);
-  return 0;
+  // the records now cover this map's obstacles, and the fingerprint its content: older records no longer load
+  const std::string ls = state_layout(*sim->state, sim->S, *sim->maps);
+  return ls.empty() ? 0 : sim->fail("%s", ls.c_str());
 }
 
 int dts_set_fisheye_lut(dts_sim* sim, const float* rmapx, const float* rmapy, int width, int height) {
@@ -241,6 +251,13 @@ int dts_set_rectify_lut(dts_sim* sim, const float* mapx, const float* mapy, int 
 
 // > 0: round-robin over that many slots; < 0: uniform draw over -n slots; 0: the env keeps its map
 static int map_select(const dts_sim* sim) { return sim->cfg.random_maps > 0 ? -sim->cfg.random_maps : sim->cfg.cycle_maps; }
+
+// status bit 1: a dts_load_state was handed a record naming no uploaded map (that env kept its state)
+static int check_loaded(dts_sim* sim) {
+  if (((volatile int32_t*)sim->h_status)[1])
+    return sim->fail("an earlier dts_load_state met a record whose map_id names no uploaded map; that env was not loaded");
+  return 0;
+}
 
 static int check_maps(dts_sim* sim) {
   if (!maps_get(*sim->maps, 0)) return sim->fail("no map uploaded in slot 0");
@@ -322,6 +339,7 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
                env_list, env_count};
   if (*(volatile int32_t*)sim->h_status & 1)
     return sim->fail("an earlier frame overflowed its render frame memory (prim slab / bin lists) and was left incomplete");
+  if (check_loaded(sim)) return 1;
   cudaEvent_t* marks = nullptr;
   if (sim->profiling && !env_list) {
     const size_t base = sim->prof_events.size();
@@ -371,7 +389,7 @@ int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, voi
   if (obs_dev && !terminal_obs_dev) return sim->fail("terminal_obs_dev is NULL");
   if (obs_dev && terminal_obs_dev == obs_dev) return sim->fail("terminal_obs_dev must be a buffer of its own, not obs_dev");
   if (sim->gather_next) return sim->fail("a fused gather is armed (dts_gather_next): dts_step_terminal does not write it");
-  if (check_maps(sim)) return 1;
+  if (check_maps(sim) || check_loaded(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   if (!sim->seeded) return sim->fail("auto-reset needs seeded streams: call dts_seed_streams first");
   cudaStream_t st = (cudaStream_t)stream;
@@ -403,7 +421,7 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
              void* stream) {
   if (!sim) return 1;
   if (!actions_dev) return sim->fail("actions_dev is NULL");
-  if (check_maps(sim)) return 1;
+  if (check_maps(sim) || check_loaded(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   if ((sim->cfg.flags & DTS_FLAG_AUTO_RESET) && !sim->seeded)
     return sim->fail("auto-reset needs seeded streams: call dts_seed_streams first");
@@ -565,7 +583,49 @@ int dts_resize_frames(dts_sim* sim, const uint8_t* src_dev, void* dst_dev, void*
   return 0;
 }
 
-int dts_status(dts_sim* sim) { return (sim && sim->h_status) ? *(volatile int32_t*)sim->h_status : 0; }
+int dts_status(dts_sim* sim) {
+  if (!sim || !sim->h_status) return 0;
+  const volatile int32_t* w = sim->h_status;
+  return (w[0] ? 1 : 0) | (w[1] ? 2 : 0);
+}
+
+// ---- snapshots: every env's state as one record, out of and back into the library's arrays (dts_state.cu) --------
+int dts_state_info(dts_sim* sim, uint64_t* record_bytes, uint64_t* fingerprint) {
+  if (!sim) return 1;
+  if (!state_record_bytes(*sim->state)) return sim->fail("no state record layout: the last map upload could not build it");
+  if (record_bytes) *record_bytes = state_record_bytes(*sim->state);
+  if (fingerprint) *fingerprint = state_fingerprint(*sim->state);
+  return 0;
+}
+
+int dts_save_state(dts_sim* sim, void* records_dev, void* stream) {
+  if (!sim) return 1;
+  if (!records_dev) return sim->fail("records_dev is NULL");
+  if (!state_record_bytes(*sim->state)) return sim->fail("no state record layout: the last map upload could not build it");
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  launch_state_save(*sim->state, records_dev, (cudaStream_t)stream);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int dts_load_state(dts_sim* sim, const uint8_t* mask_dev, const void* records_dev, uint64_t fingerprint, void* stream) {
+  if (!sim) return 1;
+  if (!records_dev) return sim->fail("records_dev is NULL");
+  if (!state_record_bytes(*sim->state)) return sim->fail("no state record layout: the last map upload could not build it");
+  const uint64_t mine = state_fingerprint(*sim->state);
+  if (fingerprint != mine)
+    return sim->fail("record fingerprint %016llx is not this handle's %016llx: the records were saved with other maps "
+                     "(or before a map upload) or another record layout", (unsigned long long)fingerprint,
+                     (unsigned long long)mine);
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  launch_state_load(*sim->state, mask_dev, records_dev, maps_table(*sim->maps), maps_slot_count(*sim->maps),
+                    sim->d_status + 1, (cudaStream_t)stream);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  sim->seeded = true;   // the envs' streams came with their records
+  return 0;
+}
 
 int dts_profile_enable(dts_sim* sim, int on) {
   if (!sim) return 1;

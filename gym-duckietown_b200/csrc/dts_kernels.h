@@ -73,6 +73,26 @@ std::string maps_upload(MapSlots& m, int slot, const dts_map_blob* b);
 const DMap* maps_table(const MapSlots& m);           // device [max_maps]
 const DMap* maps_get(const MapSlots& m, int slot);   // the slot's host record; null if out of range or empty
 const std::vector<MapCounts>& maps_counts(const MapSlots& m);   // [max_maps]
+int maps_slot_count(const MapSlots& m);                           // max_maps
+// Content hash of the blob the slot's map was built from (never 0); 0 for an empty slot
+uint64_t maps_hash(const MapSlots& m, int slot);
+
+// snapshots (dts_state.cu).  The record layout of one handle: which device arrays make up an env's state, where each
+// lands in the env's record, and the fingerprint of that layout and of the maps it refers to.
+struct StateRecords;
+StateRecords* state_create(const dts_config& cfg);   // on the current device; null if out of memory
+void state_destroy(StateRecords* s);
+// Re-lay the records out for the state `S` and the maps now in `maps` (after creation and after every map upload).
+// Synchronous; no save or load may be in flight.  Returns the error text, empty on success.
+std::string state_layout(StateRecords& s, const DState& S, const MapSlots& maps);
+uint64_t state_record_bytes(const StateRecords& s);   // one env's record, a multiple of 16
+uint64_t state_fingerprint(const StateRecords& s);
+// records u8[n_envs][record_bytes] <- every env's state
+void launch_state_save(const StateRecords& s, void* records, cudaStream_t st);
+// every env e with mask[e] (null: all) whose record names an uploaded map in `maps[0 .. n_maps)` <- record e; an env
+// whose record names none keeps its state, and `refused` (device address of a status word) is set to 1
+void launch_state_load(const StateRecords& s, const uint8_t* mask, const void* records, const DMap* maps, int n_maps,
+                       int32_t* refused, cudaStream_t st);
 
 // render (dts_render.cu).  The renderer of one handle: the launch sizes, the frame memory, sized from the uploaded maps,
 // and the fisheye tables.  Functions that can fail return the error text, empty on success.

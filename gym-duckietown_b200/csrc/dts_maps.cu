@@ -14,6 +14,7 @@ namespace dts {
 struct MapSlot {
   DMap rec{};                   // host copy of the device table's entry (valid = 0: empty)
   std::vector<void*> allocs;    // the device memory behind it
+  uint64_t hash = 0;            // content hash of the blob it was built from (0: empty)
 };
 
 struct MapSlots {
@@ -47,6 +48,71 @@ const DMap* maps_get(const MapSlots& m, int slot) {
 }
 
 const std::vector<MapCounts>& maps_counts(const MapSlots& m) { return m.counts; }
+
+int maps_slot_count(const MapSlots& m) { return (int)m.slots.size(); }
+
+uint64_t maps_hash(const MapSlots& m, int slot) { return maps_get(m, slot) ? m.slots[slot].hash : 0; }
+
+// 64-bit FNV-1a over 8-byte words (the tail byte by byte), with a final avalanche
+namespace {
+struct Hasher {
+  uint64_t h = 0xcbf29ce484222325ull;
+  void bytes(const void* p, size_t n) {
+    const uint8_t* b = static_cast<const uint8_t*>(p);
+    size_t i = 0;
+    for (; i + 8 <= n; i += 8) {
+      uint64_t w;
+      memcpy(&w, b + i, 8);
+      h = (h ^ w) * 0x100000001b3ull;
+    }
+    for (; i < n; i++) h = (h ^ b[i]) * 0x100000001b3ull;
+  }
+  template <typename T> void arr(const T* p, size_t count) {   // the element count, then the contents
+    const uint64_t c = p ? count : 0;
+    bytes(&c, sizeof c);
+    if (p && count) bytes(p, count * sizeof(T));
+  }
+  template <typename T> void val(const T& v) { bytes(&v, sizeof v); }
+  uint64_t done() const {
+    uint64_t z = h;
+    z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+    z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+    z ^= z >> 31;
+    return z ? z : 1;   // 0 stands for an empty slot
+  }
+};
+}  // namespace
+
+// Everything a blob says, pointers aside: two uploads of the same map hash alike, in any process
+static uint64_t blob_hash(const dts_map_blob& b) {
+  Hasher H;
+  const size_t T = (size_t)b.grid_w * b.grid_h;
+  H.val(b.tile_size); H.val(b.grid_w); H.val(b.grid_h);
+  H.arr(b.tile_kind, T); H.arr(b.tile_angle, T); H.arr(b.tile_drivable, T); H.arr(b.tile_tex, T);
+  H.arr(b.tile_curve_off, T); H.arr(b.tile_curve_cnt, T);
+  H.arr(b.curves, (size_t)b.n_curves * 12);
+  H.arr(b.coll_corners, (size_t)b.n_coll * 8); H.arr(b.coll_norms, (size_t)b.n_coll * 4);
+  H.arr(b.coll_centers, (size_t)b.n_coll * 3); H.arr(b.coll_radii, (size_t)b.n_coll);
+  H.val(b.n_objects);
+  for (int o = 0; o < b.n_objects; o++) { dts_object s = b.objects[o]; s.reserved = 0; H.val(s); }
+  H.val(b.n_meshes);
+  for (int i = 0; i < b.n_meshes; i++) { dts_mesh s = b.meshes[i]; s.reserved = 0; H.val(s); }
+  H.arr(b.tri_pos, (size_t)b.n_tris * 9); H.arr(b.tri_nrm, (size_t)b.n_tris * 9); H.arr(b.tri_uv, (size_t)b.n_tris * 6);
+  H.arr(b.tri_col, (size_t)b.n_tris * 9); H.arr(b.tri_tex, (size_t)b.n_tris);
+  H.val(b.n_textures);
+  for (int t = 0; t < b.n_textures; t++) {
+    const dts_texture& s = b.textures[t];
+    H.val(s.width); H.val(s.height);
+    H.arr(s.rgba, (size_t)s.width * s.height * 4);
+  }
+  H.arr(b.tex_segment, b.tex_segment ? (size_t)b.n_textures : 0);
+  H.val(b.start_tile[0]); H.val(b.start_tile[1]); H.val(b.has_start_pose);
+  for (int k = 0; k < 3; k++) H.val(b.start_pose[k]);
+  H.val(b.agent_mesh);
+  H.val(b.n_dyn);
+  for (int s = 0; s < b.n_dyn; s++) { dts_dyn_object q = b.dyn[s]; q.reserved = 0; H.val(q); }
+  return H.done();
+}
 
 static std::string format(const char* fmt, ...) {
   char buf[512];
@@ -269,6 +335,7 @@ std::string maps_upload(MapSlots& ms, int slot, const dts_map_blob* blob) {
   }
   if (err.empty()) {
     fresh.rec = m;
+    fresh.hash = blob_hash(b);
     std::swap(ms.slots[slot], fresh);   // fresh: what to release, the old map or the new one that failed
     ms.counts[slot] = counts;
   }

@@ -189,6 +189,9 @@ def load() -> C.CDLL:
     lib.dts_blend4.argtypes = [vp, vp, vp, vp, C.c_uint64, vp]
     lib.dts_set_timing.argtypes = [vp, C.c_double, i, i]
     lib.dts_status.argtypes = [vp]
+    lib.dts_state_info.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    lib.dts_save_state.argtypes = [vp, vp, vp]
+    lib.dts_load_state.argtypes = [vp, vp, vp, C.c_uint64, vp]
     lib.dts_profile_enable.argtypes = [vp, i]
     lib.dts_profile_read.argtypes = [vp, vp, vp]
     lib.dts_set_output_format.argtypes = [vp, C.POINTER(OutputFormat)]
@@ -216,7 +219,7 @@ def load() -> C.CDLL:
 
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
-           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
+           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
            "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
 
@@ -470,8 +473,23 @@ class Sim:
         self._check(self.lib.dts_set_timing(self.h, float(delta_time), int(frame_skip), int(action_mode)), "dts_set_timing")
 
     def status(self) -> int:
-        """Sticky status bits, read without synchronising (bit 0: a frame overflowed its render frame memory)."""
+        """Sticky status bits, read without synchronising (bit 0: a frame overflowed its render frame memory; bit 1: a
+        load_state met a record naming no uploaded map)."""
         return int(self.lib.dts_status(self.h))
+
+    def state_info(self):
+        """(record_bytes, fingerprint) of this handle's env records (dts_state_info)."""
+        rb, fp = C.c_uint64(), C.c_uint64()
+        self._check(self.lib.dts_state_info(self.h, C.byref(rb), C.byref(fp)), "dts_state_info")
+        return int(rb.value), int(fp.value)
+
+    def save_state(self, records_ptr: int, stream: int = 0):
+        """Every env's record -> device u8[num_envs][record_bytes] at `records_ptr` (dts_save_state)."""
+        self._check(self.lib.dts_save_state(self.h, records_ptr, stream), "dts_save_state")
+
+    def load_state(self, mask_ptr: Optional[int], records_ptr: int, fingerprint: int, stream: int = 0):
+        """The masked envs (all if None) take their records from device `records_ptr` (dts_load_state)."""
+        self._check(self.lib.dts_load_state(self.h, mask_ptr, records_ptr, int(fingerprint), stream), "dts_load_state")
 
     def profile(self, level):
         """0 / False off; 1 / True: CUDA events around k_raster only; 2: around every render kernel."""

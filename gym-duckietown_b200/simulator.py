@@ -89,13 +89,14 @@ class Simulator(Env):
             self.map_names = [m for m in list_maps() if not m.startswith(("calibration", "regress"))]
             map_arg = self.map_names
             env_kwargs = dict(env_kwargs, randomize_maps_on_reset=True)
-        self._b = BatchedDuckietownEnv(
-            1, map_arg, device=device, max_steps=max_steps, domain_rand=domain_rand, frame_rate=frame_rate,
+        self._env_kwargs = dict(
+            device=device, max_steps=max_steps, domain_rand=domain_rand, frame_rate=frame_rate,
             frame_skip=frame_skip, camera_width=camera_width, camera_height=camera_height, robot_speed=robot_speed,
             accept_start_angle_deg=accept_start_angle_deg, user_tile_start=user_tile_start, seed=seed,
             distortion=distortion, dynamics_rand=dynamics_rand, camera_rand=camera_rand,
             color_ground=color_ground, color_sky=color_sky, num_tris_distractors=num_tris_distractors,
             action_mode=self._action_mode, **env_kwargs)
+        self._b = BatchedDuckietownEnv(1, map_arg, **self._env_kwargs)
         self._adopt_map()
         self.action_space = spaces.Box(low=-1, high=1, shape=(2,), dtype=np.float32)              # S:309
         self.observation_space = spaces.Box(low=0, high=255, shape=(camera_height, camera_width, 3), dtype=np.uint8)
@@ -150,30 +151,16 @@ class Simulator(Env):
 
     def _human_view(self):
         """A second 1-env handle at WINDOW_WIDTH x WINDOW_HEIGHT (S:100-101, 340) put into this env's state: what
-        `_render_img(WINDOW_WIDTH, WINDOW_HEIGHT, multi_fbo_human, ...)` draws (S:1988-1996)."""
-        import torch
+        `_render_img(WINDOW_WIDTH, WINDOW_HEIGHT, multi_fbo_human, ...)` draws (S:1988-1996).  It is built with this
+        env's keywords and maps (so its records have the same fingerprint), without the fisheye, and takes this env's
+        whole state as a snapshot."""
         from .batched_env import BatchedDuckietownEnv
         if getattr(self, "_human", None) is None:
-            self._human = BatchedDuckietownEnv(1, list(self._b.maps), device=self._b.device_index, camera_width=WINDOW_WIDTH,
-                                               camera_height=WINDOW_HEIGHT, domain_rand=self.domain_rand, seed=0,
-                                               max_steps=self.max_steps)
-        h, b = self._human, self._b
-        ep, st = b.sim.debug_episode(0), self._scalars()
-        mid = self._map_index()
-        one = lambda v, dt: np.asarray([v], dtype=dt)
-        h.sim.reset(None, dict(
-            map_id=one(mid, np.int32), pos_x=one(st["pos_x"], np.float64), pos_z=one(st["pos_z"], np.float64),
-            angle=one(st["angle"], np.float64), wheel_dist=one(st["wheel_dist"], np.float64),
-            cam_height=one(ep["cam_height"], np.float32), cam_angle_deg=one(ep["cam_angle_deg"], np.float32),
-            cam_fov_y_deg=one(ep["cam_fov_y_deg"], np.float32), cam_noise=ep["cam_noise"][None].astype(np.float32),
-            horizon_color=ep["horizon"][None], light_ambient=ep["ambient"][None], light_diffuse=ep["diffuse"][None],
-            light_pos=ep["light_eye"][None], light_stale=one(0, np.int32), ground_color=ep["ground"][None],
-            obj_hidden=ep["hidden"][None].astype(np.uint32)), h._stream())
-        src, nd = b.sim.dyn_state(mid)
-        if nd:   # the obstacles where this env has them
-            dst, _ = h.sim.dyn_state(mid)
-            torch.as_tensor(dst, device=h.device).copy_(torch.as_tensor(src, device=b.device))
-        return h
+            kw = dict(self._env_kwargs, camera_width=WINDOW_WIDTH, camera_height=WINDOW_HEIGHT, distortion=False,
+                      terminal_obs=False)
+            self._human = BatchedDuckietownEnv(1, list(self._b.maps), **kw)
+        self._human.load_state(self._b.save_state())
+        return self._human
 
     def render(self, mode: str = "human", close: bool = False, segment: bool = False):
         """S:1974-2054.  "rgb_array" / "top_down" return the WINDOW_WIDTH x WINDOW_HEIGHT image; "human" / "free_cam" open a

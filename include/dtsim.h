@@ -343,10 +343,40 @@ int dts_comm_load(dts_sim* sim, const char* libnccl_path);
 int dts_comm_unique_id(dts_sim* sim, uint8_t out[128]);
 int dts_comm_init(dts_sim* sim, const uint8_t id[128], int rank, int world);
 int dts_allgather_obs(dts_sim* sim, const void* send_dev, void* recv_dev, uint64_t bytes_per_rank, void* stream);
-/* Sticky status, readable WITHOUT synchronising (a mapped host word the kernels write): bit 0 = some frame since
- * creation overflowed its render frame memory (prim slab / bin lists) and was left incomplete.  dts_step and
- * dts_render return non-zero once it is set (the frame that overflowed may be one or two calls back). */
+/* Sticky status, readable WITHOUT synchronising (mapped host words the kernels write): bit 0 = some frame since
+ * creation overflowed its render frame memory (prim slab / bin lists) and was left incomplete; bit 1 = a
+ * dts_load_state was handed a record whose map_id names no uploaded map (that env was not loaded).  dts_step and
+ * dts_render return non-zero once either is set (the call that set it may be one or two calls back). */
 int dts_status(dts_sim* sim);
+/* Snapshots: every env's complete simulator state as one record, saved from and loaded into the library's own arrays
+ * on the device, for resuming a run exactly or branching envs from a state.  A record holds everything a step, a reset
+ * or a render reads about its env:
+ *   - the dynamics (cartesian pose cx cy ctheta, velocities vu vw, motor trim) and the command-delay line
+ *     fifo[DTS_MAX_DELAY][2], pending duty cycles included;
+ *   - the simulator-frame pose and the per-step outputs that dts_get_state points to: pos_x pos_z angle speed reward
+ *     lane_dist lane_dot lane_angle_rad prox_penalty wheel_dist step_count tile_i tile_j map_id episode done_code
+ *     in_lane collided;
+ *   - the env's numpy PCG64 stream (as dts_seed_streams takes it);
+ *   - the per-episode render record (camera height / angle / fov and noise, horizon, light, ground colour, hidden
+ *     objects: dts_debug_episode's 144 bytes);
+ *   - for EVERY map slot that has dynamic obstacles, the env's copy of that map's obstacle state (dts_get_dyn_state,
+ *     the traffic lights' shared card included): an env that comes back to a map finds its obstacles where it left them.
+ * Not in a record, because they are not env state: reset staging buffers, frame memory, output buffers and the
+ * handle's configuration (camera size, output format, resize, render mode, timing, flags, frame_rate, DR table).
+ * Loading records into a handle configured differently is the caller's business.
+ *
+ * dts_state_info: record_bytes = one env's record size (a multiple of 16); fingerprint = a hash of the record layout
+ * version, DTS_MAX_DELAY and, per map slot, the content of the map uploaded there (0 for an empty slot).  Any map
+ * upload changes it, so records saved before one no longer load.  Host only. */
+int dts_state_info(dts_sim* sim, uint64_t* record_bytes, uint64_t* fingerprint);
+/* Every env's record -> records_dev, device u8[num_envs][record_bytes].  One launch, stream-ordered, never synchronises. */
+int dts_save_state(dts_sim* sim, void* records_dev, void* stream);
+/* Every env e of mask_dev (device u8[num_envs]; NULL = all) takes record e of records_dev as its complete state.
+ * `fingerprint` is the dts_state_info fingerprint of the handle that saved them: it is checked on the host first, and
+ * on a mismatch nothing is launched, no env changes and the call fails.  A record whose map_id names no uploaded map
+ * is not loaded (the env keeps its state) and sets status bit 1.  One launch, never synchronises.  Device resets are
+ * allowed afterwards, as after dts_seed_streams: the streams came with the records. */
+int dts_load_state(dts_sim* sim, const uint8_t* mask_dev, const void* records_dev, uint64_t fingerprint, void* stream);
 /* Per-kernel device timing of the render launches (bench.py's roofline): when enabled, every dts_render brackets its
  * kernels with CUDA events on the caller's stream.  dts_profile_read synchronises, returns the summed milliseconds of
  * [0] k_frame_setup, [1] k_geometry, [2] k_bin, [3] k_raster, [4] post passes (resize) and the number of frames
