@@ -24,15 +24,11 @@ thread_local std::string g_create_error;
 struct dts_sim {
   dts_config cfg;
   StepCfg step_cfg;
-  DState S;
   std::vector<void*> allocs;           // freed in dts_destroy
-  // reset staging (device) sized num_envs
-  struct { int32_t* map_id; double *pos_x, *pos_z, *angle, *wheel_dist, *trim; float *f1[3]; float *f3[5];
-           float* light_pos; int32_t* light_stale; uint32_t* hidden; } stage{};
+  EnvState* state = nullptr;            // the envs' simulator state, its reset staging and snapshot records
   MapSlots* maps = nullptr;             // the uploaded maps (dts_upload_map)
   Renderer* render = nullptr;           // frame memory and fisheye tables
   Resizer* resize = nullptr;            // the post-render ResizeWrapper (dts_set_resize_filter)
-  StateRecords* state = nullptr;        // the snapshot record layout (dts_save_state / dts_load_state)
   int32_t* d_err = nullptr;
   int32_t* h_status = nullptr;          // mapped pinned host words: [0] a frame overflowed its frame memory,
                                         // [1] dts_load_state met a record naming no uploaded map
@@ -55,7 +51,6 @@ struct dts_sim {
   // nccl (dlopen'ed)
   void* nccl_lib = nullptr; void* nccl_comm = nullptr;
   uint64_t launches = 0;
-  bool seeded = false;
   dts_output_format fmt{DTS_OBS_HWC, DTS_OBS_U8, DTS_REWARD_RAW, DTS_ACTIONS_CONTINUOUS, 1.0};
   std::string err;
 
@@ -151,20 +146,10 @@ int dts_create(const dts_config* cfg, dts_sim** out) {
     c.n_dr_ops = 7;
     for (int k = 0; k < 7; k++) c.dr_ops[k] = def[k];
   }
-  DState& S = sim->S;
-  S.n = n;
   int bad = 0;
-  double** dbl[] = {&S.cx, &S.cy, &S.ctheta, &S.vu, &S.vw, &S.pos_x, &S.pos_z, &S.angle, &S.speed, &S.reward,
-                    &S.lane_dist, &S.lane_dot, &S.lane_angle, &S.prox, &S.wheel_dist, &S.trim};
-  for (auto p : dbl) bad |= sim->dalloc(p, n);
-  bad |= sim->dalloc(&S.fifo, (size_t)DTS_MAX_DELAY * 2 * n);
-  int32_t** i32[] = {&S.step_count, &S.tile_i, &S.tile_j, &S.map_id, &S.episode};
-  for (auto p : i32) bad |= sim->dalloc(p, n);
-  uint8_t** u8[] = {&S.done_code, &S.in_lane, &S.collided};
-  for (auto p : u8) bad |= sim->dalloc(p, n);
-  bad |= sim->dalloc(&S.rng, 6 * (size_t)n);
-  bad |= sim->dalloc(&S.rep, n);
+  std::string se;
   if (!(sim->maps = maps_create(*cfg))) bad |= sim->fail("cudaMalloc(map table of %d slots) failed", cfg->max_maps);
+  else if (!(sim->state = state_create(*cfg, *sim->maps, se))) bad |= sim->fail("%s", se.c_str());
   bad |= sim->dalloc(&sim->d_err, 32);
   bad |= sim->dalloc(&sim->ended, n);
   bad |= sim->dalloc(&sim->n_ended, 1);
@@ -174,22 +159,8 @@ int dts_create(const dts_config* cfg, dts_sim** out) {
   } else {
     memset(sim->h_status, 0, 64);
   }
-  auto& st = sim->stage;
-  bad |= sim->dalloc(&st.map_id, n);
-  double** sd[] = {&st.pos_x, &st.pos_z, &st.angle, &st.wheel_dist, &st.trim};
-  for (auto p : sd) bad |= sim->dalloc(p, n);
-  for (auto& p : st.f1) bad |= sim->dalloc(&p, n);
-  for (auto& p : st.f3) bad |= sim->dalloc(&p, 3 * (size_t)n);
-  bad |= sim->dalloc(&st.light_pos, 4 * (size_t)n);
-  bad |= sim->dalloc(&st.light_stale, n);
-  bad |= sim->dalloc(&st.hidden, 8 * (size_t)n);
   sim->render = renderer_create(*cfg);
   sim->resize = resizer_create(*cfg);
-  if (!(sim->state = state_create(*cfg))) bad |= sim->fail("cudaMalloc(state record layout) failed");
-  else if (!bad) {
-    const std::string e = state_layout(*sim->state, S, *sim->maps);
-    if (!e.empty()) bad |= sim->fail("%s", e.c_str());
-  }
   if (bad) { g_create_error = sim->err; dts_destroy(sim); return 1; }
   *out = sim;
   return 0;
@@ -221,7 +192,7 @@ int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
   if (!e.empty()) return sim->fail("%s", e.c_str());
   renderer_release_frame(*sim->render);
   // the records now cover this map's obstacles, and the fingerprint its content: older records no longer load
-  const std::string ls = state_layout(*sim->state, sim->S, *sim->maps);
+  const std::string ls = state_layout(*sim->state, *sim->maps);
   return ls.empty() ? 0 : sim->fail("%s", ls.c_str());
 }
 
@@ -273,26 +244,16 @@ int dts_reset(dts_sim* sim, const uint8_t* mask_dev, const dts_episode_params* p
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   const size_t n = sim->cfg.num_envs;
-  ResetStaging rs{};
-  auto& sg = sim->stage;
-  dts_episode_params z{};
+  dts_episode_params z{}, dev;
   if (!p) p = &z;
   if (p->map_id) {
     for (size_t e = 0; e < n; e++)
       if (!maps_get(*sim->maps, p->map_id[e]))
         return sim->fail("episode map_id[%zu]=%d has no uploaded map", e, p->map_id[e]);
   }
-#define STAGE(field, dst, cnt)                                                                         \
-  if (p->field) { DTS_CUDA(cudaMemcpyAsync(dst, p->field, (cnt) * sizeof(*p->field), cudaMemcpyHostToDevice, st)); rs.field = dst; }
-  STAGE(map_id, sg.map_id, n)
-  STAGE(pos_x, sg.pos_x, n) STAGE(pos_z, sg.pos_z, n) STAGE(angle, sg.angle, n)
-  STAGE(wheel_dist, sg.wheel_dist, n) STAGE(trim, sg.trim, n)
-  STAGE(cam_height, sg.f1[0], n) STAGE(cam_angle_deg, sg.f1[1], n) STAGE(cam_fov_y_deg, sg.f1[2], n)
-  STAGE(cam_noise, sg.f3[0], 3 * n) STAGE(horizon_color, sg.f3[1], 3 * n) STAGE(light_ambient, sg.f3[2], 3 * n)
-  STAGE(light_diffuse, sg.f3[3], 3 * n) STAGE(ground_color, sg.f3[4], 3 * n)
-  STAGE(light_pos, sg.light_pos, 4 * n) STAGE(light_stale, sg.light_stale, n) STAGE(obj_hidden, sg.hidden, 8 * n)
-#undef STAGE
-  launch_reset_params(sim->S, maps_table(*sim->maps), sim->step_cfg, mask_dev, rs, st);
+  const std::string e = state_stage(*sim->state, *p, dev, st);
+  if (!e.empty()) return sim->fail("%s", e.c_str());
+  launch_reset_params(state_arrays(*sim->state), maps_table(*sim->maps), sim->step_cfg, mask_dev, dev, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   // the staging buffers are pageable-host copies: make them safe to reuse before returning
@@ -304,24 +265,17 @@ int dts_seed_streams(dts_sim* sim, const uint8_t* mask_host, const uint64_t* str
   if (!sim) return 1;
   if (!streams) return sim->fail("streams is NULL");
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  const size_t n = sim->cfg.num_envs;
-  std::vector<uint64_t> soa(6 * n);
-  DTS_CUDA(cudaMemcpy(soa.data(), sim->S.rng, 6 * n * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-  for (size_t e = 0; e < n; e++) {
-    if (mask_host && !mask_host[e]) continue;
-    for (int k = 0; k < 6; k++) soa[k * n + e] = streams[6 * e + k];
-  }
-  DTS_CUDA(cudaMemcpy(sim->S.rng, soa.data(), 6 * n * sizeof(uint64_t), cudaMemcpyHostToDevice));
-  sim->seeded = true;
-  return 0;
+  const std::string e = state_seed_streams(*sim->state, mask_host, streams);
+  return e.empty() ? 0 : sim->fail("%s", e.c_str());
 }
 
 int dts_reset_random(dts_sim* sim, const uint8_t* mask_dev, void* stream) {
   if (!sim) return 1;
   if (check_maps(sim)) return 1;
-  if (!sim->seeded) return sim->fail("dts_seed_streams must be called before a device-side reset");
+  if (!state_seeded(*sim->state)) return sim->fail("dts_seed_streams must be called before a device-side reset");
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  launch_reset_random(sim->S, maps_table(*sim->maps), sim->step_cfg, map_select(sim), mask_dev, (cudaStream_t)stream);
+  launch_reset_random(state_arrays(*sim->state), maps_table(*sim->maps), sim->step_cfg, map_select(sim), mask_dev,
+                      (cudaStream_t)stream);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   return 0;
@@ -363,8 +317,8 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
       gt.base[p] = reinterpret_cast<uint8_t*>(sim->gather_peer[p]) + (uint64_t)sim->gather_rank * sim->gather_bytes;
     sim->gather_next = false;
   }
-  int k = launch_render(*sim->render, sim->S, maps_table(*sim->maps), rc, target, gt, sim->d_err, sim->d_status, marks, mark_level,
-                        (cudaStream_t)stream);
+  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, target, gt, sim->d_err,
+                        sim->d_status, marks, mark_level, (cudaStream_t)stream);
   if (rz.ow) {
     launch_resize(*sim->resize, rz.staging, obs_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, env_list, env_count,
                   (cudaStream_t)stream);
@@ -391,19 +345,21 @@ int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, voi
   if (sim->gather_next) return sim->fail("a fused gather is armed (dts_gather_next): dts_step_terminal does not write it");
   if (check_maps(sim) || check_loaded(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  if (!sim->seeded) return sim->fail("auto-reset needs seeded streams: call dts_seed_streams first");
+  if (!state_seeded(*sim->state)) return sim->fail("auto-reset needs seeded streams: call dts_seed_streams first");
   cudaStream_t st = (cudaStream_t)stream;
   // 1. the step with the respawn held back: k_step_logic's only use of DTS_FLAG_AUTO_RESET is that respawn
   StepCfg deferred = sim->step_cfg;
   deferred.flags &= ~DTS_FLAG_AUTO_RESET;
-  launch_step_logic(sim->S, maps_table(*sim->maps), deferred, map_select(sim), actions_dev, reward_dev, done_dev, st);
+  launch_step_logic(state_arrays(*sim->state), maps_table(*sim->maps), deferred, map_select(sim), actions_dev, reward_dev,
+                    done_dev, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   // 2. every env's frame of the state the step left: the terminal frame where the episode ended
   if (obs_dev && render_pass(sim, obs_dev, stream, nullptr, nullptr)) return 1;
   // 3. the ended envs respawn, in the same order of draws as inside k_step_logic, and are listed
   DTS_CUDA(cudaMemsetAsync(sim->n_ended, 0, sizeof(int32_t), st));
-  launch_respawn_ended(sim->S, maps_table(*sim->maps), sim->step_cfg, map_select(sim), sim->ended, sim->n_ended, st);
+  launch_respawn_ended(state_arrays(*sim->state), maps_table(*sim->maps), sim->step_cfg, map_select(sim), sim->ended,
+                       sim->n_ended, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   if (!obs_dev) return 0;
@@ -423,9 +379,9 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
   if (!actions_dev) return sim->fail("actions_dev is NULL");
   if (check_maps(sim) || check_loaded(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  if ((sim->cfg.flags & DTS_FLAG_AUTO_RESET) && !sim->seeded)
+  if ((sim->cfg.flags & DTS_FLAG_AUTO_RESET) && !state_seeded(*sim->state))
     return sim->fail("auto-reset needs seeded streams: call dts_seed_streams first");
-  launch_step_logic(sim->S, maps_table(*sim->maps), sim->step_cfg, map_select(sim), actions_dev, reward_dev, done_dev,
+  launch_step_logic(state_arrays(*sim->state), maps_table(*sim->maps), sim->step_cfg, map_select(sim), actions_dev, reward_dev, done_dev,
                     (cudaStream_t)stream);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
@@ -435,10 +391,7 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
 
 int dts_get_state(dts_sim* sim, dts_state_view* v) {
   if (!sim || !v) return 1;
-  const DState& S = sim->S;
-  *v = dts_state_view{S.pos_x, S.pos_z, S.angle, S.speed, S.reward, S.lane_dist, S.lane_dot, S.lane_angle, S.prox,
-                      S.wheel_dist, S.step_count, S.tile_i, S.tile_j, S.map_id, S.episode, S.done_code, S.in_lane,
-                      S.collided};
+  *v = state_view(*sim->state);
   return 0;
 }
 
@@ -479,8 +432,11 @@ int dts_assign_maps(dts_sim* sim, const uint8_t* mask_dev, const int32_t* map_id
       return sim->fail("dts_assign_maps: map_id[%zu]=%d has no uploaded map", e, map_id_host[e]);
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  DTS_CUDA(cudaMemcpyAsync(sim->stage.map_id, map_id_host, n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  launch_assign_maps(sim->S, maps_table(*sim->maps), mask_dev, sim->stage.map_id, st);
+  dts_episode_params host{}, dev;
+  host.map_id = map_id_host;
+  const std::string e = state_stage(*sim->state, host, dev, st);
+  if (!e.empty()) return sim->fail("%s", e.c_str());
+  launch_assign_maps(state_arrays(*sim->state), maps_table(*sim->maps), mask_dev, dev.map_id, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   DTS_CUDA(cudaStreamSynchronize(st));   // pageable host source
@@ -623,7 +579,6 @@ int dts_load_state(dts_sim* sim, const uint8_t* mask_dev, const void* records_de
                     sim->d_status + 1, (cudaStream_t)stream);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
-  sim->seeded = true;   // the envs' streams came with their records
   return 0;
 }
 
@@ -683,7 +638,7 @@ int dts_debug_episode(dts_sim* sim, int env, void* out144) {
   if (!sim) return 1;
   if (env < 0 || env >= sim->cfg.num_envs) return sim->fail("env out of range");
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  DTS_CUDA(cudaMemcpy(out144, sim->S.rep + env, sizeof(RenderEp), cudaMemcpyDeviceToHost));
+  DTS_CUDA(cudaMemcpy(out144, state_arrays(*sim->state).rep + env, sizeof(RenderEp), cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -711,12 +666,8 @@ int dts_debug_streams(dts_sim* sim, uint64_t* out_host) {
   if (!out_host) return sim->fail("out_host is NULL");
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   DTS_CUDA(cudaDeviceSynchronize());
-  const size_t n = sim->cfg.num_envs;
-  std::vector<uint64_t> soa(6 * n);
-  DTS_CUDA(cudaMemcpy(soa.data(), sim->S.rng, 6 * n * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-  for (size_t e = 0; e < n; e++)
-    for (int k = 0; k < 6; k++) out_host[6 * e + k] = soa[k * n + e];
-  return 0;
+  const std::string e = state_read_streams(*sim->state, out_host);
+  return e.empty() ? 0 : sim->fail("%s", e.c_str());
 }
 
 /* debug: a program of NpStream draws from every env's stream (see dtsim.h) */
@@ -735,7 +686,7 @@ int dts_debug_draw(dts_sim* sim, const dts_draw_op* ops, int n_ops, uint64_t* ou
   dts_draw_op* d_ops = nullptr;
   DTS_CUDA(cudaMallocAsync((void**)&d_ops, n_ops * sizeof(dts_draw_op), st));
   DTS_CUDA(cudaMemcpyAsync(d_ops, ops, n_ops * sizeof(dts_draw_op), cudaMemcpyHostToDevice, st));
-  launch_debug_draw(sim->S, d_ops, n_ops, total, out_dev, st);
+  launch_debug_draw(state_arrays(*sim->state), d_ops, n_ops, total, out_dev, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   DTS_CUDA(cudaFreeAsync(d_ops, st));

@@ -98,7 +98,8 @@ __device__ __forceinline__ DynRef dyn_ref(const DMap& m, int n_envs, int e) {
 }
 
 // ------------------------------------------------------------------ per-env state, SoA in HBM
-// One thread per env in the logic kernels: consecutive threads touch consecutive doubles.
+// One thread per env in the logic kernels: consecutive threads touch consecutive doubles.  kStateArrays (dts_state.cu)
+// lists every array once: a new one is allocated and snapshotted by adding it there, and the build fails until it is.
 struct DState {
   int32_t n;
   // dynamics (cartesian frame of duckietown_world: x right, y up; S:1629-1652)
@@ -113,7 +114,8 @@ struct DState {
   struct RenderEp* rep;  // [n] per-episode render parameters (AoS: one CTA reads one record)
 };
 
-// Per-episode render inputs (simulator.py:546-614, 1768): 128 bytes, read by one CTA per frame.
+// Per-episode render inputs (simulator.py:546-614, 1768): 144 bytes, seven 16-byte groups and the hidden mask, read by
+// one CTA per frame.
 struct __align__(16) RenderEp {
   float cam_height, cam_angle_deg, cam_fov_y_deg, pad0;
   float cam_noise[3]; float pad1;
@@ -124,6 +126,7 @@ struct __align__(16) RenderEp {
   float ground[3]; float pad5;
   uint32_t hidden[8];                 // bit o = object o invisible
 };
+static_assert(sizeof(RenderEp) == 144, "dts_debug_episode copies 144 bytes, and the records' sizes count them");
 
 struct DynParams { double u1, u2, u3, w1, w2, w3, uar, ual, war, wal; int32_t delay_steps; };
 

@@ -7,17 +7,6 @@
 
 namespace dts {
 
-// Device copies of a dts_episode_params (NULL members keep defaults).
-struct ResetStaging {
-  const int32_t* map_id;
-  const double *pos_x, *pos_z, *angle, *wheel_dist, *trim;
-  const float *cam_height, *cam_angle_deg, *cam_fov_y_deg, *cam_noise, *horizon_color, *light_ambient,
-      *light_diffuse, *light_pos;
-  const int32_t* light_stale;
-  const float* ground_color;
-  const uint32_t* obj_hidden;
-};
-
 struct RenderCfg {
   int32_t width, height;      // output obs size
   int32_t flags;
@@ -36,8 +25,9 @@ void launch_step_logic(const DState& S, const DMap* maps, const StepCfg& c, int 
                        float* reward, uint8_t* done, cudaStream_t st);
 void launch_reset_random(const DState& S, const DMap* maps, const StepCfg& c, int n_maps_cycle, const uint8_t* mask,
                          cudaStream_t st);
+// `p` holds DEVICE copies of the host's episode parameters (state_stage); NULL members keep the defaults
 void launch_reset_params(const DState& S, const DMap* maps, const StepCfg& c, const uint8_t* mask,
-                         const ResetStaging& p, cudaStream_t st);
+                         const dts_episode_params& p, cudaStream_t st);
 void launch_assign_maps(const DState& S, const DMap* maps, const uint8_t* mask, const int32_t* map_id, cudaStream_t st);
 // The auto-reset k_step_logic does in place, deferred (dts_step_terminal): every env whose episode ended re-spawns, and
 // is appended to ended[0 .. *n_ended), which the caller zeroes first.  The list's order is not deterministic.
@@ -77,21 +67,35 @@ int maps_slot_count(const MapSlots& m);                           // max_maps
 // Content hash of the blob the slot's map was built from (never 0); 0 for an empty slot
 uint64_t maps_hash(const MapSlots& m, int slot);
 
-// snapshots (dts_state.cu).  The record layout of one handle: which device arrays make up an env's state, where each
-// lands in the env's record, and the fingerprint of that layout and of the maps it refers to.
-struct StateRecords;
-StateRecords* state_create(const dts_config& cfg);   // on the current device; null if out of memory
-void state_destroy(StateRecords* s);
-// Re-lay the records out for the state `S` and the maps now in `maps` (after creation and after every map upload).
-// Synchronous; no save or load may be in flight.  Returns the error text, empty on success.
-std::string state_layout(StateRecords& s, const DState& S, const MapSlots& maps);
-uint64_t state_record_bytes(const StateRecords& s);   // one env's record, a multiple of 16
-uint64_t state_fingerprint(const StateRecords& s);
+// per-env state (dts_state.cu).  The envs' simulator state of one handle: the DState arrays, the staging buffers of
+// dts_reset, the snapshot record layout with its fingerprint, and whether the envs' streams are seeded.  One table,
+// kStateArrays, is the single statement of the per-env state: it allocates the arrays and lays out the records.
+// Functions that can fail return the error text, empty on success.
+struct EnvState;
+// On the current device, the records laid out for the maps now in `maps`; null (and `err`) if out of memory
+EnvState* state_create(const dts_config& cfg, const MapSlots& maps, std::string& err);
+void state_destroy(EnvState* s);
+const DState& state_arrays(const EnvState& s);   // what the launchers take
+dts_state_view state_view(const EnvState& s);
+bool state_seeded(const EnvState& s);   // dts_seed_streams or dts_load_state has given the envs their streams
+// streams[N][6] (dts_seed_streams' layout, HOST) -> the streams of the envs with mask_host[e] (null: all); synchronous
+std::string state_seed_streams(EnvState& s, const uint8_t* mask_host, const uint64_t* streams);
+// every env's stream -> out[N][6] (HOST); synchronous on the legacy stream
+std::string state_read_streams(const EnvState& s, uint64_t* out);
+// The host arrays of `host` -> the staging buffers, on `st`; `dev` gets their device addresses, null where `host` has
+// none.  The host arrays must stay unchanged until `st` has passed the copies.
+std::string state_stage(EnvState& s, const dts_episode_params& host, dts_episode_params& dev, cudaStream_t st);
+// Re-lay the records out for the maps now in `maps` (after every map upload).  Synchronous; no save or load may be in
+// flight.
+std::string state_layout(EnvState& s, const MapSlots& maps);
+uint64_t state_record_bytes(const EnvState& s);   // one env's record, a multiple of 16; 0: the last layout failed
+uint64_t state_fingerprint(const EnvState& s);
 // records u8[n_envs][record_bytes] <- every env's state
-void launch_state_save(const StateRecords& s, void* records, cudaStream_t st);
+void launch_state_save(const EnvState& s, void* records, cudaStream_t st);
 // every env e with mask[e] (null: all) whose record names an uploaded map in `maps[0 .. n_maps)` <- record e; an env
-// whose record names none keeps its state, and `refused` (device address of a status word) is set to 1
-void launch_state_load(const StateRecords& s, const uint8_t* mask, const void* records, const DMap* maps, int n_maps,
+// whose record names none keeps its state, and `refused` (device address of a status word) is set to 1.  The envs'
+// streams count as seeded from then on.
+void launch_state_load(EnvState& s, const uint8_t* mask, const void* records, const DMap* maps, int n_maps,
                        int32_t* refused, cudaStream_t st);
 
 // render (dts_render.cu).  The renderer of one handle: the launch sizes, the frame memory, sized from the uploaded maps,

@@ -270,7 +270,7 @@ __global__ void __launch_bounds__(128) k_respawn_ended(DState S, const DMap* __r
 
 // dts_reset with host-drawn parameters (already copied to device staging arrays in `p`)
 __global__ void __launch_bounds__(128) k_reset_params(DState S, const DMap* __restrict__ maps, StepCfg c,
-                                                      const uint8_t* __restrict__ mask, ResetStaging p) {
+                                                      const uint8_t* __restrict__ mask, dts_episode_params p) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= S.n || (mask && !mask[e])) return;
   RenderEp old = S.rep[e];
@@ -385,7 +385,7 @@ void launch_respawn_ended(const DState& S, const DMap* maps, const StepCfg& c, i
   k_respawn_ended<<<(S.n + 127) / 128, 128, 0, st>>>(S, maps, c, n_maps_cycle, ended, n_ended);
 }
 void launch_reset_params(const DState& S, const DMap* maps, const StepCfg& c, const uint8_t* mask,
-                         const ResetStaging& p, cudaStream_t st) {
+                         const dts_episode_params& p, cudaStream_t st) {
   k_reset_params<<<(S.n + 127) / 128, 128, 0, st>>>(S, maps, c, mask, p);
 }
 void launch_assign_maps(const DState& S, const DMap* maps, const uint8_t* mask, const int32_t* map_id, cudaStream_t st) {

@@ -117,20 +117,17 @@ class MapBlob(C.Structure):
     ]
 
 
-_EP_FIELDS = ["map_id", "pos_x", "pos_z", "angle", "wheel_dist", "trim", "cam_height", "cam_angle_deg",
-              "cam_fov_y_deg", "cam_noise", "horizon_color", "light_ambient", "light_diffuse", "light_pos",
-              "light_stale", "ground_color", "obj_hidden"]
-_EP_DTYPES = {"map_id": np.int32, "pos_x": np.float64, "pos_z": np.float64, "angle": np.float64,
-              "wheel_dist": np.float64, "trim": np.float64, "cam_height": np.float32, "cam_angle_deg": np.float32,
-              "cam_fov_y_deg": np.float32, "cam_noise": np.float32, "horizon_color": np.float32,
-              "light_ambient": np.float32, "light_diffuse": np.float32, "light_pos": np.float32,
-              "light_stale": np.int32, "ground_color": np.float32, "obj_hidden": np.uint32}
-_EP_WIDTH = {"cam_noise": 3, "horizon_color": 3, "light_ambient": 3, "light_diffuse": 3, "light_pos": 4,
-             "ground_color": 3, "obj_hidden": 8}
+# dts_episode_params, in its order: (member, dtype, values per env)
+_EP_FIELDS = [("map_id", np.int32, 1), ("pos_x", np.float64, 1), ("pos_z", np.float64, 1), ("angle", np.float64, 1),
+              ("wheel_dist", np.float64, 1), ("trim", np.float64, 1), ("cam_height", np.float32, 1),
+              ("cam_angle_deg", np.float32, 1), ("cam_fov_y_deg", np.float32, 1), ("cam_noise", np.float32, 3),
+              ("horizon_color", np.float32, 3), ("light_ambient", np.float32, 3), ("light_diffuse", np.float32, 3),
+              ("light_pos", np.float32, 4), ("light_stale", np.int32, 1), ("ground_color", np.float32, 3),
+              ("obj_hidden", np.uint32, 8)]
 
 
 class EpisodeParams(C.Structure):
-    _fields_ = [(f, C.c_void_p) for f in _EP_FIELDS]
+    _fields_ = [(f, C.c_void_p) for f, _, _ in _EP_FIELDS]
 
 
 _STATE_FIELDS = [("pos_x", np.float64), ("pos_z", np.float64), ("angle", np.float64), ("speed", np.float64),
@@ -379,12 +376,12 @@ class Sim:
     def reset(self, mask_ptr: Optional[int], params: dict, stream: int = 0):
         n = self.cfg.num_envs
         keep, ep = [], EpisodeParams()
-        for f in _EP_FIELDS:
+        for f, dtype, width in _EP_FIELDS:
             v = params.get(f)
             if v is None:
                 continue
-            a = np.ascontiguousarray(v, _EP_DTYPES[f])
-            want = (n, _EP_WIDTH[f]) if f in _EP_WIDTH else (n,)
+            a = np.ascontiguousarray(v, dtype)
+            want = (n, width) if width > 1 else (n,)
             if a.shape != want:
                 raise ValueError(f"episode param {f}: shape {a.shape}, expected {want}")
             keep.append(a)
