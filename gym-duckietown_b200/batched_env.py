@@ -4,7 +4,7 @@
 observation buffers are caller-visible torch CUDA tensors, the work runs on
 `torch.cuda.current_stream()` inside libdtsim.so, nothing synchronises.  Constructor keywords are the
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
-`auto_reset`, `device_reset`, `terminal_obs`.
+`auto_reset`, `device_reset`, `terminal_obs`, `depth`.
 
 Under `auto_reset` the observation a step returns for an env whose episode ended is the first frame of its next
 episode.  `terminal_obs=True` also keeps the frame the reference's step() returns there (the terminal frame, before
@@ -12,6 +12,14 @@ the caller's reset()), in `env.terminal_obs` — what SB3's `terminal_observatio
 value bootstrapping on truncation.  Only the rows of envs that ended (`done`) are written; the others keep what they
 held.  The ended envs are drawn a second time, so the cost grows with how many ended, not with num_envs.  It holds a
 second obs-sized buffer: 236 MB at 4096 envs x 160x120 u8, 7.5 GB at 8192 envs x 640x480 u8.
+
+`depth=True` allocates `env.depth`, float32 [num_envs, camera_height, camera_width], which every render (`reset`,
+`step`, `render_obs`) fills beside the observation it draws: the eye-space depth in metres of the nearest surface a
+pixel's samples see, 0 for sky and for pixels the fisheye / rectification gives no source (dts_set_depth_target).  It is
+the depth of the frame just rendered, so it follows `undistort`, the rectification, `top_down` and `segment` (which
+leaves it unchanged), and under `auto_reset` an ended env's row is its next episode's first frame, as in `obs`.  It stays
+at the camera size and in this layout under `set_resize` and `set_output_format`.  The depth of the terminal frames
+(`terminal_obs=True`) is not kept, and the multi-GPU gathers carry observations only.
 """
 from __future__ import annotations
 
@@ -35,7 +43,8 @@ class BatchedDuckietownEnv:
                  gain=1.0, trim=0.0, radius=0.0318, k=27.0, limit=1.0,
                  action_mode: str = "vel_steer", auto_reset: bool = False, device_reset: bool = False,
                  cycle_maps: bool = False, env_id_offset: int = 0, tessellate_tiles: bool = False,
-                 randomize_maps_on_reset: bool = False, randomization_config=None, terminal_obs: bool = False):
+                 randomize_maps_on_reset: bool = False, randomization_config=None, terminal_obs: bool = False,
+                 depth: bool = False):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
         if camera_rand:
@@ -84,6 +93,9 @@ class BatchedDuckietownEnv:
             self.obs = torch.zeros((num_envs, camera_height, camera_width, 3), dtype=torch.uint8, device=self.device)
             # the terminal frames of the envs that ended on a step (terminal_obs=True), in obs's shape and dtype
             self.terminal_obs: Optional[torch.Tensor] = torch.zeros_like(self.obs) if terminal_obs else None
+            # the depth image of the frames in obs (depth=True); the renders write it on the device
+            self.depth: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, camera_height, camera_width), dtype=torch.float32, device=self.device) if depth else None
             self.reward = torch.zeros(num_envs, dtype=torch.float32, device=self.device)
             self._done_u8 = torch.zeros(num_envs, dtype=torch.uint8, device=self.device)
             self.state: Dict[str, torch.Tensor] = {
@@ -100,6 +112,8 @@ class BatchedDuckietownEnv:
         self.rectification = None    # (mapx, mapy) UndistortWrapper installed for reset / step observations
         self.output_format = dict(obs_layout="hwc", obs_dtype="uint8", reward="raw", discrete_actions=False,
                                   action_vel_scale=1.0)
+        if depth:
+            self.sim.set_depth_target(self.depth.data_ptr())
         self.seed(seed)
 
     def set_output_format(self, obs_layout: Optional[str] = None, obs_dtype: Optional[str] = None,

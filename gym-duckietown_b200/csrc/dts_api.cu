@@ -42,6 +42,7 @@ struct dts_sim {
   void* gather_peer[DTS_MAX_PEERS] = {};   // peers' buffers opened with cudaIpcOpenMemHandle (own entry = gather_buf)
   bool gather_next = false;
   int render_mode = 0;                  // dts_set_render_mode             // the next dts_render also stores into the gather buffers
+  float* depth_target = nullptr;        // dts_set_depth_target: caller-owned f32 [N][cam_h][cam_w], or null
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
   int profiling = 0;                    // 0 off, 1 events around k_raster only, 2 around every render kernel
   std::vector<cudaEvent_t> prof_events; // kProfMarks events per profiled frame
@@ -290,7 +291,7 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
   if (!e.empty()) return sim->fail("%s", e.c_str());
   RenderCfg rc{sim->cfg.cam_width, sim->cfg.cam_height, sim->cfg.flags, sim->cfg.num_envs,
                (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->render_mode,
-               env_list, env_count};
+               env_list, env_count, sim->depth_target};
   if (*(volatile int32_t*)sim->h_status & 1)
     return sim->fail("an earlier frame overflowed its render frame memory (prim slab / bin lists) and was left incomplete");
   if (check_loaded(sim)) return 1;
@@ -525,6 +526,13 @@ int dts_set_render_mode(dts_sim* sim, int mode) {
   if (mode & ~(DTS_RENDER_SEGMENT | DTS_RENDER_TOP_DOWN | DTS_RENDER_PINHOLE | DTS_RENDER_RECTIFY))
     return sim->fail("bad render mode %d", mode);
   sim->render_mode = mode;
+  return 0;
+}
+
+int dts_set_depth_target(dts_sim* sim, float* depth_dev) {
+  if (!sim) return 1;
+  if (reinterpret_cast<uintptr_t>(depth_dev) & 3) return sim->fail("depth target is not aligned to 4 bytes");
+  sim->depth_target = depth_dev;
   return 0;
 }
 

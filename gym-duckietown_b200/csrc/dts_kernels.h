@@ -19,6 +19,9 @@ struct RenderCfg {
   // the envs left out keep what the previous pass put there.  (n_envs stays the SoA stride of the per-env state.)
   const int32_t* env_list;
   const int32_t* env_count;
+  // Optional depth target (dts_set_depth_target): f32 [n_envs][height][width], written beside obs by the rasterisers'
+  // depth instances, for the listed envs only where there is a list.  NULL: no depth is computed.
+  float* depth;
 };
 
 void launch_step_logic(const DState& S, const DMap* maps, const StepCfg& c, int n_maps_cycle, const float* actions,

@@ -28,7 +28,10 @@
 // Arithmetic follows the render spec of DESIGN.md (the CPU checker implements the same spec) bit for bit
 // (compiled with -fmad=false; fmaf() is spelled out where the spec has one).
 //
-// HBM traffic per env-frame: obs store W*H*3 B (compulsory) + PrimRec slab / BinRec lists / lattice table
+// With a depth target (RenderCfg::depth, render spec item 9) the three rasterisers run their kDepth instances, which also
+// store every pixel's eye-space depth, f32 [N][H][W]; without one the launches and their kernels are the plain ones.
+//
+// HBM traffic per env-frame: obs store W*H*3 B (compulsory; + W*H*4 B of depth where asked for) + PrimRec slab / BinRec lists / lattice table
 // (tens of KB per env, written by k_geometry / k_bin and read once by k_raster) + texels (shared, L2-resident).
 #include <algorithm>
 #include <cstddef>
@@ -595,6 +598,8 @@ __device__ __forceinline__ unsigned build_binrec(const PrimRec* __restrict__ pr,
 // 5-6 and 8): perspective-correct u,v (+ rgb for meshes / ground), analytic lattice lighting for road tiles,
 // bilinear REPEAT texel, MODULATE.  Deferred shading: each lane may shade a different prim.  Split in two so that a
 // coarse bin lying inside ONE prim fetches the prim's planes once for its 256 pixels.
+// `qq_out` (depth target, render spec item 9) receives the prim's clamped 1/w at the pixel centre: the very value the
+// perspective divide uses.
 struct ShadeIn {
   const PrimRec* pr;
   int x0, y0;
@@ -616,10 +621,11 @@ __device__ __forceinline__ ShadeIn load_shade(const PrimRec* __restrict__ prims,
   return si;
 }
 __device__ __forceinline__ void shade_eval(const ShadeIn& si, const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab,
-                                           int pxa, int pya, float c3[3]) {
+                                           int pxa, int pya, float c3[3], float* qq_out = nullptr) {
   const float cdx = (float)(pxa + 32 - si.x0) * 0.015625f, cdy = (float)(pya + 32 - si.y0) * 0.015625f;
   float qq = fmaf(si.qy, cdy, fmaf(si.qx, cdx, si.q0));
   if (!(qq > 1e-20f)) qq = 1e-20f;
+  if (qq_out) *qq_out = qq;
   const float rq = 1.0f / qq;
   const float u = fmaf(si.uy, cdy, fmaf(si.ux, cdx, si.u0)) * rq;
   const float v = fmaf(si.vy, cdy, fmaf(si.vx, cdx, si.v0)) * rq;
@@ -675,9 +681,9 @@ __device__ __forceinline__ void shade_eval(const ShadeIn& si, const uint8_t* __r
   }
 }
 __device__ __forceinline__ void shade_prim(const PrimRec* __restrict__ prims, unsigned w, const uint8_t* __restrict__ tex_pool,
-                                           const float4* __restrict__ lat_tab, int pxa, int pya, float c3[3]) {
+                                           const float4* __restrict__ lat_tab, int pxa, int pya, float c3[3], float* qq_out = nullptr) {
   const ShadeIn si = load_shade(prims, w);
-  shade_eval(si, tex_pool, lat_tab, pxa, pya, c3);
+  shade_eval(si, tex_pool, lat_tab, pxa, pya, c3, qq_out);
 }
 
 // ---- bulk-async copy (TMA, 1-D) + mbarrier: global -> shared without register staging
@@ -824,6 +830,17 @@ __device__ __forceinline__ void store_bin_lean(uint8_t* __restrict__ out, const 
                                                int W, int H) {
   if (bx * kBinW + kBinW <= W) store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
   else store_bin(out, rgb, lane, bx, by, W, H);
+}
+
+// Depth target (render spec item 9): the eye-space depth of a pixel is 1 / (the largest 1/w among the distinct winners
+// of its samples), 0 where no sample is covered (`qmax` 0: a prim's 1/w is at least 1e-20) or the gather has no source.
+__device__ __forceinline__ float depth_of(float qmax, bool px_valid = true) { return (px_valid && qmax > 0.0f) ? 1.0f / qmax : 0.0f; }
+// One fine bin of the depth frame `dep` (f32 [H][W] of one env): a lane stores its own pixel.  The 8 lanes of a bin row
+// write 32 contiguous bytes — one whole sector wherever W is a multiple of 8 — so wider per-lane stores packed with
+// shuffles would move the same sectors.
+__device__ __forceinline__ void store_depth(float* __restrict__ dep, float d, int lane, int bx, int by, int W, int H) {
+  const int gx = bx * kBinW + (lane & 7), gy = by * kBinH + (lane >> 3);
+  if (gx < W && gy < H) dep[(size_t)gy * W + gx] = d;
 }
 
 // glClearColor: the env's horizon colour, or on the segment view glClearColor(255, 0, 255) clamped to magenta (S:1752)
@@ -1535,9 +1552,12 @@ __device__ __forceinline__ int sample_mask(const BinRec& br, int pxc, int pyc) {
 // in rounds of the whole warp (a lane with nothing pending idles), and the box resolve (s01 + s23) * 0.25 into c3, with
 // s01 = c(wn0) + c(wn1), s23 = c(wn2) + c(wn3).  Each shade depends only on (prim, position) and each half has two
 // addends, so neither the lane nor the order in which the winners are shaded changes a bit.  Called by the whole warp.
+// kDepth: `qmax` comes in as the first winner's 1/w (0: none) and leaves as the largest over the pixel's winners; a
+// maximum of exact values, so the order does not matter there either.
+template <bool kDepth>
 __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], const float clr[3], const PrimRec* __restrict__ prims,
                                              const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa, int pya,
-                                             int lane, int32_t* __restrict__ err) {
+                                             int lane, int32_t* __restrict__ err, float& qmax) {
   (void)lane; (void)err;   // (DTS_STATS counters)
   float s01[3] = {c3[0], c3[1], c3[2]}, s23[3] = {0.f, 0.f, 0.f};   // 0 + c == c
   unsigned pend = 0xeu;
@@ -1552,7 +1572,9 @@ __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], 
       const int s = __ffs(pend) - 1;
       const unsigned w = s == 1 ? wn[1] : (s == 2 ? wn[2] : wn[3]);
       float d3[3] = {clr[0], clr[1], clr[2]};
-      if (w != kNoPrim) shade_prim(prims, w, tex_pool, lat_tab, pxa, pya, d3);
+      float qq = 0.0f;
+      if (w != kNoPrim) shade_prim(prims, w, tex_pool, lat_tab, pxa, pya, d3, kDepth ? &qq : nullptr);
+      if (kDepth) qmax = fmaxf(qmax, qq);
 #pragma unroll
       for (int t = 1; t < 4; t++)
         if ((pend >> t & 1u) && wn[t] == w) {
@@ -1566,21 +1588,24 @@ __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], 
   for (int ch = 0; ch < 3; ch++) c3[ch] = (s01[ch] + s23[ch]) * 0.25f;
 }
 // The whole resolve of one fine bin's pixels (k_raster).  `simple`: the caller knows that every sample of the whole fine
-// bin has the same winner.
+// bin has the same winner.  kDepth: `qmax` receives the largest 1/w among the pixel's winners, 0 if it has none.
+template <bool kDepth>
 __device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool simple, const float clr[3], const PrimRec* __restrict__ prims,
                                                   const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa,
-                                                  int pya, int lane, int32_t* __restrict__ err) {
+                                                  int pya, int lane, int32_t* __restrict__ err, float& qmax) {
   const bool same = wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0];
   const bool all_same = simple || __all_sync(0xffffffffu, same);
   float c3[3] = {clr[0], clr[1], clr[2]};
-  if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3);   // every lane: its first winner
-  if (!all_same) resolve_edge(wn, c3, clr, prims, tex_pool, lat_tab, pxa, pya, lane, err);   // (four equal samples: the mean is the value itself)
+  if (kDepth) qmax = 0.0f;
+  if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3, kDepth ? &qmax : nullptr);   // every lane: its first winner
+  if (!all_same) resolve_edge<kDepth>(wn, c3, clr, prims, tex_pool, lat_tab, pxa, pya, lane, err, qmax);   // (four equal samples: the mean is the value itself)
   return pack_rgb(c3[0], c3[1], c3[2]);
 }
 
 // ------------------------------------------------------------------------------------------------ k_raster
-template <bool kWrapFmt, bool kFish>   // kWrapFmt: a dts_output_format other than packed u8 HWC is written by the resolve;
-                                       // kFish: every lane renders the SOURCE pixel the fisheye LUT names for its output pixel
+template <bool kWrapFmt, bool kFish, bool kDepth>   // kWrapFmt: a dts_output_format other than packed u8 HWC is written by the resolve;
+                                       // kFish: every lane renders the SOURCE pixel the fisheye LUT names for its output pixel;
+                                       // kDepth: every pixel's depth goes to rc.depth beside its colour (render spec item 9)
 __global__ void __launch_bounds__(kThreads, kRasterMinCtas)
 k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, FishTab ft, GatherTab gt,
          uint8_t* __restrict__ obs, int max_prims, int max_pairs, int max_lat, int32_t* __restrict__ err) {
@@ -1623,12 +1648,14 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     const size_t env_off = (size_t)env * frame_bytes * out_elem;
     uint8_t* out = obs + env_off;
+    float* dep = kDepth ? rc.depth + (size_t)env * W * H : nullptr;
     // one fine bin -> the caller's tensor and, on a gathering step, every peer's gather buffer (NVLink stores)
     // On a gathering step (gt.n > 0) the packed u8 HWC frame goes to the peers in BLOCKS: a work item is 8 whole image rows =
     // one contiguous run of bytes, copied to every rank's gather buffer with 16-byte vector stores once the item is drawn
     // (NVLink wants long writes: per-bin 4-byte stores reach a fifth of the link rate).  Other layouts store per bin.
     const bool gather_rows = gt.n > 0 && !kWrapFmt;
-    auto emit = [&](unsigned rgb, int bx, int by) {
+    auto emit = [&](unsigned rgb, float depth, int bx, int by) {
+      if (kDepth) store_depth(dep, depth, lane, bx, by, W, H);   // (the caller's depth tensor only: the gather carries obs)
       if (fast_fmt && (gt.n == 0 || gather_rows) && bx * kBinW + kBinW <= W) {   // the common case inline: packed u8 HWC, whole bin inside
         store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
       } else if (kWrapFmt && gt.n == 0) {
@@ -1696,7 +1723,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
             const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);
             unsigned rgb = clear_rgb;
             if (kFish && !fish_source(ft, bx, by, lane, W, H).valid) rgb = 0u;
-            emit(rgb, bx, by);
+            emit(rgb, 0.0f, bx, by);
           }
         continue;
       }
@@ -1906,9 +1933,10 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
             }
             // ---- deferred shading: once per distinct winner of this pixel, then the box resolve
             DTS_COUNT(11, 1);
-            unsigned rgb = shade_resolve(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane, err);
+            float qmax = 0.0f;
+            unsigned rgb = shade_resolve<kDepth>(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane, err, qmax);
             if (kFish && !px_valid) rgb = 0u;   // cv2.remap BORDER_CONSTANT
-            emit(rgb, bx, by);
+            emit(rgb, kDepth ? depth_of(qmax, px_valid) : 0.0f, bx, by);
           }
         }
       }
@@ -1927,7 +1955,8 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
 // visibility state: a warp fetches the prim's planes once and shades the bin's 256 pixels.  A separate kernel so that the
 // lean loop gets its own register allocation (the same fast path inside k_raster cost more than it saved).
 // Packed u8 HWC output with whole-word rows only (k_bin marks no bin otherwise).  Runs before k_raster.
-template <bool kFish>   // true: each lane shades the source pixel the fisheye LUT names for its output pixel
+template <bool kFish, bool kDepth>   // kFish: each lane shades the source pixel the fisheye LUT names for its output pixel;
+                                     // kDepth: the 1/w the shading divides by also gives the pixel's depth (rc.depth)
 __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
                                                                         FishTab ft, uint8_t* __restrict__ obs, int max_prims, int max_lat) {
   const int W = rc.width, H = rc.height;
@@ -1961,11 +1990,12 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
         px_valid = src.valid;
         pxa = src.x; pya = src.y;
       }
-      float c3[3];
-      shade_eval(si, tex_pool, lat_tab, pxa, pya, c3);
+      float c3[3], qq = 0.0f;
+      shade_eval(si, tex_pool, lat_tab, pxa, pya, c3, kDepth ? &qq : nullptr);
       unsigned rgb = pack_rgb(c3[0], c3[1], c3[2]);
       if (kFish && !px_valid) rgb = 0u;
       store_bin_lean(out, sl, rgb, lane, bx, by, W, H);
+      if (kDepth) store_depth(rc.depth + (size_t)env * W * H, depth_of(qq, px_valid), lane, bx, by, W, H);
     }
   }
 }
@@ -1986,9 +2016,13 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
 // Hand-back: a sample covered by two tiles (or by two ground records) is not resolved here.  The warp drops the bin's
 // queue and colours, restores its record count, and k_raster, launched next on the stream, draws the whole bin
 // depth-tested.
+// kDepth: depth needs no plane in shared memory.  A lane stores a one-winner pixel's depth as soon as it has shaded it,
+// and a queued pixel's when its other winners are resolved; the queue carries the first winner's 1/w in a third array
+// (2 KB: 46 KB per CTA, still four CTAs per SM).  A bin handed back may have stored some depths already: k_raster
+// rewrites the whole bin, colour and depth.
 // Packed u8 HWC output with whole-word rows only (k_bin lists no bin otherwise).  Runs after k_raster_solo.
 constexpr int kEdgeQ = 64;   // queue ring: flushed at 32 entries, so at most 31 + 32 wait at once
-template <bool kFish>   // true: each lane covers and shades the source pixel the fisheye LUT names for its output pixel
+template <bool kFish, bool kDepth>   // kFish: each lane covers and shades the source pixel the fisheye LUT names for its output pixel
 __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
                                                                         FishTab ft, uint8_t* __restrict__ obs, int max_prims, int max_lat,
                                                                         int32_t* __restrict__ err) {
@@ -2002,6 +2036,11 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
   BinRec* stage = stages[threadIdx.x >> 5];
   unsigned* rgb_buf = bin_rgb[threadIdx.x >> 5];
   uint4 (*q)[kEdgeQ] = edge_q[threadIdx.x >> 5];
+  float* q_qq = nullptr;   // kDepth: per queue entry, the first winner's 1/w
+  if constexpr (kDepth) {
+    __shared__ float edge_qq[kWarps][kEdgeQ];
+    q_qq = edge_qq[threadIdx.x >> 5];
+  }
   const size_t frame_bytes = (size_t)W * H * 3;
   const int pxs = (lane & 7) * kSub, pys = (lane >> 3) * kSub;   // this lane's pixel inside a fine bin (sub-pixels)
   const int warps = (gridDim.x * blockDim.x) >> 5;
@@ -2030,6 +2069,7 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
     const PrimRec* prims = fm.prims + (size_t)env * max_prims;
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     uint8_t* out = obs + (size_t)env * frame_bytes;
+    float* dep = kDepth ? rc.depth + (size_t)env * W * H : nullptr;
     float clr[3];
     clear_colour(S, rc, env, clr);
     int ox = cbx * kCoarseW * kSub, oy = cby * kCoarseH * kSub;   // coarse bin corner, sub-pixels
@@ -2100,8 +2140,8 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
       }
       // ---- every lane: its first winner.  One winner: the pixel is done.  More: it waits in the queue.  (A pixel the
       // fisheye LUT gives no source is black either way.)
-      float c3[3] = {clr[0], clr[1], clr[2]};
-      if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, ox + pxc, oy + pyc, c3);
+      float c3[3] = {clr[0], clr[1], clr[2]}, qq0 = 0.0f;
+      if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, ox + pxc, oy + pyc, c3, kDepth ? &qq0 : nullptr);
       const bool edge = px_valid && !(wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0]);
       const unsigned edges = __ballot_sync(0xffffffffu, edge);
       const unsigned slot = f * 32 + lane;
@@ -2109,8 +2149,10 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
         const int e = (qs + __popc(edges & ((1u << lane) - 1u))) & (kEdgeQ - 1);
         q[0][e] = make_uint4(slot, (unsigned)(ox + pxc), (unsigned)(oy + pyc), wn[0] | (wn[1] << 16));
         q[1][e] = make_uint4(wn[2] | (wn[3] << 16), __float_as_uint(c3[0]), __float_as_uint(c3[1]), __float_as_uint(c3[2]));
+        if (kDepth) q_qq[e] = qq0;
       } else {
         rgb_buf[slot] = (kFish && !px_valid) ? 0u : pack_rgb(c3[0], c3[1], c3[2]);
+        if (kDepth) store_depth(dep, depth_of(qq0, px_valid), lane, bx, by, W, H);
       }
       qs += __popc(edges);
       DTS_COUNT(26, __popc(edges));
@@ -2121,7 +2163,7 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
         const int take = min(nq, 32);
         __syncwarp();   // the entries were written by other lanes
         unsigned qw[4] = {0u, 0u, 0u, 0u};   // (lanes without an entry: one winner, nothing to shade)
-        float q3[3] = {0.f, 0.f, 0.f};
+        float q3[3] = {0.f, 0.f, 0.f}, qmax = 0.0f;
         unsigned qslot = 0u;
         int qx = 0, qy = 0;
         if (lane < take) {
@@ -2130,9 +2172,13 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
           qslot = a.x; qx = (int)a.y; qy = (int)a.z;
           qw[0] = a.w & 0xffffu; qw[1] = a.w >> 16; qw[2] = c.x & 0xffffu; qw[3] = c.x >> 16;
           q3[0] = __uint_as_float(c.y); q3[1] = __uint_as_float(c.z); q3[2] = __uint_as_float(c.w);
+          if (kDepth) qmax = q_qq[e];
         }
-        resolve_edge(qw, q3, clr, prims, tex_pool, lat_tab, qx, qy, lane, err);
+        resolve_edge<kDepth>(qw, q3, clr, prims, tex_pool, lat_tab, qx, qy, lane, err, qmax);
         if (lane < take) rgb_buf[qslot] = pack_rgb(q3[0], q3[1], q3[2]);
+        // the queued pixel `qslot` = fine bin * 32 + lane-in-bin: its depth goes straight to the frame (queued pixels have a source)
+        if (kDepth && lane < take)
+          store_depth(dep, depth_of(qmax), (int)(qslot & 31u), cbx * kCFX + (int)((qslot >> 5) & 3u), cby * kCFY + (int)(qslot >> 7), W, H);
         qs += (unsigned)take << 16;
         __syncwarp();   // read before the next fine bin's entries overwrite the ring
       }
@@ -2368,15 +2414,23 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, ft, r.max_prims, r.pool, err_flag);
   mark();
   const bool wrap = (rc.obs_layout | rc.obs_dtype) != 0;
+  // a depth target (RenderCfg::depth) selects the depth-writing instance of each rasteriser; without one the launches
+  // are the same kernels as ever
+  const bool depth = rc.depth != nullptr;
   if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
-    const auto solo = fisheye ? k_raster_solo<true> : k_raster_solo<false>;
-    const auto flat = fisheye ? k_raster_flat<true> : k_raster_flat<false>;
+    const auto solo = depth ? (fisheye ? k_raster_solo<true, true> : k_raster_solo<false, true>)
+                            : (fisheye ? k_raster_solo<true, false> : k_raster_solo<false, false>);
+    const auto flat = depth ? (fisheye ? k_raster_flat<true, true> : k_raster_flat<false, true>)
+                            : (fisheye ? k_raster_flat<true, false> : k_raster_flat<false, false>);
     solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat);
     // before k_raster, which draws the bins k_raster_flat hands back
     flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, err_flag);
     launches += 2;
   }
-  const auto raster = fisheye ? (wrap ? k_raster<true, true> : k_raster<false, true>) : (wrap ? k_raster<true, false> : k_raster<false, false>);
+  const auto raster = depth ? (fisheye ? (wrap ? k_raster<true, true, true> : k_raster<false, true, true>)
+                                       : (wrap ? k_raster<true, false, true> : k_raster<false, false, true>))
+                            : (fisheye ? (wrap ? k_raster<true, true, false> : k_raster<false, true, false>)
+                                       : (wrap ? k_raster<true, false, false> : k_raster<false, false, false>));
   raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, ft, gather, obs, r.max_prims, r.pool, r.max_lat, err_flag);
   mark();
   mark();   // (post passes: launched by the caller)
@@ -2391,7 +2445,9 @@ Renderer* renderer_create(const dts_config& cfg) {
   cudaDeviceGetAttribute(&r->sms, cudaDevAttrMultiProcessorCount, cfg.device);
   r->cbins = ((r->W + kCoarseW - 1) / kCoarseW) * ((r->H + kCoarseH - 1) / kCoarseH);
   // k_raster's shared memory is past the 48 KB default; the opt-in holds for the kernel as loaded on this device
-  for (const auto raster : {k_raster<true, true>, k_raster<false, true>, k_raster<true, false>, k_raster<false, false>})
+  for (const auto raster : {k_raster<true, true, false>, k_raster<false, true, false>, k_raster<true, false, false>,
+                            k_raster<false, false, false>, k_raster<true, true, true>, k_raster<false, true, true>,
+                            k_raster<true, false, true>, k_raster<false, false, true>})
     cudaFuncSetAttribute(raster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
   return r;
 }

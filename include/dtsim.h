@@ -294,6 +294,19 @@ int dts_render(dts_sim* sim, void* obs_dev, void* stream);
  *                        dts_set_rectify_lut table; implies PINHOLE.  dts_render fails while no such table is set. */
 enum { DTS_RENDER_SEGMENT = 1, DTS_RENDER_TOP_DOWN = 2, DTS_RENDER_PINHOLE = 4, DTS_RENDER_RECTIFY = 8 };
 int dts_set_render_mode(dts_sim* sim, int mode);
+/* Depth image beside every observation (render spec item 9, DESIGN.md section 5): every later render of this handle —
+ * dts_render, dts_step, dts_step_terminal, whatever the render mode — also writes depth_dev, float32
+ * [num_envs][cam_height][cam_width], always in that layout and at the camera size whatever dts_set_output_format and
+ * dts_set_resize say.  A pixel holds the eye-space depth in metres (clip-space w, the distance along the view axis) of
+ * the nearest surface any of its four samples sees: 1 / (the largest 1/w, evaluated at the pixel centre exactly as
+ * shading evaluates it, among the distinct winners of the samples).  0: no sample is covered (sky), or the fisheye /
+ * rectification table names no source pixel.  No averaging, no quantisation, no far-plane clamp.  Lighting, textures and
+ * DTS_RENDER_SEGMENT leave it unchanged; the camera values of domain randomisation do not.  Sticky, like
+ * dts_set_render_mode.  The memory is the caller's and must stay valid while it is set; NULL (the default) turns depth
+ * off, and the renders launch the very kernels they launch without this call.  A pass over listed envs (the second pass
+ * of dts_step_terminal) writes only those envs' rows, so after dts_step_terminal row e matches obs_dev row e; the
+ * terminal frames' depth is not kept.  The fused gather (dts_gather_next) carries observations only. */
+int dts_set_depth_target(dts_sim* sim, float* depth_dev);
 /* Select the fused wrapper behaviour for subsequent dts_step / dts_render calls (default: all zero, scale 1).
  * obs_dev then holds num_envs * 3 * H * W elements of uint8 or float32 in the chosen layout. */
 int dts_set_output_format(dts_sim* sim, const dts_output_format* fmt);

@@ -1,0 +1,123 @@
+"""What the depth image costs (dts_set_depth_target: the rasterisers' depth instances, one f32 store per pixel).
+
+For each benchmark shape — c2: small_loop, c3: loop_obstacles (4096 envs, 160x120), c4: udem1, 640x480, fisheye, domain
+randomisation (`--c4-envs`, default 2048: the depth tensor is 1.2 MB per env there) — ONE env under device auto-reset
+and bench.py's uniform random actions in [-1, 1], stepped with the depth target off and on in alternating arms, `rounds`
+times.  The same handle runs both arms, so the arms differ in nothing but the kernels launched.
+Reports ms per step of each arm (host clock around `steps` steps ending in a synchronise, after `warmup` steps of that
+arm), the median and the spread (min .. max) over the rounds, and, from a separate pass under dts_profile_enable(2)
+(events at every kernel boundary, so not an end-to-end number), the ms per frame of each render kernel bracket; k_raster's
+bracket holds the three rasterisers.  Prints one JSON line with the card's name, power limit and SM clocks read before
+and after in the same run.
+
+    python tools/depth_probe.py [--configs c2,c3,c4] [--steps 100] [--warmup 10] [--rounds 5] [--out FILE.json]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from gym_duckietown_b200.batched_env import BatchedDuckietownEnv  # noqa: E402
+
+SHAPES = {
+    "c2": dict(map="small_loop", envs=4096, width=160, height=120, domain_rand=False, distortion=False),
+    "c3": dict(map="loop_obstacles", envs=4096, width=160, height=120, domain_rand=False, distortion=False),
+    "c4": dict(map="udem1", envs=2048, width=640, height=480, domain_rand=True, distortion=True),
+}
+ARMS = ["off", "on"]
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
+                        "-i", "0"], capture_output=True, text=True)
+    return q.stdout.strip() or torch.cuda.get_device_name(0)
+
+
+def set_arm(env, arm):
+    env.sim.set_depth_target(env.depth.data_ptr() if arm == "on" else None)
+
+
+def run(env, acts, steps, t0=0):
+    for t in range(steps):
+        env.step(acts[(t0 + t) % len(acts)])
+
+
+def device_ms(env, arm, acts, steps, warmup):
+    set_arm(env, arm)
+    run(env, acts, warmup)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    run(env, acts, steps, warmup)
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t0) / steps * 1e3
+
+
+def kernel_ms(env, arm, acts, steps):
+    """ms per frame of each render kernel bracket, events at every boundary."""
+    set_arm(env, arm)
+    run(env, acts, 5)
+    env.sim.profile(2)
+    env.sim.profile_read()
+    run(env, acts, steps)
+    ms, frames = env.sim.profile_read()
+    env.sim.profile(0)
+    return {k: v / max(frames, 1) for k, v in ms.items()}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--configs", default="c2,c3,c4")
+    ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--c4-envs", type=int, default=SHAPES["c4"]["envs"])
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        sys.exit("needs a CUDA device")
+    res = {"card": card(), "steps": a.steps, "warmup": a.warmup, "rounds": a.rounds, "actions": "uniform [-1, 1]", "configs": {}}
+    for cfg in a.configs.split(","):
+        c = dict(SHAPES[cfg])
+        if cfg == "c4":
+            c["envs"] = a.c4_envs
+        env = BatchedDuckietownEnv(c["envs"], c["map"], camera_width=c["width"], camera_height=c["height"],
+                                   domain_rand=c["domain_rand"], distortion=c["distortion"], seed=1, device_reset=True,
+                                   auto_reset=True, depth=True)
+        env.reset()
+        g = torch.Generator(device="cuda").manual_seed(0)
+        acts = torch.rand((16, c["envs"], 2), device="cuda", generator=g) * 2 - 1
+        runs = {k: [] for k in ARMS}
+        for r in range(a.rounds):
+            for arm in (ARMS if r % 2 == 0 else ARMS[::-1]):     # neither arm always runs first
+                runs[arm].append(device_ms(env, arm, acts, a.steps, a.warmup))
+            print(f"{cfg} round {r}: " + ", ".join(f"{k} {runs[k][-1]:.3f}" for k in ARMS) + " ms/step", file=sys.stderr, flush=True)
+        kern = {arm: kernel_ms(env, arm, acts, min(a.steps, 50)) for arm in ARMS}
+        env.check()
+        med = {k: float(np.median(v)) for k, v in runs.items()}
+        px = c["envs"] * c["width"] * c["height"]
+        res["configs"][cfg] = {
+            **c, "ms_per_step": runs, "median_ms_per_step": med,
+            "spread_ms_per_step": {k: [float(min(v)), float(max(v))] for k, v in runs.items()},
+            "on_minus_off_ms": med["on"] - med["off"], "on_over_off": med["on"] / med["off"],
+            "kernel_ms_per_frame": kern, "k_raster_on_minus_off_ms": kern["on"]["k_raster"] - kern["off"]["k_raster"],
+            "obs_bytes_per_step": px * 3, "depth_bytes_per_step": px * 4}
+        env.close()
+        del env
+        torch.cuda.empty_cache()
+    res["card_after"] = card()
+    line = json.dumps(res)
+    print(line, flush=True)
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    main()
