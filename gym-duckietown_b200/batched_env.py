@@ -4,7 +4,7 @@
 observation buffers are caller-visible torch CUDA tensors, the work runs on
 `torch.cuda.current_stream()` inside libdtsim.so, nothing synchronises.  Constructor keywords are the
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
-`auto_reset`, `device_reset`, `terminal_obs`, `depth`.
+`auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`.
 
 Under `auto_reset` the observation a step returns for an env whose episode ended is the first frame of its next
 episode.  `terminal_obs=True` also keeps the frame the reference's step() returns there (the terminal frame, before
@@ -20,6 +20,13 @@ the depth of the frame just rendered, so it follows `undistort`, the rectificati
 leaves it unchanged), and under `auto_reset` an ended env's row is its next episode's first frame, as in `obs`.  It stays
 at the camera size and in this layout under `set_resize` and `set_output_format`.  The depth of the terminal frames
 (`terminal_obs=True`) is not kept, and the multi-GPU gathers carry observations only.
+
+`labels=True` allocates `env.labels`, int16 [num_envs, camera_height, camera_width], filled by the same renders: which
+draw item each pixel shows (dts_set_label_target) — 0 nothing, 1 the ground, then one value per grid cell, per object of
+the map and for the agent's own mesh; `label_table(map_id)` names them.  It is the surface the depth image measures, so
+with both on `labels != 0` exactly where `depth != 0`; it follows the render modes, sizes and auto-reset as depth does,
+and lighting, textures, domain randomisation and `segment` leave it unchanged.  `object_boxes()` reduces it to every
+object's pixel count and bounding box.
 """
 from __future__ import annotations
 
@@ -30,7 +37,21 @@ import torch
 
 from . import lib as L
 from .episode import EpisodeSampler
-from .maps import MapData, load_map
+from .maps import TILE_KINDS, MapData, load_map
+
+
+def label_table(md: MapData) -> list:
+    """What each label value of the map stands for, indexed by the value (render spec item 10): ("none",), ("ground",),
+    ("tile", i, j, kind) for every grid cell (i outer, j inner; kind is None for an empty cell, whose label never
+    appears), ("object", o, kind) for entry o of the map's object list, and ("agent",) last."""
+    table = [("none",), ("ground",)]
+    for i in range(md.grid_w):
+        for j in range(md.grid_h):
+            k = int(md.tile_kind[j * md.grid_w + i])
+            table.append(("tile", i, j, TILE_KINDS[k] if k >= 0 else None))
+    table += [("object", o, ob.kind) for o, ob in enumerate(md.objects)]
+    table.append(("agent",))
+    return table
 
 
 class BatchedDuckietownEnv:
@@ -44,7 +65,7 @@ class BatchedDuckietownEnv:
                  action_mode: str = "vel_steer", auto_reset: bool = False, device_reset: bool = False,
                  cycle_maps: bool = False, env_id_offset: int = 0, tessellate_tiles: bool = False,
                  randomize_maps_on_reset: bool = False, randomization_config=None, terminal_obs: bool = False,
-                 depth: bool = False):
+                 depth: bool = False, labels: bool = False):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
         if camera_rand:
@@ -96,6 +117,9 @@ class BatchedDuckietownEnv:
             # the depth image of the frames in obs (depth=True); the renders write it on the device
             self.depth: Optional[torch.Tensor] = torch.zeros(
                 (num_envs, camera_height, camera_width), dtype=torch.float32, device=self.device) if depth else None
+            # the label image of the frames in obs (labels=True); the renders write it on the device
+            self.labels: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, camera_height, camera_width), dtype=torch.int16, device=self.device) if labels else None
             self.reward = torch.zeros(num_envs, dtype=torch.float32, device=self.device)
             self._done_u8 = torch.zeros(num_envs, dtype=torch.uint8, device=self.device)
             self.state: Dict[str, torch.Tensor] = {
@@ -114,6 +138,8 @@ class BatchedDuckietownEnv:
                                   action_vel_scale=1.0)
         if depth:
             self.sim.set_depth_target(self.depth.data_ptr())
+        if labels:
+            self.sim.set_label_target(self.labels.data_ptr())
         self.seed(seed)
 
     def set_output_format(self, obs_layout: Optional[str] = None, obs_dtype: Optional[str] = None,
@@ -287,6 +313,41 @@ class BatchedDuckietownEnv:
         else:
             self.sim.render(tgt.data_ptr(), self._stream())
         return tgt
+
+    # labels -------------------------------------------------------------------------------------
+    def label_table(self, map_id: int = 0) -> list:
+        """What each label value of map `map_id` stands for (module-level `label_table`)."""
+        return label_table(self.maps[map_id])
+
+    def object_boxes(self):
+        """From `labels` (labels=True), on the device: (pixels int32 [num_envs, max_objects], boxes int32 [num_envs,
+        max_objects, 4]) — how many pixels of each env's frame show object o of its map, and their bounding box x0, y0,
+        x1, y1 (inclusive); -1 where the object shows no pixel.  max_objects is the most objects any of the maps has."""
+        if self.labels is None:
+            raise ValueError("object_boxes needs labels=True")
+        n, h, w = self.labels.shape
+        n_obj = max((len(md.objects) for md in self.maps), default=0)
+        dev = self.device
+        cells = torch.tensor([md.grid_w * md.grid_h for md in self.maps], dtype=torch.int64, device=dev)
+        nobj = torch.tensor([len(md.objects) for md in self.maps], dtype=torch.int64, device=dev)
+        mid = self.state["map_id"].to(torch.int64)
+        o = self.labels.to(torch.int64) - 2 - cells[mid].view(n, 1, 1)        # object index, where the label is one
+        hit = (o >= 0) & (o < nobj[mid].view(n, 1, 1))
+        env = torch.arange(n, device=dev).view(n, 1, 1).expand(n, h, w)
+        ys = torch.arange(h, device=dev).view(1, h, 1).expand(n, h, w)
+        xs = torch.arange(w, device=dev).view(1, 1, w).expand(n, h, w)
+        slot = (env * max(n_obj, 1) + o)[hit]
+        pixels = torch.zeros(n * max(n_obj, 1), dtype=torch.int64, device=dev).scatter_add_(
+            0, slot, torch.ones_like(slot))
+        big = torch.iinfo(torch.int64).max
+        lo_x = torch.full_like(pixels, big).scatter_reduce_(0, slot, xs[hit], "amin")
+        lo_y = torch.full_like(pixels, big).scatter_reduce_(0, slot, ys[hit], "amin")
+        hi_x = torch.full_like(pixels, -1).scatter_reduce_(0, slot, xs[hit], "amax")
+        hi_y = torch.full_like(pixels, -1).scatter_reduce_(0, slot, ys[hit], "amax")
+        boxes = torch.stack([lo_x, lo_y, hi_x, hi_y], dim=1)
+        boxes[pixels == 0] = -1
+        return (pixels.view(n, -1)[:, :n_obj].to(torch.int32),
+                boxes.view(n, -1, 4)[:, :n_obj].to(torch.int32))
 
     # snapshots ----------------------------------------------------------------------------------
     @property

@@ -43,6 +43,7 @@ struct dts_sim {
   bool gather_next = false;
   int render_mode = 0;                  // dts_set_render_mode             // the next dts_render also stores into the gather buffers
   float* depth_target = nullptr;        // dts_set_depth_target: caller-owned f32 [N][cam_h][cam_w], or null
+  int16_t* label_target = nullptr;      // dts_set_label_target: caller-owned i16 [N][cam_h][cam_w], or null
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
   int profiling = 0;                    // 0 off, 1 events around k_raster only, 2 around every render kernel
   std::vector<cudaEvent_t> prof_events; // kProfMarks events per profiled frame
@@ -186,8 +187,14 @@ void dts_destroy(dts_sim* sim) {
   delete sim;
 }
 
+// The largest label (render spec item 10) of a map of these sizes: the agent's mesh, after the ground, cells and objects
+static long long largest_label(long long n_cells, long long n_objects) { return 2 + n_cells + n_objects; }
+
 int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
   if (!sim) return 1;
+  if (sim->label_target && b && largest_label((long long)b->grid_w * b->grid_h, b->n_objects) > INT16_MAX)
+    return sim->fail("a label target is set and this map's largest label, %lld, does not fit in int16",
+                     largest_label((long long)b->grid_w * b->grid_h, b->n_objects));
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   const std::string e = maps_upload(*sim->maps, map_id, b);
   if (!e.empty()) return sim->fail("%s", e.c_str());
@@ -318,8 +325,8 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
       gt.base[p] = reinterpret_cast<uint8_t*>(sim->gather_peer[p]) + (uint64_t)sim->gather_rank * sim->gather_bytes;
     sim->gather_next = false;
   }
-  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, target, gt, sim->d_err,
-                        sim->d_status, marks, mark_level, (cudaStream_t)stream);
+  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, sim->label_target, target, gt,
+                        sim->d_err, sim->d_status, marks, mark_level, (cudaStream_t)stream);
   if (rz.ow) {
     launch_resize(*sim->resize, rz.staging, obs_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, env_list, env_count,
                   (cudaStream_t)stream);
@@ -533,6 +540,20 @@ int dts_set_depth_target(dts_sim* sim, float* depth_dev) {
   if (!sim) return 1;
   if (reinterpret_cast<uintptr_t>(depth_dev) & 3) return sim->fail("depth target is not aligned to 4 bytes");
   sim->depth_target = depth_dev;
+  return 0;
+}
+
+int dts_set_label_target(dts_sim* sim, int16_t* labels_dev) {
+  if (!sim) return 1;
+  if (reinterpret_cast<uintptr_t>(labels_dev) & 1) return sim->fail("label target is not aligned to 2 bytes");
+  if (labels_dev) {
+    const std::vector<MapCounts>& counts = maps_counts(*sim->maps);
+    for (size_t s = 0; s < counts.size(); s++)
+      if (counts[s].n_tiles && largest_label(counts[s].n_tiles, counts[s].n_objects) > INT16_MAX)
+        return sim->fail("map slot %zu's largest label, %lld, does not fit in int16", s,
+                         largest_label(counts[s].n_tiles, counts[s].n_objects));
+  }
+  sim->label_target = labels_dev;
   return 0;
 }
 

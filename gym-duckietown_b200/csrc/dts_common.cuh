@@ -22,7 +22,9 @@ struct DObject {
   float centre[3];   // object-space bounding-sphere centre
   int32_t dyn_slot;  // -1 static; else slot of the per-env dynamic state that supplies pos / y_rot / card
   int32_t alt_from, alt_to;   // traffic-light card swap (texture ids), -1 none
-  int32_t seg_tex, pad_;      // flat class-colour texture of the mesh under segment=True (-1 none)
+  int32_t seg_tex;            // flat class-colour texture of the mesh under segment=True (-1 none)
+  int32_t tri_base;           // triangles of the map's objects before this one (the agent: of all of them), so that its
+                              // draw ids start at 2 + the tiles' ids + tri_base (label images, render spec item 10)
   double dpos[3];    // float64 position (x.pos in _inconvenient_spawn S:1466)
 };
 

@@ -116,9 +116,13 @@ std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, 
 std::string renderer_set_lut(Renderer& r, bool rectify, const float* rmapx, const float* rmapy);
 // `marks`: NULL or kProfMarks events recorded on `st` before k_frame_setup and after each of k_frame_setup, k_geometry,
 // k_bin, k_raster and the post passes (dts_profile_*).  `status_dev`: device address of the mapped host status word.
+// `labels`: NULL, or the label target (dts_set_label_target), i16 [n_envs][height][width], written beside obs like the
+// depth target, for the listed envs only where there is a list.  It is not a RenderCfg member: RenderCfg is every render
+// kernel's parameter block, and a longer one would move each kernel's later parameters.
 constexpr int kProfMarks = 6;
-int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, void* obs, const GatherTab& gather,
-                  int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level, cudaStream_t st);
+int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, int16_t* labels, void* obs,
+                  const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level,
+                  cudaStream_t st);
 // What the last render left in frame memory for one env (dts_debug_frame), after the device has synchronised
 std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, int32_t* counts, float* lattice_by_cell,
                              int n_cells);

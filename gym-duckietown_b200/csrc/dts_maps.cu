@@ -226,6 +226,7 @@ std::string maps_upload(MapSlots& ms, int slot, const dts_map_blob* blob) {
     const dts_object& s = b.objects[o];
     float top;
     DObject& d = objs[o] = mesh_object(b, s.mesh_id, top);
+    d.tri_base = (int32_t)counts.n_tris;   // (the objects' triangles so far: the agent's are added after the loop)
     for (int k = 0; k < 3; k++) { d.pos[k] = (float)s.pos[k]; d.dpos[k] = s.pos[k]; }   // glTranslatef takes floats
     d.dyn_slot = s.dyn_slot;
     d.alt_from = s.alt_tex_from; d.alt_to = s.alt_tex_to;
@@ -239,8 +240,9 @@ std::string maps_upload(MapSlots& ms, int slot, const dts_map_blob* blob) {
     float top;
     m.agent = mesh_object(b, b.agent_mesh, top);
     m.agent.scale = 1.0f; m.agent.dyn_slot = -1; m.agent.alt_from = m.agent.alt_to = -1;
-    counts.n_tris += m.agent.tri_count;
   }
+  m.agent.tri_base = (int32_t)counts.n_tris;   // the agent's draw ids follow every object's
+  counts.n_tris += m.agent.tri_count;
   std::vector<DTexture> tex(b.n_textures);
   std::vector<size_t> off(b.n_textures);
   size_t pool_size = 0;

@@ -30,8 +30,11 @@
 //
 // With a depth target (RenderCfg::depth, render spec item 9) the three rasterisers run their kDepth instances, which also
 // store every pixel's eye-space depth, f32 [N][H][W]; without one the launches and their kernels are the plain ones.
+// A label target (dts_set_label_target, render spec item 10) selects their kLabels instances in the same way, alone or
+// with kDepth: every pixel's draw item + 1, i16 [N][H][W].  The target reaches them as their last kernel parameter, not
+// through RenderCfg: a longer RenderCfg would move every later parameter of every render kernel.
 //
-// HBM traffic per env-frame: obs store W*H*3 B (compulsory; + W*H*4 B of depth where asked for) + PrimRec slab / BinRec lists / lattice table
+// HBM traffic per env-frame: obs store W*H*3 B (compulsory; + W*H*4 B of depth and W*H*2 B of labels where asked for) + PrimRec slab / BinRec lists / lattice table
 // (tens of KB per env, written by k_geometry / k_bin and read once by k_raster) + texels (shared, L2-resident).
 #include <algorithm>
 #include <cstddef>
@@ -843,6 +846,47 @@ __device__ __forceinline__ void store_depth(float* __restrict__ dep, float d, in
   if (gx < W && gy < H) dep[(size_t)gy * W + gx] = d;
 }
 
+// Label target (render spec item 10): a pixel's label is 1 + the draw item of the winner depth selects (the largest 1/w;
+// among equal ones the smallest label), 0 where no sample is covered or the gather has no source.  Items: the ground
+// (draw ids 0, 1), grid cell t = i * grid_h + j (tile_draw_ids ids each), object o (its tri_count ids each, from
+// tri_base on), the agent's mesh.  What a label instance needs of its env's map to turn a draw id into a label:
+struct LabelMap { const DObject* objects; int n_cells, n_objects, agent_base, tess; };
+__device__ __forceinline__ LabelMap label_map(const DMap& m, int tess) {
+  return LabelMap{m.objects, m.grid_w * m.grid_h, m.n_objects, m.agent.tri_base, tess};
+}
+// ground and road tiles only (all k_raster_flat ever sees)
+__device__ __forceinline__ int tile_label(int tess, int id) {
+  return id < 2 ? 1 : 2 + (tess ? (id - 2) / kTessTris : (id - 2) >> 1);
+}
+__device__ __forceinline__ int label_of_id(const LabelMap& lm, int id) {
+  const int r = id - 2 - tile_draw_ids(lm.tess != 0) * lm.n_cells;   // triangle index among the meshes' draw ids
+  if (r < 0) return tile_label(lm.tess, id);
+  if (r >= lm.agent_base) return 2 + lm.n_cells + lm.n_objects;
+  // the last object whose tri_base <= r (objects without triangles share the tri_base of the object after them)
+  int lo = 0, hi = lm.n_objects - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(&lm.objects[mid].tri_base) <= r) lo = mid; else hi = mid - 1;
+  }
+  return 2 + lm.n_cells + lo;
+}
+// One more winner `w` of a pixel (a prim index), its 1/w `qq` (> 0) and label_of(w): (qmax, lab) keeps the largest 1/w
+// and, among equal ones, the smallest label.  A maximum over exact values with an exact tie-break: the order does not
+// matter.
+template <typename LabelOf>
+__device__ __forceinline__ void take_label(float& qmax, int& lab, float qq, unsigned w, const LabelOf& label_of) {
+  if (!(qq >= qmax)) return;   // (a farther winner: its label is not looked up)
+  const int l = label_of(w);
+  if (qq > qmax || l < lab) { qmax = qq; lab = l; }
+}
+// The label frame `lf` (i16 [H][W] of one env): a lane stores its own pixel, 2 bytes.  The 8 lanes of a bin row write 16
+// contiguous bytes — half a 32-byte sector — so pairs packed into 4-byte stores with a shuffle would write the same
+// sectors, for a shuffle more per pixel.
+__device__ __forceinline__ void store_label(int16_t* __restrict__ lf, int v, int lane, int bx, int by, int W, int H) {
+  const int gx = bx * kBinW + (lane & 7), gy = by * kBinH + (lane >> 3);
+  if (gx < W && gy < H) lf[(size_t)gy * W + gx] = (int16_t)v;
+}
+
 // glClearColor: the env's horizon colour, or on the segment view glClearColor(255, 0, 255) clamped to magenta (S:1752)
 __device__ __forceinline__ void clear_colour(const DState& S, const RenderCfg& rc, int env, float clr[3]) {
   const bool seg = (rc.mode & DTS_RENDER_SEGMENT) != 0;
@@ -1553,11 +1597,13 @@ __device__ __forceinline__ int sample_mask(const BinRec& br, int pxc, int pyc) {
 // s01 = c(wn0) + c(wn1), s23 = c(wn2) + c(wn3).  Each shade depends only on (prim, position) and each half has two
 // addends, so neither the lane nor the order in which the winners are shaded changes a bit.  Called by the whole warp.
 // kDepth: `qmax` comes in as the first winner's 1/w (0: none) and leaves as the largest over the pixel's winners; a
-// maximum of exact values, so the order does not matter there either.
-template <bool kDepth>
+// maximum of exact values, so the order does not matter there either.  kLabels: the same, and `lab` comes in as the
+// first winner's label (0: none) and leaves as the pixel's (take_label; label_of(w): the label of prim w).
+template <bool kDepth, bool kLabels, typename LabelOf>
 __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], const float clr[3], const PrimRec* __restrict__ prims,
                                              const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa, int pya,
-                                             int lane, int32_t* __restrict__ err, float& qmax) {
+                                             int lane, int32_t* __restrict__ err, float& qmax, int* lab,
+                                             const LabelOf& label_of) {
   (void)lane; (void)err;   // (DTS_STATS counters)
   float s01[3] = {c3[0], c3[1], c3[2]}, s23[3] = {0.f, 0.f, 0.f};   // 0 + c == c
   unsigned pend = 0xeu;
@@ -1573,8 +1619,12 @@ __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], 
       const unsigned w = s == 1 ? wn[1] : (s == 2 ? wn[2] : wn[3]);
       float d3[3] = {clr[0], clr[1], clr[2]};
       float qq = 0.0f;
-      if (w != kNoPrim) shade_prim(prims, w, tex_pool, lat_tab, pxa, pya, d3, kDepth ? &qq : nullptr);
-      if (kDepth) qmax = fmaxf(qmax, qq);
+      if (w != kNoPrim) shade_prim(prims, w, tex_pool, lat_tab, pxa, pya, d3, (kDepth || kLabels) ? &qq : nullptr);
+      if (kLabels) {
+        if (w != kNoPrim) take_label(qmax, *lab, qq, w, label_of);
+      } else if (kDepth) {
+        qmax = fmaxf(qmax, qq);
+      }
 #pragma unroll
       for (int t = 1; t < 4; t++)
         if ((pend >> t & 1u) && wn[t] == w) {
@@ -1589,26 +1639,36 @@ __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], 
 }
 // The whole resolve of one fine bin's pixels (k_raster).  `simple`: the caller knows that every sample of the whole fine
 // bin has the same winner.  kDepth: `qmax` receives the largest 1/w among the pixel's winners, 0 if it has none.
-template <bool kDepth>
+// kLabels: `qmax` the same, and `lab` the pixel's label, 0 if it has no winner.
+template <bool kDepth, bool kLabels, typename LabelOf>
 __device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool simple, const float clr[3], const PrimRec* __restrict__ prims,
                                                   const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa,
-                                                  int pya, int lane, int32_t* __restrict__ err, float& qmax) {
+                                                  int pya, int lane, int32_t* __restrict__ err, float& qmax, int* lab,
+                                                  const LabelOf& label_of) {
   const bool same = wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0];
   const bool all_same = simple || __all_sync(0xffffffffu, same);
   float c3[3] = {clr[0], clr[1], clr[2]};
-  if (kDepth) qmax = 0.0f;
-  if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3, kDepth ? &qmax : nullptr);   // every lane: its first winner
-  if (!all_same) resolve_edge<kDepth>(wn, c3, clr, prims, tex_pool, lat_tab, pxa, pya, lane, err, qmax);   // (four equal samples: the mean is the value itself)
+  if (kDepth || kLabels) qmax = 0.0f;
+  if (kLabels) *lab = 0;
+  if (wn[0] != kNoPrim) {   // every lane: its first winner
+    shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3, (kDepth || kLabels) ? &qmax : nullptr);
+    if (kLabels) *lab = label_of(wn[0]);
+  }
+  if (!all_same)   // (four equal samples: the mean is the value itself)
+    resolve_edge<kDepth, kLabels>(wn, c3, clr, prims, tex_pool, lat_tab, pxa, pya, lane, err, qmax, lab, label_of);
   return pack_rgb(c3[0], c3[1], c3[2]);
 }
 
 // ------------------------------------------------------------------------------------------------ k_raster
-template <bool kWrapFmt, bool kFish, bool kDepth>   // kWrapFmt: a dts_output_format other than packed u8 HWC is written by the resolve;
+template <bool kWrapFmt, bool kFish, bool kDepth, bool kLabels>
+                                       // kWrapFmt: a dts_output_format other than packed u8 HWC is written by the resolve;
                                        // kFish: every lane renders the SOURCE pixel the fisheye LUT names for its output pixel;
-                                       // kDepth: every pixel's depth goes to rc.depth beside its colour (render spec item 9)
+                                       // kDepth: every pixel's depth goes to rc.depth beside its colour (render spec item 9);
+                                       // kLabels: every pixel's label goes to `labels` (render spec item 10)
 __global__ void __launch_bounds__(kThreads, kRasterMinCtas)
 k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, FishTab ft, GatherTab gt,
-         uint8_t* __restrict__ obs, int max_prims, int max_pairs, int max_lat, int32_t* __restrict__ err) {
+         uint8_t* __restrict__ obs, int max_prims, int max_pairs, int max_lat, int32_t* __restrict__ err,
+         int16_t* __restrict__ labels) {
   // dynamic shared memory (kRasterSmem bytes): per warp two chunks of records in flight, their mbarriers, and a 128-sample
   // depth / winner buffer for the tiny triangles of the fine bin being drawn
   extern __shared__ __align__(128) unsigned char raster_smem[];
@@ -1649,13 +1709,18 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
     const size_t env_off = (size_t)env * frame_bytes * out_elem;
     uint8_t* out = obs + env_off;
     float* dep = kDepth ? rc.depth + (size_t)env * W * H : nullptr;
+    int16_t* lf = kLabels ? labels + (size_t)env * W * H : nullptr;
+    LabelMap lm{};
+    if constexpr (kLabels) lm = label_map(m, rc.tessellate);
+    auto label_of = [&](unsigned w) { return label_of_id(lm, __ldg(&prims[w].id)); };
     // one fine bin -> the caller's tensor and, on a gathering step, every peer's gather buffer (NVLink stores)
     // On a gathering step (gt.n > 0) the packed u8 HWC frame goes to the peers in BLOCKS: a work item is 8 whole image rows =
     // one contiguous run of bytes, copied to every rank's gather buffer with 16-byte vector stores once the item is drawn
     // (NVLink wants long writes: per-bin 4-byte stores reach a fifth of the link rate).  Other layouts store per bin.
     const bool gather_rows = gt.n > 0 && !kWrapFmt;
-    auto emit = [&](unsigned rgb, float depth, int bx, int by) {
+    auto emit = [&](unsigned rgb, float depth, int label, int bx, int by) {
       if (kDepth) store_depth(dep, depth, lane, bx, by, W, H);   // (the caller's depth tensor only: the gather carries obs)
+      if (kLabels) store_label(lf, label, lane, bx, by, W, H);
       if (fast_fmt && (gt.n == 0 || gather_rows) && bx * kBinW + kBinW <= W) {   // the common case inline: packed u8 HWC, whole bin inside
         store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
       } else if (kWrapFmt && gt.n == 0) {
@@ -1723,7 +1788,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
             const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);
             unsigned rgb = clear_rgb;
             if (kFish && !fish_source(ft, bx, by, lane, W, H).valid) rgb = 0u;
-            emit(rgb, 0.0f, bx, by);
+            emit(rgb, 0.0f, 0, bx, by);
           }
         continue;
       }
@@ -1934,9 +1999,11 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
             // ---- deferred shading: once per distinct winner of this pixel, then the box resolve
             DTS_COUNT(11, 1);
             float qmax = 0.0f;
-            unsigned rgb = shade_resolve<kDepth>(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane, err, qmax);
+            int lab = 0;
+            unsigned rgb = shade_resolve<kDepth, kLabels>(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane, err,
+                                                          qmax, &lab, label_of);
             if (kFish && !px_valid) rgb = 0u;   // cv2.remap BORDER_CONSTANT
-            emit(rgb, kDepth ? depth_of(qmax, px_valid) : 0.0f, bx, by);
+            emit(rgb, kDepth ? depth_of(qmax, px_valid) : 0.0f, px_valid ? lab : 0, bx, by);
           }
         }
       }
@@ -1955,10 +2022,13 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
 // visibility state: a warp fetches the prim's planes once and shades the bin's 256 pixels.  A separate kernel so that the
 // lean loop gets its own register allocation (the same fast path inside k_raster cost more than it saved).
 // Packed u8 HWC output with whole-word rows only (k_bin marks no bin otherwise).  Runs before k_raster.
-template <bool kFish, bool kDepth>   // kFish: each lane shades the source pixel the fisheye LUT names for its output pixel;
-                                     // kDepth: the 1/w the shading divides by also gives the pixel's depth (rc.depth)
+template <bool kFish, bool kDepth, bool kLabels>
+                                     // kFish: each lane shades the source pixel the fisheye LUT names for its output pixel;
+                                     // kDepth: the 1/w the shading divides by also gives the pixel's depth (rc.depth);
+                                     // kLabels: the bin's one prim gives every pixel with a source its label (`labels`)
 __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
-                                                                        FishTab ft, uint8_t* __restrict__ obs, int max_prims, int max_lat) {
+                                                                        FishTab ft, uint8_t* __restrict__ obs, int max_prims, int max_lat,
+                                                                        int16_t* __restrict__ labels) {
   const int W = rc.width, H = rc.height;
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW;
   const int lane = threadIdx.x & 31;
@@ -1975,6 +2045,9 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     const ShadeIn si = load_shade(fm.prims + (size_t)env * max_prims, p);
     uint8_t* out = obs + (size_t)env * frame_bytes;
+    int lab = 0;
+    if constexpr (kLabels)
+      lab = label_of_id(label_map(maps[S.map_id[env]], rc.tessellate), __ldg(&fm.prims[(size_t)env * max_prims + p].id));
     // fine bins inside the image as loop bounds rather than fine_in_image(): the mask test costs this loop machine code
     const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);
     const int ny = ((cby * kCFY + 1) * kBinH < H) ? 2 : 1;
@@ -1996,6 +2069,7 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
       if (kFish && !px_valid) rgb = 0u;
       store_bin_lean(out, sl, rgb, lane, bx, by, W, H);
       if (kDepth) store_depth(rc.depth + (size_t)env * W * H, depth_of(qq, px_valid), lane, bx, by, W, H);
+      if (kLabels) store_label(labels + (size_t)env * W * H, px_valid ? lab : 0, lane, bx, by, W, H);
     }
   }
 }
@@ -2020,12 +2094,15 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
 // and a queued pixel's when its other winners are resolved; the queue carries the first winner's 1/w in a third array
 // (2 KB: 46 KB per CTA, still four CTAs per SM).  A bin handed back may have stored some depths already: k_raster
 // rewrites the whole bin, colour and depth.
+// kLabels: the same for labels, with no more shared memory.  A queued pixel's first label is looked up again from its
+// first winner, which the queue holds; its 1/w comes from the depth array (kept for labels alone, too).  Only the ground
+// and road tiles come here, so a label is arithmetic on the draw id (tile_label).
 // Packed u8 HWC output with whole-word rows only (k_bin lists no bin otherwise).  Runs after k_raster_solo.
 constexpr int kEdgeQ = 64;   // queue ring: flushed at 32 entries, so at most 31 + 32 wait at once
-template <bool kFish, bool kDepth>   // kFish: each lane covers and shades the source pixel the fisheye LUT names for its output pixel
+template <bool kFish, bool kDepth, bool kLabels>   // kFish: each lane covers and shades the source pixel the fisheye LUT names for its output pixel
 __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
                                                                         FishTab ft, uint8_t* __restrict__ obs, int max_prims, int max_lat,
-                                                                        int32_t* __restrict__ err) {
+                                                                        int32_t* __restrict__ err, int16_t* __restrict__ labels) {
   __shared__ BinRec stages[kWarps][kStage];   // per warp: the records of its bin
   __shared__ unsigned bin_rgb[kWarps][kCFX * kCFY * 32];   // per warp: packed colour of pixel `lane` of fine bin f at f * 32 + lane
   // per warp: the edge-pixel queue, an entry in two words: (pixel slot, pxa, pya, wn0 | wn1 << 16), (wn2 | wn3 << 16, first colour)
@@ -2036,8 +2113,8 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
   BinRec* stage = stages[threadIdx.x >> 5];
   unsigned* rgb_buf = bin_rgb[threadIdx.x >> 5];
   uint4 (*q)[kEdgeQ] = edge_q[threadIdx.x >> 5];
-  float* q_qq = nullptr;   // kDepth: per queue entry, the first winner's 1/w
-  if constexpr (kDepth) {
+  float* q_qq = nullptr;   // kDepth, kLabels: per queue entry, the first winner's 1/w
+  if constexpr (kDepth || kLabels) {
     __shared__ float edge_qq[kWarps][kEdgeQ];
     q_qq = edge_qq[threadIdx.x >> 5];
   }
@@ -2070,6 +2147,8 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     uint8_t* out = obs + (size_t)env * frame_bytes;
     float* dep = kDepth ? rc.depth + (size_t)env * W * H : nullptr;
+    int16_t* lf = kLabels ? labels + (size_t)env * W * H : nullptr;
+    auto label_of = [&](unsigned w) { return tile_label(rc.tessellate, __ldg(&prims[w].id)); };
     float clr[3];
     clear_colour(S, rc, env, clr);
     int ox = cbx * kCoarseW * kSub, oy = cby * kCoarseH * kSub;   // coarse bin corner, sub-pixels
@@ -2141,7 +2220,7 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
       // ---- every lane: its first winner.  One winner: the pixel is done.  More: it waits in the queue.  (A pixel the
       // fisheye LUT gives no source is black either way.)
       float c3[3] = {clr[0], clr[1], clr[2]}, qq0 = 0.0f;
-      if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, ox + pxc, oy + pyc, c3, kDepth ? &qq0 : nullptr);
+      if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, ox + pxc, oy + pyc, c3, (kDepth || kLabels) ? &qq0 : nullptr);
       const bool edge = px_valid && !(wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0]);
       const unsigned edges = __ballot_sync(0xffffffffu, edge);
       const unsigned slot = f * 32 + lane;
@@ -2149,10 +2228,11 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
         const int e = (qs + __popc(edges & ((1u << lane) - 1u))) & (kEdgeQ - 1);
         q[0][e] = make_uint4(slot, (unsigned)(ox + pxc), (unsigned)(oy + pyc), wn[0] | (wn[1] << 16));
         q[1][e] = make_uint4(wn[2] | (wn[3] << 16), __float_as_uint(c3[0]), __float_as_uint(c3[1]), __float_as_uint(c3[2]));
-        if (kDepth) q_qq[e] = qq0;
+        if (kDepth || kLabels) q_qq[e] = qq0;
       } else {
         rgb_buf[slot] = (kFish && !px_valid) ? 0u : pack_rgb(c3[0], c3[1], c3[2]);
         if (kDepth) store_depth(dep, depth_of(qq0, px_valid), lane, bx, by, W, H);
+        if (kLabels) store_label(lf, (px_valid && wn[0] != kNoPrim) ? label_of(wn[0]) : 0, lane, bx, by, W, H);
       }
       qs += __popc(edges);
       DTS_COUNT(26, __popc(edges));
@@ -2164,6 +2244,7 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
         __syncwarp();   // the entries were written by other lanes
         unsigned qw[4] = {0u, 0u, 0u, 0u};   // (lanes without an entry: one winner, nothing to shade)
         float q3[3] = {0.f, 0.f, 0.f}, qmax = 0.0f;
+        int qlab = 0;
         unsigned qslot = 0u;
         int qx = 0, qy = 0;
         if (lane < take) {
@@ -2172,13 +2253,17 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
           qslot = a.x; qx = (int)a.y; qy = (int)a.z;
           qw[0] = a.w & 0xffffu; qw[1] = a.w >> 16; qw[2] = c.x & 0xffffu; qw[3] = c.x >> 16;
           q3[0] = __uint_as_float(c.y); q3[1] = __uint_as_float(c.z); q3[2] = __uint_as_float(c.w);
-          if (kDepth) qmax = q_qq[e];
+          if (kDepth || kLabels) qmax = q_qq[e];
+          if (kLabels && qw[0] != kNoPrim) qlab = label_of(qw[0]);
         }
-        resolve_edge<kDepth>(qw, q3, clr, prims, tex_pool, lat_tab, qx, qy, lane, err, qmax);
+        resolve_edge<kDepth, kLabels>(qw, q3, clr, prims, tex_pool, lat_tab, qx, qy, lane, err, qmax, &qlab, label_of);
         if (lane < take) rgb_buf[qslot] = pack_rgb(q3[0], q3[1], q3[2]);
-        // the queued pixel `qslot` = fine bin * 32 + lane-in-bin: its depth goes straight to the frame (queued pixels have a source)
+        // the queued pixel `qslot` = fine bin * 32 + lane-in-bin: its depth and label go straight to the frame (queued
+        // pixels have a source)
         if (kDepth && lane < take)
           store_depth(dep, depth_of(qmax), (int)(qslot & 31u), cbx * kCFX + (int)((qslot >> 5) & 3u), cby * kCFY + (int)(qslot >> 7), W, H);
+        if (kLabels && lane < take)
+          store_label(lf, qlab, (int)(qslot & 31u), cbx * kCFX + (int)((qslot >> 5) & 3u), cby * kCFY + (int)(qslot >> 7), W, H);
         qs += (unsigned)take << 16;
         __syncwarp();   // read before the next fine bin's entries overwrite the ring
       }
@@ -2376,8 +2461,9 @@ std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, in
   return rc ? "debug_frame_copy failed" : "";
 }
 
-int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, void* obs_any, const GatherTab& gather,
-                  int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level, cudaStream_t st) {
+int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, int16_t* labels, void* obs_any,
+                  const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level,
+                  cudaStream_t st) {
   uint8_t* obs = reinterpret_cast<uint8_t*>(obs_any);
   // the gather the frame goes through, if any: the rectification (DTS_RENDER_RECTIFY), none (DTS_RENDER_PINHOLE or no
   // DTS_FLAG_DISTORTION) or the fisheye.  Both tables run the same kFish kernels.
@@ -2417,21 +2503,35 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   // a depth target (RenderCfg::depth) selects the depth-writing instance of each rasteriser; without one the launches
   // are the same kernels as ever
   const bool depth = rc.depth != nullptr;
+  // so does a label target, alone or with depth
+  const int out = (depth ? 1 : 0) | (labels ? 2 : 0);
   if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
-    const auto solo = depth ? (fisheye ? k_raster_solo<true, true> : k_raster_solo<false, true>)
-                            : (fisheye ? k_raster_solo<true, false> : k_raster_solo<false, false>);
-    const auto flat = depth ? (fisheye ? k_raster_flat<true, true> : k_raster_flat<false, true>)
-                            : (fisheye ? k_raster_flat<true, false> : k_raster_flat<false, false>);
-    solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat);
+    const auto solo_of = [&](auto fish) {
+      constexpr bool f = decltype(fish)::value;
+      return out == 3 ? k_raster_solo<f, true, true> : out == 2 ? k_raster_solo<f, false, true>
+                                                     : out == 1 ? k_raster_solo<f, true, false> : k_raster_solo<f, false, false>;
+    };
+    const auto flat_of = [&](auto fish) {
+      constexpr bool f = decltype(fish)::value;
+      return out == 3 ? k_raster_flat<f, true, true> : out == 2 ? k_raster_flat<f, false, true>
+                                                     : out == 1 ? k_raster_flat<f, true, false> : k_raster_flat<f, false, false>;
+    };
+    const auto solo = fisheye ? solo_of(std::true_type{}) : solo_of(std::false_type{});
+    const auto flat = fisheye ? flat_of(std::true_type{}) : flat_of(std::false_type{});
+    solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, labels);
     // before k_raster, which draws the bins k_raster_flat hands back
-    flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, err_flag);
+    flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, err_flag, labels);
     launches += 2;
   }
-  const auto raster = depth ? (fisheye ? (wrap ? k_raster<true, true, true> : k_raster<false, true, true>)
-                                       : (wrap ? k_raster<true, false, true> : k_raster<false, false, true>))
-                            : (fisheye ? (wrap ? k_raster<true, true, false> : k_raster<false, true, false>)
-                                       : (wrap ? k_raster<true, false, false> : k_raster<false, false, false>));
-  raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, ft, gather, obs, r.max_prims, r.pool, r.max_lat, err_flag);
+  const auto raster_of = [&](auto wrap_fmt, auto fish) {
+    constexpr bool w = decltype(wrap_fmt)::value, f = decltype(fish)::value;
+    return out == 3 ? k_raster<w, f, true, true> : out == 2 ? k_raster<w, f, false, true>
+                                                 : out == 1 ? k_raster<w, f, true, false> : k_raster<w, f, false, false>;
+  };
+  const auto raster = fisheye ? (wrap ? raster_of(std::true_type{}, std::true_type{}) : raster_of(std::false_type{}, std::true_type{}))
+                              : (wrap ? raster_of(std::true_type{}, std::false_type{}) : raster_of(std::false_type{}, std::false_type{}));
+  raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, ft, gather, obs, r.max_prims, r.pool, r.max_lat, err_flag,
+                                                                labels);
   mark();
   mark();   // (post passes: launched by the caller)
   return launches;
@@ -2445,10 +2545,14 @@ Renderer* renderer_create(const dts_config& cfg) {
   cudaDeviceGetAttribute(&r->sms, cudaDevAttrMultiProcessorCount, cfg.device);
   r->cbins = ((r->W + kCoarseW - 1) / kCoarseW) * ((r->H + kCoarseH - 1) / kCoarseH);
   // k_raster's shared memory is past the 48 KB default; the opt-in holds for the kernel as loaded on this device
-  for (const auto raster : {k_raster<true, true, false>, k_raster<false, true, false>, k_raster<true, false, false>,
-                            k_raster<false, false, false>, k_raster<true, true, true>, k_raster<false, true, true>,
-                            k_raster<true, false, true>, k_raster<false, false, true>})
-    cudaFuncSetAttribute(raster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
+  const auto opt_in = [](auto wrap_fmt, auto fish) {
+    constexpr bool w = decltype(wrap_fmt)::value, f = decltype(fish)::value;
+    for (const auto raster : {k_raster<w, f, false, false>, k_raster<w, f, true, false>, k_raster<w, f, false, true>,
+                              k_raster<w, f, true, true>})
+      cudaFuncSetAttribute(raster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
+  };
+  opt_in(std::true_type{}, std::true_type{}); opt_in(std::false_type{}, std::true_type{});
+  opt_in(std::true_type{}, std::false_type{}); opt_in(std::false_type{}, std::false_type{});
   return r;
 }
 

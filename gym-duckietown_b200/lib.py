@@ -183,6 +183,7 @@ def load() -> C.CDLL:
     lib.dts_set_resize_filter.argtypes = [vp, i, i, i]
     lib.dts_set_render_mode.argtypes = [vp, i]
     lib.dts_set_depth_target.argtypes = [vp, vp]
+    lib.dts_set_label_target.argtypes = [vp, vp]
     lib.dts_resize_frames.argtypes = [vp, vp, vp, vp]
     lib.dts_blend4.argtypes = [vp, vp, vp, vp, C.c_uint64, vp]
     lib.dts_set_timing.argtypes = [vp, C.c_double, i, i]
@@ -217,7 +218,7 @@ def load() -> C.CDLL:
 
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
-           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
+           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
            "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
 
@@ -456,6 +457,11 @@ class Sim:
         """Every later render also writes float32 [num_envs, cam_height, cam_width] eye-space depth at `depth_ptr`, which
         the caller keeps alive; None turns it off (dts_set_depth_target)."""
         self._check(self.lib.dts_set_depth_target(self.h, depth_ptr), "dts_set_depth_target")
+
+    def set_label_target(self, labels_ptr: Optional[int]):
+        """Every later render also writes int16 [num_envs, cam_height, cam_width] labels (which draw item each pixel
+        shows) at `labels_ptr`, which the caller keeps alive; None turns it off (dts_set_label_target)."""
+        self._check(self.lib.dts_set_label_target(self.h, labels_ptr), "dts_set_label_target")
 
     def set_resize(self, out_w: int, out_h: int, filter: int = 0):
         """filter RESIZE_CV2_CUBIC (dts_set_resize) or RESIZE_PIL_BILINEAR (dts_set_resize_filter)."""

@@ -70,7 +70,8 @@ class Simulator(Env):
                  seed: Optional[int] = None, distortion: bool = False, dynamics_rand: bool = False,
                  camera_rand: bool = False, randomize_maps_on_reset: bool = False, num_tris_distractors: int = 12,
                  color_ground=(0.15, 0.15, 0.15), color_sky=(0.45, 0.82, 1), style: str = "photos",
-                 enable_leds: bool = False, device: int = 0, depth: bool = False, **env_kwargs):
+                 enable_leds: bool = False, device: int = 0, depth: bool = False, labels: bool = False,
+                 **env_kwargs):
         if draw_curve or draw_bbox or enable_leds:
             raise NotImplementedError("draw_curve / draw_bbox / enable_leds are debug modes outside the hot path "
                                       "(SURVEY 8f-4)")
@@ -95,7 +96,7 @@ class Simulator(Env):
             accept_start_angle_deg=accept_start_angle_deg, user_tile_start=user_tile_start, seed=seed,
             distortion=distortion, dynamics_rand=dynamics_rand, camera_rand=camera_rand,
             color_ground=color_ground, color_sky=color_sky, num_tris_distractors=num_tris_distractors,
-            action_mode=self._action_mode, depth=depth, **env_kwargs)
+            action_mode=self._action_mode, depth=depth, labels=labels, **env_kwargs)
         self._b = BatchedDuckietownEnv(1, map_arg, **self._env_kwargs)
         self._adopt_map()
         self.action_space = spaces.Box(low=-1, high=1, shape=(2,), dtype=np.float32)              # S:309
@@ -157,7 +158,7 @@ class Simulator(Env):
         from .batched_env import BatchedDuckietownEnv
         if getattr(self, "_human", None) is None:
             kw = dict(self._env_kwargs, camera_width=WINDOW_WIDTH, camera_height=WINDOW_HEIGHT, distortion=False,
-                      terminal_obs=False, depth=False)
+                      terminal_obs=False, depth=False, labels=False)
             self._human = BatchedDuckietownEnv(1, list(self._b.maps), **kw)
         self._human.load_state(self._b.save_state())
         return self._human
@@ -201,6 +202,13 @@ class Simulator(Env):
         reset / step / render_obs (BatchedDuckietownEnv.depth); else None."""
         d = self._b.depth
         return None if d is None else d[0].cpu().numpy()
+
+    @property
+    def labels(self) -> Optional[np.ndarray]:
+        """With labels=True: int16 [camera_height, camera_width], the label image of the observation last returned by
+        reset / step / render_obs (BatchedDuckietownEnv.labels, named by BatchedDuckietownEnv.label_table); else None."""
+        lb = self._b.labels
+        return None if lb is None else lb[0].cpu().numpy()
 
     @property
     def cur_pos(self):

@@ -307,6 +307,22 @@ int dts_set_render_mode(dts_sim* sim, int mode);
  * of dts_step_terminal) writes only those envs' rows, so after dts_step_terminal row e matches obs_dev row e; the
  * terminal frames' depth is not kept.  The fused gather (dts_gather_next) carries observations only. */
 int dts_set_depth_target(dts_sim* sim, float* depth_dev);
+/* Label image beside every observation (render spec item 10, DESIGN.md section 5): every later render of this handle —
+ * dts_render, dts_step, dts_step_terminal, whatever the render mode — also writes labels_dev, int16
+ * [num_envs][cam_height][cam_width], always in that layout and at the camera size whatever dts_set_output_format and
+ * dts_set_resize say.  A pixel holds which draw item it shows: 0 none (no sample covered, or the fisheye / rectification
+ * table names no source pixel), 1 the ground quad, 2 + i * grid_h + j the road tile at grid cell (i, j), 2 + n_cells + o
+ * object o of the map's object list (dts_map_blob.objects, static and dynamic alike), 2 + n_cells + n_objects the agent's
+ * own mesh (top-down views), where n_cells = grid_w * grid_h.  Of the distinct winners of the pixel's four samples it is
+ * the one with the largest 1/w at the pixel centre (the surface dts_set_depth_target's depth is taken from), and among
+ * equal ones the smallest label; so with both targets set, label != 0 exactly where depth != 0.  No averaging at edges.
+ * Lighting, textures, domain-randomised colours and DTS_RENDER_SEGMENT leave it unchanged.  Sticky, like
+ * dts_set_render_mode.  The memory is the caller's, 2-byte aligned, and must stay valid while it is set; NULL (the
+ * default) turns labels off, and the renders launch the very kernels they launch without this call.  Refused while an
+ * uploaded map's largest label exceeds 32767, and while it is set dts_upload_map refuses such a map.  A pass over listed
+ * envs (the second pass of dts_step_terminal) writes only those envs' rows, so after dts_step_terminal row e matches
+ * obs_dev row e; the terminal frames' labels are not kept.  The fused gather (dts_gather_next) carries observations only. */
+int dts_set_label_target(dts_sim* sim, int16_t* labels_dev);
 /* Select the fused wrapper behaviour for subsequent dts_step / dts_render calls (default: all zero, scale 1).
  * obs_dev then holds num_envs * 3 * H * W elements of uint8 or float32 in the chosen layout. */
 int dts_set_output_format(dts_sim* sim, const dts_output_format* fmt);
