@@ -4,7 +4,16 @@
 observation buffers are caller-visible torch CUDA tensors, the work runs on
 `torch.cuda.current_stream()` inside libdtsim.so, nothing synchronises.  Constructor keywords are the
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
-`auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`.
+`auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `camera_rand_pool`.
+
+`camera_rand=True` (with `distortion=True`; without it the flag does nothing, as in the reference, S:352-358) gives the
+envs a spread of lenses: `camera_rand_pool` calibrations K, D are drawn once, at construction, within the reference's
+ranges (distortion.py:58-83; `distortion.draw_calibrations`, from a stream seeded by `seed`), each gets the fisheye LUT
+the reference builds for it, and env g (global index, `env_id_offset + e`) is gathered through calibration
+`g % camera_rand_pool` in every render — frames, depth and labels.  camera_rand_pool = num_envs is the reference's one
+camera per Simulator.  Resets then apply the drawn camera height / angle / FOV even without domain_rand (S:611-614).
+The calibration belongs to the env, not to its state: snapshots do not carry it, and an env keeps its own across
+`load_state` / `copy_envs`.  Building the LUTs takes about 0.5 s per calibration at 160x120 and 1-2 s at 640x480.
 
 Under `auto_reset` the observation a step returns for an env whose episode ended is the first frame of its next
 episode.  `terminal_obs=True` also keeps the frame the reference's step() returns there (the terminal frame, before
@@ -65,11 +74,13 @@ class BatchedDuckietownEnv:
                  action_mode: str = "vel_steer", auto_reset: bool = False, device_reset: bool = False,
                  cycle_maps: bool = False, env_id_offset: int = 0, tessellate_tiles: bool = False,
                  randomize_maps_on_reset: bool = False, randomization_config=None, terminal_obs: bool = False,
-                 depth: bool = False, labels: bool = False):
+                 depth: bool = False, labels: bool = False, camera_rand_pool: int = 16):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
-        if camera_rand:
-            raise NotImplementedError("camera_rand needs carnivalmirror (distortion.py:58-83); out of scope")
+        camera_rand = bool(camera_rand and distortion)   # S:353-356: camera_rand only with distortion
+        if camera_rand and not 1 <= int(camera_rand_pool) <= 65536:
+            raise ValueError(f"camera_rand_pool must be 1 to 65536, not {camera_rand_pool}")
+        self.camera_rand = camera_rand
         names = [map_name] if isinstance(map_name, (str, MapData)) else list(map_name)
         self.maps: List[MapData] = [n if isinstance(n, MapData) else load_map(n) for n in names]   # parsed maps pass through
         self.num_envs, self.device_index = num_envs, device
@@ -90,7 +101,7 @@ class BatchedDuckietownEnv:
         self._keep_terminal = terminal_obs
         flags = (L.FLAG_AUTO_RESET if auto_reset else 0) | (L.FLAG_DOMAIN_RAND if domain_rand else 0) | \
                 (L.FLAG_DISTORTION if distortion else 0) | (L.FLAG_DYNAMICS_RAND if dynamics_rand else 0) | \
-                (L.FLAG_TESSELLATE if tessellate_tiles else 0)
+                (L.FLAG_TESSELLATE if tessellate_tiles else 0) | (L.FLAG_CAMERA_RAND if camera_rand else 0)
         self.cfg = L.default_config(
             num_envs=num_envs, device=device, cam_width=camera_width, cam_height=camera_height, max_steps=max_steps,
             frame_skip=int(frame_skip), action_mode=L.ACTION_VEL_STEER if action_mode == "vel_steer" else L.ACTION_PWM,
@@ -106,7 +117,17 @@ class BatchedDuckietownEnv:
         self.sim = L.Sim(self.cfg)
         for i, md in enumerate(self.maps):
             self.sim.upload_map(i, md, tuple(user_tile_start) if user_tile_start else None)
-        if distortion:
+        # camera_rand: the calibrations (K, D) of the pool and the one of every env, else None
+        self.calibrations: Optional[list] = None
+        self.calibration_of_env: Optional[np.ndarray] = None
+        if camera_rand:
+            from .distortion import Distortion, draw_calibrations
+            self.calibrations = draw_calibrations(int(camera_rand_pool), seed)
+            self.camera_models = [Distortion(camera_width, camera_height, K, D) for K, D in self.calibrations]
+            self.calibration_of_env = (env_id_offset + np.arange(num_envs)) % len(self.calibrations)
+            self.sim.set_fisheye_luts(np.stack([m.rmapx for m in self.camera_models]),
+                                      np.stack([m.rmapy for m in self.camera_models]), self.calibration_of_env)
+        elif distortion:
             from .distortion import Distortion
             self.camera_model = Distortion(camera_width, camera_height)
             self.sim.set_fisheye_lut(self.camera_model.rmapx, self.camera_model.rmapy)
@@ -125,7 +146,8 @@ class BatchedDuckietownEnv:
             self.state: Dict[str, torch.Tensor] = {
                 k_: torch.as_tensor(v, device=self.device) for k_, v in self.sim.state_arrays().items()}
         self.sampler = EpisodeSampler(
-            num_envs, domain_rand=domain_rand, dynamics_rand=dynamics_rand, accept_start_angle_deg=accept_start_angle_deg,
+            num_envs, domain_rand=domain_rand, dynamics_rand=dynamics_rand, camera_rand=camera_rand,
+            accept_start_angle_deg=accept_start_angle_deg,
             num_tris_distractors=num_tris_distractors, color_ground=color_ground, color_sky=color_sky,
             user_tile_start=user_tile_start, randomization_config=randomization_config)
         self.map_ids = np.zeros(num_envs, np.int32)
@@ -429,17 +451,30 @@ class BatchedDuckietownEnv:
     def state_dict(self) -> dict:
         """Everything needed to continue this batch elsewhere: every env's record (on the CPU), its fingerprint and the
         host-side reset state, in types `torch.save` / `torch.load` round-trip.  Synchronises.  Load it into an env
-        built with the same keywords (`load_state_dict`)."""
+        built with the same keywords (`load_state_dict`).  Under camera_rand it also holds the calibrations and each
+        env's, which the env must have too: a resume sees the same lenses."""
         h = self._host_state()
         recs = self.save_state()
-        return {"records": recs.cpu(), "fingerprint": int(recs.fingerprint), "rngs": h["rngs"],
-                "last_horizon": torch.from_numpy(np.stack(h["last_horizon"])),
-                "episodes": torch.from_numpy(h["episodes"]), "map_ids": torch.from_numpy(h["map_ids"]),
-                "first_reset": bool(self._first_reset)}
+        d = {"records": recs.cpu(), "fingerprint": int(recs.fingerprint), "rngs": h["rngs"],
+             "last_horizon": torch.from_numpy(np.stack(h["last_horizon"])),
+             "episodes": torch.from_numpy(h["episodes"]), "map_ids": torch.from_numpy(h["map_ids"]),
+             "first_reset": bool(self._first_reset)}
+        if self.camera_rand:
+            d["camera_rand"] = self._camera_rand_state()
+        return d
+
+    def _camera_rand_state(self) -> dict:
+        return {"K": torch.from_numpy(np.stack([K for K, _ in self.calibrations])),
+                "D": torch.from_numpy(np.stack([D for _, D in self.calibrations])),
+                "calibration_of_env": torch.from_numpy(self.calibration_of_env.astype(np.int64))}
 
     def load_state_dict(self, d: dict) -> None:
-        """Continue from `state_dict()`: every env's device and host state.  A fingerprint from other maps raises and
-        changes nothing."""
+        """Continue from `state_dict()`: every env's device and host state.  A fingerprint from other maps, or camera_rand
+        calibrations other than this env's, raise and change nothing."""
+        mine, theirs = (self._camera_rand_state() if self.camera_rand else None), d.get("camera_rand")
+        if (mine is None) != (theirs is None) or (mine is not None and any(
+                mine[k].shape != theirs[k].shape or not torch.equal(mine[k], theirs[k].to(mine[k].dtype)) for k in mine)):
+            raise ValueError("the state's camera_rand calibrations differ from this env's")
         recs = d["records"].to(self.device).contiguous()
         self.load_state(recs, fingerprint=int(d["fingerprint"]))
         h = dict(rngs=d["rngs"], last_horizon=list(d["last_horizon"].numpy()), episodes=d["episodes"].numpy(),

@@ -211,7 +211,24 @@ int dts_set_fisheye_lut(dts_sim* sim, const float* rmapx, const float* rmapy, in
     return sim->fail("fisheye LUT is %dx%d but the camera is %dx%d", width, height, sim->cfg.cam_width, sim->cfg.cam_height);
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   DTS_CUDA(cudaDeviceSynchronize());
-  const std::string e = renderer_set_lut(*sim->render, false, rmapx, rmapy);
+  const std::string e = renderer_set_lut(*sim->render, false, 1, rmapx, rmapy, nullptr);
+  return e.empty() ? 0 : sim->fail("%s", e.c_str());
+}
+
+int dts_set_fisheye_luts(dts_sim* sim, int count, const float* rmapx, const float* rmapy, int width, int height,
+                         const int32_t* lut_of_env) {
+  if (!sim) return 1;
+  if (!(sim->cfg.flags & DTS_FLAG_DISTORTION)) return sim->fail("fisheye LUT pool on a handle created without DTS_FLAG_DISTORTION");
+  if (count < 1 || count > 65536) return sim->fail("fisheye LUT pool of %d tables: 1 to 65536 are accepted", count);
+  if (!rmapx || !rmapy || !lut_of_env) return sim->fail("fisheye LUT pool: rmapx, rmapy and lut_of_env must not be NULL");
+  if (width != sim->cfg.cam_width || height != sim->cfg.cam_height)
+    return sim->fail("fisheye LUTs are %dx%d but the camera is %dx%d", width, height, sim->cfg.cam_width, sim->cfg.cam_height);
+  for (int e = 0; e < sim->cfg.num_envs; e++)
+    if (lut_of_env[e] < 0 || lut_of_env[e] >= count)
+      return sim->fail("lut_of_env[%d] = %d is not a table of the pool (0 to %d)", e, lut_of_env[e], count - 1);
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  DTS_CUDA(cudaDeviceSynchronize());
+  const std::string e = renderer_set_lut(*sim->render, false, count, rmapx, rmapy, lut_of_env);
   return e.empty() ? 0 : sim->fail("%s", e.c_str());
 }
 
@@ -224,7 +241,7 @@ int dts_set_rectify_lut(dts_sim* sim, const float* mapx, const float* mapy, int 
     return sim->fail("rectification LUT is %dx%d but the camera is %dx%d", width, height, sim->cfg.cam_width, sim->cfg.cam_height);
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   DTS_CUDA(cudaDeviceSynchronize());
-  const std::string e = renderer_set_lut(*sim->render, true, mapx, mapy);
+  const std::string e = renderer_set_lut(*sim->render, true, 1, mapx, mapy, nullptr);
   return e.empty() ? 0 : sim->fail("%s", e.c_str());
 }
 

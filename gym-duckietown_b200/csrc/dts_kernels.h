@@ -112,8 +112,11 @@ void renderer_release_frame(Renderer& r);   // the maps changed: the next render
 std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode);
 // The fused gather's tables for a LUT of the camera's size (obs[y, x] = frame[rint(rmapy), rint(rmapx)]), in the fisheye
 // slot or (`rectify`) the rectification slot; they replace that slot's previous ones, so no render may be in flight.  A
-// LUT the rasteriser cannot take leaves the previous tables; NULL maps free the slot.
-std::string renderer_set_lut(Renderer& r, bool rectify, const float* rmapx, const float* rmapy);
+// LUT the rasteriser cannot take leaves the previous tables; NULL maps free the slot.  A fisheye pool: `count` LUTs
+// back to back in rmapx / rmapy, env e gathered through LUT lut_of_env[e] (HOST, [n_envs], checked by the caller; read
+// only when count > 1).  The rectification slot takes one LUT.
+std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* rmapx, const float* rmapy,
+                             const int32_t* lut_of_env);
 // `marks`: NULL or kProfMarks events recorded on `st` before k_frame_setup and after each of k_frame_setup, k_geometry,
 // k_bin, k_raster and the post passes (dts_profile_*).  `status_dev`: device address of the mapped host status word.
 // `labels`: NULL, or the label target (dts_set_label_target), i16 [n_envs][height][width], written beside obs like the

@@ -137,10 +137,12 @@ __device__ inline void respawn(const DState& S, const DMap* maps, const StepCfg&
     for (int k = 0; k < 3; k++) r.diffuse[k] = (float)(0.35 * p4[k]);
     for (int k = 0; k < 3; k++) r.ground[k] = (float)(c.color_ground[k] * rs.uniform(1.0 - 0.3, 1.0 + 0.3));  // S:594
     wheel = 0.102 * rs.uniform(1.0 - 0.1, 1.0 + 0.1);                         // S:597
-    r.cam_height = (float)(0.108 * cam_h);                                    // S:612-614
+    for (int k = 0; k < 3; k++) r.cam_noise[k] = (float)noise[k];             // S:1768: domain_rand only
+  }
+  if (dr || (c.flags & DTS_FLAG_CAMERA_RAND)) {                               // S:611-614: domain_rand or camera_rand
+    r.cam_height = (float)(0.108 * cam_h);
     r.cam_angle_deg = (float)(19.15 * cam_angle);
     r.cam_fov_y_deg = (float)(75.0 * cam_fov);
-    for (int k = 0; k < 3; k++) r.cam_noise[k] = (float)noise[k];
   }
   // distractor triangles S:621-629: never visible (below the ground plane) but their draws are consumed
   for (int t = 0; t < 3 * c.num_tris_distractors; t++) {

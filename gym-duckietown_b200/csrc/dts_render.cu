@@ -66,6 +66,11 @@ struct FishTab {
   const int4* home_ent;
   int ext_x, ext_y;
 };
+// A pool of fisheye tables (dts_set_fisheye_luts, camera_rand) is held in one FishTab: the tables' arrays concatenated,
+// table t's src_xy / cbox / fbox / cell_start / home_start t strides in (every table has the camera's sizes), the CSR
+// starts holding positions in the concatenated cell_bins / home_ent, and ext_x / ext_y the largest over the tables.  The
+// rasterisers' kPool instances take the table of each env from a device array of table indices, their last kernel
+// parameter; the other instances, and launches with one table, read the FishTab as it is.
 
 namespace {
 
@@ -827,6 +832,16 @@ __device__ __forceinline__ FishPx fish_source(const FishTab& ft, int bx, int by,
   const int sx = (int)(short)(sxy & 0xffff), sy = sxy >> 16;
   return FishPx{sx != -32768, sx * kSub, sy * kSub};
 }
+// The tables of env `env` in a pool (`tab`: the table index of every env)
+__device__ __forceinline__ FishTab fish_of_env(FishTab ft, const uint16_t* __restrict__ tab, int env, int W, int H, int cbins) {
+  const int t = __ldg(tab + env);
+  ft.src_xy += (size_t)t * W * H;
+  ft.cbox += (size_t)t * cbins;
+  ft.fbox += (size_t)t * cbins * (kCFX * kCFY);
+  ft.cell_start += (size_t)t * (cbins + 1);
+  ft.home_start += (size_t)t * (cbins + 1);
+  return ft;
+}
 
 // One fine bin of a lean_output() frame: whole words if the bin lies inside the image, else the general form
 __device__ __forceinline__ void store_bin_lean(uint8_t* __restrict__ out, const StoreLane& sl, unsigned rgb, int lane, int bx, int by,
@@ -929,7 +944,8 @@ struct Renderer {
   int max_prims = 0, max_lat = 0, items_max = 0, pool = 0;
   void* frame = nullptr;     // frame memory (null: not reserved since the last map upload)
   FrameMem fm{};             // ... carved
-  FishTab fish{};            // fused fisheye tables (null until a LUT is set)
+  FishTab fish{};            // fused fisheye tables (null until a LUT is set): one table, or a pool of them
+  uint16_t* fish_tab = nullptr;   // [n] a pool's table index of every env (device); null with one table
   FishTab rect{};            // UndistortWrapper's rectification, gathered the same way (null unless set)
 };
 
@@ -1325,9 +1341,11 @@ constexpr int kCountMask = 0xfffff, kGroundInc = 1 << 20;   // a bin's counter: 
 constexpr int kFlatBin = -0x7fffffff - 1;   // bin_count of a flat bin (k_raster_flat); solo bins hold -(prim + 1) >= -65536
 // kListed: the frame draws the envs of rc.env_list.  (Its own instance: an env id loaded from the list stays live across
 // the kernel, where blockIdx.x is re-read for free, and would cost the fisheye instance registers and spills.)
-template <bool kFish, bool kListed>   // kFish: bins are the LUT's source boxes of the output bins (fused fisheye gather)
+template <bool kFish, bool kListed, bool kPool = false>   // kFish: bins are the LUT's source boxes of the output bins (fused fisheye gather)
+                                                       // kPool: each env's tables of a pool (fish_of_env)
 __global__ void __launch_bounds__(kBinWarps * 32)
-k_bin(RenderCfg rc, FrameMem fm, FishTab ft, int max_prims, int max_pairs, int32_t* __restrict__ err) {
+k_bin(RenderCfg rc, FrameMem fm, FishTab fts, int max_prims, int max_pairs, int32_t* __restrict__ err,
+      const uint16_t* __restrict__ fish_tab) {
   extern __shared__ int bin_smem[];
   __shared__ int s_total, s_base, s_ok;
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, tid = threadIdx.x;
@@ -1335,6 +1353,7 @@ k_bin(RenderCfg rc, FrameMem fm, FishTab ft, int max_prims, int max_pairs, int32
   const int env = kListed ? __ldg(rc.env_list + blockIdx.x) : (int)blockIdx.x, nthr = blockDim.x;   // 1 warp per env for small cameras, 4 for large ones (launch_render)
   const int W = rc.width, H = rc.height;
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW, cbins_y = (H + kCoarseH - 1) / kCoarseH, cbins = cbins_x * cbins_y;
+  const FishTab ft = kPool ? fish_of_env(fts, fish_tab, env, W, H, cbins) : fts;
   int* cnt = bin_smem;
   int* start = cnt + cbins;
   const PrimRec* prims = fm.prims + (size_t)env * max_prims;
@@ -1660,15 +1679,16 @@ __device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool sim
 }
 
 // ------------------------------------------------------------------------------------------------ k_raster
-template <bool kWrapFmt, bool kFish, bool kDepth, bool kLabels>
+template <bool kWrapFmt, bool kFish, bool kDepth, bool kLabels, bool kPool = false>
                                        // kWrapFmt: a dts_output_format other than packed u8 HWC is written by the resolve;
                                        // kFish: every lane renders the SOURCE pixel the fisheye LUT names for its output pixel;
                                        // kDepth: every pixel's depth goes to rc.depth beside its colour (render spec item 9);
-                                       // kLabels: every pixel's label goes to `labels` (render spec item 10)
+                                       // kLabels: every pixel's label goes to `labels` (render spec item 10);
+                                       // kPool: each env's tables of a pool (fish_of_env)
 __global__ void __launch_bounds__(kThreads, kRasterMinCtas)
-k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, FishTab ft, GatherTab gt,
+k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, FishTab fts, GatherTab gt,
          uint8_t* __restrict__ obs, int max_prims, int max_pairs, int max_lat, int32_t* __restrict__ err,
-         int16_t* __restrict__ labels) {
+         int16_t* __restrict__ labels, const uint16_t* __restrict__ fish_tab) {
   // dynamic shared memory (kRasterSmem bytes): per warp two chunks of records in flight, their mbarriers, and a 128-sample
   // depth / winner buffer for the tiny triangles of the fine bin being drawn
   extern __shared__ __align__(128) unsigned char raster_smem[];
@@ -1701,6 +1721,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
     if (lane == 0) next_work = atomicAdd(fm.work + kWorkRaster, 1);   // consumed after this row: latency hidden
     const int slot = work / cbins_y, cby = work - slot * cbins_y;
     const int env = listed_env(rc.env_list, slot);
+    const FishTab ft = kPool ? fish_of_env(fts, fish_tab, env, W, H, cbins) : fts;
     const DMap& m = maps[S.map_id[env]];
     const uint8_t* tex_pool = m.tex_pool;
     const PrimRec* prims = fm.prims + (size_t)env * max_prims;
@@ -2022,13 +2043,14 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
 // visibility state: a warp fetches the prim's planes once and shades the bin's 256 pixels.  A separate kernel so that the
 // lean loop gets its own register allocation (the same fast path inside k_raster cost more than it saved).
 // Packed u8 HWC output with whole-word rows only (k_bin marks no bin otherwise).  Runs before k_raster.
-template <bool kFish, bool kDepth, bool kLabels>
+template <bool kFish, bool kDepth, bool kLabels, bool kPool = false>
                                      // kFish: each lane shades the source pixel the fisheye LUT names for its output pixel;
                                      // kDepth: the 1/w the shading divides by also gives the pixel's depth (rc.depth);
-                                     // kLabels: the bin's one prim gives every pixel with a source its label (`labels`)
+                                     // kLabels: the bin's one prim gives every pixel with a source its label (`labels`);
+                                     // kPool: each env's tables of a pool (fish_of_env)
 __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
-                                                                        FishTab ft, uint8_t* __restrict__ obs, int max_prims, int max_lat,
-                                                                        int16_t* __restrict__ labels) {
+                                                                        FishTab fts, uint8_t* __restrict__ obs, int max_prims, int max_lat,
+                                                                        int16_t* __restrict__ labels, const uint16_t* __restrict__ fish_tab) {
   const int W = rc.width, H = rc.height;
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW;
   const int lane = threadIdx.x & 31;
@@ -2041,6 +2063,7 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
     const int env = (int)e.x, b = (int)(e.y & 0xffffu);
     const unsigned p = e.y >> 16;
     const int cby = b / cbins_x, cbx = b - cby * cbins_x;
+    const FishTab ft = kPool ? fish_of_env(fts, fish_tab, env, W, H, cbins_x * ((H + kCoarseH - 1) / kCoarseH)) : fts;
     const uint8_t* tex_pool = maps[S.map_id[env]].tex_pool;
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     const ShadeIn si = load_shade(fm.prims + (size_t)env * max_prims, p);
@@ -2099,10 +2122,13 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
 // and road tiles come here, so a label is arithmetic on the draw id (tile_label).
 // Packed u8 HWC output with whole-word rows only (k_bin lists no bin otherwise).  Runs after k_raster_solo.
 constexpr int kEdgeQ = 64;   // queue ring: flushed at 32 entries, so at most 31 + 32 wait at once
-template <bool kFish, bool kDepth, bool kLabels>   // kFish: each lane covers and shades the source pixel the fisheye LUT names for its output pixel
+template <bool kFish, bool kDepth, bool kLabels, bool kPool = false>
+                                 // kFish: each lane covers and shades the source pixel the fisheye LUT names for its output pixel;
+                                 // kPool: each env's tables of a pool (fish_of_env)
 __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
-                                                                        FishTab ft, uint8_t* __restrict__ obs, int max_prims, int max_lat,
-                                                                        int32_t* __restrict__ err, int16_t* __restrict__ labels) {
+                                                                        FishTab fts, uint8_t* __restrict__ obs, int max_prims, int max_lat,
+                                                                        int32_t* __restrict__ err, int16_t* __restrict__ labels,
+                                                                        const uint16_t* __restrict__ fish_tab) {
   __shared__ BinRec stages[kWarps][kStage];   // per warp: the records of its bin
   __shared__ unsigned bin_rgb[kWarps][kCFX * kCFY * 32];   // per warp: packed colour of pixel `lane` of fine bin f at f * 32 + lane
   // per warp: the edge-pixel queue, an entry in two words: (pixel slot, pxa, pya, wn0 | wn1 << 16), (wn2 | wn3 << 16, first colour)
@@ -2126,6 +2152,7 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
     const uint2 e = fm.flat[i];
     const int env = (int)e.x, b = (int)(e.y & 0xffffu), count = (int)(e.y >> 16);
     const int cby = b / cbins_x, cbx = b - cby * cbins_x;
+    const FishTab ft = kPool ? fish_of_env(fts, fish_tab, env, W, H, cbins) : fts;
     DTS_COUNT(24, 1);
     // ---- stage the records: one per lane, five 128-bit loads
     uint2 mine = make_uint2(0u, 0u);   // prim_flags, kind
@@ -2292,7 +2319,7 @@ void renderer_release_frame(Renderer& r) {
 }
 
 void renderer_destroy(Renderer* r) {
-  if (r) { renderer_release_frame(*r); free_fish(r->fish); free_fish(r->rect); }
+  if (r) { renderer_release_frame(*r); free_fish(r->fish); free_fish(r->rect); cudaFree(r->fish_tab); }
   delete r;
 }
 
@@ -2336,7 +2363,8 @@ std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, 
   return "";
 }
 
-std::string renderer_set_lut(Renderer& r, bool rectify, const float* rmapx, const float* rmapy) {
+std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* rmapx, const float* rmapy,
+                             const int32_t* lut_of_env) {
   // distortion.py:118 gathers img[rint(rmapy), rint(rmapx)], UndistortWrapper (wrappers.py:227) the same with its own
   // map.  The rasteriser renders those source pixels directly: per output pixel the source position, per fine / coarse
   // output bin the bounding box of its source pixels (the bins prims are sorted into).
@@ -2344,69 +2372,85 @@ std::string renderer_set_lut(Renderer& r, bool rectify, const float* rmapx, cons
   const char* what = rectify ? "rectification LUT" : "fisheye LUT";
   if (!rmapx || !rmapy) {
     free_fish(slot);
+    if (!rectify) { cudaFree(r.fish_tab); r.fish_tab = nullptr; }
     return "";
   }
   const int W = r.W, H = r.H, cbx_n = (W + kCoarseW - 1) / kCoarseW, cbins = r.cbins;
-  std::vector<int32_t> src((size_t)W * H);
+  const size_t px = (size_t)W * H;
+  // the tables of a pool, concatenated (FishTab): every per-table array is appended, so that the CSR starts pushed below
+  // are positions in the concatenated lists
+  std::vector<int32_t> src(px * count);
   const short4 empty = make_short4(32767, 32767, -32768, -32768);
-  std::vector<short4> cbox(cbins, empty), fbox((size_t)cbins * kCFX * kCFY, empty);
+  std::vector<short4> cbox((size_t)cbins * count, empty), fbox((size_t)cbins * count * kCFX * kCFY, empty);
+  std::vector<int32_t> cell_start, home_start;
+  std::vector<uint16_t> cell_bins;
+  std::vector<int4> home_ent;   // with the box
+  int ext_x = 0, ext_y = 0;
   auto grow = [](short4& b, int x, int y) {
     b.x = (short)(x < b.x ? x : b.x); b.y = (short)(y < b.y ? y : b.y);
     b.z = (short)(x > b.z ? x : b.z); b.w = (short)(y > b.w ? y : b.w);
   };
-  for (int y = 0; y < H; y++)
-    for (int x = 0; x < W; x++) {
-      const float fx = rmapx[(size_t)y * W + x], fy = rmapy[(size_t)y * W + x];
-      // round half to even (numpy's rint); NaN, inf and huge entries are out of range before any float -> int conversion,
-      // which would be undefined for them
-      const bool finite = fabsf(fx) < 1073741824.0f && fabsf(fy) < 1073741824.0f;
-      const int sx = finite ? (int)rintf(fx) : -1, sy = finite ? (int)rintf(fy) : -1;
-      const bool ok = sx >= 0 && sx < W && sy >= 0 && sy < H;
-      src[(size_t)y * W + x] = ok ? (int32_t)((uint32_t)(sx & 0xffff) | ((uint32_t)sy << 16)) : (int32_t)0x80008000u;
-      if (!ok) continue;
-      const int cb = (y / kCoarseH) * cbx_n + x / kCoarseW, f = (y % kCoarseH / kBinH) * kCFX + x % kCoarseW / kBinW;
-      grow(cbox[cb], sx, sy); grow(fbox[(size_t)cb * kCFX * kCFY + f], sx, sy);
+  for (int t = 0; t < count; t++) {
+    const float* mx = rmapx + px * t;
+    const float* my = rmapy + px * t;
+    int32_t* tsrc = src.data() + px * t;
+    short4* tcbox = cbox.data() + (size_t)cbins * t;
+    short4* tfbox = fbox.data() + (size_t)cbins * t * kCFX * kCFY;
+    const std::string name = count > 1 ? std::string(what) + " " + std::to_string(t) : std::string(what);
+    for (int y = 0; y < H; y++)
+      for (int x = 0; x < W; x++) {
+        const float fx = mx[(size_t)y * W + x], fy = my[(size_t)y * W + x];
+        // round half to even (numpy's rint); NaN, inf and huge entries are out of range before any float -> int conversion,
+        // which would be undefined for them
+        const bool finite = fabsf(fx) < 1073741824.0f && fabsf(fy) < 1073741824.0f;
+        const int sx = finite ? (int)rintf(fx) : -1, sy = finite ? (int)rintf(fy) : -1;
+        const bool ok = sx >= 0 && sx < W && sy >= 0 && sy < H;
+        tsrc[(size_t)y * W + x] = ok ? (int32_t)((uint32_t)(sx & 0xffff) | ((uint32_t)sy << 16)) : (int32_t)0x80008000u;
+        if (!ok) continue;
+        const int cb = (y / kCoarseH) * cbx_n + x / kCoarseW, f = (y % kCoarseH / kBinH) * kCFX + x % kCoarseW / kBinW;
+        grow(tcbox[cb], sx, sy); grow(tfbox[(size_t)cb * kCFX * kCFY + f], sx, sy);
+      }
+    // int32 edge functions inside a coarse bin need |A x + B y| < 2^30 over its source box, where (guard band) |A| <=
+    // kEdge * H, |B| <= kEdge * W, x <= kSub * w, y <= kSub * h  ->  H * w + W * h < 2^30 / (kEdge * kSub)
+    constexpr long long kEdge = (long long)(kGuard + 1) * kSub;
+    for (int b = 0; b < cbins; b++) {
+      if (tcbox[b].z < tcbox[b].x) continue;
+      const long long w = tcbox[b].z - tcbox[b].x + 2, h = tcbox[b].w - tcbox[b].y + 2;
+      if ((long long)H * w + (long long)W * h >= (1LL << 30) / (kEdge * kSub))
+        return name + " sends output bin " + std::to_string(b) + " to a " + std::to_string(w) + "x" + std::to_string(h) +
+               " px source region: too wide for the rasteriser's int32 edge functions";
     }
-  // int32 edge functions inside a coarse bin need |A x + B y| < 2^30 over its source box, where (guard band) |A| <=
-  // kEdge * H, |B| <= kEdge * W, x <= kSub * w, y <= kSub * h  ->  H * w + W * h < 2^30 / (kEdge * kSub)
-  constexpr long long kEdge = (long long)(kGuard + 1) * kSub;
-  for (int b = 0; b < cbins; b++) {
-    if (cbox[b].z < cbox[b].x) continue;
-    const long long w = cbox[b].z - cbox[b].x + 2, h = cbox[b].w - cbox[b].y + 2;
-    if ((long long)H * w + (long long)W * h >= (1LL << 30) / (kEdge * kSub))
-      return std::string(what) + " sends output bin " + std::to_string(b) + " to a " + std::to_string(w) + "x" + std::to_string(h) +
-             " px source region: too wide for the rasteriser's int32 edge functions";
-  }
-  // two inverse indices over source cells (the coarse grid laid over the source image): per cell, the output bins whose
-  // source box meets it, and the output bins whose box has its top-left corner there, each bin under one HOME cell
-  std::vector<std::vector<int>> meets(cbins), homes(cbins);
-  int ext_x = 0, ext_y = 0;
-  for (int b = 0; b < cbins; b++) {
-    const short4 q = cbox[b];
-    if (q.z < q.x) continue;
-    const int cx0 = q.x / kCoarseW, cy0 = q.y / kCoarseH, cx1 = q.z / kCoarseW, cy1 = q.w / kCoarseH;
-    for (int cy = cy0; cy <= cy1; cy++)
-      for (int cx = cx0; cx <= cx1; cx++) meets[cy * cbx_n + cx].push_back(b);
-    homes[cy0 * cbx_n + cx0].push_back(b);
-    ext_x = std::max(ext_x, cx1 - cx0);
-    ext_y = std::max(ext_y, cy1 - cy0);
-  }
-  std::vector<int32_t> cell_start, home_start;
-  std::vector<uint16_t> cell_bins;
-  std::vector<int4> home_ent;   // with the box
-  for (int c = 0; c < cbins; c++) {
+    // two inverse indices over source cells (the coarse grid laid over the source image): per cell, the output bins whose
+    // source box meets it, and the output bins whose box has its top-left corner there, each bin under one HOME cell
+    std::vector<std::vector<int>> meets(cbins), homes(cbins);
+    for (int b = 0; b < cbins; b++) {
+      const short4 q = tcbox[b];
+      if (q.z < q.x) continue;
+      const int cx0 = q.x / kCoarseW, cy0 = q.y / kCoarseH, cx1 = q.z / kCoarseW, cy1 = q.w / kCoarseH;
+      for (int cy = cy0; cy <= cy1; cy++)
+        for (int cx = cx0; cx <= cx1; cx++) meets[cy * cbx_n + cx].push_back(b);
+      homes[cy0 * cbx_n + cx0].push_back(b);
+      ext_x = std::max(ext_x, cx1 - cx0);
+      ext_y = std::max(ext_y, cy1 - cy0);
+    }
+    for (int c = 0; c < cbins; c++) {
+      cell_start.push_back((int32_t)cell_bins.size());
+      home_start.push_back((int32_t)home_ent.size());
+      for (int b : meets[c]) cell_bins.push_back((uint16_t)b);
+      for (int b : homes[c])
+        home_ent.push_back(make_int4((int)((uint32_t)(uint16_t)tcbox[b].x | ((uint32_t)(uint16_t)tcbox[b].y << 16)),
+                                     (int)((uint32_t)(uint16_t)tcbox[b].z | ((uint32_t)(uint16_t)tcbox[b].w << 16)), b, 0));
+    }
     cell_start.push_back((int32_t)cell_bins.size());
     home_start.push_back((int32_t)home_ent.size());
-    for (int b : meets[c]) cell_bins.push_back((uint16_t)b);
-    for (int b : homes[c])
-      home_ent.push_back(make_int4((int)((uint32_t)(uint16_t)cbox[b].x | ((uint32_t)(uint16_t)cbox[b].y << 16)),
-                                   (int)((uint32_t)(uint16_t)cbox[b].z | ((uint32_t)(uint16_t)cbox[b].w << 16)), b, 0));
   }
-  cell_start.push_back((int32_t)cell_bins.size());
-  home_start.push_back((int32_t)home_ent.size());
   if (cell_bins.empty()) cell_bins.push_back(0);
   if (home_ent.empty()) home_ent.push_back(make_int4(0, 0, 0, 0));
+  std::vector<uint16_t> tab;
+  if (count > 1)
+    for (int e = 0; e < r.n; e++) tab.push_back((uint16_t)lut_of_env[e]);
   FishTab t{};
+  uint16_t* d_tab = nullptr;
   cudaError_t e = cudaSuccess;
   auto upload = [&](auto& dst, const auto& v) {
     void* d = nullptr;
@@ -2418,10 +2462,15 @@ std::string renderer_set_lut(Renderer& r, bool rectify, const float* rmapx, cons
   upload(t.src_xy, src); upload(t.cbox, cbox); upload(t.fbox, fbox);
   upload(t.cell_start, cell_start); upload(t.cell_bins, cell_bins);
   upload(t.home_start, home_start); upload(t.home_ent, home_ent);
-  if (e != cudaSuccess) { free_fish(t); return std::string(what) + " table upload failed: " + cudaGetErrorString(e); }
+  if (!tab.empty()) upload(d_tab, tab);
+  if (e != cudaSuccess) {
+    free_fish(t); cudaFree(d_tab);
+    return std::string(what) + " table upload failed: " + cudaGetErrorString(e);
+  }
   t.ext_x = ext_x; t.ext_y = ext_y;
   free_fish(slot);
   slot = t;
+  if (!rectify) { cudaFree(r.fish_tab); r.fish_tab = d_tab; }
   return "";
 }
 
@@ -2471,6 +2520,9 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
                      : ((rc.flags & DTS_FLAG_DISTORTION) && !(rc.mode & DTS_RENDER_PINHOLE)) ? &r.fish : nullptr;
   const bool fisheye = lut != nullptr;
   const FishTab ft = fisheye ? *lut : FishTab{};
+  // a pool of fisheye tables selects the kPool instances; one table, the rectification and no gather the others
+  const uint16_t* fish_tab = lut == &r.fish ? r.fish_tab : nullptr;
+  const bool pool = fish_tab != nullptr;
   FrameMem fm = r.fm;
   fm.status = status_dev;
   int mk = 0;
@@ -2496,8 +2548,9 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   const int bin_grid = rc.n_envs;   // CTA per env: one warp where a frame has few bins and prims (160x120: 75 bins — more warps
   // only add barriers and CTA launches), four for large cameras (640x480)
   const int bin_threads = r.cbins > 128 ? kBinWarps * 32 : 32;
-  const auto bin = rc.env_list ? (fisheye ? k_bin<true, true> : k_bin<false, true>) : (fisheye ? k_bin<true, false> : k_bin<false, false>);
-  bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, ft, r.max_prims, r.pool, err_flag);
+  const auto bin = pool ? (rc.env_list ? k_bin<true, true, true> : k_bin<true, false, true>)
+                 : rc.env_list ? (fisheye ? k_bin<true, true> : k_bin<false, true>) : (fisheye ? k_bin<true, false> : k_bin<false, false>);
+  bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, ft, r.max_prims, r.pool, err_flag, fish_tab);
   mark();
   const bool wrap = (rc.obs_layout | rc.obs_dtype) != 0;
   // a depth target (RenderCfg::depth) selects the depth-writing instance of each rasteriser; without one the launches
@@ -2506,32 +2559,37 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   // so does a label target, alone or with depth
   const int out = (depth ? 1 : 0) | (labels ? 2 : 0);
   if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
-    const auto solo_of = [&](auto fish) {
-      constexpr bool f = decltype(fish)::value;
-      return out == 3 ? k_raster_solo<f, true, true> : out == 2 ? k_raster_solo<f, false, true>
-                                                     : out == 1 ? k_raster_solo<f, true, false> : k_raster_solo<f, false, false>;
+    const auto solo_of = [&](auto fish, auto pool_) {
+      constexpr bool f = decltype(fish)::value, p = decltype(pool_)::value;
+      return out == 3 ? k_raster_solo<f, true, true, p> : out == 2 ? k_raster_solo<f, false, true, p>
+                                                        : out == 1 ? k_raster_solo<f, true, false, p> : k_raster_solo<f, false, false, p>;
     };
-    const auto flat_of = [&](auto fish) {
-      constexpr bool f = decltype(fish)::value;
-      return out == 3 ? k_raster_flat<f, true, true> : out == 2 ? k_raster_flat<f, false, true>
-                                                     : out == 1 ? k_raster_flat<f, true, false> : k_raster_flat<f, false, false>;
+    const auto flat_of = [&](auto fish, auto pool_) {
+      constexpr bool f = decltype(fish)::value, p = decltype(pool_)::value;
+      return out == 3 ? k_raster_flat<f, true, true, p> : out == 2 ? k_raster_flat<f, false, true, p>
+                                                        : out == 1 ? k_raster_flat<f, true, false, p> : k_raster_flat<f, false, false, p>;
     };
-    const auto solo = fisheye ? solo_of(std::true_type{}) : solo_of(std::false_type{});
-    const auto flat = fisheye ? flat_of(std::true_type{}) : flat_of(std::false_type{});
-    solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, labels);
+    const auto solo = pool ? solo_of(std::true_type{}, std::true_type{})
+                    : fisheye ? solo_of(std::true_type{}, std::false_type{}) : solo_of(std::false_type{}, std::false_type{});
+    const auto flat = pool ? flat_of(std::true_type{}, std::true_type{})
+                    : fisheye ? flat_of(std::true_type{}, std::false_type{}) : flat_of(std::false_type{}, std::false_type{});
+    solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, labels, fish_tab);
     // before k_raster, which draws the bins k_raster_flat hands back
-    flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, err_flag, labels);
+    flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, err_flag, labels, fish_tab);
     launches += 2;
   }
-  const auto raster_of = [&](auto wrap_fmt, auto fish) {
-    constexpr bool w = decltype(wrap_fmt)::value, f = decltype(fish)::value;
-    return out == 3 ? k_raster<w, f, true, true> : out == 2 ? k_raster<w, f, false, true>
-                                                 : out == 1 ? k_raster<w, f, true, false> : k_raster<w, f, false, false>;
+  const auto raster_of = [&](auto wrap_fmt, auto fish, auto pool_) {
+    constexpr bool w = decltype(wrap_fmt)::value, f = decltype(fish)::value, p = decltype(pool_)::value;
+    return out == 3 ? k_raster<w, f, true, true, p> : out == 2 ? k_raster<w, f, false, true, p>
+                                                    : out == 1 ? k_raster<w, f, true, false, p> : k_raster<w, f, false, false, p>;
   };
-  const auto raster = fisheye ? (wrap ? raster_of(std::true_type{}, std::true_type{}) : raster_of(std::false_type{}, std::true_type{}))
-                              : (wrap ? raster_of(std::true_type{}, std::false_type{}) : raster_of(std::false_type{}, std::false_type{}));
+  const std::true_type yes{};
+  const std::false_type no{};
+  const auto raster = pool ? (wrap ? raster_of(yes, yes, yes) : raster_of(no, yes, yes))
+                    : fisheye ? (wrap ? raster_of(yes, yes, no) : raster_of(no, yes, no))
+                              : (wrap ? raster_of(yes, no, no) : raster_of(no, no, no));
   raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, ft, gather, obs, r.max_prims, r.pool, r.max_lat, err_flag,
-                                                                labels);
+                                                                labels, fish_tab);
   mark();
   mark();   // (post passes: launched by the caller)
   return launches;
@@ -2545,14 +2603,16 @@ Renderer* renderer_create(const dts_config& cfg) {
   cudaDeviceGetAttribute(&r->sms, cudaDevAttrMultiProcessorCount, cfg.device);
   r->cbins = ((r->W + kCoarseW - 1) / kCoarseW) * ((r->H + kCoarseH - 1) / kCoarseH);
   // k_raster's shared memory is past the 48 KB default; the opt-in holds for the kernel as loaded on this device
-  const auto opt_in = [](auto wrap_fmt, auto fish) {
-    constexpr bool w = decltype(wrap_fmt)::value, f = decltype(fish)::value;
-    for (const auto raster : {k_raster<w, f, false, false>, k_raster<w, f, true, false>, k_raster<w, f, false, true>,
-                              k_raster<w, f, true, true>})
+  const auto opt_in = [](auto wrap_fmt, auto fish, auto pool) {
+    constexpr bool w = decltype(wrap_fmt)::value, f = decltype(fish)::value, p = decltype(pool)::value;
+    for (const auto raster : {k_raster<w, f, false, false, p>, k_raster<w, f, true, false, p>, k_raster<w, f, false, true, p>,
+                              k_raster<w, f, true, true, p>})
       cudaFuncSetAttribute(raster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
   };
-  opt_in(std::true_type{}, std::true_type{}); opt_in(std::false_type{}, std::true_type{});
-  opt_in(std::true_type{}, std::false_type{}); opt_in(std::false_type{}, std::false_type{});
+  const std::true_type yes{};
+  const std::false_type no{};
+  opt_in(yes, yes, no); opt_in(no, yes, no); opt_in(yes, no, no); opt_in(no, no, no);
+  opt_in(yes, yes, yes); opt_in(no, yes, yes);
   return r;
 }
 

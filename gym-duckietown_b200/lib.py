@@ -17,6 +17,7 @@ LIB_PATH = os.path.join(HERE, "libdtsim.so")
 DTS_ABI_VERSION = 3
 ACTION_PWM, ACTION_VEL_STEER = 0, 1
 FLAG_AUTO_RESET, FLAG_DOMAIN_RAND, FLAG_DISTORTION, FLAG_DYNAMICS_RAND, FLAG_TESSELLATE = 1, 2, 4, 8, 16
+FLAG_CAMERA_RAND = 32
 IN_PROGRESS, INVALID_POSE, MAX_STEPS = 0, 1, 2
 DONE_CODE_STR = {0: "in-progress", 1: "invalid-pose", 2: "max-steps-reached"}  # S:1685-1705
 
@@ -169,6 +170,7 @@ def load() -> C.CDLL:
     lib.dts_create.argtypes = [C.POINTER(Config), C.POINTER(vp)]
     lib.dts_upload_map.argtypes = [vp, i, C.POINTER(MapBlob)]
     lib.dts_set_fisheye_lut.argtypes = [vp, vp, vp, i, i]
+    lib.dts_set_fisheye_luts.argtypes = [vp, i, vp, vp, i, i, vp]
     lib.dts_set_rectify_lut.argtypes = [vp, vp, vp, i, i]
     lib.dts_reset.argtypes = [vp, vp, C.POINTER(EpisodeParams), vp]
     lib.dts_reset_random.argtypes = [vp, vp, vp]
@@ -217,7 +219,7 @@ def load() -> C.CDLL:
     return lib
 
 
-EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
+EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_fisheye_luts", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
            "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
            "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
@@ -365,6 +367,17 @@ class Sim:
         rx, ry = self._lut("fisheye LUT", rmapx, rmapy)
         self._check(self.lib.dts_set_fisheye_lut(self.h, _ptr(rx), _ptr(ry), rx.shape[1], rx.shape[0]),
                     "dts_set_fisheye_lut")
+
+    def set_fisheye_luts(self, rmapx: np.ndarray, rmapy: np.ndarray, lut_of_env):
+        """A pool of fisheye LUTs, float32 [count][H][W] each, and the LUT of every env (dts_set_fisheye_luts)."""
+        rx, ry = np.ascontiguousarray(rmapx, np.float32), np.ascontiguousarray(rmapy, np.float32)
+        if rx.ndim != 3 or rx.shape != ry.shape:   # the library reads count x camera_height x camera_width floats
+            raise ValueError(f"fisheye LUT pool: {rx.shape} and {ry.shape} must be two 3-D arrays of one shape")
+        tab = np.ascontiguousarray(lut_of_env, np.int32)
+        if tab.shape != (self.cfg.num_envs,):
+            raise ValueError(f"lut_of_env must have one entry per env, not shape {tab.shape}")
+        self._check(self.lib.dts_set_fisheye_luts(self.h, rx.shape[0], _ptr(rx), _ptr(ry), rx.shape[2], rx.shape[1],
+                                                  _ptr(tab)), "dts_set_fisheye_luts")
 
     def set_rectify_lut(self, mapx: Optional[np.ndarray], mapy: Optional[np.ndarray]):
         """UndistortWrapper's map for DTS_RENDER_RECTIFY; None, None clears it."""

@@ -95,6 +95,7 @@ class Simulator(Env):
             frame_skip=frame_skip, camera_width=camera_width, camera_height=camera_height, robot_speed=robot_speed,
             accept_start_angle_deg=accept_start_angle_deg, user_tile_start=user_tile_start, seed=seed,
             distortion=distortion, dynamics_rand=dynamics_rand, camera_rand=camera_rand,
+            camera_rand_pool=env_kwargs.pop("camera_rand_pool", 1),   # one camera per Simulator (distortion.py:46-47)
             color_ground=color_ground, color_sky=color_sky, num_tris_distractors=num_tris_distractors,
             action_mode=self._action_mode, depth=depth, labels=labels, **env_kwargs)
         self._b = BatchedDuckietownEnv(1, map_arg, **self._env_kwargs)

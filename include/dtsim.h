@@ -33,8 +33,11 @@ enum { DTS_FLAG_AUTO_RESET = 1,   /* done envs are re-spawned on device inside d
        DTS_FLAG_DOMAIN_RAND = 2,  /* simulator.py:213  (camera noise S:1768, DR sampling in device resets) */
        DTS_FLAG_DISTORTION = 4,   /* simulator.py:223  fisheye gather fused into the render (distortion.py:118) */
        DTS_FLAG_DYNAMICS_RAND = 8,/* simulator.py:224  per-env trim on the motor gains (S:746-748) */
-       DTS_FLAG_TESSELLATE = 16   /* draw every road tile as the literal 7x7 quads of simulator.py:386-507
-                                     instead of one quad + analytic lattice lighting (DESIGN.md render spec) */ };
+       DTS_FLAG_TESSELLATE = 16,  /* draw every road tile as the literal 7x7 quads of simulator.py:386-507
+                                     instead of one quad + analytic lattice lighting (DESIGN.md render spec) */
+       DTS_FLAG_CAMERA_RAND = 32  /* simulator.py:225 camera_rand: device resets apply the drawn camera height / angle
+                                     / FOV without DTS_FLAG_DOMAIN_RAND too (S:611-614); the calibrations are the
+                                     caller's (dts_set_fisheye_luts) */ };
 
 /* One entry of the reference's domain-randomization table (randomization/randomizer.py:19-89): Randomizer.randomize
  * draws every key of the JSON config in SORTED key order from the env's np_random, whether or not domain_rand is on
@@ -247,6 +250,13 @@ int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* blob);
  * undistorted frame is materialised and no second pass runs.  Fails if the LUT scatters one 32x8 output bin over a
  * source region too wide for the rasteriser's int32 edge functions. */
 int dts_set_fisheye_lut(dts_sim* sim, const float* rmapx, const float* rmapy, int width, int height);
+/* camera_rand (distortion.py:46-83): a pool of `count` fisheye LUTs, one per camera calibration, float [count][H][W]
+ * each of rmapx / rmapy (HOST), and the LUT of every env, lut_of_env int32 [num_envs] (HOST), each entry in
+ * [0, count).  Env e's frames, and its depth and labels, are gathered through LUT lut_of_env[e], in every render.
+ * Each LUT is validated as dts_set_fisheye_lut validates its one; a refused call leaves the previous tables and
+ * assignment in effect.  Only on a DTS_FLAG_DISTORTION handle.  count = 1 is dts_set_fisheye_lut. */
+int dts_set_fisheye_luts(dts_sim* sim, int count, const float* rmapx, const float* rmapy, int width, int height,
+                         const int32_t* lut_of_env);
 /* UndistortWrapper's rectification (wrappers.py:206-227: cv2.remap(frame, mapx, mapy, INTER_NEAREST) of the pinhole
  * frame, with mapx/mapy from cv2.initUndistortRectifyMap(K, D, I, P, (W, H), CV_32FC1)): a second LUT [H][W] each (HOST
  * pointers), gathered by the same fused kernels as the fisheye's under DTS_RENDER_RECTIFY, so the rectified frame
