@@ -306,9 +306,32 @@ int dts_reset_random(dts_sim* sim, const uint8_t* mask_dev, void* stream) {
   return 0;
 }
 
+// The bytes an armed gather writes into slot `rank` of every rank's buffer: the whole batch at the camera size, in the
+// selected dtype
+static uint64_t gather_batch_bytes(const dts_sim* sim) {
+  const uint64_t elem = sim->fmt.obs_dtype == DTS_OBS_F32_UNIT ? 4 : 1;
+  return (uint64_t)sim->cfg.num_envs * sim->cfg.cam_height * sim->cfg.cam_width * 3 * elem;
+}
+static int check_gather_fits(dts_sim* sim) {
+  const uint64_t need = gather_batch_bytes(sim);
+  if (need > sim->gather_bytes)
+    return sim->fail("the fused gather holds %llu bytes per rank (dts_gather_alloc) but the observation batch is %llu bytes "
+                     "in the current output format", (unsigned long long)sim->gather_bytes, (unsigned long long)need);
+  return 0;
+}
+// An armed gather is checked before a step or render launches anything: a refused call leaves the state, every buffer
+// and the armed gather as they were
+static int check_gather(dts_sim* sim) {
+  if (!sim->gather_next) return 0;
+  if (resizer_target(*sim->resize).ow)
+    return sim->fail("the fused gather writes the rasteriser's own output: not combined with dts_set_resize");
+  return check_gather_fits(sim);
+}
+
 // dts_render of every env, or of the envs on a device list (dts_step_terminal's second pass; not profiled)
 static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t* env_list, const int32_t* env_count) {
   if (!obs_dev) return sim->fail("obs_dev is NULL");
+  if (check_gather(sim)) return 1;
   if (check_maps(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   const std::string e = renderer_prepare(*sim->render, maps_counts(*sim->maps), sim->render_mode);
@@ -335,8 +358,7 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
     target = rz.staging;
   }
   GatherTab gt{};
-  if (sim->gather_next) {
-    if (rz.ow) return sim->fail("the fused gather writes the rasteriser's own output: not combined with dts_set_resize");
+  if (sim->gather_next) {   // (check_gather: no resize target, and the batch fits the slot)
     gt.n = sim->gather_world;
     for (int p = 0; p < sim->gather_world; p++)
       gt.base[p] = reinterpret_cast<uint8_t*>(sim->gather_peer[p]) + (uint64_t)sim->gather_rank * sim->gather_bytes;
@@ -402,7 +424,7 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
              void* stream) {
   if (!sim) return 1;
   if (!actions_dev) return sim->fail("actions_dev is NULL");
-  if (check_maps(sim) || check_loaded(sim)) return 1;
+  if (check_maps(sim) || check_loaded(sim) || check_gather(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   if ((sim->cfg.flags & DTS_FLAG_AUTO_RESET) && !state_seeded(*sim->state))
     return sim->fail("auto-reset needs seeded streams: call dts_seed_streams first");
@@ -517,6 +539,7 @@ int dts_gather_next(dts_sim* sim) {
   if (!sim || !sim->gather_buf) return sim ? sim->fail("dts_gather_alloc first") : 1;
   for (int p = 0; p < sim->gather_world; p++)
     if (!sim->gather_peer[p]) return sim->fail("dts_gather_open first (rank %d not mapped)", p);
+  if (check_gather_fits(sim)) return 1;
   sim->gather_next = true;
   return 0;
 }

@@ -85,18 +85,21 @@ class ObsAllGather:
 
 class FusedObsGather:
     """The end-of-rollout observation exchange FUSED into the last step's rasteriser (dts_gather_*): every rank maps the
-    other ranks' gather buffers as peer memory (cudaIpc over NVLink / NVSwitch) and its k_raster stores each finished
-    8x4 pixel block into all of them while it renders — no separate collective pass, the transfer rides under the
-    rasterisation.  Usage per rollout:
+    other ranks' gather buffers as peer memory (cudaIpc over NVLink / NVSwitch) and its k_raster ships each finished
+    block of 8 whole image rows of a packed u8 HWC frame into all of them while it renders; the other layouts and float32
+    are stored per 8x4 pixel bin.  No separate collective pass: the transfer rides under the rasterisation.  The buffers
+    are sized for `env.obs` as it is at construction (one gather per env): `arm()` refuses while `set_output_format` /
+    `set_resize` have left it another dtype or shape.  Usage per rollout:
 
         g.arm()                      # before the rollout's LAST env.step(): that step also fills the gather buffers
         env.step(actions)
-        batch = g.finish()           # stream sync + barrier: u8[world, N, H, W, 3] (this rank's copy) is complete
+        batch = g.finish()           # stream sync + barrier: [world, *env.obs.shape] (this rank's copy) is complete
     """
 
     def __init__(self, env, rank: int, world: int):
         self.env, self.rank, self.world = env, rank, world
         sim = env.sim
+        self.dtype, self.shape = env.obs.dtype, tuple(env.obs.shape)
         nbytes = env.obs.numel() * env.obs.element_size()
         handle = (C.c_uint8 * 64)()
         buf = C.c_void_p()
@@ -117,6 +120,10 @@ class FusedObsGather:
             dist.barrier()   # every rank has opened every buffer before anyone writes
 
     def arm(self):
+        obs = self.env.obs
+        if obs.dtype != self.dtype or tuple(obs.shape) != self.shape:
+            raise ValueError(f"FusedObsGather was built for observations {self.dtype} {list(self.shape)}, but env.obs is now "
+                             f"{obs.dtype} {list(obs.shape)}: choose the output format before creating the gather")
         sim = self.env.sim
         sim._check(sim.lib.dts_gather_next(sim.h), "dts_gather_next")
 

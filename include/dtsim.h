@@ -430,7 +430,20 @@ int dts_profile_read(dts_sim* sim, double ms_out[8], int64_t* frames);
  *   dts_gather_next    the NEXT dts_step / dts_render also writes its observations, in the selected layout / dtype,
  *                      to slot `rank` of every rank's buffer while it rasterises (one extra store per peer and word).
  * A rank's buffer is complete once every rank's step has finished: the caller orders that (stream sync + barrier), exactly
- * as it orders the use of an all-gather's output.  dts_allgather_obs remains as the NCCL baseline of the same exchange. */
+ * as it orders the use of an all-gather's output.  dts_allgather_obs remains as the NCCL baseline of the same exchange.
+ * Slot `rank` starts at byte rank * bytes_per_rank, and the armed dts_step / dts_render writes its first num_envs * cam_h *
+ * cam_w * 3 * elem bytes (elem 1 for DTS_OBS_U8, 4 for DTS_OBS_F32_UNIT); no call writes the rest of the buffer, which
+ * dts_gather_alloc zeroes.
+ * bytes_per_rank is fixed here, so:
+ *   dts_gather_next    fails, and does not arm, while that batch is larger than bytes_per_rank;
+ *   dts_step, dts_render  fail while a gather is armed and a resize target is set (dts_set_resize: the gather carries the
+ *                      rasteriser's camera-sized output) or the batch, in the current output format, is larger than
+ *                      bytes_per_rank.  They check before launching anything: a refused call runs no step logic, writes
+ *                      no buffer and leaves the gather armed;
+ *   dts_step_terminal  fails while a gather is armed (it does not write one).
+ * dts_gather_alloc fails for a rank outside [0, world), a world outside [1, 8], and on a handle that has
+ * allocated one already; dts_gather_next fails before dts_gather_alloc and before dts_gather_open has mapped every other
+ * rank's buffer. */
 int dts_gather_alloc(dts_sim* sim, uint64_t bytes_per_rank, int rank, int world, uint8_t handle_out[64], void** buf_dev);
 int dts_gather_open(dts_sim* sim, const uint8_t* handles /* [world][64] */);
 int dts_gather_next(dts_sim* sim);
