@@ -4,9 +4,11 @@ Public surface (mirrors gym_duckietown's, SURVEY.md 8b):
   Simulator, DuckietownEnv, MultiMapEnv      single-env gym.Env adapters (old 4-tuple API)
   BatchedDuckietownEnv                       N envs per GPU, torch tensors in/out
   load_map, list_maps                        MapFormat1 loader
+  MARKING_NAMES                              names of the lane-marking image's values (markings=True)
 """
 __version__ = "0.1.0"
 
+from .assets import MARKING_NAMES  # noqa: F401
 from .maps import InvalidMapException, list_maps, load_map  # noqa: F401
 
 

@@ -334,6 +334,35 @@ def segment_tile_texture(kind: str, rgba: np.ndarray, style: str = "photos") -> 
     return out
 
 
+# ----------------------------------------------------------------------------- lane-marking classes (render spec item 11)
+MARKING_NAMES = ("none", "tile", "white", "yellow", "red")
+MARK_NONE, MARK_TILE, MARK_WHITE, MARK_YELLOW, MARK_RED = range(5)
+
+
+def tile_texel_classes(kind: str, rgba: np.ndarray, style: str = "photos") -> np.ndarray:
+    """uint8 [h, w], row 0 = t=0 as the texels: the marking class of every texel of road tile `kind`'s texture `rgba`.
+    Paint is what the reference's own filter keeps, segment_tile_texture(kind, rgba) not black (so a kind it flattens
+    has none, and the erosion trims a texel off each side of a line); an unpainted texel is MARK_TILE.  A painted texel's
+    class comes from OpenCV's HSV of the texel itself (H 0-179, S and V 0-255): S <= 100 white, else 11 <= H <= 45
+    yellow, else red.  The thresholds are this project's: the reference has no classes."""
+    h, w = rgba.shape[:2]
+    cls = np.full((h, w), MARK_TILE, np.uint8)
+    if should_segment_out(f"tiles-processed/{style}/{kind}/texture"):
+        return cls
+    import cv2   # (segment_tile_texture has already required it)
+    paint = segment_tile_texture(kind, rgba, style)[:, :, :3].any(axis=2)
+    hsv = cv2.cvtColor(np.ascontiguousarray(rgba[:, :, 2::-1]), cv2.COLOR_BGR2HSV)
+    hue, sat = hsv[:, :, 0], hsv[:, :, 1]
+    painted = np.where(sat <= 100, MARK_WHITE, np.where((hue >= 11) & (hue <= 45), MARK_YELLOW, MARK_RED))
+    cls[paint] = painted[paint]
+    return cls
+
+
+def mesh_texel_classes(rgba: np.ndarray) -> np.ndarray:
+    """uint8 [h, w] of zeros: a mesh's texels (signs, traffic-light cards, flat segment colours) are never road."""
+    return np.zeros(rgba.shape[:2], np.uint8)
+
+
 # ----------------------------------------------------------------------------- OBJ / MTL reader
 def load_obj(path: str, name: str, texture_loader=None) -> Mesh:
     """Wavefront reader with the reference loader's semantics (objmesh.py:65-293): triangles only,

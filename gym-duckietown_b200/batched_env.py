@@ -4,7 +4,7 @@
 observation buffers are caller-visible torch CUDA tensors, the work runs on
 `torch.cuda.current_stream()` inside libdtsim.so, nothing synchronises.  Constructor keywords are the
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
-`auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `camera_rand_pool`.
+`auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `camera_rand_pool`.
 
 `camera_rand=True` (with `distortion=True`; without it the flag does nothing, as in the reference, S:352-358) gives the
 envs a spread of lenses: `camera_rand_pool` calibrations K, D are drawn once, at construction, within the reference's
@@ -36,6 +36,12 @@ the map and for the agent's own mesh; `label_table(map_id)` names them.  It is t
 with both on `labels != 0` exactly where `depth != 0`; it follows the render modes, sizes and auto-reset as depth does,
 and lighting, textures, domain randomisation and `segment` leave it unchanged.  `object_boxes()` reduces it to every
 object's pixel count and bounding box.
+
+`markings=True` allocates `env.markings`, uint8 [num_envs, camera_height, camera_width], filled by the same renders: the
+lane paint each pixel shows (dts_set_marking_target), named by MARKING_NAMES — 0 no road tile (sky, ground, objects, no
+fisheye source), 1 a road tile's unpainted surface, 2 white, 3 yellow, 4 red — the class of the texel its label winner
+samples at the pixel centre.  It needs no label image and follows the render modes, sizes and auto-reset as labels do;
+lighting, domain randomisation and `segment` leave it unchanged.
 """
 from __future__ import annotations
 
@@ -45,6 +51,7 @@ import numpy as np
 import torch
 
 from . import lib as L
+from .assets import MARKING_NAMES  # noqa: F401  (the names of env.markings' values)
 from .episode import EpisodeSampler
 from .maps import TILE_KINDS, MapData, load_map
 
@@ -74,7 +81,7 @@ class BatchedDuckietownEnv:
                  action_mode: str = "vel_steer", auto_reset: bool = False, device_reset: bool = False,
                  cycle_maps: bool = False, env_id_offset: int = 0, tessellate_tiles: bool = False,
                  randomize_maps_on_reset: bool = False, randomization_config=None, terminal_obs: bool = False,
-                 depth: bool = False, labels: bool = False, camera_rand_pool: int = 16):
+                 depth: bool = False, labels: bool = False, camera_rand_pool: int = 16, markings: bool = False):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
         camera_rand = bool(camera_rand and distortion)   # S:353-356: camera_rand only with distortion
@@ -141,6 +148,9 @@ class BatchedDuckietownEnv:
             # the label image of the frames in obs (labels=True); the renders write it on the device
             self.labels: Optional[torch.Tensor] = torch.zeros(
                 (num_envs, camera_height, camera_width), dtype=torch.int16, device=self.device) if labels else None
+            # the lane-marking image of the frames in obs (markings=True); the renders write it on the device
+            self.markings: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, camera_height, camera_width), dtype=torch.uint8, device=self.device) if markings else None
             self.reward = torch.zeros(num_envs, dtype=torch.float32, device=self.device)
             self._done_u8 = torch.zeros(num_envs, dtype=torch.uint8, device=self.device)
             self.state: Dict[str, torch.Tensor] = {
@@ -162,6 +172,8 @@ class BatchedDuckietownEnv:
             self.sim.set_depth_target(self.depth.data_ptr())
         if labels:
             self.sim.set_label_target(self.labels.data_ptr())
+        if markings:
+            self.sim.set_marking_target(self.markings.data_ptr())
         self.seed(seed)
 
     def set_output_format(self, obs_layout: Optional[str] = None, obs_dtype: Optional[str] = None,

@@ -44,6 +44,7 @@ struct dts_sim {
   int render_mode = 0;                  // dts_set_render_mode             // the next dts_render also stores into the gather buffers
   float* depth_target = nullptr;        // dts_set_depth_target: caller-owned f32 [N][cam_h][cam_w], or null
   int16_t* label_target = nullptr;      // dts_set_label_target: caller-owned i16 [N][cam_h][cam_w], or null
+  uint8_t* marking_target = nullptr;    // dts_set_marking_target: caller-owned u8 [N][cam_h][cam_w], or null
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
   int profiling = 0;                    // 0 off, 1 events around k_raster only, 2 around every render kernel
   std::vector<cudaEvent_t> prof_events; // kProfMarks events per profiled frame
@@ -364,8 +365,8 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
       gt.base[p] = reinterpret_cast<uint8_t*>(sim->gather_peer[p]) + (uint64_t)sim->gather_rank * sim->gather_bytes;
     sim->gather_next = false;
   }
-  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, sim->label_target, target, gt,
-                        sim->d_err, sim->d_status, marks, mark_level, (cudaStream_t)stream);
+  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, sim->label_target,
+                        sim->marking_target, target, gt, sim->d_err, sim->d_status, marks, mark_level, (cudaStream_t)stream);
   if (rz.ow) {
     launch_resize(*sim->resize, rz.staging, obs_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, env_list, env_count,
                   (cudaStream_t)stream);
@@ -594,6 +595,12 @@ int dts_set_label_target(dts_sim* sim, int16_t* labels_dev) {
                          largest_label(counts[s].n_tiles, counts[s].n_objects));
   }
   sim->label_target = labels_dev;
+  return 0;
+}
+
+int dts_set_marking_target(dts_sim* sim, uint8_t* markings_dev) {
+  if (!sim) return 1;
+  sim->marking_target = markings_dev;
   return 0;
 }
 

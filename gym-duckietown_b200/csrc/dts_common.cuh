@@ -75,8 +75,10 @@ struct DMap {
   const float* tri_col;         // [T][3][3]
   const int16_t* tri_tex;
   int32_t n_textures;
+  uint32_t tex_class_off;       // the texel classes (dts_map_blob.tex_class) start at tex_pool + tex_class_off, one byte
+                                // per texel at the texture's texel offset, (info & 0xffffff) << 6 (in what was padding)
   const DTexture* textures;
-  const uint8_t* tex_pool;      // all RGBA8 textures, each 256-byte aligned
+  const uint8_t* tex_pool;      // all RGBA8 textures, each 256-byte aligned, then the texel classes
   const int16_t* tex_segment;   // [n_textures] segment=True replacement of each texture (or the same index)
   DObject agent;                // top-down views: the agent's own mesh (tri_count 0 = none)
   int32_t n_dyn;

@@ -122,8 +122,10 @@ std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* 
 // `labels`: NULL, or the label target (dts_set_label_target), i16 [n_envs][height][width], written beside obs like the
 // depth target, for the listed envs only where there is a list.  It is not a RenderCfg member: RenderCfg is every render
 // kernel's parameter block, and a longer one would move each kernel's later parameters.
+// `markings`: NULL, or the marking target (dts_set_marking_target), u8 [n_envs][height][width], the same way.
 constexpr int kProfMarks = 6;
-int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, int16_t* labels, void* obs,
+int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, int16_t* labels,
+                  uint8_t* markings, void* obs,
                   const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level,
                   cudaStream_t st);
 // What the last render left in frame memory for one env (dts_debug_frame), after the device has synchronised

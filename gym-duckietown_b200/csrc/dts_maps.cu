@@ -106,6 +106,11 @@ static uint64_t blob_hash(const dts_map_blob& b) {
     H.arr(s.rgba, (size_t)s.width * s.height * 4);
   }
   H.arr(b.tex_segment, b.tex_segment ? (size_t)b.n_textures : 0);
+  if (b.tex_class) {   // (a blob without classes hashes as before they existed)
+    size_t texels = 0;
+    for (int t = 0; t < b.n_textures; t++) texels += (size_t)b.textures[t].width * b.textures[t].height;
+    H.arr(b.tex_class, texels);
+  }
   H.val(b.start_tile[0]); H.val(b.start_tile[1]); H.val(b.has_start_pose);
   for (int k = 0; k < 3; k++) H.val(b.start_pose[k]);
   H.val(b.agent_mesh);
@@ -250,10 +255,16 @@ std::string maps_upload(MapSlots& ms, int slot, const dts_map_blob* blob) {
     off[t] = pool_size;
     pool_size += pool_bytes(b.textures[t]);
   }
-  std::vector<uint8_t> pool(pool_size ? pool_size : 256, 0);
+  // the texel classes follow the texels in the same allocation, a byte per texel at the texture's texel offset (off / 4),
+  // so that a prim's texture word finds both and a refused upload leaves the slot's classes with its texels
+  const size_t class_off = pool_size ? pool_size : 256;
+  std::vector<uint8_t> pool(class_off + class_off / 4, 0);
+  size_t class_src = 0;
   for (int t = 0; t < b.n_textures; t++) {
     const dts_texture& s = b.textures[t];
     memcpy(pool.data() + off[t], s.rgba, (size_t)s.width * s.height * 4);
+    if (b.tex_class) memcpy(pool.data() + class_off + off[t] / 4, b.tex_class + class_src, (size_t)s.width * s.height);
+    class_src += (size_t)s.width * s.height;
     int lw = 0, lh = 0;
     while ((1 << lw) < s.width) lw++;
     while ((1 << lh) < s.height) lh++;
@@ -262,6 +273,7 @@ std::string maps_upload(MapSlots& ms, int slot, const dts_map_blob* blob) {
     tex[t].pad = 0;
   }
   m.n_textures = b.n_textures;
+  m.tex_class_off = (uint32_t)class_off;   // (validate() keeps the pool below 4 GB)
   std::vector<int16_t> seg(b.n_textures > 0 ? b.n_textures : 1);
   for (int t = 0; t < b.n_textures; t++) {
     const int v = b.tex_segment ? b.tex_segment[t] : -1;

@@ -33,8 +33,12 @@
 // A label target (dts_set_label_target, render spec item 10) selects their kLabels instances in the same way, alone or
 // with kDepth: every pixel's draw item + 1, i16 [N][H][W].  The target reaches them as their last kernel parameter, not
 // through RenderCfg: a longer RenderCfg would move every later parameter of every render kernel.
+// A marking target (dts_set_marking_target, render spec item 11) selects their kMarks instances, alone or with kLabels:
+// they take the label's winners and store every pixel's texel class, u8 [N][H][W], and the depth where that target is
+// set (a pointer test in these instances only, instead of a kDepth variant of each), so the plain, depth and label
+// instances stay as they are.
 //
-// HBM traffic per env-frame: obs store W*H*3 B (compulsory; + W*H*4 B of depth and W*H*2 B of labels where asked for) + PrimRec slab / BinRec lists / lattice table
+// HBM traffic per env-frame: obs store W*H*3 B (compulsory; + W*H*4 B of depth, W*H*2 B of labels and W*H B of markings where asked for) + PrimRec slab / BinRec lists / lattice table
 // (tens of KB per env, written by k_geometry / k_bin and read once by k_raster) + texels (shared, L2-resident).
 #include <algorithm>
 #include <cstddef>
@@ -607,7 +611,9 @@ __device__ __forceinline__ unsigned build_binrec(const PrimRec* __restrict__ pr,
 // bilinear REPEAT texel, MODULATE.  Deferred shading: each lane may shade a different prim.  Split in two so that a
 // coarse bin lying inside ONE prim fetches the prim's planes once for its 256 pixels.
 // `qq_out` (depth target, render spec item 9) receives the prim's clamped 1/w at the pixel centre: the very value the
-// perspective divide uses.
+// perspective divide uses.  `cls_out` (marking target, render spec item 11) receives the class of the texel
+// (floor(u * tw) mod tw, floor(v * th) mod th) of the prim's texture from `cls_pool` (the map's texel classes, at the
+// texture's texel offset), u, v those the texel fetch uses; 0 for an untextured prim.
 struct ShadeIn {
   const PrimRec* pr;
   int x0, y0;
@@ -629,7 +635,8 @@ __device__ __forceinline__ ShadeIn load_shade(const PrimRec* __restrict__ prims,
   return si;
 }
 __device__ __forceinline__ void shade_eval(const ShadeIn& si, const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab,
-                                           int pxa, int pya, float c3[3], float* qq_out = nullptr) {
+                                           int pxa, int pya, float c3[3], float* qq_out = nullptr,
+                                           const uint8_t* __restrict__ cls_pool = nullptr, int* cls_out = nullptr) {
   const float cdx = (float)(pxa + 32 - si.x0) * 0.015625f, cdy = (float)(pya + 32 - si.y0) * 0.015625f;
   float qq = fmaf(si.qy, cdy, fmaf(si.qx, cdx, si.q0));
   if (!(qq > 1e-20f)) qq = 1e-20f;
@@ -662,6 +669,7 @@ __device__ __forceinline__ void shade_eval(const ShadeIn& si, const uint8_t* __r
     c3[1] = fmaf(w7.x, cdy, fmaf(w6.w, cdx, w6.z)) * rq;
     c3[2] = fmaf(w7.w, cdy, fmaf(w7.z, cdx, w7.y)) * rq;
   }
+  if (cls_out) *cls_out = 0;
   if (ltq & 0x00ff0000) {
     const unsigned ti = si.tex;
     const int lw = (ti >> 24) & 15, lh = ti >> 28;
@@ -686,12 +694,17 @@ __device__ __forceinline__ void shade_eval(const ShadeIn& si, const uint8_t* __r
       const float tc = fmaf(ffy, tb - ta, ta);
       c3[ch] = tc * (c3[ch] * 0.00392156862745098f);
     }
+    if (cls_out) {   // (u * twf is exact: a power of two)
+      const unsigned cu = (unsigned)__float2int_rd(u * twf) & (tw - 1), cv = (unsigned)__float2int_rd(v * thf) & (th - 1);
+      *cls_out = __ldg(cls_pool + ((size_t)(ti & 0xffffffu) << 6) + ((cv << lw) + cu));
+    }
   }
 }
 __device__ __forceinline__ void shade_prim(const PrimRec* __restrict__ prims, unsigned w, const uint8_t* __restrict__ tex_pool,
-                                           const float4* __restrict__ lat_tab, int pxa, int pya, float c3[3], float* qq_out = nullptr) {
+                                           const float4* __restrict__ lat_tab, int pxa, int pya, float c3[3], float* qq_out = nullptr,
+                                           const uint8_t* __restrict__ cls_pool = nullptr, int* cls_out = nullptr) {
   const ShadeIn si = load_shade(prims, w);
-  shade_eval(si, tex_pool, lat_tab, pxa, pya, c3, qq_out);
+  shade_eval(si, tex_pool, lat_tab, pxa, pya, c3, qq_out, cls_pool, cls_out);
 }
 
 // ---- bulk-async copy (TMA, 1-D) + mbarrier: global -> shared without register staging
@@ -893,6 +906,21 @@ __device__ __forceinline__ void take_label(float& qmax, int& lab, float qq, unsi
   if (!(qq >= qmax)) return;   // (a farther winner: its label is not looked up)
   const int l = label_of(w);
   if (qq > qmax || l < lab) { qmax = qq; lab = l; }
+}
+// Marking target (render spec item 11): as take_label, and `mk` keeps the smallest class `c` among the winners that
+// have both the kept 1/w and the kept label (two triangles of one tile, in tile mode 0 or clipped, can).  Exact values
+// and exact tie-breaks again: the order does not matter.
+template <typename LabelOf>
+__device__ __forceinline__ void take_mark(float& qmax, int& lab, int& mk, float qq, unsigned w, int c, const LabelOf& label_of) {
+  if (!(qq >= qmax)) return;
+  const int l = label_of(w);
+  if (qq > qmax || l < lab) { qmax = qq; lab = l; mk = c; }
+  else if (l == lab) mk = min(mk, c);
+}
+// The marking frame `mf` (u8 [H][W] of one env): a lane stores its own pixel, 1 byte.
+__device__ __forceinline__ void store_marking(uint8_t* __restrict__ mf, int v, int lane, int bx, int by, int W, int H) {
+  const int gx = bx * kBinW + (lane & 7), gy = by * kBinH + (lane >> 3);
+  if (gx < W && gy < H) mf[(size_t)gy * W + gx] = (uint8_t)v;
 }
 // The label frame `lf` (i16 [H][W] of one env): a lane stores its own pixel, 2 bytes.  The 8 lanes of a bin row write 16
 // contiguous bytes — half a 32-byte sector — so pairs packed into 4-byte stores with a shuffle would write the same
@@ -1617,12 +1645,13 @@ __device__ __forceinline__ int sample_mask(const BinRec& br, int pxc, int pyc) {
 // addends, so neither the lane nor the order in which the winners are shaded changes a bit.  Called by the whole warp.
 // kDepth: `qmax` comes in as the first winner's 1/w (0: none) and leaves as the largest over the pixel's winners; a
 // maximum of exact values, so the order does not matter there either.  kLabels: the same, and `lab` comes in as the
-// first winner's label (0: none) and leaves as the pixel's (take_label; label_of(w): the label of prim w).
-template <bool kDepth, bool kLabels, typename LabelOf>
+// first winner's label (0: none) and leaves as the pixel's (take_label; label_of(w): the label of prim w).  kMarks
+// (with kLabels): `mk` the same for the marking, the class coming from `cls_pool` (take_mark).
+template <bool kDepth, bool kLabels, bool kMarks, typename LabelOf>
 __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], const float clr[3], const PrimRec* __restrict__ prims,
                                              const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa, int pya,
-                                             int lane, int32_t* __restrict__ err, float& qmax, int* lab,
-                                             const LabelOf& label_of) {
+                                             int lane, int32_t* __restrict__ err, float& qmax, int* lab, int* mk,
+                                             const LabelOf& label_of, const uint8_t* __restrict__ cls_pool) {
   (void)lane; (void)err;   // (DTS_STATS counters)
   float s01[3] = {c3[0], c3[1], c3[2]}, s23[3] = {0.f, 0.f, 0.f};   // 0 + c == c
   unsigned pend = 0xeu;
@@ -1638,8 +1667,12 @@ __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], 
       const unsigned w = s == 1 ? wn[1] : (s == 2 ? wn[2] : wn[3]);
       float d3[3] = {clr[0], clr[1], clr[2]};
       float qq = 0.0f;
-      if (w != kNoPrim) shade_prim(prims, w, tex_pool, lat_tab, pxa, pya, d3, (kDepth || kLabels) ? &qq : nullptr);
-      if (kLabels) {
+      int c = 0;
+      if (w != kNoPrim)
+        shade_prim(prims, w, tex_pool, lat_tab, pxa, pya, d3, (kDepth || kLabels) ? &qq : nullptr, cls_pool, kMarks ? &c : nullptr);
+      if (kMarks) {
+        if (w != kNoPrim) take_mark(qmax, *lab, *mk, qq, w, c, label_of);
+      } else if (kLabels) {
         if (w != kNoPrim) take_label(qmax, *lab, qq, w, label_of);
       } else if (kDepth) {
         qmax = fmaxf(qmax, qq);
@@ -1658,37 +1691,43 @@ __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], 
 }
 // The whole resolve of one fine bin's pixels (k_raster).  `simple`: the caller knows that every sample of the whole fine
 // bin has the same winner.  kDepth: `qmax` receives the largest 1/w among the pixel's winners, 0 if it has none.
-// kLabels: `qmax` the same, and `lab` the pixel's label, 0 if it has no winner.
-template <bool kDepth, bool kLabels, typename LabelOf>
+// kLabels: `qmax` the same, and `lab` the pixel's label, 0 if it has no winner.  kMarks (with kLabels): `mk` the
+// pixel's marking, 0 if it has no winner.
+template <bool kDepth, bool kLabels, bool kMarks, typename LabelOf>
 __device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool simple, const float clr[3], const PrimRec* __restrict__ prims,
                                                   const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa,
-                                                  int pya, int lane, int32_t* __restrict__ err, float& qmax, int* lab,
-                                                  const LabelOf& label_of) {
+                                                  int pya, int lane, int32_t* __restrict__ err, float& qmax, int* lab, int* mk,
+                                                  const LabelOf& label_of, const uint8_t* __restrict__ cls_pool) {
   const bool same = wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0];
   const bool all_same = simple || __all_sync(0xffffffffu, same);
   float c3[3] = {clr[0], clr[1], clr[2]};
   if (kDepth || kLabels) qmax = 0.0f;
   if (kLabels) *lab = 0;
+  if (kMarks) *mk = 0;
   if (wn[0] != kNoPrim) {   // every lane: its first winner
-    shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3, (kDepth || kLabels) ? &qmax : nullptr);
+    shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3, (kDepth || kLabels) ? &qmax : nullptr, cls_pool, kMarks ? mk : nullptr);
     if (kLabels) *lab = label_of(wn[0]);
   }
   if (!all_same)   // (four equal samples: the mean is the value itself)
-    resolve_edge<kDepth, kLabels>(wn, c3, clr, prims, tex_pool, lat_tab, pxa, pya, lane, err, qmax, lab, label_of);
+    resolve_edge<kDepth, kLabels, kMarks>(wn, c3, clr, prims, tex_pool, lat_tab, pxa, pya, lane, err, qmax, lab, mk, label_of,
+                                          cls_pool);
   return pack_rgb(c3[0], c3[1], c3[2]);
 }
 
 // ------------------------------------------------------------------------------------------------ k_raster
-template <bool kWrapFmt, bool kFish, bool kDepth, bool kLabels, bool kPool = false>
+template <bool kWrapFmt, bool kFish, bool kDepth, bool kLabels, bool kPool = false, bool kMarks = false>
                                        // kWrapFmt: a dts_output_format other than packed u8 HWC is written by the resolve;
                                        // kFish: every lane renders the SOURCE pixel the fisheye LUT names for its output pixel;
                                        // kDepth: every pixel's depth goes to rc.depth beside its colour (render spec item 9);
                                        // kLabels: every pixel's label goes to `labels` (render spec item 10);
-                                       // kPool: each env's tables of a pool (fish_of_env)
+                                       // kPool: each env's tables of a pool (fish_of_env);
+                                       // kMarks (kDepth false): every pixel's marking goes to `marks` (render spec item 11),
+                                       // and its depth where rc.depth is set
 __global__ void __launch_bounds__(kThreads, kRasterMinCtas)
 k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, FishTab fts, GatherTab gt,
          uint8_t* __restrict__ obs, int max_prims, int max_pairs, int max_lat, int32_t* __restrict__ err,
-         int16_t* __restrict__ labels, const uint16_t* __restrict__ fish_tab) {
+         int16_t* __restrict__ labels, const uint16_t* __restrict__ fish_tab, uint8_t* __restrict__ marks) {
+  constexpr bool kLab = kLabels || kMarks;   // the label's winner: markings are taken from it
   // dynamic shared memory (kRasterSmem bytes): per warp two chunks of records in flight, their mbarriers, and a 128-sample
   // depth / winner buffer for the tiny triangles of the fine bin being drawn
   extern __shared__ __align__(128) unsigned char raster_smem[];
@@ -1729,19 +1768,22 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     const size_t env_off = (size_t)env * frame_bytes * out_elem;
     uint8_t* out = obs + env_off;
-    float* dep = kDepth ? rc.depth + (size_t)env * W * H : nullptr;
+    float* dep = (kDepth || (kMarks && rc.depth)) ? rc.depth + (size_t)env * W * H : nullptr;
     int16_t* lf = kLabels ? labels + (size_t)env * W * H : nullptr;
+    uint8_t* mf = kMarks ? marks + (size_t)env * W * H : nullptr;
+    const uint8_t* cls_pool = kMarks ? tex_pool + m.tex_class_off : nullptr;
     LabelMap lm{};
-    if constexpr (kLabels) lm = label_map(m, rc.tessellate);
+    if constexpr (kLab) lm = label_map(m, rc.tessellate);
     auto label_of = [&](unsigned w) { return label_of_id(lm, __ldg(&prims[w].id)); };
     // one fine bin -> the caller's tensor and, on a gathering step, every peer's gather buffer (NVLink stores)
     // On a gathering step (gt.n > 0) the packed u8 HWC frame goes to the peers in BLOCKS: a work item is 8 whole image rows =
     // one contiguous run of bytes, copied to every rank's gather buffer with 16-byte vector stores once the item is drawn
     // (NVLink wants long writes: per-bin 4-byte stores reach a fifth of the link rate).  Other layouts store per bin.
     const bool gather_rows = gt.n > 0 && !kWrapFmt;
-    auto emit = [&](unsigned rgb, float depth, int label, int bx, int by) {
-      if (kDepth) store_depth(dep, depth, lane, bx, by, W, H);   // (the caller's depth tensor only: the gather carries obs)
+    auto emit = [&](unsigned rgb, float depth, int label, int mark, int bx, int by) {
+      if (kDepth || (kMarks && dep)) store_depth(dep, depth, lane, bx, by, W, H);   // (the caller's depth tensor only: the gather carries obs)
       if (kLabels) store_label(lf, label, lane, bx, by, W, H);
+      if (kMarks) store_marking(mf, mark, lane, bx, by, W, H);
       if (fast_fmt && (gt.n == 0 || gather_rows) && bx * kBinW + kBinW <= W) {   // the common case inline: packed u8 HWC, whole bin inside
         store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
       } else if (kWrapFmt && gt.n == 0) {
@@ -1809,7 +1851,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
             const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);
             unsigned rgb = clear_rgb;
             if (kFish && !fish_source(ft, bx, by, lane, W, H).valid) rgb = 0u;
-            emit(rgb, 0.0f, 0, bx, by);
+            emit(rgb, 0.0f, 0, 0, bx, by);
           }
         continue;
       }
@@ -2020,11 +2062,11 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
             // ---- deferred shading: once per distinct winner of this pixel, then the box resolve
             DTS_COUNT(11, 1);
             float qmax = 0.0f;
-            int lab = 0;
-            unsigned rgb = shade_resolve<kDepth, kLabels>(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane, err,
-                                                          qmax, &lab, label_of);
+            int lab = 0, mk = 0;
+            unsigned rgb = shade_resolve<kDepth, kLab, kMarks>(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane,
+                                                               err, qmax, &lab, &mk, label_of, cls_pool);
             if (kFish && !px_valid) rgb = 0u;   // cv2.remap BORDER_CONSTANT
-            emit(rgb, kDepth ? depth_of(qmax, px_valid) : 0.0f, px_valid ? lab : 0, bx, by);
+            emit(rgb, (kDepth || kMarks) ? depth_of(qmax, px_valid) : 0.0f, px_valid ? lab : 0, px_valid ? mk : 0, bx, by);
           }
         }
       }
@@ -2043,14 +2085,17 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
 // visibility state: a warp fetches the prim's planes once and shades the bin's 256 pixels.  A separate kernel so that the
 // lean loop gets its own register allocation (the same fast path inside k_raster cost more than it saved).
 // Packed u8 HWC output with whole-word rows only (k_bin marks no bin otherwise).  Runs before k_raster.
-template <bool kFish, bool kDepth, bool kLabels, bool kPool = false>
+template <bool kFish, bool kDepth, bool kLabels, bool kPool = false, bool kMarks = false>
                                      // kFish: each lane shades the source pixel the fisheye LUT names for its output pixel;
                                      // kDepth: the 1/w the shading divides by also gives the pixel's depth (rc.depth);
                                      // kLabels: the bin's one prim gives every pixel with a source its label (`labels`);
-                                     // kPool: each env's tables of a pool (fish_of_env)
+                                     // kPool: each env's tables of a pool (fish_of_env);
+                                     // kMarks (kDepth false): the class of the texel the prim shows at each pixel with a
+                                     // source (`marks`), and the depth where rc.depth is set
 __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
                                                                         FishTab fts, uint8_t* __restrict__ obs, int max_prims, int max_lat,
-                                                                        int16_t* __restrict__ labels, const uint16_t* __restrict__ fish_tab) {
+                                                                        int16_t* __restrict__ labels, const uint16_t* __restrict__ fish_tab,
+                                                                        uint8_t* __restrict__ marks) {
   const int W = rc.width, H = rc.height;
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW;
   const int lane = threadIdx.x & 31;
@@ -2071,6 +2116,7 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
     int lab = 0;
     if constexpr (kLabels)
       lab = label_of_id(label_map(maps[S.map_id[env]], rc.tessellate), __ldg(&fm.prims[(size_t)env * max_prims + p].id));
+    const uint8_t* cls_pool = kMarks ? tex_pool + maps[S.map_id[env]].tex_class_off : nullptr;
     // fine bins inside the image as loop bounds rather than fine_in_image(): the mask test costs this loop machine code
     const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);
     const int ny = ((cby * kCFY + 1) * kBinH < H) ? 2 : 1;
@@ -2087,12 +2133,14 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
         pxa = src.x; pya = src.y;
       }
       float c3[3], qq = 0.0f;
-      shade_eval(si, tex_pool, lat_tab, pxa, pya, c3, kDepth ? &qq : nullptr);
+      int mk = 0;
+      shade_eval(si, tex_pool, lat_tab, pxa, pya, c3, (kDepth || kMarks) ? &qq : nullptr, cls_pool, kMarks ? &mk : nullptr);
       unsigned rgb = pack_rgb(c3[0], c3[1], c3[2]);
       if (kFish && !px_valid) rgb = 0u;
       store_bin_lean(out, sl, rgb, lane, bx, by, W, H);
-      if (kDepth) store_depth(rc.depth + (size_t)env * W * H, depth_of(qq, px_valid), lane, bx, by, W, H);
+      if (kDepth || (kMarks && rc.depth)) store_depth(rc.depth + (size_t)env * W * H, depth_of(qq, px_valid), lane, bx, by, W, H);
       if (kLabels) store_label(labels + (size_t)env * W * H, px_valid ? lab : 0, lane, bx, by, W, H);
+      if (kMarks) store_marking(marks + (size_t)env * W * H, px_valid ? mk : 0, lane, bx, by, W, H);
     }
   }
 }
@@ -2120,15 +2168,18 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
 // kLabels: the same for labels, with no more shared memory.  A queued pixel's first label is looked up again from its
 // first winner, which the queue holds; its 1/w comes from the depth array (kept for labels alone, too).  Only the ground
 // and road tiles come here, so a label is arithmetic on the draw id (tile_label).
+// kMarks (kDepth false): markings, and the depth where rc.depth is set.  A queued pixel's
+// first winner's class rides in the high half of its entry's slot word: still no more shared memory.
 // Packed u8 HWC output with whole-word rows only (k_bin lists no bin otherwise).  Runs after k_raster_solo.
 constexpr int kEdgeQ = 64;   // queue ring: flushed at 32 entries, so at most 31 + 32 wait at once
-template <bool kFish, bool kDepth, bool kLabels, bool kPool = false>
+template <bool kFish, bool kDepth, bool kLabels, bool kPool = false, bool kMarks = false>
                                  // kFish: each lane covers and shades the source pixel the fisheye LUT names for its output pixel;
                                  // kPool: each env's tables of a pool (fish_of_env)
 __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
                                                                         FishTab fts, uint8_t* __restrict__ obs, int max_prims, int max_lat,
                                                                         int32_t* __restrict__ err, int16_t* __restrict__ labels,
-                                                                        const uint16_t* __restrict__ fish_tab) {
+                                                                        const uint16_t* __restrict__ fish_tab, uint8_t* __restrict__ marks) {
+  constexpr bool kLab = kLabels || kMarks;   // the label's winner: markings are taken from it
   __shared__ BinRec stages[kWarps][kStage];   // per warp: the records of its bin
   __shared__ unsigned bin_rgb[kWarps][kCFX * kCFY * 32];   // per warp: packed colour of pixel `lane` of fine bin f at f * 32 + lane
   // per warp: the edge-pixel queue, an entry in two words: (pixel slot, pxa, pya, wn0 | wn1 << 16), (wn2 | wn3 << 16, first colour)
@@ -2139,8 +2190,8 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
   BinRec* stage = stages[threadIdx.x >> 5];
   unsigned* rgb_buf = bin_rgb[threadIdx.x >> 5];
   uint4 (*q)[kEdgeQ] = edge_q[threadIdx.x >> 5];
-  float* q_qq = nullptr;   // kDepth, kLabels: per queue entry, the first winner's 1/w
-  if constexpr (kDepth || kLabels) {
+  float* q_qq = nullptr;   // kDepth, kLabels, kMarks: per queue entry, the first winner's 1/w
+  if constexpr (kDepth || kLab) {
     __shared__ float edge_qq[kWarps][kEdgeQ];
     q_qq = edge_qq[threadIdx.x >> 5];
   }
@@ -2173,8 +2224,10 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
     const PrimRec* prims = fm.prims + (size_t)env * max_prims;
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     uint8_t* out = obs + (size_t)env * frame_bytes;
-    float* dep = kDepth ? rc.depth + (size_t)env * W * H : nullptr;
+    float* dep = (kDepth || (kMarks && rc.depth)) ? rc.depth + (size_t)env * W * H : nullptr;
     int16_t* lf = kLabels ? labels + (size_t)env * W * H : nullptr;
+    uint8_t* mf = kMarks ? marks + (size_t)env * W * H : nullptr;
+    const uint8_t* cls_pool = kMarks ? tex_pool + maps[S.map_id[env]].tex_class_off : nullptr;
     auto label_of = [&](unsigned w) { return tile_label(rc.tessellate, __ldg(&prims[w].id)); };
     float clr[3];
     clear_colour(S, rc, env, clr);
@@ -2247,19 +2300,23 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
       // ---- every lane: its first winner.  One winner: the pixel is done.  More: it waits in the queue.  (A pixel the
       // fisheye LUT gives no source is black either way.)
       float c3[3] = {clr[0], clr[1], clr[2]}, qq0 = 0.0f;
-      if (wn[0] != kNoPrim) shade_prim(prims, wn[0], tex_pool, lat_tab, ox + pxc, oy + pyc, c3, (kDepth || kLabels) ? &qq0 : nullptr);
+      int c0 = 0;
+      if (wn[0] != kNoPrim)
+        shade_prim(prims, wn[0], tex_pool, lat_tab, ox + pxc, oy + pyc, c3, (kDepth || kLab) ? &qq0 : nullptr, cls_pool,
+                   kMarks ? &c0 : nullptr);
       const bool edge = px_valid && !(wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0]);
       const unsigned edges = __ballot_sync(0xffffffffu, edge);
       const unsigned slot = f * 32 + lane;
       if (edge) {
         const int e = (qs + __popc(edges & ((1u << lane) - 1u))) & (kEdgeQ - 1);
-        q[0][e] = make_uint4(slot, (unsigned)(ox + pxc), (unsigned)(oy + pyc), wn[0] | (wn[1] << 16));
+        q[0][e] = make_uint4(kMarks ? slot | (unsigned)c0 << 16 : slot, (unsigned)(ox + pxc), (unsigned)(oy + pyc), wn[0] | (wn[1] << 16));
         q[1][e] = make_uint4(wn[2] | (wn[3] << 16), __float_as_uint(c3[0]), __float_as_uint(c3[1]), __float_as_uint(c3[2]));
-        if (kDepth || kLabels) q_qq[e] = qq0;
+        if (kDepth || kLab) q_qq[e] = qq0;
       } else {
         rgb_buf[slot] = (kFish && !px_valid) ? 0u : pack_rgb(c3[0], c3[1], c3[2]);
-        if (kDepth) store_depth(dep, depth_of(qq0, px_valid), lane, bx, by, W, H);
+        if (kDepth || (kMarks && dep)) store_depth(dep, depth_of(qq0, px_valid), lane, bx, by, W, H);
         if (kLabels) store_label(lf, (px_valid && wn[0] != kNoPrim) ? label_of(wn[0]) : 0, lane, bx, by, W, H);
+        if (kMarks) store_marking(mf, px_valid ? c0 : 0, lane, bx, by, W, H);   // (c0 = 0 without a winner)
       }
       qs += __popc(edges);
       DTS_COUNT(26, __popc(edges));
@@ -2271,26 +2328,30 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
         __syncwarp();   // the entries were written by other lanes
         unsigned qw[4] = {0u, 0u, 0u, 0u};   // (lanes without an entry: one winner, nothing to shade)
         float q3[3] = {0.f, 0.f, 0.f}, qmax = 0.0f;
-        int qlab = 0;
+        int qlab = 0, qmk = 0;
         unsigned qslot = 0u;
         int qx = 0, qy = 0;
         if (lane < take) {
           const int e = ((qs >> 16) + lane) & (kEdgeQ - 1);
           const uint4 a = q[0][e], c = q[1][e];
-          qslot = a.x; qx = (int)a.y; qy = (int)a.z;
+          qslot = kMarks ? a.x & 0xffffu : a.x; qx = (int)a.y; qy = (int)a.z;
+          if (kMarks) qmk = (int)(a.x >> 16);
           qw[0] = a.w & 0xffffu; qw[1] = a.w >> 16; qw[2] = c.x & 0xffffu; qw[3] = c.x >> 16;
           q3[0] = __uint_as_float(c.y); q3[1] = __uint_as_float(c.z); q3[2] = __uint_as_float(c.w);
-          if (kDepth || kLabels) qmax = q_qq[e];
-          if (kLabels && qw[0] != kNoPrim) qlab = label_of(qw[0]);
+          if (kDepth || kLab) qmax = q_qq[e];
+          if (kLab && qw[0] != kNoPrim) qlab = label_of(qw[0]);
         }
-        resolve_edge<kDepth, kLabels>(qw, q3, clr, prims, tex_pool, lat_tab, qx, qy, lane, err, qmax, &qlab, label_of);
+        resolve_edge<kDepth, kLab, kMarks>(qw, q3, clr, prims, tex_pool, lat_tab, qx, qy, lane, err, qmax, &qlab, &qmk, label_of,
+                                           cls_pool);
         if (lane < take) rgb_buf[qslot] = pack_rgb(q3[0], q3[1], q3[2]);
-        // the queued pixel `qslot` = fine bin * 32 + lane-in-bin: its depth and label go straight to the frame (queued
-        // pixels have a source)
-        if (kDepth && lane < take)
+        // the queued pixel `qslot` = fine bin * 32 + lane-in-bin: its depth, label and marking go straight to the frame
+        // (queued pixels have a source)
+        if ((kDepth || (kMarks && dep)) && lane < take)
           store_depth(dep, depth_of(qmax), (int)(qslot & 31u), cbx * kCFX + (int)((qslot >> 5) & 3u), cby * kCFY + (int)(qslot >> 7), W, H);
         if (kLabels && lane < take)
           store_label(lf, qlab, (int)(qslot & 31u), cbx * kCFX + (int)((qslot >> 5) & 3u), cby * kCFY + (int)(qslot >> 7), W, H);
+        if (kMarks && lane < take)
+          store_marking(mf, qmk, (int)(qslot & 31u), cbx * kCFX + (int)((qslot >> 5) & 3u), cby * kCFY + (int)(qslot >> 7), W, H);
         qs += (unsigned)take << 16;
         __syncwarp();   // read before the next fine bin's entries overwrite the ring
       }
@@ -2510,8 +2571,8 @@ std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, in
   return rc ? "debug_frame_copy failed" : "";
 }
 
-int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, int16_t* labels, void* obs_any,
-                  const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level,
+int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, int16_t* labels,
+                  uint8_t* markings, void* obs_any, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level,
                   cudaStream_t st) {
   uint8_t* obs = reinterpret_cast<uint8_t*>(obs_any);
   // the gather the frame goes through, if any: the rectification (DTS_RENDER_RECTIFY), none (DTS_RENDER_PINHOLE or no
@@ -2558,14 +2619,19 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   const bool depth = rc.depth != nullptr;
   // so does a label target, alone or with depth
   const int out = (depth ? 1 : 0) | (labels ? 2 : 0);
+  // a marking target selects the kMarks instances, with kLabels where a label target is set; they write the depth
+  // where that target is set
+  const bool marking = markings != nullptr;
   if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
     const auto solo_of = [&](auto fish, auto pool_) {
       constexpr bool f = decltype(fish)::value, p = decltype(pool_)::value;
+      if (marking) return labels ? k_raster_solo<f, false, true, p, true> : k_raster_solo<f, false, false, p, true>;
       return out == 3 ? k_raster_solo<f, true, true, p> : out == 2 ? k_raster_solo<f, false, true, p>
                                                         : out == 1 ? k_raster_solo<f, true, false, p> : k_raster_solo<f, false, false, p>;
     };
     const auto flat_of = [&](auto fish, auto pool_) {
       constexpr bool f = decltype(fish)::value, p = decltype(pool_)::value;
+      if (marking) return labels ? k_raster_flat<f, false, true, p, true> : k_raster_flat<f, false, false, p, true>;
       return out == 3 ? k_raster_flat<f, true, true, p> : out == 2 ? k_raster_flat<f, false, true, p>
                                                         : out == 1 ? k_raster_flat<f, true, false, p> : k_raster_flat<f, false, false, p>;
     };
@@ -2573,13 +2639,16 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
                     : fisheye ? solo_of(std::true_type{}, std::false_type{}) : solo_of(std::false_type{}, std::false_type{});
     const auto flat = pool ? flat_of(std::true_type{}, std::true_type{})
                     : fisheye ? flat_of(std::true_type{}, std::false_type{}) : flat_of(std::false_type{}, std::false_type{});
-    solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, labels, fish_tab);
+    solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, labels, fish_tab,
+                                                     markings);
     // before k_raster, which draws the bins k_raster_flat hands back
-    flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, err_flag, labels, fish_tab);
+    flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, err_flag, labels, fish_tab,
+                                                     markings);
     launches += 2;
   }
   const auto raster_of = [&](auto wrap_fmt, auto fish, auto pool_) {
     constexpr bool w = decltype(wrap_fmt)::value, f = decltype(fish)::value, p = decltype(pool_)::value;
+    if (marking) return labels ? k_raster<w, f, false, true, p, true> : k_raster<w, f, false, false, p, true>;
     return out == 3 ? k_raster<w, f, true, true, p> : out == 2 ? k_raster<w, f, false, true, p>
                                                     : out == 1 ? k_raster<w, f, true, false, p> : k_raster<w, f, false, false, p>;
   };
@@ -2589,7 +2658,7 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
                     : fisheye ? (wrap ? raster_of(yes, yes, no) : raster_of(no, yes, no))
                               : (wrap ? raster_of(yes, no, no) : raster_of(no, no, no));
   raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, ft, gather, obs, r.max_prims, r.pool, r.max_lat, err_flag,
-                                                                labels, fish_tab);
+                                                                labels, fish_tab, markings);
   mark();
   mark();   // (post passes: launched by the caller)
   return launches;
@@ -2606,7 +2675,8 @@ Renderer* renderer_create(const dts_config& cfg) {
   const auto opt_in = [](auto wrap_fmt, auto fish, auto pool) {
     constexpr bool w = decltype(wrap_fmt)::value, f = decltype(fish)::value, p = decltype(pool)::value;
     for (const auto raster : {k_raster<w, f, false, false, p>, k_raster<w, f, true, false, p>, k_raster<w, f, false, true, p>,
-                              k_raster<w, f, true, true, p>})
+                              k_raster<w, f, true, true, p>, k_raster<w, f, false, false, p, true>,
+                              k_raster<w, f, false, true, p, true>})
       cudaFuncSetAttribute(raster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
   };
   const std::true_type yes{};

@@ -114,7 +114,7 @@ class MapBlob(C.Structure):
         ("tri_uv", C.c_void_p), ("tri_col", C.c_void_p), ("tri_tex", C.c_void_p), ("n_textures", C.c_int32),
         ("textures", C.c_void_p), ("start_tile", C.c_int32 * 2), ("n_dyn", C.c_int32), ("has_start_pose", C.c_int32),
         ("dyn", C.c_void_p), ("start_pose", C.c_double * 3),
-        ("tex_segment", C.c_void_p), ("agent_mesh", C.c_int32), ("reserved2", C.c_int32),
+        ("tex_segment", C.c_void_p), ("agent_mesh", C.c_int32), ("reserved2", C.c_int32), ("tex_class", C.c_void_p),
     ]
 
 
@@ -186,6 +186,7 @@ def load() -> C.CDLL:
     lib.dts_set_render_mode.argtypes = [vp, i]
     lib.dts_set_depth_target.argtypes = [vp, vp]
     lib.dts_set_label_target.argtypes = [vp, vp]
+    lib.dts_set_marking_target.argtypes = [vp, vp]
     lib.dts_resize_frames.argtypes = [vp, vp, vp, vp]
     lib.dts_blend4.argtypes = [vp, vp, vp, vp, C.c_uint64, vp]
     lib.dts_set_timing.argtypes = [vp, C.c_double, i, i]
@@ -220,7 +221,7 @@ def load() -> C.CDLL:
 
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_fisheye_luts", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
-           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
+           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
            "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
 
@@ -272,6 +273,9 @@ class MapBlobHolder:
             off += len(m.tri_pos)
             pos.append(m.tri_pos); nrm.append(m.tri_nrm); uv.append(m.tri_uv); col.append(m.tri_col)
             ttex.append(np.where(m.tri_tex >= 0, m.tri_tex + base, -1).astype(np.int16))
+        # lane-marking classes of every texture (render spec item 11): the tiles' from their paint, 0 for the meshes'
+        tex_cls = [assets.tile_texel_classes(TILE_KINDS[kid], tex_imgs[ti]) for kid, ti in kind_tex.items()]
+        tex_cls += [assets.mesh_texel_classes(im) for im in tex_imgs[n_tile_tex:]]
         # segment=True assets: tiles keep their lane markings or go black (graphics.py:70-130); every chunk of a mesh
         # shows the flat class colour gen_segmentation_color(mesh_name) (objmesh.py:260-290)
         seg_of = np.arange(len(tex_imgs), dtype=np.int64)
@@ -279,14 +283,22 @@ class MapBlobHolder:
         for kid, ti in kind_tex.items():
             seg_of[ti] = len(tex_imgs)
             tex_imgs.append(np.ascontiguousarray(assets.segment_tile_texture(TILE_KINDS[kid], tex_imgs[ti])))
+            # a segment replacement carries the classes of the texture it replaces, so segment=True keeps the markings
+            # (a flattened kind's 1x1 replacement: one texel of MARK_TILE)
+            tex_cls.append(tex_cls[ti] if tex_imgs[-1].shape[:2] == tex_cls[ti].shape
+                           else np.full(tex_imgs[-1].shape[:2], assets.MARK_TILE, np.uint8))
         for mi, m in enumerate(mesh_list):
             name = "sign_generic" if m.name.startswith("sign") else m.name
             meshes[mi].seg_flat_tex = len(tex_imgs)
             seg_of[mesh_tex_range[mi][0]:mesh_tex_range[mi][1]] = len(tex_imgs)
             tex_imgs.append(assets.flat_texture(assets.gen_segmentation_color(name)))
+            tex_cls.append(assets.mesh_texel_classes(tex_imgs[-1]))
         seg_full = np.arange(len(tex_imgs), dtype=np.int16)
         seg_full[:n_plain] = seg_of
         k["seg"] = seg_full
+        k["tex_cls"] = tex_cls     # uint8 [h, w] per texture, in texture order
+        k["tex_class"] = np.ascontiguousarray(np.concatenate([c.ravel() for c in tex_cls]) if tex_cls
+                                              else np.zeros(1, np.uint8))
         cat = lambda lst, shape, dt: (np.ascontiguousarray(np.concatenate(lst, 0), dt) if lst else np.zeros(shape, dt))
         k["tpos"] = cat(pos, (0, 3, 3), np.float32); k["tnrm"] = cat(nrm, (0, 3, 3), np.float32)
         k["tuv"] = cat(uv, (0, 3, 2), np.float32); k["tcol"] = cat(col, (0, 3, 3), np.float32)
@@ -326,7 +338,7 @@ class MapBlobHolder:
             len(md.dyn_objects), int(md.start_pose is not None), C.cast(dyn, C.c_void_p),
             (C.c_double * 3)(*((float(md.start_pose[0][0]), float(md.start_pose[0][2]), float(md.start_pose[1]))
                                if md.start_pose is not None else (0.0, 0.0, 0.0))),
-            _ptr(k["seg"]), agent_mesh, 0)
+            _ptr(k["seg"]), agent_mesh, 0, _ptr(k["tex_class"]))
         self.agent_mesh, self.n_tile_tex = agent_mesh, n_tile_tex
 
 
@@ -470,6 +482,12 @@ class Sim:
         """Every later render also writes float32 [num_envs, cam_height, cam_width] eye-space depth at `depth_ptr`, which
         the caller keeps alive; None turns it off (dts_set_depth_target)."""
         self._check(self.lib.dts_set_depth_target(self.h, depth_ptr), "dts_set_depth_target")
+
+    def set_marking_target(self, markings_ptr: Optional[int]):
+        """Write every later render's lane-marking image (uint8 [num_envs][cam_h][cam_w], render spec item 11: the class
+        of the texel each pixel's label winner samples, named by MARKING_NAMES) at `markings_ptr`, which the caller keeps
+        alive; None turns it off (dts_set_marking_target)."""
+        self._check(self.lib.dts_set_marking_target(self.h, markings_ptr), "dts_set_marking_target")
 
     def set_label_target(self, labels_ptr: Optional[int]):
         """Every later render also writes int16 [num_envs, cam_height, cam_width] labels (which draw item each pixel

@@ -195,6 +195,8 @@ typedef struct {
                                      (graphics.py:52-56, 70-130; objmesh.py:268-290); NULL or -1 = unchanged */
   int32_t agent_mesh;             /* mesh drawn at the agent's pose in top-down views (self.mesh, S:864, S:1923-1929); -1 = none */
   int32_t reserved2;
+  const uint8_t* tex_class;       /* texel classes of every texture in texture order, width*height each (row 0 = t=0, as
+                                     rgba), values of dts_set_marking_target; NULL = all 0 */
 } dts_map_blob;
 
 /* Per-episode inputs produced by Simulator.reset() (simulator.py:528-763, SURVEY 8a row P0), one
@@ -333,6 +335,21 @@ int dts_set_depth_target(dts_sim* sim, float* depth_dev);
  * envs (the second pass of dts_step_terminal) writes only those envs' rows, so after dts_step_terminal row e matches
  * obs_dev row e; the terminal frames' labels are not kept.  The fused gather (dts_gather_next) carries observations only. */
 int dts_set_label_target(dts_sim* sim, int16_t* labels_dev);
+/* Lane-marking image beside every observation (render spec item 11, DESIGN.md section 5): every later render of this
+ * handle — dts_render, dts_step, dts_step_terminal, whatever the render mode — also writes markings_dev, uint8
+ * [num_envs][cam_height][cam_width], always in that layout and at the camera size whatever dts_set_output_format and
+ * dts_set_resize say.  A pixel holds the class of the texel its label winner samples (dts_map_blob.tex_class): 0 none
+ * (no road tile: sky, no fisheye / rectification source, the ground, objects, the agent, untextured prims), 1 a road
+ * tile's unpainted surface, 2 white, 3 yellow, 4 red paint.  Of the pixel's distinct winners with the label's 1/w and
+ * the label's value (dts_set_label_target), each gives the class at texel (floor(u * w) mod w, floor(v * h) mod h) of
+ * its texture, u, v as shading computes them at the pixel centre; the pixel takes the smallest.  So markings != 0
+ * exactly where the label is a grid cell whose tile has a texture.  Lighting, domain-randomised colours and
+ * DTS_RENDER_SEGMENT leave it unchanged.  Independent of the depth and label targets: any of the three may be set.
+ * Sticky, like dts_set_render_mode.  The memory is the caller's and must stay valid while it is set; NULL (the default)
+ * turns markings off, and the renders launch the very kernels they launch without this call.  A pass over listed envs
+ * (the second pass of dts_step_terminal) writes only those envs' rows; the terminal frames' markings are not kept.  The
+ * fused gather (dts_gather_next) carries observations only. */
+int dts_set_marking_target(dts_sim* sim, uint8_t* markings_dev);
 /* Select the fused wrapper behaviour for subsequent dts_step / dts_render calls (default: all zero, scale 1).
  * obs_dev then holds num_envs * 3 * H * W elements of uint8 or float32 in the chosen layout. */
 int dts_set_output_format(dts_sim* sim, const dts_output_format* fmt);
