@@ -42,9 +42,7 @@ struct dts_sim {
   void* gather_peer[DTS_MAX_PEERS] = {};   // peers' buffers opened with cudaIpcOpenMemHandle (own entry = gather_buf)
   bool gather_next = false;
   int render_mode = 0;                  // dts_set_render_mode             // the next dts_render also stores into the gather buffers
-  float* depth_target = nullptr;        // dts_set_depth_target: caller-owned f32 [N][cam_h][cam_w], or null
-  int16_t* label_target = nullptr;      // dts_set_label_target: caller-owned i16 [N][cam_h][cam_w], or null
-  uint8_t* marking_target = nullptr;    // dts_set_marking_target: caller-owned u8 [N][cam_h][cam_w], or null
+  AuxTargets aux{};                     // dts_set_{depth,label,marking}_target: caller-owned images, or null
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
   int profiling = 0;                    // 0 off, 1 events around k_raster only, 2 around every render kernel
   std::vector<cudaEvent_t> prof_events; // kProfMarks events per profiled frame
@@ -193,7 +191,7 @@ static long long largest_label(long long n_cells, long long n_objects) { return 
 
 int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
   if (!sim) return 1;
-  if (sim->label_target && b && largest_label((long long)b->grid_w * b->grid_h, b->n_objects) > INT16_MAX)
+  if (sim->aux.labels && b && largest_label((long long)b->grid_w * b->grid_h, b->n_objects) > INT16_MAX)
     return sim->fail("a label target is set and this map's largest label, %lld, does not fit in int16",
                      largest_label((long long)b->grid_w * b->grid_h, b->n_objects));
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
@@ -339,7 +337,7 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
   if (!e.empty()) return sim->fail("%s", e.c_str());
   RenderCfg rc{sim->cfg.cam_width, sim->cfg.cam_height, sim->cfg.flags, sim->cfg.num_envs,
                (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->render_mode,
-               env_list, env_count, sim->depth_target};
+               env_list, env_count};
   if (*(volatile int32_t*)sim->h_status & 1)
     return sim->fail("an earlier frame overflowed its render frame memory (prim slab / bin lists) and was left incomplete");
   if (check_loaded(sim)) return 1;
@@ -365,8 +363,8 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
       gt.base[p] = reinterpret_cast<uint8_t*>(sim->gather_peer[p]) + (uint64_t)sim->gather_rank * sim->gather_bytes;
     sim->gather_next = false;
   }
-  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, sim->label_target,
-                        sim->marking_target, target, gt, sim->d_err, sim->d_status, marks, mark_level, (cudaStream_t)stream);
+  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, sim->aux, target, gt,
+                        sim->d_err, sim->d_status, marks, mark_level, (cudaStream_t)stream);
   if (rz.ow) {
     launch_resize(*sim->resize, rz.staging, obs_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, env_list, env_count,
                   (cudaStream_t)stream);
@@ -580,7 +578,7 @@ int dts_set_render_mode(dts_sim* sim, int mode) {
 int dts_set_depth_target(dts_sim* sim, float* depth_dev) {
   if (!sim) return 1;
   if (reinterpret_cast<uintptr_t>(depth_dev) & 3) return sim->fail("depth target is not aligned to 4 bytes");
-  sim->depth_target = depth_dev;
+  sim->aux.depth = depth_dev;
   return 0;
 }
 
@@ -594,13 +592,13 @@ int dts_set_label_target(dts_sim* sim, int16_t* labels_dev) {
         return sim->fail("map slot %zu's largest label, %lld, does not fit in int16", s,
                          largest_label(counts[s].n_tiles, counts[s].n_objects));
   }
-  sim->label_target = labels_dev;
+  sim->aux.labels = labels_dev;
   return 0;
 }
 
 int dts_set_marking_target(dts_sim* sim, uint8_t* markings_dev) {
   if (!sim) return 1;
-  sim->marking_target = markings_dev;
+  sim->aux.marks = markings_dev;
   return 0;
 }
 

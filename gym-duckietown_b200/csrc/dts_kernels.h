@@ -19,9 +19,16 @@ struct RenderCfg {
   // the envs left out keep what the previous pass put there.  (n_envs stays the SoA stride of the per-env state.)
   const int32_t* env_list;
   const int32_t* env_count;
-  // Optional depth target (dts_set_depth_target): f32 [n_envs][height][width], written beside obs by the rasterisers'
-  // depth instances, for the listed envs only where there is a list.  NULL: no depth is computed.
+};
+
+// The per-pixel images the rasterisers write beside obs, for the listed envs only where there is a list; NULL: that
+// image is not computed.  Each is [n_envs][height][width]: eye-space depth (dts_set_depth_target), the label
+// (dts_set_label_target) and the lane marking (dts_set_marking_target).  Not RenderCfg members: RenderCfg is every render
+// kernel's parameter block, and only the rasterisers read these.
+struct AuxTargets {
   float* depth;
+  int16_t* labels;
+  uint8_t* marks;
 };
 
 void launch_step_logic(const DState& S, const DMap* maps, const StepCfg& c, int n_maps_cycle, const float* actions,
@@ -119,15 +126,10 @@ std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* 
                              const int32_t* lut_of_env);
 // `marks`: NULL or kProfMarks events recorded on `st` before k_frame_setup and after each of k_frame_setup, k_geometry,
 // k_bin, k_raster and the post passes (dts_profile_*).  `status_dev`: device address of the mapped host status word.
-// `labels`: NULL, or the label target (dts_set_label_target), i16 [n_envs][height][width], written beside obs like the
-// depth target, for the listed envs only where there is a list.  It is not a RenderCfg member: RenderCfg is every render
-// kernel's parameter block, and a longer one would move each kernel's later parameters.
-// `markings`: NULL, or the marking target (dts_set_marking_target), u8 [n_envs][height][width], the same way.
 constexpr int kProfMarks = 6;
-int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, int16_t* labels,
-                  uint8_t* markings, void* obs,
-                  const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level,
-                  cudaStream_t st);
+int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, const AuxTargets& aux,
+                  void* obs, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks,
+                  int mark_level, cudaStream_t st);
 // What the last render left in frame memory for one env (dts_debug_frame), after the device has synchronised
 std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, int32_t* counts, float* lattice_by_cell,
                              int n_cells);

@@ -28,22 +28,22 @@
 // Arithmetic follows the render spec of DESIGN.md (the CPU checker implements the same spec) bit for bit
 // (compiled with -fmad=false; fmaf() is spelled out where the spec has one).
 //
-// With a depth target (RenderCfg::depth, render spec item 9) the three rasterisers run their kDepth instances, which also
-// store every pixel's eye-space depth, f32 [N][H][W]; without one the launches and their kernels are the plain ones.
-// A label target (dts_set_label_target, render spec item 10) selects their kLabels instances in the same way, alone or
-// with kDepth: every pixel's draw item + 1, i16 [N][H][W].  The target reaches them as their last kernel parameter, not
-// through RenderCfg: a longer RenderCfg would move every later parameter of every render kernel.
-// A marking target (dts_set_marking_target, render spec item 11) selects their kMarks instances, alone or with kLabels:
-// they take the label's winners and store every pixel's texel class, u8 [N][H][W], and the depth where that target is
-// set (a pointer test in these instances only, instead of a kDepth variant of each), so the plain, depth and label
-// instances stay as they are.
+// Image targets (AuxTargets, the three rasterisers' last kernel parameter): besides obs, every pixel's eye-space depth
+// (f32 [N][H][W], render spec item 9), label (the draw item + 1, i16, item 10) and lane marking (the texel class, u8,
+// item 11).  Template parameter kAux, a set of kAuxDepth / kAuxLabels / kAuxMarks, is the images an instance writes,
+// and launch_render picks it from the targets that are set (aux_set); without targets the launches are the plain
+// kernels.  Labels and markings both take the label's winner among a pixel's winners.  A marking instance stores the
+// depth where that target is set, a pointer test in these instances only (stores_depth), instead of a compiled depth +
+// markings variant of each.  The instances are kAuxSets.
 //
 // HBM traffic per env-frame: obs store W*H*3 B (compulsory; + W*H*4 B of depth, W*H*2 B of labels and W*H B of markings where asked for) + PrimRec slab / BinRec lists / lattice table
 // (tens of KB per env, written by k_geometry / k_bin and read once by k_raster) + texels (shared, L2-resident).
 #include <algorithm>
 #include <cstddef>
 #include <cstdlib>
+#include <iterator>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "dts_camera.cuh"
@@ -898,25 +898,6 @@ __device__ __forceinline__ int label_of_id(const LabelMap& lm, int id) {
   }
   return 2 + lm.n_cells + lo;
 }
-// One more winner `w` of a pixel (a prim index), its 1/w `qq` (> 0) and label_of(w): (qmax, lab) keeps the largest 1/w
-// and, among equal ones, the smallest label.  A maximum over exact values with an exact tie-break: the order does not
-// matter.
-template <typename LabelOf>
-__device__ __forceinline__ void take_label(float& qmax, int& lab, float qq, unsigned w, const LabelOf& label_of) {
-  if (!(qq >= qmax)) return;   // (a farther winner: its label is not looked up)
-  const int l = label_of(w);
-  if (qq > qmax || l < lab) { qmax = qq; lab = l; }
-}
-// Marking target (render spec item 11): as take_label, and `mk` keeps the smallest class `c` among the winners that
-// have both the kept 1/w and the kept label (two triangles of one tile, in tile mode 0 or clipped, can).  Exact values
-// and exact tie-breaks again: the order does not matter.
-template <typename LabelOf>
-__device__ __forceinline__ void take_mark(float& qmax, int& lab, int& mk, float qq, unsigned w, int c, const LabelOf& label_of) {
-  if (!(qq >= qmax)) return;
-  const int l = label_of(w);
-  if (qq > qmax || l < lab) { qmax = qq; lab = l; mk = c; }
-  else if (l == lab) mk = min(mk, c);
-}
 // The marking frame `mf` (u8 [H][W] of one env): a lane stores its own pixel, 1 byte.
 __device__ __forceinline__ void store_marking(uint8_t* __restrict__ mf, int v, int lane, int bx, int by, int W, int H) {
   const int gx = bx * kBinW + (lane & 7), gy = by * kBinH + (lane >> 3);
@@ -928,6 +909,52 @@ __device__ __forceinline__ void store_marking(uint8_t* __restrict__ mf, int v, i
 __device__ __forceinline__ void store_label(int16_t* __restrict__ lf, int v, int lane, int bx, int by, int W, int H) {
   const int gx = bx * kBinW + (lane & 7), gy = by * kBinH + (lane >> 3);
   if (gx < W && gy < H) lf[(size_t)gy * W + gx] = (int16_t)v;
+}
+
+// The images a rasteriser instance writes (kAux, a set of these) and what they ask of it
+constexpr int kAuxDepth = 1, kAuxLabels = 2, kAuxMarks = 4;
+// the label's winner is taken: for the label, and for the marking, which is the class that winner shows
+__host__ __device__ constexpr bool takes_winner(int aux) { return (aux & (kAuxLabels | kAuxMarks)) != 0; }
+// depth may be stored: by a depth instance, and by a marking instance where the depth target is set
+__host__ __device__ constexpr bool may_store_depth(int aux) { return (aux & (kAuxDepth | kAuxMarks)) != 0; }
+// a winner's 1/w is needed: for the depth, or to take the label's winner
+__host__ __device__ constexpr bool needs_qq(int aux) { return takes_winner(aux) || may_store_depth(aux); }
+// depth is stored: always by a depth instance, by a marking instance where the depth target `depth` is set
+template <int kAux>
+__device__ __forceinline__ bool stores_depth(const float* depth) { return (kAux & kAuxDepth) || ((kAux & kAuxMarks) && depth); }
+
+// One env's frames of the image targets, each [H][W] at `off`.  (The targets and an offset rather than three frame
+// pointers: the depth test then reads the kernel parameter, and the pointers cost no registers across a bin.)
+struct AuxFrames { AuxTargets t; size_t off; };
+__device__ __forceinline__ AuxFrames aux_frames(const AuxTargets& aux, int env, int W, int H) {
+  return AuxFrames{aux, (size_t)env * W * H};
+}
+// One fine bin of each image the instance writes, in the order depth, label, marking: a lane stores its own pixel
+template <int kAux>
+__device__ __forceinline__ void store_aux(const AuxFrames& af, float depth, int label, int mark, int lane, int bx, int by, int W,
+                                          int H) {
+  if (stores_depth<kAux>(af.t.depth)) store_depth(af.t.depth + af.off, depth, lane, bx, by, W, H);
+  if (kAux & kAuxLabels) store_label(af.t.labels + af.off, label, lane, bx, by, W, H);
+  if (kAux & kAuxMarks) store_marking(af.t.marks + af.off, mark, lane, bx, by, W, H);
+}
+
+// A pixel's image state over its winners: the largest 1/w (0: none yet), the label of the winner it picks and the
+// marking (0: none)
+struct AuxPx { float qmax; int lab, mk; };
+// One more winner `w` of a pixel (a prim index), its 1/w `qq` (> 0), label_of(w) and texel class `c`: the pixel keeps
+// the largest 1/w and, among equal ones, the smallest label; with markings, the smallest class among the winners that
+// have both (two triangles of one tile, in tile mode 0 or clipped, can).  Maxima over exact values with exact
+// tie-breaks: the order does not matter.
+template <int kAux, typename LabelOf>
+__device__ __forceinline__ void take_winner(AuxPx& pix, float qq, unsigned w, int c, const LabelOf& label_of) {
+  if (!(qq >= pix.qmax)) return;   // (a farther winner: its label is not looked up)
+  const int l = label_of(w);
+  if (qq > pix.qmax || l < pix.lab) {
+    pix.qmax = qq; pix.lab = l;
+    if constexpr ((kAux & kAuxMarks) != 0) pix.mk = c;
+  } else if constexpr ((kAux & kAuxMarks) != 0) {
+    if (l == pix.lab) pix.mk = min(pix.mk, c);
+  }
 }
 
 // glClearColor: the env's horizon colour, or on the segment view glClearColor(255, 0, 255) clamped to magenta (S:1752)
@@ -1643,15 +1670,14 @@ __device__ __forceinline__ int sample_mask(const BinRec& br, int pxc, int pyc) {
 // in rounds of the whole warp (a lane with nothing pending idles), and the box resolve (s01 + s23) * 0.25 into c3, with
 // s01 = c(wn0) + c(wn1), s23 = c(wn2) + c(wn3).  Each shade depends only on (prim, position) and each half has two
 // addends, so neither the lane nor the order in which the winners are shaded changes a bit.  Called by the whole warp.
-// kDepth: `qmax` comes in as the first winner's 1/w (0: none) and leaves as the largest over the pixel's winners; a
-// maximum of exact values, so the order does not matter there either.  kLabels: the same, and `lab` comes in as the
-// first winner's label (0: none) and leaves as the pixel's (take_label; label_of(w): the label of prim w).  kMarks
-// (with kLabels): `mk` the same for the marking, the class coming from `cls_pool` (take_mark).
-template <bool kDepth, bool kLabels, bool kMarks, typename LabelOf>
+// `pix` comes in as the first winner's (0s: none) and leaves as the pixel's: the largest 1/w over its winners (a maximum
+// of exact values, so the order does not matter there either), and where kAux takes the label's winner, its label and
+// marking (take_winner; label_of(w): the label of prim w; the class coming from `cls_pool`).
+template <int kAux, typename LabelOf>
 __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], const float clr[3], const PrimRec* __restrict__ prims,
                                              const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa, int pya,
-                                             int lane, int32_t* __restrict__ err, float& qmax, int* lab, int* mk,
-                                             const LabelOf& label_of, const uint8_t* __restrict__ cls_pool) {
+                                             int lane, int32_t* __restrict__ err, AuxPx& pix, const LabelOf& label_of,
+                                             const uint8_t* __restrict__ cls_pool) {
   (void)lane; (void)err;   // (DTS_STATS counters)
   float s01[3] = {c3[0], c3[1], c3[2]}, s23[3] = {0.f, 0.f, 0.f};   // 0 + c == c
   unsigned pend = 0xeu;
@@ -1669,13 +1695,12 @@ __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], 
       float qq = 0.0f;
       int c = 0;
       if (w != kNoPrim)
-        shade_prim(prims, w, tex_pool, lat_tab, pxa, pya, d3, (kDepth || kLabels) ? &qq : nullptr, cls_pool, kMarks ? &c : nullptr);
-      if (kMarks) {
-        if (w != kNoPrim) take_mark(qmax, *lab, *mk, qq, w, c, label_of);
-      } else if (kLabels) {
-        if (w != kNoPrim) take_label(qmax, *lab, qq, w, label_of);
-      } else if (kDepth) {
-        qmax = fmaxf(qmax, qq);
+        shade_prim(prims, w, tex_pool, lat_tab, pxa, pya, d3, needs_qq(kAux) ? &qq : nullptr, cls_pool,
+                   (kAux & kAuxMarks) ? &c : nullptr);
+      if (takes_winner(kAux)) {
+        if (w != kNoPrim) take_winner<kAux>(pix, qq, w, c, label_of);
+      } else if (kAux & kAuxDepth) {
+        pix.qmax = fmaxf(pix.qmax, qq);
       }
 #pragma unroll
       for (int t = 1; t < 4; t++)
@@ -1690,44 +1715,36 @@ __device__ __forceinline__ void resolve_edge(const unsigned wn[4], float c3[3], 
   for (int ch = 0; ch < 3; ch++) c3[ch] = (s01[ch] + s23[ch]) * 0.25f;
 }
 // The whole resolve of one fine bin's pixels (k_raster).  `simple`: the caller knows that every sample of the whole fine
-// bin has the same winner.  kDepth: `qmax` receives the largest 1/w among the pixel's winners, 0 if it has none.
-// kLabels: `qmax` the same, and `lab` the pixel's label, 0 if it has no winner.  kMarks (with kLabels): `mk` the
-// pixel's marking, 0 if it has no winner.
-template <bool kDepth, bool kLabels, bool kMarks, typename LabelOf>
+// bin has the same winner.  `pix` receives the pixel's image state (resolve_edge), 0s if it has no winner.
+template <int kAux, typename LabelOf>
 __device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool simple, const float clr[3], const PrimRec* __restrict__ prims,
                                                   const uint8_t* __restrict__ tex_pool, const float4* __restrict__ lat_tab, int pxa,
-                                                  int pya, int lane, int32_t* __restrict__ err, float& qmax, int* lab, int* mk,
-                                                  const LabelOf& label_of, const uint8_t* __restrict__ cls_pool) {
+                                                  int pya, int lane, int32_t* __restrict__ err, AuxPx& pix, const LabelOf& label_of,
+                                                  const uint8_t* __restrict__ cls_pool) {
   const bool same = wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0];
   const bool all_same = simple || __all_sync(0xffffffffu, same);
   float c3[3] = {clr[0], clr[1], clr[2]};
-  if (kDepth || kLabels) qmax = 0.0f;
-  if (kLabels) *lab = 0;
-  if (kMarks) *mk = 0;
+  pix = AuxPx{};
   if (wn[0] != kNoPrim) {   // every lane: its first winner
-    shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3, (kDepth || kLabels) ? &qmax : nullptr, cls_pool, kMarks ? mk : nullptr);
-    if (kLabels) *lab = label_of(wn[0]);
+    shade_prim(prims, wn[0], tex_pool, lat_tab, pxa, pya, c3, needs_qq(kAux) ? &pix.qmax : nullptr, cls_pool,
+               (kAux & kAuxMarks) ? &pix.mk : nullptr);
+    if (takes_winner(kAux)) pix.lab = label_of(wn[0]);
   }
   if (!all_same)   // (four equal samples: the mean is the value itself)
-    resolve_edge<kDepth, kLabels, kMarks>(wn, c3, clr, prims, tex_pool, lat_tab, pxa, pya, lane, err, qmax, lab, mk, label_of,
-                                          cls_pool);
+    resolve_edge<kAux>(wn, c3, clr, prims, tex_pool, lat_tab, pxa, pya, lane, err, pix, label_of, cls_pool);
   return pack_rgb(c3[0], c3[1], c3[2]);
 }
 
 // ------------------------------------------------------------------------------------------------ k_raster
-template <bool kWrapFmt, bool kFish, bool kDepth, bool kLabels, bool kPool = false, bool kMarks = false>
+template <bool kWrapFmt, bool kFish, bool kPool, int kAux>
                                        // kWrapFmt: a dts_output_format other than packed u8 HWC is written by the resolve;
                                        // kFish: every lane renders the SOURCE pixel the fisheye LUT names for its output pixel;
-                                       // kDepth: every pixel's depth goes to rc.depth beside its colour (render spec item 9);
-                                       // kLabels: every pixel's label goes to `labels` (render spec item 10);
                                        // kPool: each env's tables of a pool (fish_of_env);
-                                       // kMarks (kDepth false): every pixel's marking goes to `marks` (render spec item 11),
-                                       // and its depth where rc.depth is set
+                                       // kAux: the images written beside obs (AuxTargets)
 __global__ void __launch_bounds__(kThreads, kRasterMinCtas)
 k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, FishTab fts, GatherTab gt,
          uint8_t* __restrict__ obs, int max_prims, int max_pairs, int max_lat, int32_t* __restrict__ err,
-         int16_t* __restrict__ labels, const uint16_t* __restrict__ fish_tab, uint8_t* __restrict__ marks) {
-  constexpr bool kLab = kLabels || kMarks;   // the label's winner: markings are taken from it
+         const uint16_t* __restrict__ fish_tab, AuxTargets aux) {
   // dynamic shared memory (kRasterSmem bytes): per warp two chunks of records in flight, their mbarriers, and a 128-sample
   // depth / winner buffer for the tiny triangles of the fine bin being drawn
   extern __shared__ __align__(128) unsigned char raster_smem[];
@@ -1768,12 +1785,10 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     const size_t env_off = (size_t)env * frame_bytes * out_elem;
     uint8_t* out = obs + env_off;
-    float* dep = (kDepth || (kMarks && rc.depth)) ? rc.depth + (size_t)env * W * H : nullptr;
-    int16_t* lf = kLabels ? labels + (size_t)env * W * H : nullptr;
-    uint8_t* mf = kMarks ? marks + (size_t)env * W * H : nullptr;
-    const uint8_t* cls_pool = kMarks ? tex_pool + m.tex_class_off : nullptr;
+    const AuxFrames af = aux_frames(aux, env, W, H);
+    const uint8_t* cls_pool = (kAux & kAuxMarks) ? tex_pool + m.tex_class_off : nullptr;
     LabelMap lm{};
-    if constexpr (kLab) lm = label_map(m, rc.tessellate);
+    if constexpr (takes_winner(kAux)) lm = label_map(m, rc.tessellate);
     auto label_of = [&](unsigned w) { return label_of_id(lm, __ldg(&prims[w].id)); };
     // one fine bin -> the caller's tensor and, on a gathering step, every peer's gather buffer (NVLink stores)
     // On a gathering step (gt.n > 0) the packed u8 HWC frame goes to the peers in BLOCKS: a work item is 8 whole image rows =
@@ -1781,9 +1796,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
     // (NVLink wants long writes: per-bin 4-byte stores reach a fifth of the link rate).  Other layouts store per bin.
     const bool gather_rows = gt.n > 0 && !kWrapFmt;
     auto emit = [&](unsigned rgb, float depth, int label, int mark, int bx, int by) {
-      if (kDepth || (kMarks && dep)) store_depth(dep, depth, lane, bx, by, W, H);   // (the caller's depth tensor only: the gather carries obs)
-      if (kLabels) store_label(lf, label, lane, bx, by, W, H);
-      if (kMarks) store_marking(mf, mark, lane, bx, by, W, H);
+      store_aux<kAux>(af, depth, label, mark, lane, bx, by, W, H);   // (the caller's tensors only: the gather carries obs)
       if (fast_fmt && (gt.n == 0 || gather_rows) && bx * kBinW + kBinW <= W) {   // the common case inline: packed u8 HWC, whole bin inside
         store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
       } else if (kWrapFmt && gt.n == 0) {
@@ -2061,12 +2074,11 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
             }
             // ---- deferred shading: once per distinct winner of this pixel, then the box resolve
             DTS_COUNT(11, 1);
-            float qmax = 0.0f;
-            int lab = 0, mk = 0;
-            unsigned rgb = shade_resolve<kDepth, kLab, kMarks>(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane,
-                                                               err, qmax, &lab, &mk, label_of, cls_pool);
+            AuxPx pix;
+            unsigned rgb = shade_resolve<kAux>(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane, err, pix,
+                                               label_of, cls_pool);
             if (kFish && !px_valid) rgb = 0u;   // cv2.remap BORDER_CONSTANT
-            emit(rgb, (kDepth || kMarks) ? depth_of(qmax, px_valid) : 0.0f, px_valid ? lab : 0, px_valid ? mk : 0, bx, by);
+            emit(rgb, depth_of(pix.qmax, px_valid), px_valid ? pix.lab : 0, px_valid ? pix.mk : 0, bx, by);
           }
         }
       }
@@ -2085,17 +2097,14 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
 // visibility state: a warp fetches the prim's planes once and shades the bin's 256 pixels.  A separate kernel so that the
 // lean loop gets its own register allocation (the same fast path inside k_raster cost more than it saved).
 // Packed u8 HWC output with whole-word rows only (k_bin marks no bin otherwise).  Runs before k_raster.
-template <bool kFish, bool kDepth, bool kLabels, bool kPool = false, bool kMarks = false>
+// Images: the 1/w the shading divides by gives the depth, the bin's one prim the label of every pixel with a source, and
+// the texel it shows there the marking.
+template <bool kFish, bool kPool, int kAux>
                                      // kFish: each lane shades the source pixel the fisheye LUT names for its output pixel;
-                                     // kDepth: the 1/w the shading divides by also gives the pixel's depth (rc.depth);
-                                     // kLabels: the bin's one prim gives every pixel with a source its label (`labels`);
-                                     // kPool: each env's tables of a pool (fish_of_env);
-                                     // kMarks (kDepth false): the class of the texel the prim shows at each pixel with a
-                                     // source (`marks`), and the depth where rc.depth is set
+                                     // kPool: each env's tables of a pool (fish_of_env)
 __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
                                                                         FishTab fts, uint8_t* __restrict__ obs, int max_prims, int max_lat,
-                                                                        int16_t* __restrict__ labels, const uint16_t* __restrict__ fish_tab,
-                                                                        uint8_t* __restrict__ marks) {
+                                                                        const uint16_t* __restrict__ fish_tab, AuxTargets aux) {
   const int W = rc.width, H = rc.height;
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW;
   const int lane = threadIdx.x & 31;
@@ -2114,9 +2123,10 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
     const ShadeIn si = load_shade(fm.prims + (size_t)env * max_prims, p);
     uint8_t* out = obs + (size_t)env * frame_bytes;
     int lab = 0;
-    if constexpr (kLabels)
+    if constexpr ((kAux & kAuxLabels) != 0)
       lab = label_of_id(label_map(maps[S.map_id[env]], rc.tessellate), __ldg(&fm.prims[(size_t)env * max_prims + p].id));
-    const uint8_t* cls_pool = kMarks ? tex_pool + maps[S.map_id[env]].tex_class_off : nullptr;
+    const uint8_t* cls_pool = (kAux & kAuxMarks) ? tex_pool + maps[S.map_id[env]].tex_class_off : nullptr;
+    const AuxFrames af = aux_frames(aux, env, W, H);
     // fine bins inside the image as loop bounds rather than fine_in_image(): the mask test costs this loop machine code
     const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);
     const int ny = ((cby * kCFY + 1) * kBinH < H) ? 2 : 1;
@@ -2134,13 +2144,12 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
       }
       float c3[3], qq = 0.0f;
       int mk = 0;
-      shade_eval(si, tex_pool, lat_tab, pxa, pya, c3, (kDepth || kMarks) ? &qq : nullptr, cls_pool, kMarks ? &mk : nullptr);
+      shade_eval(si, tex_pool, lat_tab, pxa, pya, c3, may_store_depth(kAux) ? &qq : nullptr, cls_pool,
+                 (kAux & kAuxMarks) ? &mk : nullptr);
       unsigned rgb = pack_rgb(c3[0], c3[1], c3[2]);
       if (kFish && !px_valid) rgb = 0u;
       store_bin_lean(out, sl, rgb, lane, bx, by, W, H);
-      if (kDepth || (kMarks && rc.depth)) store_depth(rc.depth + (size_t)env * W * H, depth_of(qq, px_valid), lane, bx, by, W, H);
-      if (kLabels) store_label(labels + (size_t)env * W * H, px_valid ? lab : 0, lane, bx, by, W, H);
-      if (kMarks) store_marking(marks + (size_t)env * W * H, px_valid ? mk : 0, lane, bx, by, W, H);
+      store_aux<kAux>(af, depth_of(qq, px_valid), px_valid ? lab : 0, px_valid ? mk : 0, lane, bx, by, W, H);
     }
   }
 }
@@ -2161,25 +2170,21 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
 // Hand-back: a sample covered by two tiles (or by two ground records) is not resolved here.  The warp drops the bin's
 // queue and colours, restores its record count, and k_raster, launched next on the stream, draws the whole bin
 // depth-tested.
-// kDepth: depth needs no plane in shared memory.  A lane stores a one-winner pixel's depth as soon as it has shaded it,
-// and a queued pixel's when its other winners are resolved; the queue carries the first winner's 1/w in a third array
-// (2 KB: 46 KB per CTA, still four CTAs per SM).  A bin handed back may have stored some depths already: k_raster
-// rewrites the whole bin, colour and depth.
-// kLabels: the same for labels, with no more shared memory.  A queued pixel's first label is looked up again from its
-// first winner, which the queue holds; its 1/w comes from the depth array (kept for labels alone, too).  Only the ground
-// and road tiles come here, so a label is arithmetic on the draw id (tile_label).
-// kMarks (kDepth false): markings, and the depth where rc.depth is set.  A queued pixel's
-// first winner's class rides in the high half of its entry's slot word: still no more shared memory.
+// Images need no plane in shared memory.  A lane stores a one-winner pixel's images as soon as it has shaded it, and a
+// queued pixel's when its other winners are resolved; the queue carries the first winner's 1/w in a third array (2 KB:
+// 46 KB per CTA, still four CTAs per SM) and its class in the high half of the entry's slot word, and the first label
+// is looked up again from the first winner, which the queue holds.  Only the ground and road tiles come here, so a label
+// is arithmetic on the draw id (tile_label).  A bin handed back may have stored some images already: k_raster rewrites
+// the whole bin, colour and images.
 // Packed u8 HWC output with whole-word rows only (k_bin lists no bin otherwise).  Runs after k_raster_solo.
 constexpr int kEdgeQ = 64;   // queue ring: flushed at 32 entries, so at most 31 + 32 wait at once
-template <bool kFish, bool kDepth, bool kLabels, bool kPool = false, bool kMarks = false>
+template <bool kFish, bool kPool, int kAux>
                                  // kFish: each lane covers and shades the source pixel the fisheye LUT names for its output pixel;
                                  // kPool: each env's tables of a pool (fish_of_env)
 __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
                                                                         FishTab fts, uint8_t* __restrict__ obs, int max_prims, int max_lat,
-                                                                        int32_t* __restrict__ err, int16_t* __restrict__ labels,
-                                                                        const uint16_t* __restrict__ fish_tab, uint8_t* __restrict__ marks) {
-  constexpr bool kLab = kLabels || kMarks;   // the label's winner: markings are taken from it
+                                                                        int32_t* __restrict__ err, const uint16_t* __restrict__ fish_tab,
+                                                                        AuxTargets aux) {
   __shared__ BinRec stages[kWarps][kStage];   // per warp: the records of its bin
   __shared__ unsigned bin_rgb[kWarps][kCFX * kCFY * 32];   // per warp: packed colour of pixel `lane` of fine bin f at f * 32 + lane
   // per warp: the edge-pixel queue, an entry in two words: (pixel slot, pxa, pya, wn0 | wn1 << 16), (wn2 | wn3 << 16, first colour)
@@ -2190,8 +2195,8 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
   BinRec* stage = stages[threadIdx.x >> 5];
   unsigned* rgb_buf = bin_rgb[threadIdx.x >> 5];
   uint4 (*q)[kEdgeQ] = edge_q[threadIdx.x >> 5];
-  float* q_qq = nullptr;   // kDepth, kLabels, kMarks: per queue entry, the first winner's 1/w
-  if constexpr (kDepth || kLab) {
+  float* q_qq = nullptr;   // per queue entry, the first winner's 1/w
+  if constexpr (needs_qq(kAux)) {
     __shared__ float edge_qq[kWarps][kEdgeQ];
     q_qq = edge_qq[threadIdx.x >> 5];
   }
@@ -2224,10 +2229,8 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
     const PrimRec* prims = fm.prims + (size_t)env * max_prims;
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     uint8_t* out = obs + (size_t)env * frame_bytes;
-    float* dep = (kDepth || (kMarks && rc.depth)) ? rc.depth + (size_t)env * W * H : nullptr;
-    int16_t* lf = kLabels ? labels + (size_t)env * W * H : nullptr;
-    uint8_t* mf = kMarks ? marks + (size_t)env * W * H : nullptr;
-    const uint8_t* cls_pool = kMarks ? tex_pool + maps[S.map_id[env]].tex_class_off : nullptr;
+    const AuxFrames af = aux_frames(aux, env, W, H);
+    const uint8_t* cls_pool = (kAux & kAuxMarks) ? tex_pool + maps[S.map_id[env]].tex_class_off : nullptr;
     auto label_of = [&](unsigned w) { return tile_label(rc.tessellate, __ldg(&prims[w].id)); };
     float clr[3];
     clear_colour(S, rc, env, clr);
@@ -2302,21 +2305,21 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
       float c3[3] = {clr[0], clr[1], clr[2]}, qq0 = 0.0f;
       int c0 = 0;
       if (wn[0] != kNoPrim)
-        shade_prim(prims, wn[0], tex_pool, lat_tab, ox + pxc, oy + pyc, c3, (kDepth || kLab) ? &qq0 : nullptr, cls_pool,
-                   kMarks ? &c0 : nullptr);
+        shade_prim(prims, wn[0], tex_pool, lat_tab, ox + pxc, oy + pyc, c3, needs_qq(kAux) ? &qq0 : nullptr, cls_pool,
+                   (kAux & kAuxMarks) ? &c0 : nullptr);
       const bool edge = px_valid && !(wn[1] == wn[0] && wn[2] == wn[0] && wn[3] == wn[0]);
       const unsigned edges = __ballot_sync(0xffffffffu, edge);
       const unsigned slot = f * 32 + lane;
       if (edge) {
         const int e = (qs + __popc(edges & ((1u << lane) - 1u))) & (kEdgeQ - 1);
-        q[0][e] = make_uint4(kMarks ? slot | (unsigned)c0 << 16 : slot, (unsigned)(ox + pxc), (unsigned)(oy + pyc), wn[0] | (wn[1] << 16));
+        q[0][e] = make_uint4((kAux & kAuxMarks) ? slot | (unsigned)c0 << 16 : slot, (unsigned)(ox + pxc), (unsigned)(oy + pyc),
+                             wn[0] | (wn[1] << 16));
         q[1][e] = make_uint4(wn[2] | (wn[3] << 16), __float_as_uint(c3[0]), __float_as_uint(c3[1]), __float_as_uint(c3[2]));
-        if (kDepth || kLab) q_qq[e] = qq0;
+        if (needs_qq(kAux)) q_qq[e] = qq0;
       } else {
         rgb_buf[slot] = (kFish && !px_valid) ? 0u : pack_rgb(c3[0], c3[1], c3[2]);
-        if (kDepth || (kMarks && dep)) store_depth(dep, depth_of(qq0, px_valid), lane, bx, by, W, H);
-        if (kLabels) store_label(lf, (px_valid && wn[0] != kNoPrim) ? label_of(wn[0]) : 0, lane, bx, by, W, H);
-        if (kMarks) store_marking(mf, px_valid ? c0 : 0, lane, bx, by, W, H);   // (c0 = 0 without a winner)
+        const int lab = ((kAux & kAuxLabels) && px_valid && wn[0] != kNoPrim) ? label_of(wn[0]) : 0;
+        store_aux<kAux>(af, depth_of(qq0, px_valid), lab, px_valid ? c0 : 0, lane, bx, by, W, H);   // (c0 = 0 without a winner)
       }
       qs += __popc(edges);
       DTS_COUNT(26, __popc(edges));
@@ -2327,31 +2330,27 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
         const int take = min(nq, 32);
         __syncwarp();   // the entries were written by other lanes
         unsigned qw[4] = {0u, 0u, 0u, 0u};   // (lanes without an entry: one winner, nothing to shade)
-        float q3[3] = {0.f, 0.f, 0.f}, qmax = 0.0f;
-        int qlab = 0, qmk = 0;
+        float q3[3] = {0.f, 0.f, 0.f};
+        AuxPx qpix{};
         unsigned qslot = 0u;
         int qx = 0, qy = 0;
         if (lane < take) {
           const int e = ((qs >> 16) + lane) & (kEdgeQ - 1);
           const uint4 a = q[0][e], c = q[1][e];
-          qslot = kMarks ? a.x & 0xffffu : a.x; qx = (int)a.y; qy = (int)a.z;
-          if (kMarks) qmk = (int)(a.x >> 16);
+          qslot = (kAux & kAuxMarks) ? a.x & 0xffffu : a.x; qx = (int)a.y; qy = (int)a.z;
+          if (kAux & kAuxMarks) qpix.mk = (int)(a.x >> 16);
           qw[0] = a.w & 0xffffu; qw[1] = a.w >> 16; qw[2] = c.x & 0xffffu; qw[3] = c.x >> 16;
           q3[0] = __uint_as_float(c.y); q3[1] = __uint_as_float(c.z); q3[2] = __uint_as_float(c.w);
-          if (kDepth || kLab) qmax = q_qq[e];
-          if (kLab && qw[0] != kNoPrim) qlab = label_of(qw[0]);
+          if (needs_qq(kAux)) qpix.qmax = q_qq[e];
+          if (takes_winner(kAux) && qw[0] != kNoPrim) qpix.lab = label_of(qw[0]);
         }
-        resolve_edge<kDepth, kLab, kMarks>(qw, q3, clr, prims, tex_pool, lat_tab, qx, qy, lane, err, qmax, &qlab, &qmk, label_of,
-                                           cls_pool);
+        resolve_edge<kAux>(qw, q3, clr, prims, tex_pool, lat_tab, qx, qy, lane, err, qpix, label_of, cls_pool);
         if (lane < take) rgb_buf[qslot] = pack_rgb(q3[0], q3[1], q3[2]);
-        // the queued pixel `qslot` = fine bin * 32 + lane-in-bin: its depth, label and marking go straight to the frame
-        // (queued pixels have a source)
-        if ((kDepth || (kMarks && dep)) && lane < take)
-          store_depth(dep, depth_of(qmax), (int)(qslot & 31u), cbx * kCFX + (int)((qslot >> 5) & 3u), cby * kCFY + (int)(qslot >> 7), W, H);
-        if (kLabels && lane < take)
-          store_label(lf, qlab, (int)(qslot & 31u), cbx * kCFX + (int)((qslot >> 5) & 3u), cby * kCFY + (int)(qslot >> 7), W, H);
-        if (kMarks && lane < take)
-          store_marking(mf, qmk, (int)(qslot & 31u), cbx * kCFX + (int)((qslot >> 5) & 3u), cby * kCFY + (int)(qslot >> 7), W, H);
+        // the queued pixel `qslot` = fine bin * 32 + lane-in-bin: its images go straight to the frames (queued pixels
+        // have a source)
+        if (lane < take)
+          store_aux<kAux>(af, depth_of(qpix.qmax), qpix.lab, qpix.mk, (int)(qslot & 31u), cbx * kCFX + (int)((qslot >> 5) & 3u),
+                          cby * kCFY + (int)(qslot >> 7), W, H);
         qs += (unsigned)take << 16;
         __syncwarp();   // read before the next fine bin's entries overwrite the ring
       }
@@ -2571,9 +2570,29 @@ std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, in
   return rc ? "debug_frame_copy failed" : "";
 }
 
-int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, int16_t* labels,
-                  uint8_t* markings, void* obs_any, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks, int mark_level,
-                  cudaStream_t st) {
+// The image sets the rasterisers are compiled for.  Depth + markings has none of its own: it runs the marking instance,
+// which stores the depth where that target is set.
+constexpr int kAuxSets[] = {0, kAuxDepth, kAuxLabels, kAuxDepth | kAuxLabels, kAuxMarks, kAuxLabels | kAuxMarks};
+// The image set a render with these targets runs
+static int aux_set(const AuxTargets& a) {
+  return (a.labels ? kAuxLabels : 0) | (a.marks ? kAuxMarks : a.depth ? kAuxDepth : 0);
+}
+// f(std::integral_constant<int, a>{}) for every image set a of kAuxSets
+template <typename F, size_t... I>
+static void each_aux_set(F& f, std::index_sequence<I...>) { (f(std::integral_constant<int, kAuxSets[I]>{}), ...); }
+template <typename F>
+static void for_each_aux_set(F f) { each_aux_set(f, std::make_index_sequence<std::size(kAuxSets)>{}); }
+// k_raster's instance for a wrapper output format, a gather through one table, or through a pool of them
+template <int kAux>
+static auto raster_of(bool wrap, bool fish, bool pool) {
+  return pool ? (wrap ? k_raster<true, true, true, kAux> : k_raster<false, true, true, kAux>)
+       : fish ? (wrap ? k_raster<true, true, false, kAux> : k_raster<false, true, false, kAux>)
+              : (wrap ? k_raster<true, false, false, kAux> : k_raster<false, false, false, kAux>);
+}
+
+int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, const AuxTargets& aux,
+                  void* obs_any, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks,
+                  int mark_level, cudaStream_t st) {
   uint8_t* obs = reinterpret_cast<uint8_t*>(obs_any);
   // the gather the frame goes through, if any: the rectification (DTS_RENDER_RECTIFY), none (DTS_RENDER_PINHOLE or no
   // DTS_FLAG_DISTORTION) or the fisheye.  Both tables run the same kFish kernels.
@@ -2614,51 +2633,22 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, ft, r.max_prims, r.pool, err_flag, fish_tab);
   mark();
   const bool wrap = (rc.obs_layout | rc.obs_dtype) != 0;
-  // a depth target (RenderCfg::depth) selects the depth-writing instance of each rasteriser; without one the launches
-  // are the same kernels as ever
-  const bool depth = rc.depth != nullptr;
-  // so does a label target, alone or with depth
-  const int out = (depth ? 1 : 0) | (labels ? 2 : 0);
-  // a marking target selects the kMarks instances, with kLabels where a label target is set; they write the depth
-  // where that target is set
-  const bool marking = markings != nullptr;
-  if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
-    const auto solo_of = [&](auto fish, auto pool_) {
-      constexpr bool f = decltype(fish)::value, p = decltype(pool_)::value;
-      if (marking) return labels ? k_raster_solo<f, false, true, p, true> : k_raster_solo<f, false, false, p, true>;
-      return out == 3 ? k_raster_solo<f, true, true, p> : out == 2 ? k_raster_solo<f, false, true, p>
-                                                        : out == 1 ? k_raster_solo<f, true, false, p> : k_raster_solo<f, false, false, p>;
-    };
-    const auto flat_of = [&](auto fish, auto pool_) {
-      constexpr bool f = decltype(fish)::value, p = decltype(pool_)::value;
-      if (marking) return labels ? k_raster_flat<f, false, true, p, true> : k_raster_flat<f, false, false, p, true>;
-      return out == 3 ? k_raster_flat<f, true, true, p> : out == 2 ? k_raster_flat<f, false, true, p>
-                                                        : out == 1 ? k_raster_flat<f, true, false, p> : k_raster_flat<f, false, false, p>;
-    };
-    const auto solo = pool ? solo_of(std::true_type{}, std::true_type{})
-                    : fisheye ? solo_of(std::true_type{}, std::false_type{}) : solo_of(std::false_type{}, std::false_type{});
-    const auto flat = pool ? flat_of(std::true_type{}, std::true_type{})
-                    : fisheye ? flat_of(std::true_type{}, std::false_type{}) : flat_of(std::false_type{}, std::false_type{});
-    solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, labels, fish_tab,
-                                                     markings);
-    // before k_raster, which draws the bins k_raster_flat hands back
-    flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, err_flag, labels, fish_tab,
-                                                     markings);
-    launches += 2;
-  }
-  const auto raster_of = [&](auto wrap_fmt, auto fish, auto pool_) {
-    constexpr bool w = decltype(wrap_fmt)::value, f = decltype(fish)::value, p = decltype(pool_)::value;
-    if (marking) return labels ? k_raster<w, f, false, true, p, true> : k_raster<w, f, false, false, p, true>;
-    return out == 3 ? k_raster<w, f, true, true, p> : out == 2 ? k_raster<w, f, false, true, p>
-                                                    : out == 1 ? k_raster<w, f, true, false, p> : k_raster<w, f, false, false, p>;
-  };
-  const std::true_type yes{};
-  const std::false_type no{};
-  const auto raster = pool ? (wrap ? raster_of(yes, yes, yes) : raster_of(no, yes, yes))
-                    : fisheye ? (wrap ? raster_of(yes, yes, no) : raster_of(no, yes, no))
-                              : (wrap ? raster_of(yes, no, no) : raster_of(no, no, no));
-  raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, ft, gather, obs, r.max_prims, r.pool, r.max_lat, err_flag,
-                                                                labels, fish_tab, markings);
+  const int aux_run = aux_set(aux);   // the rasterisers' instances for the images asked for (no target: the plain ones)
+  for_each_aux_set([&](auto aux_c) {
+    constexpr int A = decltype(aux_c)::value;
+    if (A != aux_run) return;
+    if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
+      const auto solo = pool ? k_raster_solo<true, true, A> : fisheye ? k_raster_solo<true, false, A> : k_raster_solo<false, false, A>;
+      const auto flat = pool ? k_raster_flat<true, true, A> : fisheye ? k_raster_flat<true, false, A> : k_raster_flat<false, false, A>;
+      solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, fish_tab, aux);
+      // before k_raster, which draws the bins k_raster_flat hands back
+      flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, err_flag, fish_tab, aux);
+      launches += 2;
+    }
+    const auto raster = raster_of<A>(wrap, fisheye, pool);
+    raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, ft, gather, obs, r.max_prims, r.pool,
+                                                                  r.max_lat, err_flag, fish_tab, aux);
+  });
   mark();
   mark();   // (post passes: launched by the caller)
   return launches;
@@ -2672,17 +2662,12 @@ Renderer* renderer_create(const dts_config& cfg) {
   cudaDeviceGetAttribute(&r->sms, cudaDevAttrMultiProcessorCount, cfg.device);
   r->cbins = ((r->W + kCoarseW - 1) / kCoarseW) * ((r->H + kCoarseH - 1) / kCoarseH);
   // k_raster's shared memory is past the 48 KB default; the opt-in holds for the kernel as loaded on this device
-  const auto opt_in = [](auto wrap_fmt, auto fish, auto pool) {
-    constexpr bool w = decltype(wrap_fmt)::value, f = decltype(fish)::value, p = decltype(pool)::value;
-    for (const auto raster : {k_raster<w, f, false, false, p>, k_raster<w, f, true, false, p>, k_raster<w, f, false, true, p>,
-                              k_raster<w, f, true, true, p>, k_raster<w, f, false, false, p, true>,
-                              k_raster<w, f, false, true, p, true>})
-      cudaFuncSetAttribute(raster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
-  };
-  const std::true_type yes{};
-  const std::false_type no{};
-  opt_in(yes, yes, no); opt_in(no, yes, no); opt_in(yes, no, no); opt_in(no, no, no);
-  opt_in(yes, yes, yes); opt_in(no, yes, yes);
+  for_each_aux_set([](auto aux_c) {
+    for (const bool wrap : {false, true})
+      for (const int gather : {0, 1, 2})   // none, one table, a pool
+        cudaFuncSetAttribute(raster_of<decltype(aux_c)::value>(wrap, gather > 0, gather > 1),
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
+  });
   return r;
 }
 
