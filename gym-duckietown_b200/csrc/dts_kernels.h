@@ -117,11 +117,11 @@ void renderer_release_frame(Renderer& r);   // the maps changed: the next render
 // Before every render: reserves frame memory for the maps of `counts` unless it is reserved, and checks that a fisheye
 // LUT is set if the camera needs one and a rectification LUT if render `mode` asks for it.
 std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode);
-// The fused gather's tables for a LUT of the camera's size (obs[y, x] = frame[rint(rmapy), rint(rmapx)]), in the fisheye
-// slot or (`rectify`) the rectification slot; they replace that slot's previous ones, so no render may be in flight.  A
-// LUT the rasteriser cannot take leaves the previous tables; NULL maps free the slot.  A fisheye pool: `count` LUTs
-// back to back in rmapx / rmapy, env e gathered through LUT lut_of_env[e] (HOST, [n_envs], checked by the caller; read
-// only when count > 1).  The rectification slot takes one LUT.
+// The rasteriser's remap table for a LUT of the camera's size (obs[y, x] = frame[rint(rmapy), rint(rmapx)]), in the
+// fisheye slot or (`rectify`) the rectification slot; it replaces that slot's previous one, so no render may be in
+// flight.  A LUT the rasteriser cannot take leaves the previous table; NULL maps free the slot.  A fisheye pool: `count`
+// LUTs back to back in rmapx / rmapy, env e remapped through LUT lut_of_env[e] (HOST, [n_envs], checked by the caller;
+// read only when count > 1, and then kept in the table).  The rectification slot takes one LUT.
 std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* rmapx, const float* rmapy,
                              const int32_t* lut_of_env);
 // `marks`: NULL or kProfMarks events recorded on `st` before k_frame_setup and after each of k_frame_setup, k_geometry,

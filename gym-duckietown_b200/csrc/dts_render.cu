@@ -51,11 +51,16 @@
 
 namespace dts {
 
-// Fused fisheye gather (distortion.py:118, obs[y, x] = undistorted[rint(rmapy), rint(rmapx)]): the rasteriser renders
-// each OUTPUT pixel at the source position the LUT names, so no undistorted frame is ever written.  Prims are binned
-// against the source-pixel bounding boxes of the output bins.  All device pointers, built by renderer_set_lut, for the
-// fisheye LUT or UndistortWrapper's rectification map alike.
-struct FishTab {
+// LUT remap, fused into the rasteriser (distortion.py:118 for the fisheye, UndistortWrapper's rectification alike:
+// obs[y, x] = undistorted[rint(rmapy), rint(rmapx)]): the rasteriser renders each OUTPUT pixel at the source position
+// the table names, so no undistorted frame is ever written.  Prims are binned against the source-pixel bounding boxes of
+// the output bins.  All device pointers, built by renderer_set_lut.
+// A pool of tables (dts_set_fisheye_luts, camera_rand) is held in one RemapTab: the tables' arrays concatenated, table
+// t's src_xy / cbox / fbox / cell_start / home_start t strides in (every table has the camera's sizes), the CSR starts
+// holding positions in the concatenated cell_bins / home_ent, ext_x / ext_y the largest over the tables, and
+// table_of_env naming each env's table.  The kRemapPool instances offset the pointers by it (remap_of_env); the
+// kRemapTable instances read the table as it is.
+struct RemapTab {
   const int32_t* src_xy;   // [H][W]  sx | sy << 16 (int16 each); sx = -32768: source outside the image -> 0
   const short4* cbox;      // [cbins]    source bounding box (x0, y0, x1, y1) of a 32x8 coarse output bin; x1 < x0: empty
   const short4* fbox;      // [cbins][8] the same for each of its 8x4 fine bins
@@ -69,12 +74,11 @@ struct FishTab {
   const int32_t* home_start;   // [cbins + 1]
   const int4* home_ent;
   int ext_x, ext_y;
+  const uint16_t* table_of_env;   // [n_envs] a pool's table index of every env; null unless a pool of more than one table
 };
-// A pool of fisheye tables (dts_set_fisheye_luts, camera_rand) is held in one FishTab: the tables' arrays concatenated,
-// table t's src_xy / cbox / fbox / cell_start / home_start t strides in (every table has the camera's sizes), the CSR
-// starts holding positions in the concatenated cell_bins / home_ent, and ext_x / ext_y the largest over the tables.  The
-// rasterisers' kPool instances take the table of each env from a device array of table indices, their last kernel
-// parameter; the other instances, and launches with one table, read the FishTab as it is.
+// How the rasterisers map output pixels to source pixels: not at all, through one table, or through each env's table of
+// a pool (the template value kRemap of k_bin and the rasterisers)
+constexpr int kRemapNone = 0, kRemapTable = 1, kRemapPool = 2;
 
 namespace {
 
@@ -523,7 +527,7 @@ __device__ __forceinline__ bool bin_overlaps(const int qx[4], const int qy[4], i
 // The visibility record of prim `p` for the coarse bin whose corner is (ox, oy) sub-pixels: edge functions re-based
 // to the corner (exact in 64 bits, then int32: inside the coarse bin |A*x + B*y| < 2^30), exact reject /
 // trivial-accept bits for each of the bin's 8 fine bins, depth plane, draw id.
-// With `fb` (fused fisheye) the bin's pixels are wherever the LUT sends its output pixels: (ox, oy) is the corner of
+// With `fb` (LUT remap) the bin's pixels are wherever the LUT sends its output pixels: (ox, oy) is the corner of
 // their source bounding box and fb[f] the source box of fine bin f; the bits then speak about every pixel of that box.
 // Returns the fine bins every sample of which the prim covers (bits 0-7) | kRecGround | kRecFlatOk.
 constexpr unsigned kRecGround = 0x100u;   // the ground quad
@@ -553,7 +557,7 @@ __device__ __forceinline__ unsigned build_binrec(const PrimRec* __restrict__ pr,
     const int a = -dy, b = dx, e = (int)e0;
     E0[k] = e; A[k] = a; B[k] = b;
     if (fb) {
-      // (fisheye: the fine bins' source boxes are handled after the edge loop, one box load per fine bin)
+      // (remap: the fine bins' source boxes are handled after the edge loop, one box load per fine bin)
     } else {
       // extremes of A*x + B*y over one fine bin's sample span x in [8, 504], y in [8, 248]
       const int hi = (a > 0 ? a * 504 : a * 8) + (b > 0 ? b * 248 : b * 8);
@@ -835,25 +839,25 @@ __device__ __forceinline__ unsigned fine_in_image(int cbx, unsigned rows, int W)
   return rows & (cols | (cols << 4));
 }
 
-// Fused fisheye: the source pixel the LUT names for this lane's output pixel of fine bin (bx, by), in sub-pixels, and
+// LUT remap: the source pixel the table names for this lane's output pixel of fine bin (bx, by), in sub-pixels, and
 // whether there is one (none: cv2.remap BORDER_CONSTANT, black).  Lanes past the image edge read a clamped entry; their
 // pixels are not stored.
-struct FishPx { bool valid; int x, y; };
-__device__ __forceinline__ FishPx fish_source(const FishTab& ft, int bx, int by, int lane, int W, int H) {
+struct RemapPx { bool valid; int x, y; };
+__device__ __forceinline__ RemapPx remap_source(const RemapTab& rt, int bx, int by, int lane, int W, int H) {
   const int gx = min(bx * kBinW + (lane & 7), W - 1), gy = min(by * kBinH + (lane >> 3), H - 1);
-  const int sxy = __ldg(ft.src_xy + gy * W + gx);
+  const int sxy = __ldg(rt.src_xy + gy * W + gx);
   const int sx = (int)(short)(sxy & 0xffff), sy = sxy >> 16;
-  return FishPx{sx != -32768, sx * kSub, sy * kSub};
+  return RemapPx{sx != -32768, sx * kSub, sy * kSub};
 }
-// The tables of env `env` in a pool (`tab`: the table index of every env)
-__device__ __forceinline__ FishTab fish_of_env(FishTab ft, const uint16_t* __restrict__ tab, int env, int W, int H, int cbins) {
-  const int t = __ldg(tab + env);
-  ft.src_xy += (size_t)t * W * H;
-  ft.cbox += (size_t)t * cbins;
-  ft.fbox += (size_t)t * cbins * (kCFX * kCFY);
-  ft.cell_start += (size_t)t * (cbins + 1);
-  ft.home_start += (size_t)t * (cbins + 1);
-  return ft;
+// The table of env `env` in a pool
+__device__ __forceinline__ RemapTab remap_of_env(RemapTab rt, int env, int W, int H, int cbins) {
+  const int t = __ldg(rt.table_of_env + env);
+  rt.src_xy += (size_t)t * W * H;
+  rt.cbox += (size_t)t * cbins;
+  rt.fbox += (size_t)t * cbins * (kCFX * kCFY);
+  rt.cell_start += (size_t)t * (cbins + 1);
+  rt.home_start += (size_t)t * (cbins + 1);
+  return rt;
 }
 
 // One fine bin of a lean_output() frame: whole words if the bin lies inside the image, else the general form
@@ -999,9 +1003,8 @@ struct Renderer {
   int max_prims = 0, max_lat = 0, items_max = 0, pool = 0;
   void* frame = nullptr;     // frame memory (null: not reserved since the last map upload)
   FrameMem fm{};             // ... carved
-  FishTab fish{};            // fused fisheye tables (null until a LUT is set): one table, or a pool of them
-  uint16_t* fish_tab = nullptr;   // [n] a pool's table index of every env (device); null with one table
-  FishTab rect{};            // UndistortWrapper's rectification, gathered the same way (null unless set)
+  RemapTab fish{};           // the fisheye remap (null until a LUT is set): one table, or a pool of them
+  RemapTab rect{};           // UndistortWrapper's rectification (null unless set)
 };
 
 // The one statement of the frame-memory layout: points `f` into the allocation at `base` and returns its size, so
@@ -1395,12 +1398,10 @@ constexpr int kBinWarps = 4;
 constexpr int kCountMask = 0xfffff, kGroundInc = 1 << 20;   // a bin's counter: records | ground-quad records << 20
 constexpr int kFlatBin = -0x7fffffff - 1;   // bin_count of a flat bin (k_raster_flat); solo bins hold -(prim + 1) >= -65536
 // kListed: the frame draws the envs of rc.env_list.  (Its own instance: an env id loaded from the list stays live across
-// the kernel, where blockIdx.x is re-read for free, and would cost the fisheye instance registers and spills.)
-template <bool kFish, bool kListed, bool kPool = false>   // kFish: bins are the LUT's source boxes of the output bins (fused fisheye gather)
-                                                       // kPool: each env's tables of a pool (fish_of_env)
+// the kernel, where blockIdx.x is re-read for free, and would cost the remap instances registers and spills.)
+template <int kRemap, bool kListed>   // kRemap other than kRemapNone: bins are the LUT's source boxes of the output bins
 __global__ void __launch_bounds__(kBinWarps * 32)
-k_bin(RenderCfg rc, FrameMem fm, FishTab fts, int max_prims, int max_pairs, int32_t* __restrict__ err,
-      const uint16_t* __restrict__ fish_tab) {
+k_bin(RenderCfg rc, FrameMem fm, RemapTab rts, int max_prims, int max_pairs, int32_t* __restrict__ err) {
   extern __shared__ int bin_smem[];
   __shared__ int s_total, s_base, s_ok;
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, tid = threadIdx.x;
@@ -1408,7 +1409,7 @@ k_bin(RenderCfg rc, FrameMem fm, FishTab fts, int max_prims, int max_pairs, int3
   const int env = kListed ? __ldg(rc.env_list + blockIdx.x) : (int)blockIdx.x, nthr = blockDim.x;   // 1 warp per env for small cameras, 4 for large ones (launch_render)
   const int W = rc.width, H = rc.height;
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW, cbins_y = (H + kCoarseH - 1) / kCoarseH, cbins = cbins_x * cbins_y;
-  const FishTab ft = kPool ? fish_of_env(fts, fish_tab, env, W, H, cbins) : fts;
+  const RemapTab rt = kRemap == kRemapPool ? remap_of_env(rts, env, W, H, cbins) : rts;
   int* cnt = bin_smem;
   int* start = cnt + cbins;
   const PrimRec* prims = fm.prims + (size_t)env * max_prims;
@@ -1436,18 +1437,18 @@ k_bin(RenderCfg rc, FrameMem fm, FishTab fts, int max_prims, int max_pairs, int3
       const int bx0 = pminx / kCoarseW, by0 = pminy / kCoarseH, bx1 = pmaxx / kCoarseW, by1 = pmaxy / kCoarseH;
       // A prim that may meet many bins is handed to the whole warp (one bin per lane and round) instead of one lane
       // walking all of them while 31 wait: the ground quad and the near tiles span hundreds of bins.
-      const bool big = have && (bx1 - bx0 + 1) * (by1 - by0 + 1) > 8;   // (fisheye: source cells under the prim's box)
+      const bool big = have && (bx1 - bx0 + 1) * (by1 - by0 + 1) > 8;   // (remap: source cells under the prim's box)
       if (have && !big) {
-        if (kFish) {
+        if (kRemap != kRemapNone) {
           // the output bins whose SOURCE box meets the prim, through the inverse index: the source cells under the prim's
           // pixel box (the same 32x8 grid), each with its list of output bins.  A bin listed by several of those cells
           // is taken from the first one only (the cell holding the top-left corner of box ∩ prim-cell-range).
           for (int cy = by0; cy <= by1; cy++)
             for (int cx = bx0; cx <= bx1; cx++) {
               const int c = cy * cbins_x + cx;
-              for (int q = ft.cell_start[c]; q < ft.cell_start[c + 1]; q++) {
-                const int b = ft.cell_bins[q];
-                const short4 cb = ft.cbox[b];
+              for (int q = rt.cell_start[c]; q < rt.cell_start[c + 1]; q++) {
+                const int b = rt.cell_bins[q];
+                const short4 cb = rt.cbox[b];
                 if (pmaxx < cb.x || pminx > cb.z || pmaxy < cb.y || pminy > cb.w) continue;
                 if (cx != max(bx0, cb.x / kCoarseW) || cy != max(by0, cb.y / kCoarseH)) continue;   // counted from another cell
                 const int pos = atomicAdd(&cnt[b], ginc) & kCountMask;
@@ -1473,20 +1474,20 @@ k_bin(RenderCfg rc, FrameMem fm, FishTab fts, int max_prims, int max_pairs, int3
 #pragma unroll
         for (int k = 0; k < 4; k++) { vx[k] = __shfl_sync(0xffffffffu, qx[k], src); vy[k] = __shfl_sync(0xffffffffu, qy[k], src); }
         const int snv = __shfl_sync(0xffffffffu, nv, src), sp = p0 + src, sginc = __shfl_sync(0xffffffffu, ginc, src);
-        if (kFish) {
+        if (kRemap != kRemapNone) {
           // one HOME cell per lane and round: every output bin is listed once, under the source cell holding the top-left
           // corner of its source box (second inverse index), so a prim spanning many cells meets each candidate bin once;
           // the range of home cells is the prim's cell range grown up / left by the largest box extent of the LUT
           const int sminx = __shfl_sync(0xffffffffu, pminx, src), smaxx = __shfl_sync(0xffffffffu, pmaxx, src);
           const int sminy = __shfl_sync(0xffffffffu, pminy, src), smaxy = __shfl_sync(0xffffffffu, pmaxy, src);
-          const int hx0 = max(__shfl_sync(0xffffffffu, bx0, src) - ft.ext_x, 0), sbx1 = __shfl_sync(0xffffffffu, bx1, src);
-          const int hy0 = max(__shfl_sync(0xffffffffu, by0, src) - ft.ext_y, 0), sby1 = __shfl_sync(0xffffffffu, by1, src);
+          const int hx0 = max(__shfl_sync(0xffffffffu, bx0, src) - rt.ext_x, 0), sbx1 = __shfl_sync(0xffffffffu, bx1, src);
+          const int hy0 = max(__shfl_sync(0xffffffffu, by0, src) - rt.ext_y, 0), sby1 = __shfl_sync(0xffffffffu, by1, src);
           const int nbx = sbx1 - hx0 + 1, nb = nbx * (sby1 - hy0 + 1);
           for (int i = lane; i < nb; i += 32) {
             const int cy = hy0 + i / nbx, cx = hx0 + i % nbx, c = cy * cbins_x + cx;
-            const int q1 = __ldg(ft.home_start + c + 1);
-            for (int q = __ldg(ft.home_start + c); q < q1; q++) {
-              const int4 e = __ldg(ft.home_ent + q);   // x0 | y0 << 16, x1 | y1 << 16, bin
+            const int q1 = __ldg(rt.home_start + c + 1);
+            for (int q = __ldg(rt.home_start + c); q < q1; q++) {
+              const int4 e = __ldg(rt.home_ent + q);   // x0 | y0 << 16, x1 | y1 << 16, bin
               const int x0 = (int)(short)(e.x & 0xffff), y0 = e.x >> 16, x1 = (int)(short)(e.y & 0xffff), y1 = e.y >> 16;
               if (smaxx < x0 || sminx > x1 || smaxy < y0 || sminy > y1) continue;
               if (!box_overlaps(vx, vy, snv, x0 * kSub + 8, x1 * kSub + 56, y0 * kSub + 8, y1 * kSub + 56)) continue;
@@ -1558,9 +1559,9 @@ k_bin(RenderCfg rc, FrameMem fm, FishTab fts, int max_prims, int max_pairs, int3
     const int p = (int)(pair & 0xffffu), b = (int)(pair >> 16);
     const int cby = b / cbins_x, cbx = b - cby * cbins_x;
     unsigned r;
-    if (kFish) {
-      const short4 cb = ft.cbox[b];
-      r = build_binrec(prims + p, p, cb.x * kSub, cb.y * kSub, recs + i, ft.fbox + (size_t)b * 8);
+    if (kRemap != kRemapNone) {
+      const short4 cb = rt.cbox[b];
+      r = build_binrec(prims + p, p, cb.x * kSub, cb.y * kSub, recs + i, rt.fbox + (size_t)b * 8);
     } else {
       r = build_binrec(prims + p, p, cbx * kCoarseW * kSub, cby * kCoarseH * kSub, recs + i);
     }
@@ -1736,15 +1737,14 @@ __device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool sim
 }
 
 // ------------------------------------------------------------------------------------------------ k_raster
-template <bool kWrapFmt, bool kFish, bool kPool, int kAux>
+template <bool kWrapFmt, int kRemap, int kAux>
                                        // kWrapFmt: a dts_output_format other than packed u8 HWC is written by the resolve;
-                                       // kFish: every lane renders the SOURCE pixel the fisheye LUT names for its output pixel;
-                                       // kPool: each env's tables of a pool (fish_of_env);
+                                       // kRemap other than kRemapNone: every lane renders the SOURCE pixel the LUT names
+                                       // for its output pixel;
                                        // kAux: the images written beside obs (AuxTargets)
 __global__ void __launch_bounds__(kThreads, kRasterMinCtas)
-k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, FishTab fts, GatherTab gt,
-         uint8_t* __restrict__ obs, int max_prims, int max_pairs, int max_lat, int32_t* __restrict__ err,
-         const uint16_t* __restrict__ fish_tab, AuxTargets aux) {
+k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, RemapTab rts, GatherTab gt,
+         uint8_t* __restrict__ obs, int max_prims, int max_pairs, int max_lat, int32_t* __restrict__ err, AuxTargets aux) {
   // dynamic shared memory (kRasterSmem bytes): per warp two chunks of records in flight, their mbarriers, and a 128-sample
   // depth / winner buffer for the tiny triangles of the fine bin being drawn
   extern __shared__ __align__(128) unsigned char raster_smem[];
@@ -1777,7 +1777,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
     if (lane == 0) next_work = atomicAdd(fm.work + kWorkRaster, 1);   // consumed after this row: latency hidden
     const int slot = work / cbins_y, cby = work - slot * cbins_y;
     const int env = listed_env(rc.env_list, slot);
-    const FishTab ft = kPool ? fish_of_env(fts, fish_tab, env, W, H, cbins) : fts;
+    const RemapTab rt = kRemap == kRemapPool ? remap_of_env(rts, env, W, H, cbins) : rts;
     const DMap& m = maps[S.map_id[env]];
     const uint8_t* tex_pool = m.tex_pool;
     const PrimRec* prims = fm.prims + (size_t)env * max_prims;
@@ -1863,7 +1863,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
           if ((fvalid >> f) & 1u) {
             const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);
             unsigned rgb = clear_rgb;
-            if (kFish && !fish_source(ft, bx, by, lane, W, H).valid) rgb = 0u;
+            if (kRemap != kRemapNone && !remap_source(rt, bx, by, lane, W, H).valid) rgb = 0u;
             emit(rgb, 0.0f, 0, 0, bx, by);
           }
         continue;
@@ -1872,7 +1872,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
       DTS_COUNT(10, count);
       if (!single) { DTS_COUNT(14, 1); DTS_COUNT(15, count); }
       int ox = cbx * kCoarseW * kSub, oy = cby * kCoarseH * kSub;   // coarse bin corner, sub-pixels
-      if (kFish) { const short4 cb = ft.cbox[cby * cbins_x + cbx]; ox = cb.x * kSub; oy = cb.y * kSub; }   // ... of its source box
+      if (kRemap != kRemapNone) { const short4 cb = rt.cbox[cby * cbins_x + cbx]; ox = cb.x * kSub; oy = cb.y * kSub; }   // ... of its source box
 #pragma unroll 1
       for (int g = 0; g < (single ? 1 : kCFX * kCFY); g++) {
         if (!single && !((fvalid >> g) & 1u)) continue;
@@ -1893,7 +1893,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
           if (lane < nch) mine = *reinterpret_cast<const uint2*>(&stage[lane].prim_flags);
           const bool first = c0 == 0, last = c0 + kStage >= count;
           const unsigned ground_bits = __ballot_sync(0xffffffffu, (mine.y & kKindGround) != 0u);   // the ground quad's records in this chunk
-          const unsigned tiny_bits = kFish ? 0u : __ballot_sync(0xffffffffu, (mine.y & kKindTiny) != 0u);   // one-per-lane triangles
+          const unsigned tiny_bits = kRemap != kRemapNone ? 0u : __ballot_sync(0xffffffffu, (mine.y & kKindTiny) != 0u);   // one-per-lane triangles
           const unsigned flat_bits = __ballot_sync(0xffffffffu, (mine.y & kKindFlat) != 0u);   // road tiles (plane y = 0)
 #if DTS_STATS
           if (single) {   // census: coarse bins lying inside ONE prim (besides the ground)
@@ -1908,8 +1908,8 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
             const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);   // fine bin
             int pxc = pxs + (f & 3) * kBinW * kSub, pyc = pys + (f >> 2) * kBinH * kSub;   // this lane's pixel, coarse-relative
             bool px_valid = true;
-            if (kFish) {
-              const FishPx src = fish_source(ft, bx, by, lane, W, H);
+            if (kRemap != kRemapNone) {
+              const RemapPx src = remap_source(rt, bx, by, lane, W, H);
               px_valid = src.valid;
               pxc = src.x - ox; pyc = src.y - oy;
             }
@@ -2017,7 +2017,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
                 }
               }
             }
-            if (!kFish && !simple && (live_mask & tiny_bits)) {
+            if (kRemap == kRemapNone && !simple && (live_mask & tiny_bits)) {
               // ---- tiny triangles, ONE PER LANE: each lane walks the few pixels of its triangle inside this fine bin and
               // resolves GL_LESS (ties to the lower draw id) with a 64-bit atomicMin on depth | id | prim per sample —
               // 32 triangles per pass instead of one warp-wide visit per triangle
@@ -2059,7 +2059,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
               __syncwarp();
             }
             if (!(last || simple)) continue;
-            if (!kFish && !simple && zb_used) {
+            if (kRemap == kRemapNone && !simple && zb_used) {
               // merge the tiny triangles' winners into the per-sample state: GL_LESS, ties to the lower draw id
 #pragma unroll
               for (int s = 0; s < 4; s++) {
@@ -2077,7 +2077,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
             AuxPx pix;
             unsigned rgb = shade_resolve<kAux>(wn, simple, clr, prims, tex_pool, lat_tab, ox + pxc, oy + pyc, lane, err, pix,
                                                label_of, cls_pool);
-            if (kFish && !px_valid) rgb = 0u;   // cv2.remap BORDER_CONSTANT
+            if (kRemap != kRemapNone && !px_valid) rgb = 0u;   // cv2.remap BORDER_CONSTANT
             emit(rgb, depth_of(pix.qmax, px_valid), px_valid ? pix.lab : 0, px_valid ? pix.mk : 0, bx, by);
           }
         }
@@ -2099,12 +2099,10 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
 // Packed u8 HWC output with whole-word rows only (k_bin marks no bin otherwise).  Runs before k_raster.
 // Images: the 1/w the shading divides by gives the depth, the bin's one prim the label of every pixel with a source, and
 // the texel it shows there the marking.
-template <bool kFish, bool kPool, int kAux>
-                                     // kFish: each lane shades the source pixel the fisheye LUT names for its output pixel;
-                                     // kPool: each env's tables of a pool (fish_of_env)
+template <int kRemap, int kAux>   // kRemap other than kRemapNone: each lane shades the source pixel the LUT names for its output pixel
 __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
-                                                                        FishTab fts, uint8_t* __restrict__ obs, int max_prims, int max_lat,
-                                                                        const uint16_t* __restrict__ fish_tab, AuxTargets aux) {
+                                                                        RemapTab rts, uint8_t* __restrict__ obs, int max_prims, int max_lat,
+                                                                        AuxTargets aux) {
   const int W = rc.width, H = rc.height;
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW;
   const int lane = threadIdx.x & 31;
@@ -2117,7 +2115,7 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
     const int env = (int)e.x, b = (int)(e.y & 0xffffu);
     const unsigned p = e.y >> 16;
     const int cby = b / cbins_x, cbx = b - cby * cbins_x;
-    const FishTab ft = kPool ? fish_of_env(fts, fish_tab, env, W, H, cbins_x * ((H + kCoarseH - 1) / kCoarseH)) : fts;
+    const RemapTab rt = kRemap == kRemapPool ? remap_of_env(rts, env, W, H, cbins_x * ((H + kCoarseH - 1) / kCoarseH)) : rts;
     const uint8_t* tex_pool = maps[S.map_id[env]].tex_pool;
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     const ShadeIn si = load_shade(fm.prims + (size_t)env * max_prims, p);
@@ -2137,8 +2135,8 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
       const int bx = cbx * kCFX + fx, by = cby * kCFY + fy;
       int pxa = (bx * kBinW + (lane & 7)) * kSub, pya = (by * kBinH + (lane >> 3)) * kSub;
       bool px_valid = true;
-      if (kFish) {
-        const FishPx src = fish_source(ft, bx, by, lane, W, H);
+      if (kRemap != kRemapNone) {
+        const RemapPx src = remap_source(rt, bx, by, lane, W, H);
         px_valid = src.valid;
         pxa = src.x; pya = src.y;
       }
@@ -2147,7 +2145,7 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
       shade_eval(si, tex_pool, lat_tab, pxa, pya, c3, may_store_depth(kAux) ? &qq : nullptr, cls_pool,
                  (kAux & kAuxMarks) ? &mk : nullptr);
       unsigned rgb = pack_rgb(c3[0], c3[1], c3[2]);
-      if (kFish && !px_valid) rgb = 0u;
+      if (kRemap != kRemapNone && !px_valid) rgb = 0u;
       store_bin_lean(out, sl, rgb, lane, bx, by, W, H);
       store_aux<kAux>(af, depth_of(qq, px_valid), px_valid ? lab : 0, px_valid ? mk : 0, lane, bx, by, W, H);
     }
@@ -2178,13 +2176,11 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
 // the whole bin, colour and images.
 // Packed u8 HWC output with whole-word rows only (k_bin lists no bin otherwise).  Runs after k_raster_solo.
 constexpr int kEdgeQ = 64;   // queue ring: flushed at 32 entries, so at most 31 + 32 wait at once
-template <bool kFish, bool kPool, int kAux>
-                                 // kFish: each lane covers and shades the source pixel the fisheye LUT names for its output pixel;
-                                 // kPool: each env's tables of a pool (fish_of_env)
+template <int kRemap, int kAux>   // kRemap other than kRemapNone: each lane covers and shades the source pixel the LUT names
+                                  // for its output pixel
 __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm,
-                                                                        FishTab fts, uint8_t* __restrict__ obs, int max_prims, int max_lat,
-                                                                        int32_t* __restrict__ err, const uint16_t* __restrict__ fish_tab,
-                                                                        AuxTargets aux) {
+                                                                        RemapTab rts, uint8_t* __restrict__ obs, int max_prims, int max_lat,
+                                                                        int32_t* __restrict__ err, AuxTargets aux) {
   __shared__ BinRec stages[kWarps][kStage];   // per warp: the records of its bin
   __shared__ unsigned bin_rgb[kWarps][kCFX * kCFY * 32];   // per warp: packed colour of pixel `lane` of fine bin f at f * 32 + lane
   // per warp: the edge-pixel queue, an entry in two words: (pixel slot, pxa, pya, wn0 | wn1 << 16), (wn2 | wn3 << 16, first colour)
@@ -2208,7 +2204,7 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
     const uint2 e = fm.flat[i];
     const int env = (int)e.x, b = (int)(e.y & 0xffffu), count = (int)(e.y >> 16);
     const int cby = b / cbins_x, cbx = b - cby * cbins_x;
-    const FishTab ft = kPool ? fish_of_env(fts, fish_tab, env, W, H, cbins) : fts;
+    const RemapTab rt = kRemap == kRemapPool ? remap_of_env(rts, env, W, H, cbins) : rts;
     DTS_COUNT(24, 1);
     // ---- stage the records: one per lane, five 128-bit loads
     uint2 mine = make_uint2(0u, 0u);   // prim_flags, kind
@@ -2235,7 +2231,7 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
     float clr[3];
     clear_colour(S, rc, env, clr);
     int ox = cbx * kCoarseW * kSub, oy = cby * kCoarseH * kSub;   // coarse bin corner, sub-pixels
-    if (kFish) { const short4 cb = ft.cbox[b]; ox = cb.x * kSub; oy = cb.y * kSub; }   // ... of its source box
+    if (kRemap != kRemapNone) { const short4 cb = rt.cbox[b]; ox = cb.x * kSub; oy = cb.y * kSub; }   // ... of its source box
     // fine bins inside the image as column / row counts rather than fine_in_image(), as in k_raster_solo
     const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);
     const int ny = ((cby * kCFY + 1) * kBinH < H) ? 2 : 1;
@@ -2247,8 +2243,8 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
       const int bx = cbx * kCFX + (f & 3), by = cby * kCFY + (f >> 2);   // fine bin
       int pxc = pxs + (f & 3) * kBinW * kSub, pyc = pys + (f >> 2) * kBinH * kSub;   // this lane's pixel, coarse-relative
       bool px_valid = true;
-      if (kFish) {
-        const FishPx src = fish_source(ft, bx, by, lane, W, H);
+      if (kRemap != kRemapNone) {
+        const RemapPx src = remap_source(rt, bx, by, lane, W, H);
         px_valid = src.valid;
         pxc = src.x - ox; pyc = src.y - oy;
       }
@@ -2301,7 +2297,7 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
         }
       }
       // ---- every lane: its first winner.  One winner: the pixel is done.  More: it waits in the queue.  (A pixel the
-      // fisheye LUT gives no source is black either way.)
+      // LUT gives no source is black either way.)
       float c3[3] = {clr[0], clr[1], clr[2]}, qq0 = 0.0f;
       int c0 = 0;
       if (wn[0] != kNoPrim)
@@ -2317,7 +2313,7 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
         q[1][e] = make_uint4(wn[2] | (wn[3] << 16), __float_as_uint(c3[0]), __float_as_uint(c3[1]), __float_as_uint(c3[2]));
         if (needs_qq(kAux)) q_qq[e] = qq0;
       } else {
-        rgb_buf[slot] = (kFish && !px_valid) ? 0u : pack_rgb(c3[0], c3[1], c3[2]);
+        rgb_buf[slot] = (kRemap != kRemapNone && !px_valid) ? 0u : pack_rgb(c3[0], c3[1], c3[2]);
         const int lab = ((kAux & kAuxLabels) && px_valid && wn[0] != kNoPrim) ? label_of(wn[0]) : 0;
         store_aux<kAux>(af, depth_of(qq0, px_valid), lab, px_valid ? c0 : 0, lane, bx, by, W, H);   // (c0 = 0 without a winner)
       }
@@ -2367,10 +2363,10 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
 }
 
 // ------------------------------------------------------------------------------------------------ the renderer
-static void free_fish(FishTab& f) {
-  const void* p[] = {f.src_xy, f.cbox, f.fbox, f.cell_start, f.cell_bins, f.home_start, f.home_ent};
+static void free_remap(RemapTab& t) {
+  const void* p[] = {t.src_xy, t.cbox, t.fbox, t.cell_start, t.cell_bins, t.home_start, t.home_ent, t.table_of_env};
   for (const void* q : p) cudaFree(const_cast<void*>(q));
-  f = FishTab{};
+  t = RemapTab{};
 }
 
 void renderer_release_frame(Renderer& r) {
@@ -2379,7 +2375,7 @@ void renderer_release_frame(Renderer& r) {
 }
 
 void renderer_destroy(Renderer* r) {
-  if (r) { renderer_release_frame(*r); free_fish(r->fish); free_fish(r->rect); cudaFree(r->fish_tab); }
+  if (r) { renderer_release_frame(*r); free_remap(r->fish); free_remap(r->rect); }
   delete r;
 }
 
@@ -2428,16 +2424,15 @@ std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* 
   // distortion.py:118 gathers img[rint(rmapy), rint(rmapx)], UndistortWrapper (wrappers.py:227) the same with its own
   // map.  The rasteriser renders those source pixels directly: per output pixel the source position, per fine / coarse
   // output bin the bounding box of its source pixels (the bins prims are sorted into).
-  FishTab& slot = rectify ? r.rect : r.fish;
+  RemapTab& slot = rectify ? r.rect : r.fish;
   const char* what = rectify ? "rectification LUT" : "fisheye LUT";
   if (!rmapx || !rmapy) {
-    free_fish(slot);
-    if (!rectify) { cudaFree(r.fish_tab); r.fish_tab = nullptr; }
+    free_remap(slot);
     return "";
   }
   const int W = r.W, H = r.H, cbx_n = (W + kCoarseW - 1) / kCoarseW, cbins = r.cbins;
   const size_t px = (size_t)W * H;
-  // the tables of a pool, concatenated (FishTab): every per-table array is appended, so that the CSR starts pushed below
+  // the tables of a pool, concatenated (RemapTab): every per-table array is appended, so that the CSR starts pushed below
   // are positions in the concatenated lists
   std::vector<int32_t> src(px * count);
   const short4 empty = make_short4(32767, 32767, -32768, -32768);
@@ -2509,8 +2504,7 @@ std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* 
   std::vector<uint16_t> tab;
   if (count > 1)
     for (int e = 0; e < r.n; e++) tab.push_back((uint16_t)lut_of_env[e]);
-  FishTab t{};
-  uint16_t* d_tab = nullptr;
+  RemapTab t{};
   cudaError_t e = cudaSuccess;
   auto upload = [&](auto& dst, const auto& v) {
     void* d = nullptr;
@@ -2522,15 +2516,14 @@ std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* 
   upload(t.src_xy, src); upload(t.cbox, cbox); upload(t.fbox, fbox);
   upload(t.cell_start, cell_start); upload(t.cell_bins, cell_bins);
   upload(t.home_start, home_start); upload(t.home_ent, home_ent);
-  if (!tab.empty()) upload(d_tab, tab);
+  if (!tab.empty()) upload(t.table_of_env, tab);
   if (e != cudaSuccess) {
-    free_fish(t); cudaFree(d_tab);
+    free_remap(t);
     return std::string(what) + " table upload failed: " + cudaGetErrorString(e);
   }
   t.ext_x = ext_x; t.ext_y = ext_y;
-  free_fish(slot);
+  free_remap(slot);
   slot = t;
-  if (!rectify) { cudaFree(r.fish_tab); r.fish_tab = d_tab; }
   return "";
 }
 
@@ -2577,32 +2570,25 @@ constexpr int kAuxSets[] = {0, kAuxDepth, kAuxLabels, kAuxDepth | kAuxLabels, kA
 static int aux_set(const AuxTargets& a) {
   return (a.labels ? kAuxLabels : 0) | (a.marks ? kAuxMarks : a.depth ? kAuxDepth : 0);
 }
-// f(std::integral_constant<int, a>{}) for every image set a of kAuxSets
-template <typename F, size_t... I>
-static void each_aux_set(F& f, std::index_sequence<I...>) { (f(std::integral_constant<int, kAuxSets[I]>{}), ...); }
-template <typename F>
-static void for_each_aux_set(F f) { each_aux_set(f, std::make_index_sequence<std::size(kAuxSets)>{}); }
-// k_raster's instance for a wrapper output format, a gather through one table, or through a pool of them
-template <int kAux>
-static auto raster_of(bool wrap, bool fish, bool pool) {
-  return pool ? (wrap ? k_raster<true, true, true, kAux> : k_raster<false, true, true, kAux>)
-       : fish ? (wrap ? k_raster<true, true, false, kAux> : k_raster<false, true, false, kAux>)
-              : (wrap ? k_raster<true, false, false, kAux> : k_raster<false, false, false, kAux>);
-}
+// The remap modes k_bin and the rasterisers are compiled for
+constexpr int kRemapModes[] = {kRemapNone, kRemapTable, kRemapPool};
+// f(std::integral_constant<int, v>{}) for every value v of kList (kAuxSets, kRemapModes)
+template <const auto& kList, typename F, size_t... I>
+static void each_of(F& f, std::index_sequence<I...>) { (f(std::integral_constant<int, kList[I]>{}), ...); }
+template <const auto& kList, typename F>
+static void for_each_of(F f) { each_of<kList>(f, std::make_index_sequence<std::size(kList)>{}); }
 
 int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, const AuxTargets& aux,
                   void* obs_any, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks,
                   int mark_level, cudaStream_t st) {
   uint8_t* obs = reinterpret_cast<uint8_t*>(obs_any);
-  // the gather the frame goes through, if any: the rectification (DTS_RENDER_RECTIFY), none (DTS_RENDER_PINHOLE or no
-  // DTS_FLAG_DISTORTION) or the fisheye.  Both tables run the same kFish kernels.
-  const FishTab* lut = (rc.mode & DTS_RENDER_RECTIFY) ? &r.rect
-                     : ((rc.flags & DTS_FLAG_DISTORTION) && !(rc.mode & DTS_RENDER_PINHOLE)) ? &r.fish : nullptr;
-  const bool fisheye = lut != nullptr;
-  const FishTab ft = fisheye ? *lut : FishTab{};
-  // a pool of fisheye tables selects the kPool instances; one table, the rectification and no gather the others
-  const uint16_t* fish_tab = lut == &r.fish ? r.fish_tab : nullptr;
-  const bool pool = fish_tab != nullptr;
+  // the table the frame is remapped through, if any: the rectification (DTS_RENDER_RECTIFY), none (DTS_RENDER_PINHOLE
+  // or no DTS_FLAG_DISTORTION) or the fisheye.  A table with a per-env index is a pool (kRemapPool); one table, of
+  // either kind, is kRemapTable.
+  const RemapTab* lut = (rc.mode & DTS_RENDER_RECTIFY) ? &r.rect
+                      : ((rc.flags & DTS_FLAG_DISTORTION) && !(rc.mode & DTS_RENDER_PINHOLE)) ? &r.fish : nullptr;
+  const RemapTab rt = lut ? *lut : RemapTab{};
+  const int remap = !lut ? kRemapNone : rt.table_of_env ? kRemapPool : kRemapTable;
   FrameMem fm = r.fm;
   fm.status = status_dev;
   int mk = 0;
@@ -2628,26 +2614,30 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   const int bin_grid = rc.n_envs;   // CTA per env: one warp where a frame has few bins and prims (160x120: 75 bins — more warps
   // only add barriers and CTA launches), four for large cameras (640x480)
   const int bin_threads = r.cbins > 128 ? kBinWarps * 32 : 32;
-  const auto bin = pool ? (rc.env_list ? k_bin<true, true, true> : k_bin<true, false, true>)
-                 : rc.env_list ? (fisheye ? k_bin<true, true> : k_bin<false, true>) : (fisheye ? k_bin<true, false> : k_bin<false, false>);
-  bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, ft, r.max_prims, r.pool, err_flag, fish_tab);
+  for_each_of<kRemapModes>([&](auto remap_c) {
+    constexpr int R = decltype(remap_c)::value;
+    if (R != remap) return;
+    const auto bin = rc.env_list ? k_bin<R, true> : k_bin<R, false>;
+    bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, rt, r.max_prims, r.pool, err_flag);
+  });
   mark();
   const bool wrap = (rc.obs_layout | rc.obs_dtype) != 0;
   const int aux_run = aux_set(aux);   // the rasterisers' instances for the images asked for (no target: the plain ones)
-  for_each_aux_set([&](auto aux_c) {
-    constexpr int A = decltype(aux_c)::value;
-    if (A != aux_run) return;
-    if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
-      const auto solo = pool ? k_raster_solo<true, true, A> : fisheye ? k_raster_solo<true, false, A> : k_raster_solo<false, false, A>;
-      const auto flat = pool ? k_raster_flat<true, true, A> : fisheye ? k_raster_flat<true, false, A> : k_raster_flat<false, false, A>;
-      solo<<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, fish_tab, aux);
-      // before k_raster, which draws the bins k_raster_flat hands back
-      flat<<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, ft, obs, r.max_prims, r.max_lat, err_flag, fish_tab, aux);
-      launches += 2;
-    }
-    const auto raster = raster_of<A>(wrap, fisheye, pool);
-    raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, ft, gather, obs, r.max_prims, r.pool,
-                                                                  r.max_lat, err_flag, fish_tab, aux);
+  for_each_of<kAuxSets>([&](auto aux_c) {
+    for_each_of<kRemapModes>([&](auto remap_c) {
+      constexpr int A = decltype(aux_c)::value, R = decltype(remap_c)::value;
+      if (A != aux_run || R != remap) return;
+      if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
+        k_raster_solo<R, A><<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, rt, obs, r.max_prims, r.max_lat, aux);
+        // before k_raster, which draws the bins k_raster_flat hands back
+        k_raster_flat<R, A><<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, rt, obs, r.max_prims, r.max_lat,
+                                                                        err_flag, aux);
+        launches += 2;
+      }
+      const auto raster = wrap ? k_raster<true, R, A> : k_raster<false, R, A>;
+      raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, rt, gather, obs, r.max_prims, r.pool,
+                                                                    r.max_lat, err_flag, aux);
+    });
   });
   mark();
   mark();   // (post passes: launched by the caller)
@@ -2662,11 +2652,12 @@ Renderer* renderer_create(const dts_config& cfg) {
   cudaDeviceGetAttribute(&r->sms, cudaDevAttrMultiProcessorCount, cfg.device);
   r->cbins = ((r->W + kCoarseW - 1) / kCoarseW) * ((r->H + kCoarseH - 1) / kCoarseH);
   // k_raster's shared memory is past the 48 KB default; the opt-in holds for the kernel as loaded on this device
-  for_each_aux_set([](auto aux_c) {
-    for (const bool wrap : {false, true})
-      for (const int gather : {0, 1, 2})   // none, one table, a pool
-        cudaFuncSetAttribute(raster_of<decltype(aux_c)::value>(wrap, gather > 0, gather > 1),
-                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
+  for_each_of<kAuxSets>([](auto aux_c) {
+    for_each_of<kRemapModes>([&](auto remap_c) {
+      constexpr int A = decltype(aux_c)::value, R = decltype(remap_c)::value;
+      for (const auto raster : {k_raster<false, R, A>, k_raster<true, R, A>})
+        cudaFuncSetAttribute(raster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
+    });
   });
   return r;
 }

@@ -156,10 +156,10 @@ def _check_kinds(env, torch, md, kinds, px, pz, ang, chw_f32=False):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["small_loop", "loop_obstacles"])
 @pytest.mark.parametrize("W,H,fmt", [
-    (160, 120, "hwc_u8"),    # k_raster_solo / k_raster_flat / k_raster<false, true>
+    (160, 120, "hwc_u8"),    # k_raster_solo / k_raster_flat / k_raster<false, kRemapTable>
     (84, 84, "hwc_u8"),      # lean, partial fine bins on the right and bottom edges; square: the transpose LUT
-    (90, 70, "hwc_u8"),      # W % 4 != 0: k_raster<false, true> alone, partial bins on both edges
-    (160, 120, "chw_f32"),   # k_raster<true, true>
+    (90, 70, "hwc_u8"),      # W % 4 != 0: k_raster<false, kRemapTable> alone, partial bins on both edges
+    (160, 120, "chw_f32"),   # k_raster<true, kRemapTable>
     (640, 480, "hwc_u8"),    # > 128 coarse bins: k_bin with 4 warps
 ])
 def test_lut_family_vs_oracle(name, W, H, fmt, torch_cuda):

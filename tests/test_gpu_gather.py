@@ -215,8 +215,8 @@ def test_wrapper_formats_are_stored_per_bin(layout, dtype, W, H, torch_cuda):
 
 @pytest.mark.parametrize("lens", ["fisheye", "camera_rand_pool", "rectified"])
 def test_fisheye_pool_and_rectification(lens, torch_cuda):
-    """The kFish rasterisers: the fisheye LUT, a camera_rand pool of four LUTs (the kPool instances, each env through its
-    own table) and UndistortWrapper's rectification."""
+    """The remapping rasterisers: the fisheye LUT, a camera_rand pool of four LUTs (the kRemapPool instances, each env
+    through its own table) and UndistortWrapper's rectification."""
     torch = torch_cuda
     kw = dict(distortion=True)
     if lens == "camera_rand_pool":

@@ -1,5 +1,5 @@
-"""What a pool of fisheye LUTs costs (camera_rand: dts_set_fisheye_luts, the rasterisers' kPool instances) against the
-one-LUT path (dts_set_fisheye_lut).
+"""What a pool of fisheye LUTs costs (camera_rand: dts_set_fisheye_luts, the rasterisers' kRemapPool instances) against
+the one-LUT path (dts_set_fisheye_lut).
 
 Shapes: c4 (udem1, 640x480, fisheye, domain randomisation, `--c4-envs`, default 2048) and f160 (loop_obstacles, 160x120,
 fisheye, domain randomisation, 4096 envs).  ONE env per shape under device auto-reset and bench.py's uniform random
