@@ -400,9 +400,9 @@ __device__ __forceinline__ void dynamics_step(double& x, double& y, double& th, 
   const double dw = -p.w1 * w - p.w2 * u - p.w3 * u * w + (war * r - wal * l);
   const double u1 = u + dt * du, w1 = w + dt * dw;
   const double a = dt * w1, vx = dt * u1;
-  double sa, ca;  // sin(a)/a, (1-cos a)/a
+  double sa, ca;  // sin(a)/a, (1-cos a)/a, the latter as 2 sin^2(a/2)/a: 1 - cos(a) cancels to nothing below |a| ~ 1e-7
   if (fabs(a) < 1e-9) { sa = 1.0 - a * a / 6.0; ca = a / 2.0; }
-  else { double s_, c_; sincos(a, &s_, &c_); sa = s_ / a; ca = (1.0 - c_) / a; }
+  else { double sh, ch; sincos(0.5 * a, &sh, &ch); sa = 2.0 * sh * ch / a; ca = 2.0 * sh * sh / a; }
   const double tx = sa * vx, ty = ca * vx;
   double sn, cs;
   sincos(th, &sn, &cs);

@@ -3,7 +3,7 @@
 #define DT_ORACLE_H
 #include <stdint.h>
 
-#define ORC_MAX_DELAY 8
+#define ORC_MAX_DELAY 16 /* = DTS_MAX_DELAY (include/dtsim.h); tests/test_dynamics_ref.py holds the two equal */
 
 typedef struct {
   double tile_size;

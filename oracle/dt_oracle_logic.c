@@ -59,8 +59,9 @@ void orc_dyn_step(orc_dyn_state* s, const orc_dyn_params* p, const double cmd_lr
   /* q' = q * expm(dt * [[0,-w,u],[w,0,0],[0,0,0]]) : closed form of the SE(2) exponential */
   double a = dt * w1, vx = dt * u1;
   double sa, ca;
-  if (fabs(a) < 1e-9) { sa = 1.0 - a * a / 6.0; ca = a / 2.0; }  /* sin(a)/a , (1-cos a)/a */
-  else { sa = sin(a) / a; ca = (1.0 - cos(a)) / a; }
+  /* sin(a)/a , (1-cos a)/a, the latter as 2 sin^2(a/2)/a: 1 - cos(a) cancels to nothing below |a| ~ 1e-7 */
+  if (fabs(a) < 1e-9) { sa = 1.0 - a * a / 6.0; ca = a / 2.0; }
+  else { double sh = sin(0.5 * a), ch = cos(0.5 * a); sa = 2.0 * sh * ch / a; ca = 2.0 * sh * sh / a; }
   double tx = sa * vx, ty = ca * vx; /* body-frame translation (lateral velocity is 0) */
   double c = cos(s->theta), sn = sin(s->theta);
   s->x += c * tx - sn * ty;

@@ -56,9 +56,12 @@ class OrcDynParams(C.Structure):
                [("delay_steps", C.c_int32)]
 
 
+ORC_MAX_DELAY = 16   # dt_oracle.h; the delay line is as deep as the device's (DTS_MAX_DELAY)
+
+
 class OrcDynState(C.Structure):
     _fields_ = [("x", C.c_double), ("y", C.c_double), ("theta", C.c_double), ("u", C.c_double),
-                ("w", C.c_double), ("fifo", (C.c_double * 2) * 8)]
+                ("w", C.c_double), ("fifo", (C.c_double * 2) * ORC_MAX_DELAY)]
 
 
 class OrcStepOut(C.Structure):
@@ -111,11 +114,38 @@ def action_map(vel, steer, wheel_dist, gain=1.0, trim=0.0, radius=0.0318, k=27.0
     return out[0], out[1]
 
 
+# get_DB18_nominal as restated in DESIGN.md §4 (parity unpinned): the ten model constants and the command delay in
+# seconds, under the names dts_config gives them without their `dyn_` prefix.
+DB18_NOMINAL = dict(u1=5.0, u2=0.0, u3=0.0, w1=4.0, w2=0.0, w3=0.0, uar=1.5, ual=1.5, war=15.0, wal=15.0, delay=0.15)
+
+
+def delay_steps(delay: float, dt: float) -> int:
+    """Integration steps a command waits before it acts: the fewest whose span reaches `delay` (dts_create /
+    dts_set_timing, the same expression in the same float64 arithmetic)."""
+    d = 0
+    while d * dt < delay - 1e-12:
+        d += 1
+    return d
+
+
+def dyn_params(dt=1.0 / 30, trim=0.0, **model) -> OrcDynParams:
+    """OrcDynParams of the model `DB18_NOMINAL` updated with `model` (any of its keys), stepped at `dt`, with the
+    per-env `trim` folded into the gains as the device folds it in (get_DB18_uncalibrated: right gains * (1 + trim),
+    left gains * (1 - trim)).  A delay longer than the delay line can hold is refused, as dts_create refuses it."""
+    unknown = set(model) - set(DB18_NOMINAL)
+    if unknown:
+        raise TypeError(f"unknown dynamics constants {sorted(unknown)}")
+    p = dict(DB18_NOMINAL, **model)
+    d = delay_steps(p["delay"], dt)
+    if d > ORC_MAX_DELAY:
+        raise ValueError(f"a delay of {p['delay']} s is {d} steps of {dt} s: the delay line holds {ORC_MAX_DELAY}")
+    return OrcDynParams(p["u1"], p["u2"], p["u3"], p["w1"], p["w2"], p["w3"], p["uar"] * (1.0 + trim),
+                        p["ual"] * (1.0 - trim), p["war"] * (1.0 + trim), p["wal"] * (1.0 - trim), d)
+
+
 def default_dyn_params(dt=1.0 / 30, delay=0.15, trim=0.0) -> OrcDynParams:
     """get_DB18_nominal / get_DB18_uncalibrated as restated in DESIGN.md (parity unpinned)."""
-    d = int(np.ceil(delay / dt - 1e-9)) if delay > 0 else 0
-    return OrcDynParams(5.0, 0.0, 0.0, 4.0, 0.0, 0.0, 1.5 * (1 + trim), 1.5 * (1 - trim), 15.0 * (1 + trim),
-                        15.0 * (1 - trim), d)
+    return dyn_params(dt, trim, delay=delay)
 
 
 class OracleEnv:
@@ -123,10 +153,12 @@ class OracleEnv:
 
     def __init__(self, omap: OracleMap, px, pz, angle, *, wheel_dist=0.102, action_mode=1, max_steps=1500,
                  frame_skip=1, dt=1.0 / 30, robot_speed=1.2, env5=(1.0, 0.0, 0.0318, 27.0, 1.0), trim=0.0,
-                 dynamics=None):
+                 dynamics=None, model=None):
+        """model: the wheel model's constants and command delay, any keys of DB18_NOMINAL (the dts_config fields
+        dyn_u1 ... dyn_wal, dyn_delay); the others keep their nominal values."""
         self.m = omap
         self.dynamics = dynamics          # OracleDynamics: this env's moving obstacles (stepped with the agent)
-        self.dp = default_dyn_params(dt, 0.15, trim)
+        self.dp = dyn_params(dt, trim, **(model or {}))
         self.s = OrcDynState()
         lib().orc_cartesian_from_weird(C.byref(omap.c), C.c_double(px), C.c_double(pz), C.c_double(angle), C.byref(self.s))
         self.step_count = C.c_int(0)
