@@ -4,7 +4,7 @@
 observation buffers are caller-visible torch CUDA tensors, the work runs on
 `torch.cuda.current_stream()` inside libdtsim.so, nothing synchronises.  Constructor keywords are the
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
-`auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `camera_rand_pool`.
+`auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `camera_rand_pool` and the `bev*` keywords.
 
 `camera_rand=True` (with `distortion=True`; without it the flag does nothing, as in the reference, S:352-358) gives the
 envs a spread of lenses: `camera_rand_pool` calibrations K, D are drawn once, at construction, within the reference's
@@ -42,6 +42,18 @@ lane paint each pixel shows (dts_set_marking_target), named by MARKING_NAMES —
 fisheye source), 1 a road tile's unpainted surface, 2 white, 3 yellow, 4 red — the class of the texel its label winner
 samples at the pixel centre.  It needs no label image and follows the render modes, sizes and auto-reset as labels do;
 lighting, domain randomisation and `segment` leave it unchanged.
+
+`bev=True` allocates `env.bev_labels`, int16, and `env.bev_markings`, uint8, both [num_envs, height, width] for
+`bev_shape=(height, width)`: a bird's-eye grid fixed to each agent (dts_set_bev_target), sampled from the map rather than
+rendered.  Row 0 is the farthest ahead and column 0 the leftmost, so it reads like an image of the ground seen from
+above with the agent facing up; a cell is `bev_cell` metres, and the agent sits at `bev_origin=(x, y)` in cells, by
+default (width / 2, 3 * height / 4): 1.44 m ahead and 0.48 m behind at the defaults.  A cell's label uses the label
+image's numbering (`label_table`): the first object whose footprint holds the cell centre (hidden optional objects
+skipped, moving obstacles where they are now), else the road tile under it, else 1, the ground; its marking is the
+MARKING_NAMES class of the texel under it, 0 off the tiles, objects or not.  Every `step` writes them, with
+`render=False` too (under `auto_reset`, an ended env's row is its next episode's first state, as in `obs`), and so
+does every render; `render_bev()` writes them alone, e.g. after `reset(render=False)`, `load_state` or `copy_envs`.
+They do not depend on the camera, the render modes, sizes or formats, and snapshots and gathers do not carry them.
 """
 from __future__ import annotations
 
@@ -81,7 +93,8 @@ class BatchedDuckietownEnv:
                  action_mode: str = "vel_steer", auto_reset: bool = False, device_reset: bool = False,
                  cycle_maps: bool = False, env_id_offset: int = 0, tessellate_tiles: bool = False,
                  randomize_maps_on_reset: bool = False, randomization_config=None, terminal_obs: bool = False,
-                 depth: bool = False, labels: bool = False, camera_rand_pool: int = 16, markings: bool = False):
+                 depth: bool = False, labels: bool = False, camera_rand_pool: int = 16, markings: bool = False,
+                 bev: bool = False, bev_shape=(64, 64), bev_cell: float = 0.03, bev_origin=None):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
         camera_rand = bool(camera_rand and distortion)   # S:353-356: camera_rand only with distortion
@@ -151,6 +164,12 @@ class BatchedDuckietownEnv:
             # the lane-marking image of the frames in obs (markings=True); the renders write it on the device
             self.markings: Optional[torch.Tensor] = torch.zeros(
                 (num_envs, camera_height, camera_width), dtype=torch.uint8, device=self.device) if markings else None
+            # the bird's-eye grids (bev=True); every step and render writes them on the device
+            bh, bw = (int(v) for v in bev_shape)
+            self.bev_labels: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, bh, bw), dtype=torch.int16, device=self.device) if bev else None
+            self.bev_markings: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, bh, bw), dtype=torch.uint8, device=self.device) if bev else None
             self.reward = torch.zeros(num_envs, dtype=torch.float32, device=self.device)
             self._done_u8 = torch.zeros(num_envs, dtype=torch.uint8, device=self.device)
             self.state: Dict[str, torch.Tensor] = {
@@ -174,6 +193,10 @@ class BatchedDuckietownEnv:
             self.sim.set_label_target(self.labels.data_ptr())
         if markings:
             self.sim.set_marking_target(self.markings.data_ptr())
+        if bev:
+            ox, oy = (bw / 2, 3 * bh / 4) if bev_origin is None else (float(v) for v in bev_origin)
+            self.bev_config = L.BevConfig(bw, bh, float(bev_cell), float(ox), float(oy))
+            self.sim.set_bev_target(self.bev_config, self.bev_labels.data_ptr(), self.bev_markings.data_ptr())
         self.seed(seed)
 
     def set_output_format(self, obs_layout: Optional[str] = None, obs_dtype: Optional[str] = None,
@@ -347,6 +370,13 @@ class BatchedDuckietownEnv:
         else:
             self.sim.render(tgt.data_ptr(), self._stream())
         return tgt
+
+    def render_bev(self):
+        """Write `bev_labels` / `bev_markings` for the current state (dts_render_bev), without rendering a frame."""
+        if self.bev_labels is None:
+            raise ValueError("render_bev needs bev=True")
+        self.sim.render_bev(self._stream())
+        return self.bev_labels, self.bev_markings
 
     # labels -------------------------------------------------------------------------------------
     def label_table(self, map_id: int = 0) -> list:

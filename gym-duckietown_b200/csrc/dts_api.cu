@@ -1,5 +1,6 @@
 // dts_api.cu — the C ABI of libdtsim.so (include/dtsim.h): handle management, host->device
 // staging of episode parameters, and stream-ordered launches of the kernels.
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -43,6 +44,7 @@ struct dts_sim {
   bool gather_next = false;
   int render_mode = 0;                  // dts_set_render_mode             // the next dts_render also stores into the gather buffers
   AuxTargets aux{};                     // dts_set_{depth,label,marking}_target: caller-owned images, or null
+  BevTarget bev{};                      // dts_set_bev_target: caller-owned grids, both null = off
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
   int profiling = 0;                    // 0 off, 1 events around k_raster only, 2 around every render kernel
   std::vector<cudaEvent_t> prof_events; // kProfMarks events per profiled frame
@@ -191,7 +193,7 @@ static long long largest_label(long long n_cells, long long n_objects) { return 
 
 int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
   if (!sim) return 1;
-  if (sim->aux.labels && b && largest_label((long long)b->grid_w * b->grid_h, b->n_objects) > INT16_MAX)
+  if ((sim->aux.labels || sim->bev.labels) && b && largest_label((long long)b->grid_w * b->grid_h, b->n_objects) > INT16_MAX)
     return sim->fail("a label target is set and this map's largest label, %lld, does not fit in int16",
                      largest_label((long long)b->grid_w * b->grid_h, b->n_objects));
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
@@ -376,9 +378,27 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
   return 0;
 }
 
+// The bird's-eye grids of every env's current state, where a target is set (dts_set_bev_target)
+static int bev_pass(dts_sim* sim, void* stream) {
+  if (!sim->bev.labels && !sim->bev.marks) return 0;
+  if (check_maps(sim)) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  launch_bev(state_arrays(*sim->state), maps_table(*sim->maps), sim->bev, (cudaStream_t)stream);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  return 0;
+}
+
 int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
   if (!sim) return 1;
-  return render_pass(sim, obs_dev, stream, nullptr, nullptr);
+  if (render_pass(sim, obs_dev, stream, nullptr, nullptr)) return 1;
+  return bev_pass(sim, stream);
+}
+
+int dts_render_bev(dts_sim* sim, void* stream) {
+  if (!sim) return 1;
+  if (!sim->bev.labels && !sim->bev.marks) return sim->fail("no bird's-eye target is set (dts_set_bev_target)");
+  return bev_pass(sim, stream);
 }
 
 int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, void* terminal_obs_dev, float* reward_dev,
@@ -408,6 +428,8 @@ int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, voi
                        sim->n_ended, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
+  // the grids of the state obs_dev will show: the ended envs' first states (every env's row, as the others did not move)
+  if (bev_pass(sim, stream)) return 1;
   if (!obs_dev) return 0;
   // 4. their terminal frames -> terminal_obs_dev; 5. their first frames -> obs_dev
   const ResizeTarget rz = resizer_target(*sim->resize);
@@ -431,7 +453,8 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
                     (cudaStream_t)stream);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
-  if (obs_dev) return dts_render(sim, obs_dev, stream);
+  if (bev_pass(sim, stream)) return 1;
+  if (obs_dev) return render_pass(sim, obs_dev, stream, nullptr, nullptr);
   return 0;
 }
 
@@ -582,17 +605,39 @@ int dts_set_depth_target(dts_sim* sim, float* depth_dev) {
   return 0;
 }
 
+// Every uploaded map's labels fit in int16, as a label target needs
+static int check_labels_fit(dts_sim* sim) {
+  const std::vector<MapCounts>& counts = maps_counts(*sim->maps);
+  for (size_t s = 0; s < counts.size(); s++)
+    if (counts[s].n_tiles && largest_label(counts[s].n_tiles, counts[s].n_objects) > INT16_MAX)
+      return sim->fail("map slot %zu's largest label, %lld, does not fit in int16", s,
+                       largest_label(counts[s].n_tiles, counts[s].n_objects));
+  return 0;
+}
+
 int dts_set_label_target(dts_sim* sim, int16_t* labels_dev) {
   if (!sim) return 1;
   if (reinterpret_cast<uintptr_t>(labels_dev) & 1) return sim->fail("label target is not aligned to 2 bytes");
-  if (labels_dev) {
-    const std::vector<MapCounts>& counts = maps_counts(*sim->maps);
-    for (size_t s = 0; s < counts.size(); s++)
-      if (counts[s].n_tiles && largest_label(counts[s].n_tiles, counts[s].n_objects) > INT16_MAX)
-        return sim->fail("map slot %zu's largest label, %lld, does not fit in int16", s,
-                         largest_label(counts[s].n_tiles, counts[s].n_objects));
-  }
+  if (labels_dev && check_labels_fit(sim)) return 1;
   sim->aux.labels = labels_dev;
+  return 0;
+}
+
+int dts_set_bev_target(dts_sim* sim, const dts_bev_config* cfg, int16_t* labels_dev, uint8_t* markings_dev) {
+  if (!sim) return 1;
+  if (!cfg || (!labels_dev && !markings_dev)) {
+    sim->bev = BevTarget{};
+    return 0;
+  }
+  if (cfg->width < 1 || cfg->width > 2048 || cfg->height < 1 || cfg->height > 2048)
+    return sim->fail("bird's-eye grid of %d x %d cells: 1 to 2048 per side are accepted", cfg->width, cfg->height);
+  if (!std::isfinite(cfg->cell) || !(cfg->cell > 0))
+    return sim->fail("bird's-eye cell size %g: a finite size > 0 is needed", cfg->cell);
+  if (!std::isfinite(cfg->origin_x) || !std::isfinite(cfg->origin_y))
+    return sim->fail("bird's-eye origin (%g, %g) is not finite", cfg->origin_x, cfg->origin_y);
+  if (reinterpret_cast<uintptr_t>(labels_dev) & 1) return sim->fail("bird's-eye label target is not aligned to 2 bytes");
+  if (labels_dev && check_labels_fit(sim)) return 1;
+  sim->bev = BevTarget{*cfg, labels_dev, markings_dev};
   return 0;
 }
 

@@ -1,0 +1,173 @@
+// dts_bev.cu — the bird's-eye map (dts_set_bev_target, DESIGN.md section 5 item 12): a grid of cells fixed to every
+// agent, each point-sampled from the map's own tables at its centre — the tile under it, the class of the texel under it
+// and the first object whose footprint holds it.  No rasteriser: a thread per cell, float64 in the order the spec states
+// (-fmad=false keeps every product and sum separately rounded, as numpy's are).
+#include "dts_kernels.h"
+
+namespace dts {
+namespace {
+
+constexpr int kBevThreads = 256;
+constexpr int kBevCellsPerThread = 4;   // cells per CTA = 1024: a 64 x 64 grid is four CTAs per env
+constexpr int kBevCellsPerCta = kBevThreads * kBevCellsPerThread;
+
+struct BevFootprint { double x[4], z[4]; };
+
+// (b - a) x (p - a)
+__device__ __forceinline__ double edge_cross(double ax, double az, double bx, double bz, double px, double pz) {
+  return (bx - ax) * (pz - az) - (bz - az) * (px - ax);
+}
+
+// the four cross products (c[k+1] - c[k]) x (p - c[k]) all >= 0 or all <= 0
+__device__ __forceinline__ bool footprint_holds(const BevFootprint& q, double px, double pz) {
+  bool pos = true, neg = true;
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    const int n = (k + 1) & 3;
+    const double c = edge_cross(q.x[k], q.z[k], q.x[n], q.z[n], px, pz);
+    pos &= c >= 0.0;
+    neg &= c <= 0.0;
+  }
+  return pos || neg;
+}
+
+// A strictly convex quad holds exactly its own closed area, up to the rounding of the cross products, so none of its
+// points lies outside the corners' box widened by `margin`: cells and objects outside it are skipped without changing
+// the result.  Any other quad (degenerate: its rule can hold points outside it) gets an unbounded box.
+__device__ __forceinline__ void footprint_box(const BevFootprint& q, double box[4]) {
+  bool pos = true, neg = true;
+  double x0 = q.x[0], x1 = q.x[0], z0 = q.z[0], z1 = q.z[0];
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    const int n = (k + 1) & 3, n2 = (k + 2) & 3;
+    const double t = edge_cross(q.x[k], q.z[k], q.x[n], q.z[n], q.x[n2], q.z[n2]);
+    pos &= t > 0.0;
+    neg &= t < 0.0;
+    x0 = fmin(x0, q.x[k]); x1 = fmax(x1, q.x[k]);
+    z0 = fmin(z0, q.z[k]); z1 = fmax(z1, q.z[k]);
+  }
+  const double margin = 1e-9 * (1.0 + fmax(fmax(fabs(x0), fabs(x1)), fmax(fabs(z0), fabs(z1))));
+  const bool bounded = pos || neg;
+  box[0] = bounded ? x0 - margin : -INFINITY; box[1] = bounded ? x1 + margin : INFINITY;
+  box[2] = bounded ? z0 - margin : -INFINITY; box[3] = bounded ? z1 + margin : INFINITY;
+}
+
+// Can a footprint with this box hold a point of the disc (wx, wz, wr)?  (The disc's own rounding is covered by a margin.)
+__device__ __forceinline__ bool box_meets(const double box[4], double wx, double wz, double wr) {
+  const double m = wr + 1e-9 * (1.0 + fabs(wx) + fabs(wz) + wr);
+  return box[0] <= wx + m && box[1] >= wx - m && box[2] <= wz + m && box[3] >= wz - m;
+}
+
+// grid (env, chunk of kBevCellsPerCta cells), one thread per cell of the chunk at a time, rows stored contiguously
+__global__ void __launch_bounds__(kBevThreads) k_bev(DState S, const DMap* __restrict__ maps, BevTarget b) {
+  __shared__ BevFootprint foot[DTS_MAX_OBJECTS];   // the objects whose footprint can meet the window, in index order
+  __shared__ double foot_box[DTS_MAX_OBJECTS][4];   // x0 x1 z0 z1 outside which the footprint holds no point
+  __shared__ int16_t foot_obj[DTS_MAX_OBJECTS];     // (room for every object a map may have: no fallback is needed)
+  __shared__ int n_foot;
+  __shared__ double pose[4];                        // pos_x, pos_z, cos, sin of the env's angle
+  const int env = blockIdx.x;
+  const DMap& m = maps[S.map_id[env]];
+  const dts_bev_config g = b.cfg;
+  if (threadIdx.x < 32) {
+    const int lane = threadIdx.x;
+    const double px = S.pos_x[env], pz = S.pos_z[env];
+    double sa, ca;
+    sincos(S.angle[env], &sa, &ca);
+    if (lane == 0) { pose[0] = px; pose[1] = pz; pose[2] = ca; pose[3] = sa; }
+    int count = 0;
+    if (b.labels) {
+      // the window's bounding disc: the grid's middle, half its diagonal
+      const double fc = (g.origin_y - 0.5 * g.height) * g.cell, lc = (0.5 * g.width - g.origin_x) * g.cell;
+      const double wx = px + fc * ca + lc * sa, wz = pz - fc * sa + lc * ca;
+      const double wr = 0.5 * g.cell * sqrt((double)g.width * g.width + (double)g.height * g.height);
+      const uint32_t* hidden = S.rep[env].hidden;
+      const size_t nd = m.n_dyn, ne = S.n;
+      for (int base = 0; base < m.n_objects; base += 32) {
+        const int o = base + lane;
+        BevFootprint q;
+        double box[4];
+        bool keep = false;
+        if (o < m.n_objects && !(hidden[o >> 5] >> (o & 31) & 1u)) {
+          const int slot = m.objects[o].dyn_slot;
+          if (slot >= 0) {   // this env's copy of the obstacle's corners
+            for (int k = 0; k < 4; k++) {
+              q.x[k] = m.dyn_state[((size_t)(DTS_DYN_CORNERS + 2 * k) * nd + slot) * ne + env];
+              q.z[k] = m.dyn_state[((size_t)(DTS_DYN_CORNERS + 2 * k + 1) * nd + slot) * ne + env];
+            }
+            keep = true;
+          } else if (m.obj_corners) {
+            for (int k = 0; k < 4; k++) {
+              q.x[k] = __ldg(m.obj_corners + (size_t)o * 8 + 2 * k);
+              q.z[k] = __ldg(m.obj_corners + (size_t)o * 8 + 2 * k + 1);
+            }
+            keep = true;
+          }
+          if (keep) footprint_box(q, box);
+          keep = keep && box_meets(box, wx, wz, wr);
+        }
+        const unsigned ball = __ballot_sync(0xffffffffu, keep);
+        if (keep) {
+          const int at = count + __popc(ball & ((1u << lane) - 1u));
+          foot[at] = q;
+          for (int k = 0; k < 4; k++) foot_box[at][k] = box[k];
+          foot_obj[at] = (int16_t)o;
+        }
+        count += __popc(ball);
+      }
+    }
+    if (lane == 0) n_foot = count;
+  }
+  __syncthreads();
+  const double px = pose[0], pz = pose[1], ca = pose[2], sa = pose[3];
+  const double ts = m.tile_size;
+  const int gw = m.grid_w, gh = m.grid_h, n_foot_env = n_foot;
+  const int n_cells = g.width * g.height;
+  const size_t row = (size_t)env * n_cells;
+  const uint8_t* cls_pool = m.tex_pool + m.tex_class_off;
+  for (int k = 0; k < kBevCellsPerThread; k++) {
+    const int t = blockIdx.y * kBevCellsPerCta + k * kBevThreads + threadIdx.x;
+    if (t >= n_cells) break;
+    const int r = t / g.width, c = t - r * g.width;
+    const double f = (g.origin_y - (r + 0.5)) * g.cell, l = ((c + 0.5) - g.origin_x) * g.cell;
+    const double x = px + f * ca + l * sa, z = pz - f * sa + l * ca;
+    int label = 1, mark = 0;
+    const double fi = floor(x / ts), fj = floor(z / ts);   // get_grid_coords S:1134, compared before any int conversion
+    if (fi >= 0.0 && fi < gw && fj >= 0.0 && fj < gh) {
+      const int i = (int)fi, j = (int)fj, idx = j * gw + i;
+      if (__ldg(m.tile_kind + idx) >= 0) {
+        label = 2 + i * gh + j;
+        const int tex = __ldg(m.tile_tex + idx);
+        if (b.marks && tex >= 0) {
+          // tile-local point: T((i + .5) ts, 0, (j + .5) ts) Ry(angle * 90 + 180) inverted, its cos / sin exact 0 / +-1
+          const double lx = x - (i + 0.5) * ts, lz = z - (j + 0.5) * ts;
+          const int q = (__ldg(m.tile_angle + idx) + 2) & 3;
+          const double ax = q == 0 ? lx : q == 1 ? -lz : q == 2 ? -lx : lz;
+          const double az = q == 0 ? lz : q == 1 ? lx : q == 2 ? -lz : -lx;
+          const double u = (ax + 0.5 * ts) / ts, v = 1.0 - (az + 0.5 * ts) / ts;   // _init_vlists S:394-401
+          const int tw = __ldg(&m.textures[tex].w), th = __ldg(&m.textures[tex].h);
+          const uint32_t info = __ldg(&m.textures[tex].info);
+          const int tu = (int)floor(u * tw) & (tw - 1), tv = (int)floor(v * th) & (th - 1);   // power-of-two sides
+          mark = __ldg(cls_pool + ((size_t)(info & 0xffffffu) << 6) + (size_t)tv * tw + tu);
+        }
+      }
+    }
+    if (b.labels) {
+      for (int s = 0; s < n_foot_env; s++) {
+        if (x < foot_box[s][0] || x > foot_box[s][1] || z < foot_box[s][2] || z > foot_box[s][3]) continue;
+        if (footprint_holds(foot[s], x, z)) { label = 2 + m.n_tiles + foot_obj[s]; break; }
+      }
+      b.labels[row + t] = (int16_t)label;
+    }
+    if (b.marks) b.marks[row + t] = (uint8_t)mark;
+  }
+}
+
+}  // namespace
+
+void launch_bev(const DState& S, const DMap* maps, const BevTarget& b, cudaStream_t st) {
+  const int n_cells = b.cfg.width * b.cfg.height;
+  const dim3 grid(S.n, (n_cells + kBevCellsPerCta - 1) / kBevCellsPerCta);
+  k_bev<<<grid, kBevThreads, 0, st>>>(S, maps, b);
+}
+
+}  // namespace dts

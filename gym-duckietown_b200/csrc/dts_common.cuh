@@ -86,6 +86,7 @@ struct DMap {
   double* dyn_state;            // [DTS_DYN_FIELDS][n_dyn][num_envs]: mutable, per env, survives resets
   const double* dyn_init;       // [DTS_DYN_FIELDS][n_dyn] load-time values (a map reload re-creates the obstacles)
   int32_t valid;
+  const double* obj_corners;    // [n_objects][4][2] footprints (x, z) of the bird's-eye map; null: the blob had none
 };
 
 // One env's view of its map's dynamic obstacles.

@@ -152,4 +152,13 @@ void launch_copy_rows(const void* src, void* dst, size_t row_bytes, const int32_
                       cudaStream_t st);
 void launch_blend4(const uint8_t* const f[4], const double w[4], double* out, size_t n, cudaStream_t st);
 
+// bird's-eye map (dts_bev.cu): the grid of dts_set_bev_target and its outputs, each [n_envs][height][width] or null
+struct BevTarget {
+  dts_bev_config cfg;
+  int16_t* labels;
+  uint8_t* marks;
+};
+// every env's grid of its current state, one launch
+void launch_bev(const DState& S, const DMap* maps, const BevTarget& b, cudaStream_t st);
+
 }  // namespace dts

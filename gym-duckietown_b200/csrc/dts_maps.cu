@@ -1,5 +1,6 @@
 // dts_maps.cu — the map slots of one handle (dts_upload_map): a dts_map_blob checked, built into a DMap on the host and
 // copied to the device, and the device table of every slot's DMap that the kernels index by S.map_id.
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -111,6 +112,7 @@ static uint64_t blob_hash(const dts_map_blob& b) {
     for (int t = 0; t < b.n_textures; t++) texels += (size_t)b.textures[t].width * b.textures[t].height;
     H.arr(b.tex_class, texels);
   }
+  if (b.obj_corners) H.arr(b.obj_corners, (size_t)b.n_objects * 8);   // (likewise for footprints)
   H.val(b.start_tile[0]); H.val(b.start_tile[1]); H.val(b.has_start_pose);
   for (int k = 0; k < 3; k++) H.val(b.start_pose[k]);
   H.val(b.agent_mesh);
@@ -142,6 +144,8 @@ static std::string validate(const dts_map_blob* b, int slot, int n_slots) {
     if (s.mesh_id < 0 || s.mesh_id >= b->n_meshes) return format("object %d: bad mesh_id", o);
     if (s.alt_tex_to >= b->n_textures || s.alt_tex_from >= b->n_textures) return format("object %d: alt texture out of range", o);
     if (s.dyn_slot >= b->n_dyn) return format("object %d: dyn_slot %d out of range", o, s.dyn_slot);
+    for (int k = 0; b->obj_corners && k < 8; k++)
+      if (!std::isfinite(b->obj_corners[(size_t)o * 8 + k])) return format("object %d: footprint corner is not finite", o);
   }
   // the bounding spheres are computed from tri_pos on the host
   for (int i = 0; i < b->n_meshes; i++) {
@@ -340,6 +344,7 @@ std::string maps_upload(MapSlots& ms, int slot, const dts_map_blob* blob) {
   put(m.dyn, par.data(), par.size());
   put(m.dyn_state, st.data(), st.size());
   put(m.dyn_init, init.data(), init.size());
+  if (b.obj_corners) put(m.obj_corners, b.obj_corners, (size_t)b.n_objects * 8);
   m.valid = 1;
   // 3. once no kernel still reads the slot's old map: the table entry, the host record, and the old map's memory
   if (err.empty()) {

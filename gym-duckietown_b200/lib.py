@@ -115,7 +115,14 @@ class MapBlob(C.Structure):
         ("textures", C.c_void_p), ("start_tile", C.c_int32 * 2), ("n_dyn", C.c_int32), ("has_start_pose", C.c_int32),
         ("dyn", C.c_void_p), ("start_pose", C.c_double * 3),
         ("tex_segment", C.c_void_p), ("agent_mesh", C.c_int32), ("reserved2", C.c_int32), ("tex_class", C.c_void_p),
+        ("obj_corners", C.c_void_p),
     ]
+
+
+class BevConfig(C.Structure):
+    """dts_bev_config: the bird's-eye grid (cells, metres per cell, the agent's position in cells)"""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("cell", C.c_double), ("origin_x", C.c_double),
+                ("origin_y", C.c_double)]
 
 
 # dts_episode_params, in its order: (member, dtype, values per env)
@@ -187,6 +194,8 @@ def load() -> C.CDLL:
     lib.dts_set_depth_target.argtypes = [vp, vp]
     lib.dts_set_label_target.argtypes = [vp, vp]
     lib.dts_set_marking_target.argtypes = [vp, vp]
+    lib.dts_set_bev_target.argtypes = [vp, C.POINTER(BevConfig), vp, vp]
+    lib.dts_render_bev.argtypes = [vp, vp]
     lib.dts_resize_frames.argtypes = [vp, vp, vp, vp]
     lib.dts_blend4.argtypes = [vp, vp, vp, vp, C.c_uint64, vp]
     lib.dts_set_timing.argtypes = [vp, C.c_double, i, i]
@@ -221,7 +230,7 @@ def load() -> C.CDLL:
 
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_fisheye_luts", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
-           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
+           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
            "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
 
@@ -323,6 +332,9 @@ class MapBlobHolder:
                 setattr(c, n, float(getattr(d, n)))
             c.freq, c.pattern = float(d.freq), int(d.pattern)
         k["dyn"] = dyn
+        # every object's footprint (obj_corners, computed for collidable and non-collidable objects alike)
+        k["obj_corners"] = np.ascontiguousarray(np.reshape([o.corners for o in md.objects], (len(md.objects), 4, 2))
+                                                if md.objects else np.zeros((1, 4, 2)), np.float64)
         texs = (Texture * max(1, len(tex_imgs)))()
         for ti, im in enumerate(tex_imgs):
             texs[ti] = Texture(im.shape[1], im.shape[0], im.ctypes.data)
@@ -338,7 +350,7 @@ class MapBlobHolder:
             len(md.dyn_objects), int(md.start_pose is not None), C.cast(dyn, C.c_void_p),
             (C.c_double * 3)(*((float(md.start_pose[0][0]), float(md.start_pose[0][2]), float(md.start_pose[1]))
                                if md.start_pose is not None else (0.0, 0.0, 0.0))),
-            _ptr(k["seg"]), agent_mesh, 0, _ptr(k["tex_class"]))
+            _ptr(k["seg"]), agent_mesh, 0, _ptr(k["tex_class"]), _ptr(k["obj_corners"]))
         self.agent_mesh, self.n_tile_tex = agent_mesh, n_tile_tex
 
 
@@ -493,6 +505,17 @@ class Sim:
         """Every later render also writes int16 [num_envs, cam_height, cam_width] labels (which draw item each pixel
         shows) at `labels_ptr`, which the caller keeps alive; None turns it off (dts_set_label_target)."""
         self._check(self.lib.dts_set_label_target(self.h, labels_ptr), "dts_set_label_target")
+
+    def set_bev_target(self, cfg: Optional[BevConfig], labels_ptr: Optional[int], markings_ptr: Optional[int]):
+        """Write the bird's-eye grids of cfg (int16 labels / uint8 markings [num_envs][cfg.height][cfg.width], at
+        caller-kept device pointers) on every later step and render; None for both, or cfg None, turns it off
+        (dts_set_bev_target)."""
+        self._check(self.lib.dts_set_bev_target(self.h, None if cfg is None else C.byref(cfg), labels_ptr, markings_ptr),
+                    "dts_set_bev_target")
+
+    def render_bev(self, stream: int = 0):
+        """The bird's-eye grids of the current state (dts_render_bev)."""
+        self._check(self.lib.dts_render_bev(self.h, stream), "dts_render_bev")
 
     def set_resize(self, out_w: int, out_h: int, filter: int = 0):
         """filter RESIZE_CV2_CUBIC (dts_set_resize) or RESIZE_PIL_BILINEAR (dts_set_resize_filter)."""

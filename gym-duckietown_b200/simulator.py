@@ -71,7 +71,7 @@ class Simulator(Env):
                  camera_rand: bool = False, randomize_maps_on_reset: bool = False, num_tris_distractors: int = 12,
                  color_ground=(0.15, 0.15, 0.15), color_sky=(0.45, 0.82, 1), style: str = "photos",
                  enable_leds: bool = False, device: int = 0, depth: bool = False, labels: bool = False,
-                 markings: bool = False, **env_kwargs):
+                 markings: bool = False, bev: bool = False, **env_kwargs):
         if draw_curve or draw_bbox or enable_leds:
             raise NotImplementedError("draw_curve / draw_bbox / enable_leds are debug modes outside the hot path "
                                       "(SURVEY 8f-4)")
@@ -97,7 +97,7 @@ class Simulator(Env):
             distortion=distortion, dynamics_rand=dynamics_rand, camera_rand=camera_rand,
             camera_rand_pool=env_kwargs.pop("camera_rand_pool", 1),   # one camera per Simulator (distortion.py:46-47)
             color_ground=color_ground, color_sky=color_sky, num_tris_distractors=num_tris_distractors,
-            action_mode=self._action_mode, depth=depth, labels=labels, markings=markings, **env_kwargs)
+            action_mode=self._action_mode, depth=depth, labels=labels, markings=markings, bev=bev, **env_kwargs)
         self._b = BatchedDuckietownEnv(1, map_arg, **self._env_kwargs)
         self._adopt_map()
         self.action_space = spaces.Box(low=-1, high=1, shape=(2,), dtype=np.float32)              # S:309
@@ -159,7 +159,7 @@ class Simulator(Env):
         from .batched_env import BatchedDuckietownEnv
         if getattr(self, "_human", None) is None:
             kw = dict(self._env_kwargs, camera_width=WINDOW_WIDTH, camera_height=WINDOW_HEIGHT, distortion=False,
-                      terminal_obs=False, depth=False, labels=False, markings=False)
+                      terminal_obs=False, depth=False, labels=False, markings=False, bev=False)
             self._human = BatchedDuckietownEnv(1, list(self._b.maps), **kw)
         self._human.load_state(self._b.save_state())
         return self._human
@@ -217,6 +217,21 @@ class Simulator(Env):
         returned by reset / step / render_obs (BatchedDuckietownEnv.markings, named by MARKING_NAMES); else None."""
         mk = self._b.markings
         return None if mk is None else mk[0].cpu().numpy()
+
+    @property
+    def bev_labels(self) -> Optional[np.ndarray]:
+        """With bev=True: int16 [height, width], the bird's-eye label grid around the agent in the state last returned by
+        reset / step / render_obs (BatchedDuckietownEnv.bev_labels, named by BatchedDuckietownEnv.label_table); else
+        None.  `bev_shape`, `bev_cell` and `bev_origin` pass through to the batched env."""
+        g = self._b.bev_labels
+        return None if g is None else g[0].cpu().numpy()
+
+    @property
+    def bev_markings(self) -> Optional[np.ndarray]:
+        """With bev=True: uint8 [height, width], the lane paint under each cell of the bird's-eye grid
+        (BatchedDuckietownEnv.bev_markings, named by MARKING_NAMES); else None."""
+        g = self._b.bev_markings
+        return None if g is None else g[0].cpu().numpy()
 
     @property
     def cur_pos(self):

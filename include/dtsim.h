@@ -197,6 +197,10 @@ typedef struct {
   int32_t reserved2;
   const uint8_t* tex_class;       /* texel classes of every texture in texture order, width*height each (row 0 = t=0, as
                                      rgba), values of dts_set_marking_target; NULL = all 0 */
+  const double* obj_corners;      /* [n_objects][4][2] (x, z): every object's footprint obj_corners (generate_corners
+                                     C:64-79, O:60, computed for every object S:885), for dts_set_bev_target; finite.
+                                     Objects with a dyn_slot take their env's DTS_DYN_CORNERS instead.  NULL = static
+                                     objects have no footprint in the bird's-eye map */
 } dts_map_blob;
 
 /* Per-episode inputs produced by Simulator.reset() (simulator.py:528-763, SURVEY 8a row P0), one
@@ -288,7 +292,7 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
  * (the respawn, state and draws bit for bit those of dts_step, and a device list of the ended envs), k_copy_rows (their
  * rows -> terminal_obs_dev) and a second render into obs_dev over the listed envs only, whose kernels exit at once when
  * nothing ended.  Launches: 2 R + 3, R being dts_render's (5, or 7 when the rasteriser writes packed u8 HWC of a width divisible by 4, +1
- * with a resize), plus a 4-byte memset; obs_dev = NULL (no render): 2.  Fails without DTS_FLAG_AUTO_RESET, with
+ * with a resize), plus a 4-byte memset; obs_dev = NULL (no render): 2; one more with a bird's-eye target (dts_set_bev_target).  Fails without DTS_FLAG_AUTO_RESET, with
  * terminal_obs_dev == obs_dev, and while a fused gather is armed (dts_gather_next), which it does not write.  The
  * second pass is not timed by dts_profile_*.  Never synchronises. */
 int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, void* terminal_obs_dev, float* reward_dev,
@@ -350,6 +354,39 @@ int dts_set_label_target(dts_sim* sim, int16_t* labels_dev);
  * (the second pass of dts_step_terminal) writes only those envs' rows; the terminal frames' markings are not kept.  The
  * fused gather (dts_gather_next) carries observations only. */
 int dts_set_marking_target(dts_sim* sim, uint8_t* markings_dev);
+/* Bird's-eye map around every agent (DESIGN.md section 5, item 12): a grid of `height` x `width` cells fixed to the
+ * agent, sampled from the map itself rather than rendered.  Row 0 is the farthest ahead and column 0 the leftmost, so
+ * the grid reads like an image of the ground seen from above with the agent facing up.  The agent sits at (origin_x,
+ * origin_y), in cells, and a cell is `cell` metres on a side.  In float64: with ca, sa = cos, sin of the env's angle,
+ * cell (r, c) has f = (origin_y - (r + 0.5)) * cell, l = ((c + 0.5) - origin_x) * cell and its centre at
+ * x = pos_x + f * ca + l * sa, z = pos_z - f * sa + l * ca (get_dir_vec, get_right_vec S:2056-2073). */
+typedef struct {
+  int32_t width, height;    /* cells, 1 to 2048 each */
+  double cell;              /* metres per cell, finite and > 0 */
+  double origin_x, origin_y;/* the agent's position in grid coordinates (cells), finite */
+} dts_bev_config;
+/* Sets the bird's-eye targets: labels_dev int16 [num_envs][height][width] (2-byte aligned) and markings_dev uint8
+ * [num_envs][height][width], either of them NULL.  A cell's label uses the numbering of dts_set_label_target: 2 + n_cells
+ * + o for the smallest object index o whose footprint (dts_map_blob.obj_corners, or the env's DTS_DYN_CORNERS for an
+ * object with a dyn_slot) contains the cell centre, the four cross products (c[k+1] - c[k]) x (p - c[k]) all >= 0 or
+ * all <= 0, objects hidden this episode skipped (the reference still collides with a hidden optional object); else
+ * 2 + i * grid_h + j on the road tile at (i, j) = (floor(x / tile_size), floor(z / tile_size)) (get_grid_coords S:1134);
+ * else 1, the ground, outside the grid included.  0 and the agent's label never appear.  A cell's marking is the
+ * class (dts_set_marking_target's values) of the texel of its tile's texture under the centre: the inverse of the
+ * tile's model transform T((i + .5) ts, 0, (j + .5) ts) Ry(angle * 90 + 180) gives lx, lz, then u = (lx + ts/2) / ts,
+ * v = 1 - (lz + ts/2) / ts and the texel (floor(u * w) mod w, floor(v * h) mod h); 0 off the tiles or on a tile without
+ * texture.  Objects do not change markings.
+ * Written once per dts_step and dts_step_terminal (after the respawn: a row shows the state the returned obs row shows,
+ * whether or not obs_dev is NULL), once per dts_render and by dts_render_bev; not by a call refused before it launches.
+ * Independent of the render mode, fisheye, rectification, resize, output format and the per-pixel targets.  Sticky; the
+ * memory is the caller's and must stay valid while it is set.  A NULL config, or both pointers NULL, turns it off, and
+ * then no call launches anything for it.  A refused config returns 1 and leaves the previous target in effect.  Refused
+ * with labels while an uploaded map's largest label exceeds 32767, and while so set dts_upload_map refuses such a map.
+ * An output, not state: snapshots and the gathers do not carry it. */
+int dts_set_bev_target(dts_sim* sim, const dts_bev_config* cfg, int16_t* labels_dev, uint8_t* markings_dev);
+/* The bird's-eye targets of the current state (after dts_reset without a render, dts_load_state, ...): one launch,
+ * stream-ordered.  Fails while no target is set. */
+int dts_render_bev(dts_sim* sim, void* stream);
 /* Select the fused wrapper behaviour for subsequent dts_step / dts_render calls (default: all zero, scale 1).
  * obs_dev then holds num_envs * 3 * H * W elements of uint8 or float32 in the chosen layout. */
 int dts_set_output_format(dts_sim* sim, const dts_output_format* fmt);
