@@ -4,7 +4,8 @@
 observation buffers are caller-visible torch CUDA tensors, the work runs on
 `torch.cuda.current_stream()` inside libdtsim.so, nothing synchronises.  Constructor keywords are the
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
-`auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `camera_rand_pool` and the `bev*` keywords.
+`auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `flow`, `camera_rand_pool` and the `bev*`
+keywords.
 
 `camera_rand=True` (with `distortion=True`; without it the flag does nothing, as in the reference, S:352-358) gives the
 envs a spread of lenses: `camera_rand_pool` calibrations K, D are drawn once, at construction, within the reference's
@@ -54,6 +55,20 @@ MARKING_NAMES class of the texel under it, 0 off the tiles, objects or not.  Eve
 `render=False` too (under `auto_reset`, an ended env's row is its next episode's first state, as in `obs`), and so
 does every render; `render_bev()` writes them alone, e.g. after `reset(render=False)`, `load_state` or `copy_envs`.
 They do not depend on the camera, the render modes, sizes or formats, and snapshots and gathers do not carry them.
+
+`flow=True` allocates `env.flow`, float32 [num_envs, camera_height, camera_width, 2], filled by the same renders: the
+backward motion flow (dts_set_flow_target) — for each pixel, (dx, dy) in pixels, x right and y down, from where the
+surface point it shows is now to where it was in the previous frame, the camera and scene at the start of the env's
+last `step`.  It is computed from the depth and label images, so it turns on `depth` and `labels` (allocating
+`env.depth` and `env.labels` if they were not asked for); the ground, tiles, static objects and traffic lights stay put,
+moving obstacles and the agent's own mesh (top-down) move with their poses.  Under the fisheye both ends go through the
+env's camera model's forward map (`camera_model(s).mapx / mapy`).  NaN for sky, for points behind the previous camera,
+and for every pixel of an env without a previous frame in its episode: after `reset` (host or device), in the rows
+auto-reset respawned, and after `load_state` / `copy_envs` until the next step.  No occlusion mask: a point hidden in the
+previous frame still gets its motion.  `render_obs()` after a step gives the step's flow again, and after
+`step(render=False)` that step's.  It stays at the camera size and in this layout under `set_resize` and
+`set_output_format`; a flow env refuses `set_rectification`, whose remap has no forward map.  Snapshots and gathers do
+not carry it.
 """
 from __future__ import annotations
 
@@ -94,10 +109,11 @@ class BatchedDuckietownEnv:
                  cycle_maps: bool = False, env_id_offset: int = 0, tessellate_tiles: bool = False,
                  randomize_maps_on_reset: bool = False, randomization_config=None, terminal_obs: bool = False,
                  depth: bool = False, labels: bool = False, camera_rand_pool: int = 16, markings: bool = False,
-                 bev: bool = False, bev_shape=(64, 64), bev_cell: float = 0.03, bev_origin=None):
+                 bev: bool = False, bev_shape=(64, 64), bev_cell: float = 0.03, bev_origin=None, flow: bool = False):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
         camera_rand = bool(camera_rand and distortion)   # S:353-356: camera_rand only with distortion
+        depth, labels = depth or flow, labels or flow    # the flow image is taken from both
         if camera_rand and not 1 <= int(camera_rand_pool) <= 65536:
             raise ValueError(f"camera_rand_pool must be 1 to 65536, not {camera_rand_pool}")
         self.camera_rand = camera_rand
@@ -170,6 +186,9 @@ class BatchedDuckietownEnv:
                 (num_envs, bh, bw), dtype=torch.int16, device=self.device) if bev else None
             self.bev_markings: Optional[torch.Tensor] = torch.zeros(
                 (num_envs, bh, bw), dtype=torch.uint8, device=self.device) if bev else None
+            # the backward flow of the frames in obs (flow=True); the renders write it on the device
+            self.flow: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, camera_height, camera_width, 2), dtype=torch.float32, device=self.device) if flow else None
             self.reward = torch.zeros(num_envs, dtype=torch.float32, device=self.device)
             self._done_u8 = torch.zeros(num_envs, dtype=torch.uint8, device=self.device)
             self.state: Dict[str, torch.Tensor] = {
@@ -197,6 +216,10 @@ class BatchedDuckietownEnv:
             ox, oy = (bw / 2, 3 * bh / 4) if bev_origin is None else (float(v) for v in bev_origin)
             self.bev_config = L.BevConfig(bw, bh, float(bev_cell), float(ox), float(oy))
             self.sim.set_bev_target(self.bev_config, self.bev_labels.data_ptr(), self.bev_markings.data_ptr())
+        if flow:   # the forward maps of the fisheye tables, in the pool's order
+            models = self.camera_models if camera_rand else [self.camera_model] if distortion else None
+            self.sim.set_flow_target(self.flow.data_ptr(), *((np.stack([m.mapx for m in models]),
+                                                              np.stack([m.mapy for m in models])) if models else ()))
         self.seed(seed)
 
     def set_output_format(self, obs_layout: Optional[str] = None, obs_dtype: Optional[str] = None,
@@ -274,7 +297,11 @@ class BatchedDuckietownEnv:
         """UndistortWrapper's `cv2.remap(obs, mapx, mapy, INTER_NEAREST)` of reset / step observations, fused into the
         render (dts_set_rectify_lut): each output pixel is rendered at the source pixel the map names.  Applies while
         `undistort` is True; needs an env built with distortion=True.  None, None removes it.  A map the device refuses
-        raises and leaves the previous one in effect."""
+        raises and leaves the previous one in effect.  Refused (ValueError) on a flow env: the rectification's remap has
+        no forward map, so its frames would have no flow."""
+        if self.flow is not None:
+            raise ValueError("set_rectification: the flow image cannot follow the rectification (no forward map); "
+                             "build the env without flow=True")
         self.sim.set_rectify_lut(mapx, mapy)
         self.rectification = None if mapx is None and mapy is None else (mapx, mapy)
         self.sim.set_render_mode(**self._base_mode())

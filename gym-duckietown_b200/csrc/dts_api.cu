@@ -45,6 +45,7 @@ struct dts_sim {
   int render_mode = 0;                  // dts_set_render_mode             // the next dts_render also stores into the gather buffers
   AuxTargets aux{};                     // dts_set_{depth,label,marking}_target: caller-owned images, or null
   BevTarget bev{};                      // dts_set_bev_target: caller-owned grids, both null = off
+  FlowTarget flow{};                    // dts_set_flow_target: caller-owned image and the record it owns, null = off
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
   int profiling = 0;                    // 0 off, 1 events around k_raster only, 2 around every render kernel
   std::vector<cudaEvent_t> prof_events; // kProfMarks events per profiled frame
@@ -178,6 +179,7 @@ void dts_destroy(dts_sim* sim) {
   renderer_destroy(sim->render);
   resizer_destroy(sim->resize);
   state_destroy(sim->state);
+  flow_record_free(sim->flow.rec);
   void* extra[] = {sim->q_in, sim->q_outd, sim->q_outi, sim->q_hidden};
   for (void* p : extra) if (p) cudaFree(p);
   for (int p = 0; p < sim->gather_world; p++)
@@ -191,6 +193,14 @@ void dts_destroy(dts_sim* sim) {
 // The largest label (render spec item 10) of a map of these sizes: the agent's mesh, after the ground, cells and objects
 static long long largest_label(long long n_cells, long long n_objects) { return 2 + n_cells + n_objects; }
 
+// The most dynamic slots any uploaded map has (the flow record's size)
+static int largest_n_dyn(dts_sim* sim) {
+  int n = 0;
+  for (int s = 0; s < maps_slot_count(*sim->maps); s++)
+    if (const DMap* m = maps_get(*sim->maps, s)) n = m->n_dyn > n ? m->n_dyn : n;
+  return n;
+}
+
 int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
   if (!sim) return 1;
   if ((sim->aux.labels || sim->bev.labels) && b && largest_label((long long)b->grid_w * b->grid_h, b->n_objects) > INT16_MAX)
@@ -202,7 +212,20 @@ int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
   renderer_release_frame(*sim->render);
   // the records now cover this map's obstacles, and the fingerprint its content: older records no longer load
   const std::string ls = state_layout(*sim->state, *sim->maps);
-  return ls.empty() ? 0 : sim->fail("%s", ls.c_str());
+  if (!ls.empty()) return sim->fail("%s", ls.c_str());
+  // the flow record, sized for the maps now uploaded: every env's previous frame is forgotten
+  if (sim->flow.out) {
+    FlowRecord rec;
+    const std::string fe = flow_record_alloc(rec, sim->cfg.num_envs, largest_n_dyn(sim));
+    if (!fe.empty()) {   // (the map is in: flow goes off rather than run against a record too small for it)
+      flow_record_free(sim->flow.rec);
+      sim->flow = FlowTarget{};
+      return sim->fail("%s; the flow target is cleared", fe.c_str());
+    }
+    flow_record_free(sim->flow.rec);
+    sim->flow.rec = rec;
+  }
+  return 0;
 }
 
 int dts_set_fisheye_lut(dts_sim* sim, const float* rmapx, const float* rmapy, int width, int height) {
@@ -335,7 +358,7 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
   if (check_gather(sim)) return 1;
   if (check_maps(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  const std::string e = renderer_prepare(*sim->render, maps_counts(*sim->maps), sim->render_mode);
+  const std::string e = renderer_prepare(*sim->render, maps_counts(*sim->maps), sim->render_mode, sim->flow.out != nullptr);
   if (!e.empty()) return sim->fail("%s", e.c_str());
   RenderCfg rc{sim->cfg.cam_width, sim->cfg.cam_height, sim->cfg.flags, sim->cfg.num_envs,
                (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->render_mode,
@@ -365,8 +388,8 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
       gt.base[p] = reinterpret_cast<uint8_t*>(sim->gather_peer[p]) + (uint64_t)sim->gather_rank * sim->gather_bytes;
     sim->gather_next = false;
   }
-  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, sim->aux, target, gt,
-                        sim->d_err, sim->d_status, marks, mark_level, (cudaStream_t)stream);
+  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, sim->aux, sim->flow, target,
+                        gt, sim->d_err, sim->d_status, marks, mark_level, (cudaStream_t)stream);
   if (rz.ow) {
     launch_resize(*sim->resize, rz.staging, obs_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, env_list, env_count,
                   (cudaStream_t)stream);
@@ -401,6 +424,15 @@ int dts_render_bev(dts_sim* sim, void* stream) {
   return bev_pass(sim, stream);
 }
 
+// With a flow target: every env's camera and obstacles before the step, the previous frame of the next render's flow
+static int flow_record(dts_sim* sim, cudaStream_t st) {
+  if (!sim->flow.out) return 0;
+  launch_flow_record(state_arrays(*sim->state), maps_table(*sim->maps), sim->flow.rec, st);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  return 0;
+}
+
 int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, void* terminal_obs_dev, float* reward_dev,
                       uint8_t* done_dev, void* stream) {
   if (!sim) return 1;
@@ -416,6 +448,7 @@ int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, voi
   // 1. the step with the respawn held back: k_step_logic's only use of DTS_FLAG_AUTO_RESET is that respawn
   StepCfg deferred = sim->step_cfg;
   deferred.flags &= ~DTS_FLAG_AUTO_RESET;
+  if (flow_record(sim, st)) return 1;
   launch_step_logic(state_arrays(*sim->state), maps_table(*sim->maps), deferred, map_select(sim), actions_dev, reward_dev,
                     done_dev, st);
   sim->launches++;
@@ -449,6 +482,7 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   if ((sim->cfg.flags & DTS_FLAG_AUTO_RESET) && !state_seeded(*sim->state))
     return sim->fail("auto-reset needs seeded streams: call dts_seed_streams first");
+  if (flow_record(sim, (cudaStream_t)stream)) return 1;
   launch_step_logic(state_arrays(*sim->state), maps_table(*sim->maps), sim->step_cfg, map_select(sim), actions_dev, reward_dev, done_dev,
                     (cudaStream_t)stream);
   sim->launches++;
@@ -600,6 +634,7 @@ int dts_set_render_mode(dts_sim* sim, int mode) {
 
 int dts_set_depth_target(dts_sim* sim, float* depth_dev) {
   if (!sim) return 1;
+  if (!depth_dev && sim->flow.out) return sim->fail("the flow target reads the depth image: clear it (dts_set_flow_target) first");
   if (reinterpret_cast<uintptr_t>(depth_dev) & 3) return sim->fail("depth target is not aligned to 4 bytes");
   sim->aux.depth = depth_dev;
   return 0;
@@ -618,6 +653,7 @@ static int check_labels_fit(dts_sim* sim) {
 int dts_set_label_target(dts_sim* sim, int16_t* labels_dev) {
   if (!sim) return 1;
   if (reinterpret_cast<uintptr_t>(labels_dev) & 1) return sim->fail("label target is not aligned to 2 bytes");
+  if (!labels_dev && sim->flow.out) return sim->fail("the flow target reads the label image: clear it (dts_set_flow_target) first");
   if (labels_dev && check_labels_fit(sim)) return 1;
   sim->aux.labels = labels_dev;
   return 0;
@@ -638,6 +674,37 @@ int dts_set_bev_target(dts_sim* sim, const dts_bev_config* cfg, int16_t* labels_
   if (reinterpret_cast<uintptr_t>(labels_dev) & 1) return sim->fail("bird's-eye label target is not aligned to 2 bytes");
   if (labels_dev && check_labels_fit(sim)) return 1;
   sim->bev = BevTarget{*cfg, labels_dev, markings_dev};
+  return 0;
+}
+
+int dts_set_flow_target(dts_sim* sim, float* flow_dev, const float* fwd_x, const float* fwd_y, int n_tables) {
+  if (!sim) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  if (!flow_dev) {
+    DTS_CUDA(cudaDeviceSynchronize());   // no step or render in flight still writes the record or reads the maps
+    flow_record_free(sim->flow.rec);
+    sim->flow = FlowTarget{};
+    renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
+    return 0;
+  }
+  if (reinterpret_cast<uintptr_t>(flow_dev) & 7) return sim->fail("flow target is not aligned to 8 bytes");
+  if (!sim->aux.depth || !sim->aux.labels)
+    return sim->fail("the flow image is taken from the depth and label images: set both targets first");
+  const bool fish = (sim->cfg.flags & DTS_FLAG_DISTORTION) != 0;
+  if (fish && (!fwd_x || !fwd_y || n_tables < 1))
+    return sim->fail("a DTS_FLAG_DISTORTION handle needs the forward map of every fisheye table (fwd_x, fwd_y, n_tables)");
+  if (!fish && (fwd_x || fwd_y || n_tables))
+    return sim->fail("forward maps on a handle without DTS_FLAG_DISTORTION: pass NULL, NULL, 0");
+  DTS_CUDA(cudaDeviceSynchronize());
+  FlowRecord rec;
+  std::string e = flow_record_alloc(rec, sim->cfg.num_envs, largest_n_dyn(sim));
+  if (e.empty() && fish) {
+    e = renderer_set_flow_maps(*sim->render, n_tables, fwd_x, fwd_y);
+    if (!e.empty()) flow_record_free(rec);
+  }
+  if (!e.empty()) return sim->fail("%s", e.c_str());
+  flow_record_free(sim->flow.rec);
+  sim->flow = FlowTarget{flow_dev, rec};
   return 0;
 }
 
@@ -697,6 +764,10 @@ int dts_load_state(dts_sim* sim, const uint8_t* mask_dev, const void* records_de
   launch_state_load(*sim->state, mask_dev, records_dev, maps_table(*sim->maps), maps_slot_count(*sim->maps),
                     sim->d_status + 1, (cudaStream_t)stream);
   sim->launches++;
+  if (sim->flow.out) {   // a loaded env's flow record would pair its episode number with another state's pose
+    launch_flow_forget(sim->flow.rec, mask_dev, sim->cfg.num_envs, (cudaStream_t)stream);
+    sim->launches++;
+  }
   DTS_CUDA(cudaGetLastError());
   return 0;
 }

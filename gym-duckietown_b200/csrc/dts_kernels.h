@@ -31,6 +31,23 @@ struct AuxTargets {
   uint8_t* marks;
 };
 
+// The camera of one env's frame, per env in frame memory: written by k_frame_setup, read by the render kernels and the
+// flow pass (dts_flow.cu)
+struct __align__(16) FrameCtx {
+  double V[12];                  // agent camera modelview (S:1780-1803)
+  float P00, P11, P22, P23;      // gluPerspective (S:1761)
+  int32_t n_prims, n_lat, overflow, pad;
+};
+
+// The previous frame of the flow image (dts_set_flow_target, dts_flow.cu): what every env's camera and obstacles were at
+// the start of its last step, recorded by k_flow_record just before k_step_logic.  `episode` null: no record.
+struct FlowRecord {
+  double* pose;        // [3][n_envs] pos_x, pos_z, angle
+  double* dyn;         // [3][max_dyn][n_envs] DTS_DYN_PX, DTS_DYN_PZ, DTS_DYN_YROT of every dynamic slot of the env's map
+  int32_t* episode;    // [n_envs] the episode the record belongs to (DState::episode); -1: none
+  int32_t max_dyn;     // the largest n_dyn over the uploaded maps
+};
+
 void launch_step_logic(const DState& S, const DMap* maps, const StepCfg& c, int n_maps_cycle, const float* actions,
                        float* reward, uint8_t* done, cudaStream_t st);
 void launch_reset_random(const DState& S, const DMap* maps, const StepCfg& c, int n_maps_cycle, const uint8_t* mask,
@@ -115,8 +132,9 @@ Renderer* renderer_create(const dts_config& cfg);   // on cfg.device, which must
 void renderer_destroy(Renderer* r);
 void renderer_release_frame(Renderer& r);   // the maps changed: the next render re-sizes frame memory for them
 // Before every render: reserves frame memory for the maps of `counts` unless it is reserved, and checks that a fisheye
-// LUT is set if the camera needs one and a rectification LUT if render `mode` asks for it.
-std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode);
+// LUT is set if the camera needs one, a rectification LUT if render `mode` asks for it, and (`flow`: a flow target is
+// set) the fisheye tables' forward maps if the frame goes through them.
+std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode, bool flow);
 // The rasteriser's remap table for a LUT of the camera's size (obs[y, x] = frame[rint(rmapy), rint(rmapx)]), in the
 // fisheye slot or (`rectify`) the rectification slot; it replaces that slot's previous one, so no render may be in
 // flight.  A LUT the rasteriser cannot take leaves the previous table; NULL maps free the slot.  A fisheye pool: `count`
@@ -124,12 +142,19 @@ std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, 
 // read only when count > 1, and then kept in the table).  The rectification slot takes one LUT.
 std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* rmapx, const float* rmapy,
                              const int32_t* lut_of_env);
+// The forward maps of the fisheye tables (the flow image's F, dts_set_flow_target): `count` float32 [H][W] tables of x
+// and of y back to back, one per table of the fisheye pool and in its order; they replace the previous ones.  Refused
+// (error text, previous maps kept) unless the fisheye slot holds exactly `count` tables.  NULL maps free them.  A new
+// fisheye LUT (renderer_set_lut) drops them with the tables they belong to.
+std::string renderer_set_flow_maps(Renderer& r, int count, const float* fwd_x, const float* fwd_y);
 // `marks`: NULL or kProfMarks events recorded on `st` before k_frame_setup and after each of k_frame_setup, k_geometry,
 // k_bin, k_raster and the post passes (dts_profile_*).  `status_dev`: device address of the mapped host status word.
+// `flow`: the flow image's target (dts_flow.cu), launched after the rasterisers over the same envs; null `out`: none.
+struct FlowTarget;
 constexpr int kProfMarks = 6;
 int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, const AuxTargets& aux,
-                  void* obs, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks,
-                  int mark_level, cudaStream_t st);
+                  const FlowTarget& flow, void* obs, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev,
+                  cudaEvent_t* marks, int mark_level, cudaStream_t st);
 // What the last render left in frame memory for one env (dts_debug_frame), after the device has synchronised
 std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, int32_t* counts, float* lattice_by_cell,
                              int n_cells);
@@ -160,5 +185,33 @@ struct BevTarget {
 };
 // every env's grid of its current state, one launch
 void launch_bev(const DState& S, const DMap* maps, const BevTarget& b, cudaStream_t st);
+
+// motion flow (dts_flow.cu): the image of dts_set_flow_target, float32 [n_envs][H][W][2], and the record it is taken
+// against.  Null `out`: off, and then the record is unallocated.
+struct FlowTarget {
+  float* out;
+  FlowRecord rec;
+};
+// What the flow pass reads of the frame's remap: nothing (src_xy null: the pinhole frame), the fisheye table or pool
+// with its forward maps (fwd: [tables][H][W], the env's table named by table_of_env where that is not null), or the
+// rectification, whose forward map does not exist: every pixel NaN.
+struct FlowRemap {
+  const int32_t* src_xy;
+  const uint16_t* table_of_env;
+  const float2* fwd;
+  bool rectify;
+};
+// A record for n_envs envs and max_dyn dynamic slots, every env's record invalid (episode -1); synchronous.  On failure
+// (error text) `rec` is untouched.
+std::string flow_record_alloc(FlowRecord& rec, int n_envs, int max_dyn);
+void flow_record_free(FlowRecord& rec);
+// every env's camera and obstacles now, as the previous frame of its next render: launched just before k_step_logic
+void launch_flow_record(const DState& S, const DMap* maps, const FlowRecord& rec, cudaStream_t st);
+// every env e with mask[e] (null: all) forgets its previous frame (episode -1), stream-ordered
+void launch_flow_forget(const FlowRecord& rec, const uint8_t* mask, int n_envs, cudaStream_t st);
+// The flow image of the listed envs (rc.env_list, or all) from the depth and label images the render just wrote and
+// the frames' cameras in `ctx`
+void launch_flow(const DState& S, const DMap* maps, const RenderCfg& rc, const FrameCtx* ctx, const AuxTargets& aux,
+                 const FlowTarget& f, const FlowRemap& rm, cudaStream_t st);
 
 }  // namespace dts

@@ -75,6 +75,8 @@ struct RemapTab {
   const int4* home_ent;
   int ext_x, ext_y;
   const uint16_t* table_of_env;   // [n_envs] a pool's table index of every env; null unless a pool of more than one table
+  int count;                      // tables held
+  const float2* fwd;              // [count][H][W] forward maps of the flow image (renderer_set_flow_maps), or null
 };
 // How the rasterisers map output pixels to source pixels: not at all, through one table, or through each env's table of
 // a pool (the template value kRemap of k_bin and the rasterisers)
@@ -155,12 +157,6 @@ constexpr int kKindFlat = 8;     // road tile of tile mode 1: lies in the plane 
 constexpr unsigned kNoPrim = 0xffffu;   // sample not covered by any prim: clear colour
 
 struct Xform { float MV[12], N[9]; };
-
-struct __align__(16) FrameCtx {   // per env, global memory
-  double V[12];                  // agent camera modelview (S:1780-1803)
-  float P00, P11, P22, P23;      // gluPerspective (S:1761)
-  int32_t n_prims, n_lat, overflow, pad;
-};
 
 struct __align__(16) GeoWarp {    // per warp of k_geometry, shared memory
   int32_t unlit, pad_[3];        // segment=True: GL_LIGHTING off, the vertex colour is the material colour (S:1730-1733)
@@ -2364,7 +2360,7 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
 
 // ------------------------------------------------------------------------------------------------ the renderer
 static void free_remap(RemapTab& t) {
-  const void* p[] = {t.src_xy, t.cbox, t.fbox, t.cell_start, t.cell_bins, t.home_start, t.home_ent, t.table_of_env};
+  const void* p[] = {t.src_xy, t.cbox, t.fbox, t.cell_start, t.cell_bins, t.home_start, t.home_ent, t.table_of_env, t.fwd};
   for (const void* q : p) cudaFree(const_cast<void*>(q));
   t = RemapTab{};
 }
@@ -2379,7 +2375,7 @@ void renderer_destroy(Renderer* r) {
   delete r;
 }
 
-std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode) {
+std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode, bool flow) {
   if (!r.frame) {
     // prims k_geometry emits per road tile: the literal triangles of tile mode 0, or the quad of tile mode 1, which a
     // clip splits into two triangles and fans into a few more
@@ -2416,6 +2412,33 @@ std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, 
   }
   if ((r.flags & DTS_FLAG_DISTORTION) && !r.fish.src_xy) return "distortion enabled but no fisheye LUT set";
   if ((mode & DTS_RENDER_RECTIFY) && !r.rect.src_xy) return "DTS_RENDER_RECTIFY but no rectification LUT set";
+  if (flow && (r.flags & DTS_FLAG_DISTORTION) && !(mode & (DTS_RENDER_PINHOLE | DTS_RENDER_RECTIFY)) && !r.fish.fwd)
+    return "a flow target is set but the fisheye tables have no forward maps: a fisheye LUT set after "
+           "dts_set_flow_target drops them, so set the flow target again";
+  return "";
+}
+
+std::string renderer_set_flow_maps(Renderer& r, int count, const float* fwd_x, const float* fwd_y) {
+  if (!fwd_x || !fwd_y) {
+    cudaFree(const_cast<float2*>(r.fish.fwd));
+    r.fish.fwd = nullptr;
+    return "";
+  }
+  if (!r.fish.src_xy || count != r.fish.count)
+    return "the flow image's forward maps are " + std::to_string(count) + " tables but the fisheye pool holds " +
+           std::to_string(r.fish.src_xy ? r.fish.count : 0);
+  const size_t n = (size_t)count * r.W * r.H;
+  std::vector<float2> f(n);
+  for (size_t k = 0; k < n; k++) f[k] = make_float2(fwd_x[k], fwd_y[k]);
+  void* d = nullptr;
+  cudaError_t e = cudaMalloc(&d, n * sizeof(float2));
+  if (e == cudaSuccess) e = cudaMemcpy(d, f.data(), n * sizeof(float2), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaFree(d);
+    return std::string("flow forward map upload failed: ") + cudaGetErrorString(e);
+  }
+  cudaFree(const_cast<float2*>(r.fish.fwd));
+  r.fish.fwd = static_cast<const float2*>(d);
   return "";
 }
 
@@ -2521,7 +2544,7 @@ std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* 
     free_remap(t);
     return std::string(what) + " table upload failed: " + cudaGetErrorString(e);
   }
-  t.ext_x = ext_x; t.ext_y = ext_y;
+  t.ext_x = ext_x; t.ext_y = ext_y; t.count = count;
   free_remap(slot);
   slot = t;
   return "";
@@ -2579,8 +2602,8 @@ template <const auto& kList, typename F>
 static void for_each_of(F f) { each_of<kList>(f, std::make_index_sequence<std::size(kList)>{}); }
 
 int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, const AuxTargets& aux,
-                  void* obs_any, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev, cudaEvent_t* marks,
-                  int mark_level, cudaStream_t st) {
+                  const FlowTarget& flow, void* obs_any, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev,
+                  cudaEvent_t* marks, int mark_level, cudaStream_t st) {
   uint8_t* obs = reinterpret_cast<uint8_t*>(obs_any);
   // the table the frame is remapped through, if any: the rectification (DTS_RENDER_RECTIFY), none (DTS_RENDER_PINHOLE
   // or no DTS_FLAG_DISTORTION) or the fisheye.  A table with a per-env index is a pool (kRemapPool); one table, of
@@ -2640,6 +2663,11 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
     });
   });
   mark();
+  if (flow.out) {   // (inside the post-pass event bracket)
+    const FlowRemap fr{lut ? rt.src_xy : nullptr, rt.table_of_env, rt.fwd, (rc.mode & DTS_RENDER_RECTIFY) != 0};
+    launch_flow(S, maps, rc, fm.ctx, aux, flow, fr, st);
+    launches++;
+  }
   mark();   // (post passes: launched by the caller)
   return launches;
 }

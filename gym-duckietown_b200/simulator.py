@@ -71,7 +71,7 @@ class Simulator(Env):
                  camera_rand: bool = False, randomize_maps_on_reset: bool = False, num_tris_distractors: int = 12,
                  color_ground=(0.15, 0.15, 0.15), color_sky=(0.45, 0.82, 1), style: str = "photos",
                  enable_leds: bool = False, device: int = 0, depth: bool = False, labels: bool = False,
-                 markings: bool = False, bev: bool = False, **env_kwargs):
+                 markings: bool = False, bev: bool = False, flow: bool = False, **env_kwargs):
         if draw_curve or draw_bbox or enable_leds:
             raise NotImplementedError("draw_curve / draw_bbox / enable_leds are debug modes outside the hot path "
                                       "(SURVEY 8f-4)")
@@ -97,7 +97,8 @@ class Simulator(Env):
             distortion=distortion, dynamics_rand=dynamics_rand, camera_rand=camera_rand,
             camera_rand_pool=env_kwargs.pop("camera_rand_pool", 1),   # one camera per Simulator (distortion.py:46-47)
             color_ground=color_ground, color_sky=color_sky, num_tris_distractors=num_tris_distractors,
-            action_mode=self._action_mode, depth=depth, labels=labels, markings=markings, bev=bev, **env_kwargs)
+            action_mode=self._action_mode, depth=depth, labels=labels, markings=markings, bev=bev, flow=flow,
+            **env_kwargs)
         self._b = BatchedDuckietownEnv(1, map_arg, **self._env_kwargs)
         self._adopt_map()
         self.action_space = spaces.Box(low=-1, high=1, shape=(2,), dtype=np.float32)              # S:309
@@ -159,7 +160,7 @@ class Simulator(Env):
         from .batched_env import BatchedDuckietownEnv
         if getattr(self, "_human", None) is None:
             kw = dict(self._env_kwargs, camera_width=WINDOW_WIDTH, camera_height=WINDOW_HEIGHT, distortion=False,
-                      terminal_obs=False, depth=False, labels=False, markings=False, bev=False)
+                      terminal_obs=False, depth=False, labels=False, markings=False, bev=False, flow=False)
             self._human = BatchedDuckietownEnv(1, list(self._b.maps), **kw)
         self._human.load_state(self._b.save_state())
         return self._human
@@ -232,6 +233,15 @@ class Simulator(Env):
         (BatchedDuckietownEnv.bev_markings, named by MARKING_NAMES); else None."""
         g = self._b.bev_markings
         return None if g is None else g[0].cpu().numpy()
+
+    @property
+    def flow(self) -> Optional[np.ndarray]:
+        """With flow=True: float32 [camera_height, camera_width, 2], the backward flow of the frame last returned by reset /
+        step / render_obs — for each pixel, where the surface point it shows was at the start of the last step minus
+        where it is now, in pixels, x right and y down; NaN for sky and when there is no earlier frame in the episode
+        (BatchedDuckietownEnv.flow); else None.  flow=True also turns on depth and labels."""
+        f = self._b.flow
+        return None if f is None else f[0].cpu().numpy()
 
     @property
     def cur_pos(self):

@@ -387,6 +387,36 @@ int dts_set_bev_target(dts_sim* sim, const dts_bev_config* cfg, int16_t* labels_
 /* The bird's-eye targets of the current state (after dts_reset without a render, dts_load_state, ...): one launch,
  * stream-ordered.  Fails while no target is set. */
 int dts_render_bev(dts_sim* sim, void* stream);
+/* Motion-flow image beside every observation (DESIGN.md section 5, item 13): every later render of this handle that
+ * writes obs — dts_render, dts_step, dts_step_terminal, whatever the render mode — also writes flow_dev, float32
+ * [num_envs][cam_height][cam_width][2], always in that layout and at the camera size whatever dts_set_output_format and
+ * dts_set_resize say.  A pixel holds (dx, dy) in output pixels, x to the right and y down: BACKWARD flow, the position
+ * the surface point it shows had in the previous frame minus its position in this one.  The previous frame is the
+ * camera and scene at the start of the env's most recent dts_step / dts_step_terminal (before its frame_skip ticks),
+ * in the same episode: a kernel launched just before k_step_logic (k_flow_record) records the agent's pose, every dynamic
+ * slot's position and heading and the episode number.  The surface point is the one the depth and label images name (dts_set_depth_target,
+ * dts_set_label_target): unprojected from the pixel centre of its pinhole source pixel (under the fisheye, the table's
+ * source), moved with its draw item (ground, tiles, static objects and traffic lights stay; a moving obstacle and, in
+ * top-down views, the agent's mesh move with their pose, rounded to float as the render places them), and projected
+ * through the previous camera.  Under the fisheye the pinhole positions at both ends go through the forward map of the
+ * env's table, sampled bilinearly (OpenCV's convention: index = position - 0.5).  NaN where: the depth is 0 (sky, no
+ * source pixel); the env has no previous frame (nothing stepped since dts_set_flow_target, a map upload, a reset or
+ * respawn, or a dts_load_state of that env); the render is DTS_RENDER_RECTIFY; the point was not in front of the previous
+ * camera's near plane; or, under the fisheye, the forward map's footprint leaves the table.  No occlusion mask: a point
+ * hidden in the previous frame still gets its motion.  After a step, dts_render gives the step's flow again; after a step
+ * without a render, the next render gives that step's.  A pass over listed envs (the second pass of dts_step_terminal)
+ * writes only those envs' rows — NaN, as they respawned — so row e matches obs_dev row e; the terminal frames' flow is
+ * not kept.
+ * fwd_x / fwd_y: HOST float32 [n_tables][cam_height][cam_width], the forward maps F (distortion.Distortion's mapx / mapy:
+ * the distorted output position of every pinhole position) of the fisheye tables, one per table of the pool and in its
+ * order, on a DTS_FLAG_DISTORTION handle; NULL, NULL, 0 without.  A fisheye LUT set afterwards drops them, and renders
+ * through it fail until this is called again.  Refused (non-zero, the previous setting kept) unless the depth and label
+ * targets are set, with a wrong n_tables, or a flow_dev not 8-byte aligned; while it is set, clearing the depth or
+ * label target is refused.  Sticky; the memory is the caller's and must stay valid while it is set.  NULL turns it off,
+ * and then the renders launch the very kernels they launch without this call.  With it set, every render launches one
+ * more kernel (k_flow), and dts_step, dts_step_terminal and dts_load_state one more each.  Synchronises.  An output, not state: snapshots and the gathers do not
+ * carry it, nor the record. */
+int dts_set_flow_target(dts_sim* sim, float* flow_dev, const float* fwd_x, const float* fwd_y, int n_tables);
 /* Select the fused wrapper behaviour for subsequent dts_step / dts_render calls (default: all zero, scale 1).
  * obs_dev then holds num_envs * 3 * H * W elements of uint8 or float32 in the chosen layout. */
 int dts_set_output_format(dts_sim* sim, const dts_output_format* fmt);

@@ -2,21 +2,24 @@
 with --labels what the label image costs (dts_set_label_target: their label instances, one i16 store per pixel and a
 draw-item lookup per winner), alone and together with depth, and with --markings what the lane-marking image costs
 (dts_set_marking_target: the rasterisers' marking instances, one u8 store per pixel and a texel-class load per winner),
-alone and together with labels.
+alone and together with labels, and with --flow what the motion-flow image costs (dts_set_flow_target: k_flow after the
+rasterisers, reading depth, labels and the remap, one float2 store per pixel) on top of depth and labels.
 
 For each benchmark shape — c2: small_loop, c3: loop_obstacles (4096 envs, 160x120), c4: udem1, 640x480, fisheye, domain
 randomisation (`--c4-envs`, default 2048: the depth tensor is 1.2 MB per env there) — ONE env under device auto-reset
 and bench.py's uniform random actions in [-1, 1], stepped with the depth target off and on in alternating arms, `rounds`
 times.  The same handle runs both arms, so the arms differ in nothing but the kernels launched.
 With --labels the arms are off / depth / labels / both, with --markings off / labels / markings / labels+markings (no
-depth target in either), taken in an order that rotates from round to round.
+depth target in either), taken in an order that rotates from round to round; with --flow depth+labels / flow (depth,
+labels and flow), alternated.  k_flow's own time is the "post" bracket of the flow arm less that of depth+labels (the
+bracket holds nothing else without a resize).
 Reports ms per step of each arm (host clock around `steps` steps ending in a synchronise, after `warmup` steps of that
 arm), the median and the spread (min .. max) over the rounds, and, from a separate pass under dts_profile_enable(2)
 (events at every kernel boundary, so not an end-to-end number), the ms per frame of each render kernel bracket; k_raster's
 bracket holds the three rasterisers.  Prints one JSON line with the card's name, power limit and SM clocks read before
 and after in the same run.
 
-    python tools/depth_probe.py [--configs c2,c3,c4] [--steps 100] [--warmup 10] [--rounds 5] [--labels | --markings]
+    python tools/depth_probe.py [--configs c2,c3,c4] [--steps 100] [--warmup 10] [--rounds 5] [--labels | --markings | --flow]
                                 [--out FILE.json]
 """
 import argparse
@@ -40,6 +43,7 @@ SHAPES = {
 ARMS = ["off", "on"]
 LABEL_ARMS = ["off", "depth", "labels", "both"]
 MARKING_ARMS = ["off", "labels", "markings", "labels+markings"]
+FLOW_ARMS = ["depth+labels", "flow"]
 
 
 def card():
@@ -49,6 +53,9 @@ def card():
 
 
 def set_arm(env, arm):
+    if env.flow is not None:   # depth and labels stay on: the flow image reads them
+        env.sim.set_flow_target(env.flow.data_ptr() if arm == "flow" else None)
+        return
     env.sim.set_depth_target(env.depth.data_ptr() if arm in ("on", "depth", "both") else None)
     if env.labels is not None:
         env.sim.set_label_target(env.labels.data_ptr() if arm in ("labels", "both", "labels+markings") else None)
@@ -92,9 +99,10 @@ def main():
     ap.add_argument("--c4-envs", type=int, default=SHAPES["c4"]["envs"])
     ap.add_argument("--labels", action="store_true", help="arms off / depth / labels / both")
     ap.add_argument("--markings", action="store_true", help="arms off / labels / markings / labels+markings")
+    ap.add_argument("--flow", action="store_true", help="arms depth+labels / depth+labels+flow")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    arms = MARKING_ARMS if a.markings else LABEL_ARMS if a.labels else ARMS
+    arms = FLOW_ARMS if a.flow else MARKING_ARMS if a.markings else LABEL_ARMS if a.labels else ARMS
     if not torch.cuda.is_available():
         sys.exit("needs a CUDA device")
     res = {"card": card(), "steps": a.steps, "warmup": a.warmup, "rounds": a.rounds, "actions": "uniform [-1, 1]", "configs": {}}
@@ -104,7 +112,8 @@ def main():
             c["envs"] = a.c4_envs
         env = BatchedDuckietownEnv(c["envs"], c["map"], camera_width=c["width"], camera_height=c["height"],
                                    domain_rand=c["domain_rand"], distortion=c["distortion"], seed=1, device_reset=True,
-                                   auto_reset=True, depth=True, labels=a.labels or a.markings, markings=a.markings)
+                                   auto_reset=True, depth=True, labels=a.labels or a.markings, markings=a.markings,
+                                   flow=a.flow)
         env.reset()
         g = torch.Generator(device="cuda").manual_seed(0)
         acts = torch.rand((16, c["envs"], 2), device="cuda", generator=g) * 2 - 1
@@ -122,10 +131,13 @@ def main():
             **c, "ms_per_step": runs, "median_ms_per_step": med,
             "spread_ms_per_step": {k: [float(min(v)), float(max(v))] for k, v in runs.items()},
             "kernel_ms_per_frame": kern, "obs_bytes_per_step": px * 3, "depth_bytes_per_step": px * 4,
-            "labels_bytes_per_step": px * 2, "markings_bytes_per_step": px}
+            "labels_bytes_per_step": px * 2, "markings_bytes_per_step": px, "flow_bytes_per_step": px * 8}
+        base = arms[0]
         for arm in arms[1:]:
-            res["configs"][cfg].update({f"{arm}_minus_off_ms": med[arm] - med["off"], f"{arm}_over_off": med[arm] / med["off"],
-                                        f"k_raster_{arm}_minus_off_ms": kern[arm]["k_raster"] - kern["off"]["k_raster"]})
+            res["configs"][cfg].update({f"{arm}_minus_{base}_ms": med[arm] - med[base], f"{arm}_over_{base}": med[arm] / med[base],
+                                        f"k_raster_{arm}_minus_{base}_ms": kern[arm]["k_raster"] - kern[base]["k_raster"]})
+        if a.flow:
+            res["configs"][cfg]["k_flow_ms_per_frame"] = kern["flow"]["post"] - kern[base]["post"]
         env.close()
         del env
         torch.cuda.empty_cache()
