@@ -5,10 +5,12 @@ Public surface (mirrors gym_duckietown's, SURVEY.md 8b):
   BatchedDuckietownEnv                       N envs per GPU, torch tensors in/out
   load_map, list_maps                        MapFormat1 loader
   MARKING_NAMES                              names of the lane-marking image's values (markings=True)
+  OCCLUSION_NAMES                            names of the occlusion mask's values (flow_occlusion=True)
 """
 __version__ = "0.1.0"
 
 from .assets import MARKING_NAMES  # noqa: F401
+from .lib import OCCLUSION_NAMES  # noqa: F401
 from .maps import InvalidMapException, list_maps, load_map  # noqa: F401
 
 

@@ -4,8 +4,8 @@
 observation buffers are caller-visible torch CUDA tensors, the work runs on
 `torch.cuda.current_stream()` inside libdtsim.so, nothing synchronises.  Constructor keywords are the
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
-`auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `flow`, `camera_rand_pool` and the `bev*`
-keywords.
+`auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `flow`, `flow_occlusion`,
+`camera_rand_pool` and the `bev*` keywords.
 
 `camera_rand=True` (with `distortion=True`; without it the flag does nothing, as in the reference, S:352-358) gives the
 envs a spread of lenses: `camera_rand_pool` calibrations K, D are drawn once, at construction, within the reference's
@@ -64,11 +64,22 @@ last `step`.  It is computed from the depth and label images, so it turns on `de
 moving obstacles and the agent's own mesh (top-down) move with their poses.  Under the fisheye both ends go through the
 env's camera model's forward map (`camera_model(s).mapx / mapy`).  NaN for sky, for points behind the previous camera,
 and for every pixel of an env without a previous frame in its episode: after `reset` (host or device), in the rows
-auto-reset respawned, and after `load_state` / `copy_envs` until the next step.  No occlusion mask: a point hidden in the
-previous frame still gets its motion.  `render_obs()` after a step gives the step's flow again, and after
-`step(render=False)` that step's.  It stays at the camera size and in this layout under `set_resize` and
-`set_output_format`; a flow env refuses `set_rectification`, whose remap has no forward map.  Snapshots and gathers do
-not carry it.
+auto-reset respawned, and after `load_state` / `copy_envs` until the next step.  A point hidden in the previous frame
+still gets its motion; `flow_occlusion` says which were in view.  `render_obs()` after a step gives the step's flow
+again, and after `step(render=False)` that step's.  It stays at the camera size and in this layout under `set_resize`
+and `set_output_format`; a flow env refuses `set_rectification`, whose remap has no forward map.  Snapshots and gathers
+do not carry it.
+
+`flow_occlusion=True` allocates `env.flow_occlusion`, uint8 [num_envs, camera_height, camera_width], written with
+`env.flow` (dts_set_occlusion_target; it turns on `flow`, and through it `depth` and `labels`): whether each pixel's
+surface point was in view at its position q = pixel centre + flow in the previous frame, named by OCCLUSION_NAMES —
+0 none (flow is NaN), 1 visible (one of the four pixels around q showed the same item there, and a mesh at the
+point's depth within 2 %), 2 occluded (something else was there), 3 outside (q leaves the frame), 4 unknown (the
+previous frame was never rendered in this view, e.g. after `step(render=False)`).  Under the fisheye most points that
+leave the view have NaN flow, so 0.  The library keeps the previous frames itself, two depth and label images per env
+(12 bytes per camera pixel: 944 MB at 4096 envs of 160 x 120), so `render_obs()` after a step repeats the step's mask,
+and a `render_obs(top_down=True)` between two steps leaves the next step's mask intact.  The terminal frames' masks are
+not kept; `load_state`, `copy_envs` and a map upload forget the envs' previous frames.
 """
 from __future__ import annotations
 
@@ -79,6 +90,7 @@ import torch
 
 from . import lib as L
 from .assets import MARKING_NAMES  # noqa: F401  (the names of env.markings' values)
+from .lib import OCCLUSION_NAMES  # noqa: F401  (the names of env.flow_occlusion's values)
 from .episode import EpisodeSampler
 from .maps import TILE_KINDS, MapData, load_map
 
@@ -109,10 +121,12 @@ class BatchedDuckietownEnv:
                  cycle_maps: bool = False, env_id_offset: int = 0, tessellate_tiles: bool = False,
                  randomize_maps_on_reset: bool = False, randomization_config=None, terminal_obs: bool = False,
                  depth: bool = False, labels: bool = False, camera_rand_pool: int = 16, markings: bool = False,
-                 bev: bool = False, bev_shape=(64, 64), bev_cell: float = 0.03, bev_origin=None, flow: bool = False):
+                 bev: bool = False, bev_shape=(64, 64), bev_cell: float = 0.03, bev_origin=None, flow: bool = False,
+                 flow_occlusion: bool = False):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
         camera_rand = bool(camera_rand and distortion)   # S:353-356: camera_rand only with distortion
+        flow = flow or flow_occlusion                    # the mask is taken with the flow image
         depth, labels = depth or flow, labels or flow    # the flow image is taken from both
         if camera_rand and not 1 <= int(camera_rand_pool) <= 65536:
             raise ValueError(f"camera_rand_pool must be 1 to 65536, not {camera_rand_pool}")
@@ -189,6 +203,9 @@ class BatchedDuckietownEnv:
             # the backward flow of the frames in obs (flow=True); the renders write it on the device
             self.flow: Optional[torch.Tensor] = torch.zeros(
                 (num_envs, camera_height, camera_width, 2), dtype=torch.float32, device=self.device) if flow else None
+            # which of those pixels were in view in the previous frame (flow_occlusion=True), OCCLUSION_NAMES
+            self.flow_occlusion: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, camera_height, camera_width), dtype=torch.uint8, device=self.device) if flow_occlusion else None
             self.reward = torch.zeros(num_envs, dtype=torch.float32, device=self.device)
             self._done_u8 = torch.zeros(num_envs, dtype=torch.uint8, device=self.device)
             self.state: Dict[str, torch.Tensor] = {
@@ -220,6 +237,8 @@ class BatchedDuckietownEnv:
             models = self.camera_models if camera_rand else [self.camera_model] if distortion else None
             self.sim.set_flow_target(self.flow.data_ptr(), *((np.stack([m.mapx for m in models]),
                                                               np.stack([m.mapy for m in models])) if models else ()))
+        if flow_occlusion:
+            self.sim.set_occlusion_target(self.flow_occlusion.data_ptr())
         self.seed(seed)
 
     def set_output_format(self, obs_layout: Optional[str] = None, obs_dtype: Optional[str] = None,

@@ -46,6 +46,7 @@ struct dts_sim {
   AuxTargets aux{};                     // dts_set_{depth,label,marking}_target: caller-owned images, or null
   BevTarget bev{};                      // dts_set_bev_target: caller-owned grids, both null = off
   FlowTarget flow{};                    // dts_set_flow_target: caller-owned image and the record it owns, null = off
+  OcclusionTarget occ{};                // dts_set_occlusion_target: caller-owned mask and the slots it owns, null = off
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
   int profiling = 0;                    // 0 off, 1 events around k_raster only, 2 around every render kernel
   std::vector<cudaEvent_t> prof_events; // kProfMarks events per profiled frame
@@ -180,6 +181,7 @@ void dts_destroy(dts_sim* sim) {
   resizer_destroy(sim->resize);
   state_destroy(sim->state);
   flow_record_free(sim->flow.rec);
+  occlusion_free(sim->occ);
   void* extra[] = {sim->q_in, sim->q_outd, sim->q_outi, sim->q_hidden};
   for (void* p : extra) if (p) cudaFree(p);
   for (int p = 0; p < sim->gather_world; p++)
@@ -220,10 +222,15 @@ int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
     if (!fe.empty()) {   // (the map is in: flow goes off rather than run against a record too small for it)
       flow_record_free(sim->flow.rec);
       sim->flow = FlowTarget{};
-      return sim->fail("%s; the flow target is cleared", fe.c_str());
+      occlusion_free(sim->occ);
+      return sim->fail("%s; the flow and occlusion targets are cleared", fe.c_str());
     }
     flow_record_free(sim->flow.rec);
     sim->flow.rec = rec;
+  }
+  if (sim->occ.out) {   // the slots' frames were drawn from the old map
+    const std::string oe = occlusion_empty(sim->occ, sim->cfg.num_envs);
+    if (!oe.empty()) return sim->fail("%s", oe.c_str());
   }
   return 0;
 }
@@ -388,7 +395,7 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
       gt.base[p] = reinterpret_cast<uint8_t*>(sim->gather_peer[p]) + (uint64_t)sim->gather_rank * sim->gather_bytes;
     sim->gather_next = false;
   }
-  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, sim->aux, sim->flow, target,
+  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, sim->aux, sim->flow, sim->occ, target,
                         gt, sim->d_err, sim->d_status, marks, mark_level, (cudaStream_t)stream);
   if (rz.ow) {
     launch_resize(*sim->resize, rz.staging, obs_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, env_list, env_count,
@@ -680,6 +687,8 @@ int dts_set_bev_target(dts_sim* sim, const dts_bev_config* cfg, int16_t* labels_
 int dts_set_flow_target(dts_sim* sim, float* flow_dev, const float* fwd_x, const float* fwd_y, int n_tables) {
   if (!sim) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  if (!flow_dev && sim->occ.out)
+    return sim->fail("the occlusion mask is taken with the flow image: clear it (dts_set_occlusion_target) first");
   if (!flow_dev) {
     DTS_CUDA(cudaDeviceSynchronize());   // no step or render in flight still writes the record or reads the maps
     flow_record_free(sim->flow.rec);
@@ -705,6 +714,26 @@ int dts_set_flow_target(dts_sim* sim, float* flow_dev, const float* fwd_x, const
   if (!e.empty()) return sim->fail("%s", e.c_str());
   flow_record_free(sim->flow.rec);
   sim->flow = FlowTarget{flow_dev, rec};
+  if (sim->occ.out) {   // the new record, and perhaps new forward maps and fisheye tables, start from no frame
+    e = occlusion_empty(sim->occ, sim->cfg.num_envs);
+    if (!e.empty()) return sim->fail("%s", e.c_str());
+  }
+  return 0;
+}
+
+int dts_set_occlusion_target(dts_sim* sim, uint8_t* occ_dev) {
+  if (!sim) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  if (occ_dev && !sim->flow.out)
+    return sim->fail("the occlusion mask is taken with the flow image: set the flow target (dts_set_flow_target) first");
+  DTS_CUDA(cudaDeviceSynchronize());   // no render in flight still reads or writes the slots
+  OcclusionTarget occ{};
+  if (occ_dev) {
+    const std::string e = occlusion_alloc(occ, occ_dev, sim->cfg.num_envs, sim->cfg.cam_width, sim->cfg.cam_height);
+    if (!e.empty()) return sim->fail("%s", e.c_str());
+  }
+  occlusion_free(sim->occ);
+  sim->occ = occ;
   return 0;
 }
 
@@ -765,7 +794,7 @@ int dts_load_state(dts_sim* sim, const uint8_t* mask_dev, const void* records_de
                     sim->d_status + 1, (cudaStream_t)stream);
   sim->launches++;
   if (sim->flow.out) {   // a loaded env's flow record would pair its episode number with another state's pose
-    launch_flow_forget(sim->flow.rec, mask_dev, sim->cfg.num_envs, (cudaStream_t)stream);
+    launch_flow_forget(sim->flow.rec, sim->occ, mask_dev, sim->cfg.num_envs, (cudaStream_t)stream);
     sim->launches++;
   }
   DTS_CUDA(cudaGetLastError());

@@ -17,6 +17,8 @@ constexpr int kFlowPxPerCta = kFlowThreads * kFlowPxPerThread;
 constexpr int kFlowBatch = 8;          // pixels per thread whose depth and label loads are issued together
 constexpr int kFlowMats = 2 + DTS_MAX_OBJECTS;   // the scene's, the agent's, one per dynamic slot (at most one per object)
 constexpr float kNear = 0.04f;                    // gluPerspective's near plane (S:1761)
+constexpr float kOccTau = 0.02f;                  // a mesh point is visible within this share of its depth (DESIGN.md
+                                                  // section 5 item 14 measures it)
 
 // out = A * B for row-major 3x4 rigid transforms (the implied fourth row 0 0 0 1)
 __device__ inline void compose(const double* A, const double* B, double* out) {
@@ -54,10 +56,34 @@ __device__ __forceinline__ bool forward_map(const float2* __restrict__ F, int W,
   return true;
 }
 
-// grid (listed env, chunk of kFlowPxPerCta output pixels); one thread per pixel of the chunk at a time
+// The render-mode bits that change a frame's depth and labels: an occlusion slot's frame is of one view
+__device__ __forceinline__ int occ_view(int mode) {
+  return mode & (DTS_RENDER_TOP_DOWN | DTS_RENDER_PINHOLE | DTS_RENDER_RECTIFY);
+}
+
+// An env's occlusion slots for this render (valid: its flow record is this episode's): .x the slot holding the frame of
+// the recorded state in this view, -1 if none; .y the slot this frame goes to, the other one, or with no match the one
+// written less recently.  k_flow and k_occ_commit compute it from the same tags, which only k_occ_commit changes.
+__device__ __forceinline__ int2 occ_slots(const OcclusionTarget& o, const FlowRecord& rec, const DState& S, int env,
+                                          int view, bool valid) {
+  const size_t n = S.n;
+  int rs = -1;
+  if (valid) {
+    const int ep = __ldg(rec.episode + env), sc = __ldg(rec.episode + n + env);
+    for (int s = 0; s < 2; s++)
+      if (__ldg(o.tag + (3 * s) * n + env) == ep && __ldg(o.tag + (3 * s + 1) * n + env) == sc &&
+          __ldg(o.tag + (3 * s + 2) * n + env) == view)
+        rs = s;
+  }
+  return make_int2(rs, rs >= 0 ? 1 - rs : 1 - (int)__ldg(o.newest + env));
+}
+
+// grid (listed env, chunk of kFlowPxPerCta output pixels); one thread per pixel of the chunk at a time.  kOcc: also the
+// occlusion mask (dts_set_occlusion_target) from the slot of the recorded state, and this frame into the other slot.
+template <bool kOcc>
 __global__ void __launch_bounds__(kFlowThreads) k_flow(DState S, const DMap* __restrict__ maps, RenderCfg rc,
                                                        const FrameCtx* __restrict__ ctx, AuxTargets aux, FlowTarget f,
-                                                       FlowRemap rm) {
+                                                       FlowRemap rm, OcclusionTarget o) {
   __shared__ float mats[kFlowMats][12];   // 0: ground, tiles and static objects; 1: the agent's mesh; 2 + s: dynamic slot s
   __shared__ double Vp[12], Vi[12];       // the previous frame's camera, the inverse of this frame's
   const int slot = blockIdx.x;
@@ -113,6 +139,11 @@ __global__ void __launch_bounds__(kFlowThreads) k_flow(DState S, const DMap* __r
   const float2* fwd = rm.fwd ? rm.fwd + (size_t)table * hw : nullptr;
   float2* out = reinterpret_cast<float2*>(f.out) + row;
   const float nan = __int_as_float(0x7fc00000);
+  int2 occ = make_int2(-1, 0);   // (the slot read, -1: none; the slot written)
+  if constexpr (kOcc) occ = occ_slots(o, f.rec, S, env, occ_view(rc.mode), valid);
+  const size_t slot_px = (size_t)S.n * hw;
+  const float* dprev = o.depth + max(occ.x, 0) * slot_px + row;   // (read only where occ.x >= 0)
+  const int16_t* lprev = o.labels + max(occ.x, 0) * slot_px + row;
   const int t0 = blockIdx.y * kFlowPxPerCta + threadIdx.x;
   for (int k0 = 0; k0 < kFlowPxPerThread; k0 += kFlowBatch) {
     if (t0 + k0 * kFlowThreads >= hw) break;
@@ -121,16 +152,17 @@ __global__ void __launch_bounds__(kFlowThreads) k_flow(DState S, const DMap* __r
 #pragma unroll
     for (int b = 0; b < kFlowBatch; b++) {
       const int t = t0 + (k0 + b) * kFlowThreads;
-      db[b] = valid && t < hw ? __ldg(aux.depth + row + t) : 0.0f;
-      lb[b] = valid && t < hw ? __ldg(aux.labels + row + t) : (int16_t)0;
+      db[b] = (kOcc || valid) && t < hw ? __ldg(aux.depth + row + t) : 0.0f;   // (kOcc: every frame goes to a slot)
+      lb[b] = (kOcc || valid) && t < hw ? __ldg(aux.labels + row + t) : (int16_t)0;
     }
 #pragma unroll
     for (int b = 0; b < kFlowBatch; b++) {
     const int t = t0 + (k0 + b) * kFlowThreads;
     if (t >= hw) break;
     float2 flow = make_float2(nan, nan);
+    float zp = 0.0f;   // the point's depth in the previous camera, where flow is defined
     const float d = db[b];
-    if (d > 0.0f) {   // (0: sky, or no source pixel)
+    if ((!kOcc || valid) && d > 0.0f) {   // (0: sky, or no source pixel)
       int sx, sy;
       if (src) {
         const int v = __ldg(src + t);
@@ -152,6 +184,7 @@ __global__ void __launch_bounds__(kFlowThreads) k_flow(DState S, const DMap* __r
       const float qy = M[4] * ex + M[5] * ey + M[6] * ez + M[7];
       const float qz = M[8] * ex + M[9] * ey + M[10] * ez + M[11];
       if (qz < -kNear) {
+        zp = -qz;
         const float iz = 1.0f / -qz;
         const float x1 = (P00 * qx * iz + 1.0f) * fw * 0.5f, y1 = (1.0f - P11 * qy * iz) * fh * 0.5f;
         if (!fwd) {
@@ -163,8 +196,53 @@ __global__ void __launch_bounds__(kFlowThreads) k_flow(DState S, const DMap* __r
       }
     }
     out[t] = flow;
+    if constexpr (kOcc) {   // DESIGN.md section 5 item 14
+      const int lab = lb[b];
+      uint8_t mv = DTS_OCC_NONE;
+      if (flow.x == flow.x) {   // (NaN in both components or neither)
+        const int py = t / W, px = t - py * W;
+        const float qx = (float)px + 0.5f + flow.x, qy = (float)py + 0.5f + flow.y;
+        if (!(qx >= 0.0f && qx < fw && qy >= 0.0f && qy < fh)) {
+          mv = DTS_OCC_OUTSIDE;
+        } else if (occ.x < 0) {
+          mv = DTS_OCC_UNKNOWN;
+        } else {   // visible where one of the four pixels around q shows the item, and a mesh at the point's depth
+          mv = DTS_OCC_OCCLUDED;
+          const bool flat = lab <= 1 + n_tiles;   // ground or a road tile: cannot hide part of itself
+          const int cx = (int)floorf(qx - 0.5f), cy = (int)floorf(qy - 0.5f);
+#pragma unroll
+          for (int j = 0; j < 2; j++)
+#pragma unroll
+            for (int i = 0; i < 2; i++) {
+              const int x = cx + i, y = cy + j;
+              if (x < 0 || x >= W || y < 0 || y >= H) continue;
+              const int c = y * W + x;
+              if (__ldg(lprev + c) == lab && (flat || fabsf(__ldg(dprev + c) - zp) <= kOccTau * zp)) mv = DTS_OCC_VISIBLE;
+            }
+        }
+      }
+      o.out[row + t] = mv;
+      o.depth[occ.y * slot_px + row + t] = d;   // this frame, the previous one of the next step's mask
+      o.labels[occ.y * slot_px + row + t] = (int16_t)lab;
+    }
     }
   }
+}
+
+// thread per listed env, after k_flow: the slot k_flow wrote now holds this frame.  (Not in k_flow itself, whose other
+// CTAs of the env may still be choosing their slots from the tags.)
+__global__ void __launch_bounds__(128) k_occ_commit(DState S, RenderCfg rc, FlowRecord rec, OcclusionTarget o,
+                                                    bool rectify) {
+  const int slot = blockIdx.x * blockDim.x + threadIdx.x;
+  if (slot >= n_listed(rc.env_list, rc.env_count, rc.n_envs)) return;
+  const int env = listed_env(rc.env_list, slot);
+  const int view = occ_view(rc.mode);
+  const int ws = occ_slots(o, rec, S, env, view, !rectify && __ldg(rec.episode + env) == S.episode[env]).y;
+  const size_t n = S.n;
+  o.tag[(3 * ws) * n + env] = S.episode[env];
+  o.tag[(3 * ws + 1) * n + env] = S.step_count[env];
+  o.tag[(3 * ws + 2) * n + env] = view;
+  o.newest[env] = (uint8_t)ws;
 }
 
 // thread per env: the pose and obstacles the step is about to move, and the episode they belong to
@@ -178,11 +256,17 @@ __global__ void __launch_bounds__(128) k_flow_record(DState S, const DMap* __res
     for (int f = 0; f < 3; f++)
       rec.dyn[((size_t)f * rec.max_dyn + k) * S.n + e] = m.dyn_state[((size_t)fields[f] * m.n_dyn + k) * S.n + e];
   rec.episode[e] = S.episode[e];
+  rec.episode[S.n + e] = S.step_count[e];
 }
 
-__global__ void k_flow_forget(int32_t* __restrict__ episode, const uint8_t* __restrict__ mask, int n) {
+// occ_tag: null, or the occlusion slots' tags, whose frames the env forgets with its record
+__global__ void k_flow_forget(int32_t* __restrict__ episode, int32_t* __restrict__ occ_tag,
+                              const uint8_t* __restrict__ mask, int n) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e < n && (!mask || mask[e])) episode[e] = -1;
+  if (e < n && (!mask || mask[e])) {
+    episode[e] = -1;
+    if (occ_tag) occ_tag[e] = occ_tag[3 * (size_t)n + e] = -1;
+  }
 }
 
 }  // namespace
@@ -192,8 +276,8 @@ std::string flow_record_alloc(FlowRecord& rec, int n_envs, int max_dyn) {
   const size_t n = n_envs;
   cudaError_t e = cudaMalloc(&r.pose, 3 * n * sizeof(double));
   if (e == cudaSuccess) e = cudaMalloc(&r.dyn, 3 * (size_t)(max_dyn > 0 ? max_dyn : 1) * n * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&r.episode, n * sizeof(int32_t));
-  if (e == cudaSuccess) e = cudaMemset(r.episode, 0xff, n * sizeof(int32_t));   // -1: no previous frame
+  if (e == cudaSuccess) e = cudaMalloc(&r.episode, 2 * n * sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaMemset(r.episode, 0xff, 2 * n * sizeof(int32_t));   // -1: no previous frame
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
     flow_record_free(r);
@@ -214,15 +298,56 @@ void launch_flow_record(const DState& S, const DMap* maps, const FlowRecord& rec
   k_flow_record<<<(S.n + 127) / 128, 128, 0, st>>>(S, maps, rec);
 }
 
-void launch_flow_forget(const FlowRecord& rec, const uint8_t* mask, int n_envs, cudaStream_t st) {
-  k_flow_forget<<<(n_envs + 127) / 128, 128, 0, st>>>(rec.episode, mask, n_envs);
+void launch_flow_forget(const FlowRecord& rec, const OcclusionTarget& occ, const uint8_t* mask, int n_envs,
+                        cudaStream_t st) {
+  k_flow_forget<<<(n_envs + 127) / 128, 128, 0, st>>>(rec.episode, occ.tag, mask, n_envs);
 }
 
-void launch_flow(const DState& S, const DMap* maps, const RenderCfg& rc, const FrameCtx* ctx, const AuxTargets& aux,
-                 const FlowTarget& f, const FlowRemap& rm, cudaStream_t st) {
+std::string occlusion_alloc(OcclusionTarget& occ, uint8_t* out, int n_envs, int width, int height) {
+  OcclusionTarget o{out, nullptr, nullptr, nullptr, nullptr};
+  const size_t n = n_envs, px = 2 * n * width * height;
+  cudaError_t e = cudaMalloc(&o.depth, px * sizeof(float));
+  if (e == cudaSuccess) e = cudaMalloc(&o.labels, px * sizeof(int16_t));
+  if (e == cudaSuccess) e = cudaMalloc(&o.tag, 6 * n * sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaMalloc(&o.newest, n);
+  if (e == cudaSuccess) e = cudaMemset(o.newest, 0, n);
+  if (e == cudaSuccess) e = cudaMemset(o.tag, 0xff, 6 * n * sizeof(int32_t));   // episode -1: empty
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    occlusion_free(o);
+    cudaGetLastError();   // (a failed allocation is refused, not left for the next launch to report)
+    return std::string("occlusion slot allocation (") + std::to_string(px * 6 + 25 * n) + " B) failed: " +
+           cudaGetErrorString(e);
+  }
+  occ = o;
+  return "";
+}
+
+std::string occlusion_empty(const OcclusionTarget& occ, int n_envs) {
+  cudaError_t e = cudaMemset(occ.tag, 0xff, 6 * (size_t)n_envs * sizeof(int32_t));
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  return e == cudaSuccess ? "" : std::string("emptying the occlusion slots failed: ") + cudaGetErrorString(e);
+}
+
+void occlusion_free(OcclusionTarget& occ) {
+  cudaFree(occ.depth);
+  cudaFree(occ.labels);
+  cudaFree(occ.tag);
+  cudaFree(occ.newest);
+  occ = OcclusionTarget{};
+}
+
+int launch_flow(const DState& S, const DMap* maps, const RenderCfg& rc, const FrameCtx* ctx, const AuxTargets& aux,
+                const FlowTarget& f, const FlowRemap& rm, const OcclusionTarget& occ, cudaStream_t st) {
   const int hw = rc.width * rc.height;
   const dim3 grid(rc.n_envs, (hw + kFlowPxPerCta - 1) / kFlowPxPerCta);
-  k_flow<<<grid, kFlowThreads, 0, st>>>(S, maps, rc, ctx, aux, f, rm);
+  if (!occ.out) {
+    k_flow<false><<<grid, kFlowThreads, 0, st>>>(S, maps, rc, ctx, aux, f, rm, occ);
+    return 1;
+  }
+  k_flow<true><<<grid, kFlowThreads, 0, st>>>(S, maps, rc, ctx, aux, f, rm, occ);
+  k_occ_commit<<<(rc.n_envs + 127) / 128, 128, 0, st>>>(S, rc, f.rec, occ, rm.rectify);
+  return 2;
 }
 
 }  // namespace dts

@@ -44,7 +44,7 @@ struct __align__(16) FrameCtx {
 struct FlowRecord {
   double* pose;        // [3][n_envs] pos_x, pos_z, angle
   double* dyn;         // [3][max_dyn][n_envs] DTS_DYN_PX, DTS_DYN_PZ, DTS_DYN_YROT of every dynamic slot of the env's map
-  int32_t* episode;    // [n_envs] the episode the record belongs to (DState::episode); -1: none
+  int32_t* episode;    // [2][n_envs] the episode the record belongs to (DState::episode; -1: none), then its step_count
   int32_t max_dyn;     // the largest n_dyn over the uploaded maps
 };
 
@@ -150,10 +150,12 @@ std::string renderer_set_flow_maps(Renderer& r, int count, const float* fwd_x, c
 // `marks`: NULL or kProfMarks events recorded on `st` before k_frame_setup and after each of k_frame_setup, k_geometry,
 // k_bin, k_raster and the post passes (dts_profile_*).  `status_dev`: device address of the mapped host status word.
 // `flow`: the flow image's target (dts_flow.cu), launched after the rasterisers over the same envs; null `out`: none.
+// `occ`: its occlusion mask; null `out`: none.
 struct FlowTarget;
+struct OcclusionTarget;
 constexpr int kProfMarks = 6;
 int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, const AuxTargets& aux,
-                  const FlowTarget& flow, void* obs, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev,
+                  const FlowTarget& flow, const OcclusionTarget& occ, void* obs, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev,
                   cudaEvent_t* marks, int mark_level, cudaStream_t st);
 // What the last render left in frame memory for one env (dts_debug_frame), after the device has synchronised
 std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, int32_t* counts, float* lattice_by_cell,
@@ -192,6 +194,15 @@ struct FlowTarget {
   float* out;
   FlowRecord rec;
 };
+// The occlusion mask of dts_set_occlusion_target (DESIGN.md section 5 item 14), uint8 [n_envs][H][W], and the two
+// slots per env holding the frames it is taken against.  Null `out`: off, and then nothing is allocated.
+struct OcclusionTarget {
+  uint8_t* out;
+  float* depth;        // [2][n_envs][H][W] each slot's depth image
+  int16_t* labels;     // [2][n_envs][H][W] each slot's label image
+  int32_t* tag;        // [2][3][n_envs] each slot's frame: its episode (-1: empty), step_count and view (occ_view)
+  uint8_t* newest;     // [n_envs] the slot written last
+};
 // What the flow pass reads of the frame's remap: nothing (src_xy null: the pinhole frame), the fisheye table or pool
 // with its forward maps (fwd: [tables][H][W], the env's table named by table_of_env where that is not null), or the
 // rectification, whose forward map does not exist: every pixel NaN.
@@ -207,11 +218,18 @@ std::string flow_record_alloc(FlowRecord& rec, int n_envs, int max_dyn);
 void flow_record_free(FlowRecord& rec);
 // every env's camera and obstacles now, as the previous frame of its next render: launched just before k_step_logic
 void launch_flow_record(const DState& S, const DMap* maps, const FlowRecord& rec, cudaStream_t st);
-// every env e with mask[e] (null: all) forgets its previous frame (episode -1), stream-ordered
-void launch_flow_forget(const FlowRecord& rec, const uint8_t* mask, int n_envs, cudaStream_t st);
+// every env e with mask[e] (null: all) forgets its previous frame (episode -1) and, where `occ` is set, empties its
+// occlusion slots; stream-ordered
+void launch_flow_forget(const FlowRecord& rec, const OcclusionTarget& occ, const uint8_t* mask, int n_envs,
+                        cudaStream_t st);
+// Slots for n_envs frames of width x height, all empty, and the mask at `out`; synchronous.  On failure (error text)
+// `occ` is untouched.
+std::string occlusion_alloc(OcclusionTarget& occ, uint8_t* out, int n_envs, int width, int height);
+std::string occlusion_empty(const OcclusionTarget& occ, int n_envs);   // every slot; synchronous
+void occlusion_free(OcclusionTarget& occ);
 // The flow image of the listed envs (rc.env_list, or all) from the depth and label images the render just wrote and
-// the frames' cameras in `ctx`
-void launch_flow(const DState& S, const DMap* maps, const RenderCfg& rc, const FrameCtx* ctx, const AuxTargets& aux,
-                 const FlowTarget& f, const FlowRemap& rm, cudaStream_t st);
+// the frames' cameras in `ctx`; with `occ.out`, also the occlusion mask, then the slots' tags.  Returns the launches.
+int launch_flow(const DState& S, const DMap* maps, const RenderCfg& rc, const FrameCtx* ctx, const AuxTargets& aux,
+                const FlowTarget& f, const FlowRemap& rm, const OcclusionTarget& occ, cudaStream_t st);
 
 }  // namespace dts

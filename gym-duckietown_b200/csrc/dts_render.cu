@@ -2602,7 +2602,7 @@ template <const auto& kList, typename F>
 static void for_each_of(F f) { each_of<kList>(f, std::make_index_sequence<std::size(kList)>{}); }
 
 int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, const AuxTargets& aux,
-                  const FlowTarget& flow, void* obs_any, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev,
+                  const FlowTarget& flow, const OcclusionTarget& occ, void* obs_any, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev,
                   cudaEvent_t* marks, int mark_level, cudaStream_t st) {
   uint8_t* obs = reinterpret_cast<uint8_t*>(obs_any);
   // the table the frame is remapped through, if any: the rectification (DTS_RENDER_RECTIFY), none (DTS_RENDER_PINHOLE
@@ -2665,8 +2665,7 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   mark();
   if (flow.out) {   // (inside the post-pass event bracket)
     const FlowRemap fr{lut ? rt.src_xy : nullptr, rt.table_of_env, rt.fwd, (rc.mode & DTS_RENDER_RECTIFY) != 0};
-    launch_flow(S, maps, rc, fm.ctx, aux, flow, fr, st);
-    launches++;
+    launches += launch_flow(S, maps, rc, fm.ctx, aux, flow, fr, occ, st);
   }
   mark();   // (post passes: launched by the caller)
   return launches;

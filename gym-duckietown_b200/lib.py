@@ -20,6 +20,8 @@ FLAG_AUTO_RESET, FLAG_DOMAIN_RAND, FLAG_DISTORTION, FLAG_DYNAMICS_RAND, FLAG_TES
 FLAG_CAMERA_RAND = 32
 IN_PROGRESS, INVALID_POSE, MAX_STEPS = 0, 1, 2
 DONE_CODE_STR = {0: "in-progress", 1: "invalid-pose", 2: "max-steps-reached"}  # S:1685-1705
+# the occlusion mask's values (DTS_OCC_*, dts_set_occlusion_target), by value
+OCCLUSION_NAMES = ("none", "visible", "occluded", "outside", "unknown")
 
 
 class DtsError(RuntimeError):
@@ -197,6 +199,7 @@ def load() -> C.CDLL:
     lib.dts_set_bev_target.argtypes = [vp, C.POINTER(BevConfig), vp, vp]
     lib.dts_render_bev.argtypes = [vp, vp]
     lib.dts_set_flow_target.argtypes = [vp, vp, vp, vp, i]
+    lib.dts_set_occlusion_target.argtypes = [vp, vp]
     lib.dts_resize_frames.argtypes = [vp, vp, vp, vp]
     lib.dts_blend4.argtypes = [vp, vp, vp, vp, C.c_uint64, vp]
     lib.dts_set_timing.argtypes = [vp, C.c_double, i, i]
@@ -231,7 +234,7 @@ def load() -> C.CDLL:
 
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_fisheye_luts", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
-           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_set_flow_target", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
+           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_set_flow_target", "dts_set_occlusion_target", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
            "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
 
@@ -533,6 +536,12 @@ class Sim:
         if fx.ndim != 3 or fx.shape != fy.shape or fx.shape[1:] != (self.cfg.cam_height, self.cfg.cam_width):
             raise ValueError(f"flow forward maps: {fx.shape} and {fy.shape} must both be [tables, cam_height, cam_width]")
         self._check(self.lib.dts_set_flow_target(self.h, flow_ptr, _ptr(fx), _ptr(fy), fx.shape[0]), "dts_set_flow_target")
+
+    def set_occlusion_target(self, occ_ptr: Optional[int]):
+        """Every later render that writes flow also writes the uint8 [num_envs, cam_height, cam_width] occlusion mask
+        (OCCLUSION_NAMES) at `occ_ptr`, which the caller keeps alive; needs the flow target.  None turns it off
+        (dts_set_occlusion_target)."""
+        self._check(self.lib.dts_set_occlusion_target(self.h, occ_ptr), "dts_set_occlusion_target")
 
     def set_resize(self, out_w: int, out_h: int, filter: int = 0):
         """filter RESIZE_CV2_CUBIC (dts_set_resize) or RESIZE_PIL_BILINEAR (dts_set_resize_filter)."""

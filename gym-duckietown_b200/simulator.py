@@ -71,7 +71,8 @@ class Simulator(Env):
                  camera_rand: bool = False, randomize_maps_on_reset: bool = False, num_tris_distractors: int = 12,
                  color_ground=(0.15, 0.15, 0.15), color_sky=(0.45, 0.82, 1), style: str = "photos",
                  enable_leds: bool = False, device: int = 0, depth: bool = False, labels: bool = False,
-                 markings: bool = False, bev: bool = False, flow: bool = False, **env_kwargs):
+                 markings: bool = False, bev: bool = False, flow: bool = False, flow_occlusion: bool = False,
+                 **env_kwargs):
         if draw_curve or draw_bbox or enable_leds:
             raise NotImplementedError("draw_curve / draw_bbox / enable_leds are debug modes outside the hot path "
                                       "(SURVEY 8f-4)")
@@ -98,7 +99,7 @@ class Simulator(Env):
             camera_rand_pool=env_kwargs.pop("camera_rand_pool", 1),   # one camera per Simulator (distortion.py:46-47)
             color_ground=color_ground, color_sky=color_sky, num_tris_distractors=num_tris_distractors,
             action_mode=self._action_mode, depth=depth, labels=labels, markings=markings, bev=bev, flow=flow,
-            **env_kwargs)
+            flow_occlusion=flow_occlusion, **env_kwargs)
         self._b = BatchedDuckietownEnv(1, map_arg, **self._env_kwargs)
         self._adopt_map()
         self.action_space = spaces.Box(low=-1, high=1, shape=(2,), dtype=np.float32)              # S:309
@@ -160,7 +161,8 @@ class Simulator(Env):
         from .batched_env import BatchedDuckietownEnv
         if getattr(self, "_human", None) is None:
             kw = dict(self._env_kwargs, camera_width=WINDOW_WIDTH, camera_height=WINDOW_HEIGHT, distortion=False,
-                      terminal_obs=False, depth=False, labels=False, markings=False, bev=False, flow=False)
+                      terminal_obs=False, depth=False, labels=False, markings=False, bev=False, flow=False,
+                      flow_occlusion=False)
             self._human = BatchedDuckietownEnv(1, list(self._b.maps), **kw)
         self._human.load_state(self._b.save_state())
         return self._human
@@ -242,6 +244,14 @@ class Simulator(Env):
         (BatchedDuckietownEnv.flow); else None.  flow=True also turns on depth and labels."""
         f = self._b.flow
         return None if f is None else f[0].cpu().numpy()
+
+    @property
+    def flow_occlusion(self) -> Optional[np.ndarray]:
+        """With flow_occlusion=True: uint8 [camera_height, camera_width], whether each pixel of `flow` was in view at its
+        previous position, named by OCCLUSION_NAMES (BatchedDuckietownEnv.flow_occlusion); else None.
+        flow_occlusion=True also turns on flow, depth and labels."""
+        o = self._b.flow_occlusion
+        return None if o is None else o[0].cpu().numpy()
 
     @property
     def cur_pos(self):

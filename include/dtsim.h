@@ -402,8 +402,8 @@ int dts_render_bev(dts_sim* sim, void* stream);
  * env's table, sampled bilinearly (OpenCV's convention: index = position - 0.5).  NaN where: the depth is 0 (sky, no
  * source pixel); the env has no previous frame (nothing stepped since dts_set_flow_target, a map upload, a reset or
  * respawn, or a dts_load_state of that env); the render is DTS_RENDER_RECTIFY; the point was not in front of the previous
- * camera's near plane; or, under the fisheye, the forward map's footprint leaves the table.  No occlusion mask: a point
- * hidden in the previous frame still gets its motion.  After a step, dts_render gives the step's flow again; after a step
+ * camera's near plane; or, under the fisheye, the forward map's footprint leaves the table.  A point hidden in the
+ * previous frame still gets its motion: dts_set_occlusion_target says which pixels were in view there.  After a step, dts_render gives the step's flow again; after a step
  * without a render, the next render gives that step's.  A pass over listed envs (the second pass of dts_step_terminal)
  * writes only those envs' rows — NaN, as they respawned — so row e matches obs_dev row e; the terminal frames' flow is
  * not kept.
@@ -417,6 +417,33 @@ int dts_render_bev(dts_sim* sim, void* stream);
  * more kernel (k_flow), and dts_step, dts_step_terminal and dts_load_state one more each.  Synchronises.  An output, not state: snapshots and the gathers do not
  * carry it, nor the record. */
 int dts_set_flow_target(dts_sim* sim, float* flow_dev, const float* fwd_x, const float* fwd_y, int n_tables);
+/* Occlusion mask beside the flow image (DESIGN.md section 5, item 14): every later render that writes flow_dev also
+ * writes occ_dev, uint8 [num_envs][cam_height][cam_width], one DTS_OCC_* value per pixel, checked in this order:
+ *   DTS_OCC_NONE      the pixel's flow is NaN
+ *   DTS_OCC_OUTSIDE   q = p + 0.5 + flow, the pixel's position in the previous frame, lies outside [0, W) x [0, H)
+ *   DTS_OCC_UNKNOWN   no render of the recorded state (the start of the env's last step) in this view was kept
+ *   DTS_OCC_VISIBLE   one of the up to four pixels around q, (floor(q - 0.5) + {0, 1}) clipped to the frame, showed the
+ *                     same label in that render and, unless the label is the ground or a road tile, a depth within
+ *                     2 % of the point's depth in the previous camera
+ *   DTS_OCC_OCCLUDED  otherwise: the previous frame shows something else at q
+ * Under the fisheye most points that leave the view already have NaN flow (F's footprint leaves the table): NONE.
+ * The previous frames are kept by the library: two slots per env of a depth and a label image (12 bytes per pixel
+ * across both), each tagged with the episode, step_count and view (the DTS_RENDER_TOP_DOWN, _PINHOLE and _RECTIFY bits;
+ * not _SEGMENT) of the frame it holds.  A render reads the slot of its flow record's state in its view, if there is one,
+ * and writes its own frame into the other slot, or with no match into the one written less recently.  So dts_render
+ * after a step repeats the step's mask; after a step without a render the next step's mask is UNKNOWN; a render in
+ * another view between two steps leaves the next step's mask intact; after dts_step_terminal row e matches obs_dev row
+ * e (respawned envs NONE; the terminal frames' masks are not kept, but the respawned frames are, so their next step
+ * has a mask).  The slots are emptied by this call, dts_set_flow_target, a map upload, and dts_load_state for the
+ * loaded envs.
+ * Refused (non-zero, the previous setting kept) unless a flow target is set, or when the slots cannot be allocated;
+ * while it is set, clearing the flow target is refused.  Sticky; the memory is the caller's and must stay valid while
+ * it is set.  NULL turns it off, and then the renders launch the very kernels they launch without this call.  With it
+ * set, every render launches one more kernel (k_occ_commit, after k_flow) and k_flow is its mask-writing instance;
+ * dts_step, dts_step_terminal and dts_load_state launch what they launch with flow alone.  Synchronises.  An output,
+ * not state: snapshots and the gathers carry neither it nor the slots. */
+enum { DTS_OCC_NONE = 0, DTS_OCC_VISIBLE = 1, DTS_OCC_OCCLUDED = 2, DTS_OCC_OUTSIDE = 3, DTS_OCC_UNKNOWN = 4 };
+int dts_set_occlusion_target(dts_sim* sim, uint8_t* occ_dev);
 /* Select the fused wrapper behaviour for subsequent dts_step / dts_render calls (default: all zero, scale 1).
  * obs_dev then holds num_envs * 3 * H * W elements of uint8 or float32 in the chosen layout. */
 int dts_set_output_format(dts_sim* sim, const dts_output_format* fmt);

@@ -1,5 +1,5 @@
 """A small tour of every kernel for compute-sanitizer (memcheck / racecheck / initcheck): meshes, fisheye at 640x480,
-wrapper layouts, the device resize, device resets, the literal tile mode."""
+wrapper layouts, the device resize, device resets, the literal tile mode, the flow image with its occlusion mask."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from gym_duckietown_b200.batched_env import BatchedDuckietownEnv
@@ -21,3 +21,5 @@ print("pil resize", run(24, "udem1", 640, 480, fmt=("chw", "float32"), resize=(1
 print("pil resize odd", run(7, "loop_obstacles", 162, 121, resize=(53, 40), method="pil_bilinear"))
 print("literal tiles", run(16, "small_loop", 160, 120, tessellate_tiles=True))
 print("dynamic", run(32, "loop_pedestrians", 160, 120, steps=4))
+print("flow occlusion", run(8, "loop_dyn_duckiebots", 160, 120, steps=4, flow_occlusion=True))
+print("flow occlusion fisheye", run(3, "udem1", 640, 480, steps=2, distortion=True, flow_occlusion=True))
