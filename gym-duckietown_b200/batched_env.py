@@ -5,7 +5,7 @@ observation buffers are caller-visible torch CUDA tensors, the work runs on
 `torch.cuda.current_stream()` inside libdtsim.so, nothing synchronises.  Constructor keywords are the
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
 `auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `flow`, `flow_occlusion`,
-`camera_rand_pool` and the `bev*` keywords.
+`camera_rand_pool` and the `bev*` keywords (`bev_visibility` among them).
 
 `camera_rand=True` (with `distortion=True`; without it the flag does nothing, as in the reference, S:352-358) gives the
 envs a spread of lenses: `camera_rand_pool` calibrations K, D are drawn once, at construction, within the reference's
@@ -80,6 +80,19 @@ leave the view have NaN flow, so 0.  The library keeps the previous frames itsel
 (12 bytes per camera pixel: 944 MB at 4096 envs of 160 x 120), so `render_obs()` after a step repeats the step's mask,
 and a `render_obs(top_down=True)` between two steps leaves the next step's mask intact.  The terminal frames' masks are
 not kept; `load_state`, `copy_envs` and a map upload forget the envs' previous frames.
+
+`bev_visibility=True` allocates `env.bev_visibility`, uint8 [num_envs, height, width], and `env.bev_pixels`, float32
+[num_envs, height, width, 2], in the bird's-eye grid's shape (dts_set_bev_visibility_target; it turns on `bev` and
+`labels`): for each cell, whether the frame in `obs` shows it and where.  The cell's surface point — its centre on the
+road tile or on the ground quad, 8 mm lower (for an object cell, the surface under the object) — is projected through
+that frame's camera, and under the fisheye through the env's forward map, to q in camera pixels (pixel centres at +0.5,
+as `flow`), which `bev_pixels` holds.  `bev_visibility` names the answer by BEV_VISIBILITY_NAMES: 0 unknown (no frame
+was drawn: `step(render=False)`, `render_bev()`), 1 visible (one of the four pixels around q shows the cell's grid
+label), 3 outside (behind the camera, beyond its near or far plane, off the frame, off the forward map, or all four
+pixels show nothing: sky or no fisheye source), 2 occluded (something else is in front of it).  `bev_pixels` is NaN
+for unknown and outside.  Under `auto_reset` a row matches its `obs` row.  A visibility env refuses
+`set_rectification`, whose remap has no forward map.  `frame_cameras()` returns every env's camera of its last frame,
+on the device, to turn `bev_pixels` or `depth` into rays.  Snapshots and gathers do not carry them.
 """
 from __future__ import annotations
 
@@ -90,6 +103,7 @@ import torch
 
 from . import lib as L
 from .assets import MARKING_NAMES  # noqa: F401  (the names of env.markings' values)
+from .lib import BEV_VISIBILITY_NAMES  # noqa: F401  (the names of env.bev_visibility's values)
 from .lib import OCCLUSION_NAMES  # noqa: F401  (the names of env.flow_occlusion's values)
 from .episode import EpisodeSampler
 from .maps import TILE_KINDS, MapData, load_map
@@ -122,12 +136,13 @@ class BatchedDuckietownEnv:
                  randomize_maps_on_reset: bool = False, randomization_config=None, terminal_obs: bool = False,
                  depth: bool = False, labels: bool = False, camera_rand_pool: int = 16, markings: bool = False,
                  bev: bool = False, bev_shape=(64, 64), bev_cell: float = 0.03, bev_origin=None, flow: bool = False,
-                 flow_occlusion: bool = False):
+                 flow_occlusion: bool = False, bev_visibility: bool = False):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
         camera_rand = bool(camera_rand and distortion)   # S:353-356: camera_rand only with distortion
         flow = flow or flow_occlusion                    # the mask is taken with the flow image
         depth, labels = depth or flow, labels or flow    # the flow image is taken from both
+        bev, labels = bev or bev_visibility, labels or bev_visibility   # the visibility compares their labels
         if camera_rand and not 1 <= int(camera_rand_pool) <= 65536:
             raise ValueError(f"camera_rand_pool must be 1 to 65536, not {camera_rand_pool}")
         self.camera_rand = camera_rand
@@ -206,6 +221,11 @@ class BatchedDuckietownEnv:
             # which of those pixels were in view in the previous frame (flow_occlusion=True), OCCLUSION_NAMES
             self.flow_occlusion: Optional[torch.Tensor] = torch.zeros(
                 (num_envs, camera_height, camera_width), dtype=torch.uint8, device=self.device) if flow_occlusion else None
+            # whether the frames in obs show each cell of the grid, and where (bev_visibility=True), BEV_VISIBILITY_NAMES
+            self.bev_visibility: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, bh, bw), dtype=torch.uint8, device=self.device) if bev_visibility else None
+            self.bev_pixels: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, bh, bw, 2), dtype=torch.float32, device=self.device) if bev_visibility else None
             self.reward = torch.zeros(num_envs, dtype=torch.float32, device=self.device)
             self._done_u8 = torch.zeros(num_envs, dtype=torch.uint8, device=self.device)
             self.state: Dict[str, torch.Tensor] = {
@@ -233,12 +253,15 @@ class BatchedDuckietownEnv:
             ox, oy = (bw / 2, 3 * bh / 4) if bev_origin is None else (float(v) for v in bev_origin)
             self.bev_config = L.BevConfig(bw, bh, float(bev_cell), float(ox), float(oy))
             self.sim.set_bev_target(self.bev_config, self.bev_labels.data_ptr(), self.bev_markings.data_ptr())
-        if flow:   # the forward maps of the fisheye tables, in the pool's order
-            models = self.camera_models if camera_rand else [self.camera_model] if distortion else None
-            self.sim.set_flow_target(self.flow.data_ptr(), *((np.stack([m.mapx for m in models]),
-                                                              np.stack([m.mapy for m in models])) if models else ()))
+        # the forward maps of the fisheye tables, in the pool's order
+        models = self.camera_models if camera_rand else [self.camera_model] if distortion else None
+        fwd = (np.stack([m.mapx for m in models]), np.stack([m.mapy for m in models])) if models else ()
+        if flow:
+            self.sim.set_flow_target(self.flow.data_ptr(), *fwd)
         if flow_occlusion:
             self.sim.set_occlusion_target(self.flow_occlusion.data_ptr())
+        if bev_visibility:
+            self.sim.set_bev_visibility_target(self.bev_visibility.data_ptr(), self.bev_pixels.data_ptr(), *fwd)
         self.seed(seed)
 
     def set_output_format(self, obs_layout: Optional[str] = None, obs_dtype: Optional[str] = None,
@@ -316,11 +339,14 @@ class BatchedDuckietownEnv:
         """UndistortWrapper's `cv2.remap(obs, mapx, mapy, INTER_NEAREST)` of reset / step observations, fused into the
         render (dts_set_rectify_lut): each output pixel is rendered at the source pixel the map names.  Applies while
         `undistort` is True; needs an env built with distortion=True.  None, None removes it.  A map the device refuses
-        raises and leaves the previous one in effect.  Refused (ValueError) on a flow env: the rectification's remap has
-        no forward map, so its frames would have no flow."""
+        raises and leaves the previous one in effect.  Refused (ValueError) on a flow or bev_visibility env: the
+        rectification's remap has no forward map, so its frames would have neither."""
         if self.flow is not None:
             raise ValueError("set_rectification: the flow image cannot follow the rectification (no forward map); "
                              "build the env without flow=True")
+        if self.bev_visibility is not None:
+            raise ValueError("set_rectification: the bird's-eye visibility cannot follow the rectification (no forward "
+                             "map); build the env without bev_visibility=True")
         self.sim.set_rectify_lut(mapx, mapy)
         self.rectification = None if mapx is None and mapy is None else (mapx, mapy)
         self.sim.set_render_mode(**self._base_mode())
@@ -416,6 +442,16 @@ class BatchedDuckietownEnv:
         else:
             self.sim.render(tgt.data_ptr(), self._stream())
         return tgt
+
+    def frame_cameras(self):
+        """(V float64 [num_envs, 3, 4], P float32 [num_envs, 4]) on the device: every env's camera of its last frame,
+        the model-view [R|t] and gluPerspective's P00, P11, P22, P23 (dts_get_frame_cameras), written on the current
+        stream.  Raises before the first render."""
+        with torch.cuda.device(self.device):
+            V = torch.empty((self.num_envs, 3, 4), dtype=torch.float64, device=self.device)
+            P = torch.empty((self.num_envs, 4), dtype=torch.float32, device=self.device)
+            self.sim.get_frame_cameras(V.data_ptr(), P.data_ptr(), self._stream())
+        return V, P
 
     def render_bev(self):
         """Write `bev_labels` / `bev_markings` for the current state (dts_render_bev), without rendering a frame."""

@@ -47,6 +47,8 @@ struct dts_sim {
   BevTarget bev{};                      // dts_set_bev_target: caller-owned grids, both null = off
   FlowTarget flow{};                    // dts_set_flow_target: caller-owned image and the record it owns, null = off
   OcclusionTarget occ{};                // dts_set_occlusion_target: caller-owned mask and the slots it owns, null = off
+  BevViewTarget bev_view{};             // dts_set_bev_visibility_target: caller-owned outputs, both null = off
+  bool drawn = false;                   // frame memory holds a frame of every env (dts_get_frame_cameras)
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
   int profiling = 0;                    // 0 off, 1 events around k_raster only, 2 around every render kernel
   std::vector<cudaEvent_t> prof_events; // kProfMarks events per profiled frame
@@ -212,6 +214,7 @@ int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
   const std::string e = maps_upload(*sim->maps, map_id, b);
   if (!e.empty()) return sim->fail("%s", e.c_str());
   renderer_release_frame(*sim->render);
+  sim->drawn = false;
   // the records now cover this map's obstacles, and the fingerprint its content: older records no longer load
   const std::string ls = state_layout(*sim->state, *sim->maps);
   if (!ls.empty()) return sim->fail("%s", ls.c_str());
@@ -365,7 +368,8 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
   if (check_gather(sim)) return 1;
   if (check_maps(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  const std::string e = renderer_prepare(*sim->render, maps_counts(*sim->maps), sim->render_mode, sim->flow.out != nullptr);
+  const bool forward = sim->flow.out || sim->bev_view.vis || sim->bev_view.pix;   // a pass reads the forward maps
+  const std::string e = renderer_prepare(*sim->render, maps_counts(*sim->maps), sim->render_mode, forward);
   if (!e.empty()) return sim->fail("%s", e.c_str());
   RenderCfg rc{sim->cfg.cam_width, sim->cfg.cam_height, sim->cfg.flags, sim->cfg.num_envs,
                (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->render_mode,
@@ -405,6 +409,7 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
   if (marks && mark_level >= 2) cudaEventRecord(marks[kProfMarks - 1], (cudaStream_t)stream);   // closes the "post" interval
   sim->launches += k;
   DTS_CUDA(cudaGetLastError());
+  sim->drawn = sim->drawn || !env_list;
   return 0;
 }
 
@@ -419,16 +424,30 @@ static int bev_pass(dts_sim* sim, void* stream) {
   return 0;
 }
 
+// The camera visibility of the grids bev_pass wrote, where a target is set (dts_set_bev_visibility_target): launched
+// last in the call, against the frame the call drew (its camera, labels and remap), or with none every cell UNKNOWN
+static int bev_view_pass(dts_sim* sim, void* stream, bool drew_frame) {
+  if (!sim->bev_view.vis && !sim->bev_view.pix) return 0;
+  launch_bev_view(state_arrays(*sim->state), maps_table(*sim->maps), sim->bev, sim->bev_view,
+                  drew_frame ? renderer_frame_ctx(*sim->render) : nullptr, sim->aux.labels, sim->cfg.cam_width,
+                  sim->cfg.cam_height, renderer_remap(*sim->render, sim->render_mode), drew_frame, (cudaStream_t)stream);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  return 0;
+}
+
 int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
   if (!sim) return 1;
   if (render_pass(sim, obs_dev, stream, nullptr, nullptr)) return 1;
-  return bev_pass(sim, stream);
+  if (bev_pass(sim, stream)) return 1;
+  return bev_view_pass(sim, stream, true);
 }
 
 int dts_render_bev(dts_sim* sim, void* stream) {
   if (!sim) return 1;
   if (!sim->bev.labels && !sim->bev.marks) return sim->fail("no bird's-eye target is set (dts_set_bev_target)");
-  return bev_pass(sim, stream);
+  if (bev_pass(sim, stream)) return 1;
+  return bev_view_pass(sim, stream, false);
 }
 
 // With a flow target: every env's camera and obstacles before the step, the previous frame of the next render's flow
@@ -470,7 +489,7 @@ int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, voi
   DTS_CUDA(cudaGetLastError());
   // the grids of the state obs_dev will show: the ended envs' first states (every env's row, as the others did not move)
   if (bev_pass(sim, stream)) return 1;
-  if (!obs_dev) return 0;
+  if (!obs_dev) return bev_view_pass(sim, stream, false);
   // 4. their terminal frames -> terminal_obs_dev; 5. their first frames -> obs_dev
   const ResizeTarget rz = resizer_target(*sim->resize);
   const size_t px = rz.ow ? (size_t)rz.ow * rz.oh : (size_t)sim->cfg.cam_width * sim->cfg.cam_height;
@@ -478,7 +497,8 @@ int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, voi
   launch_copy_rows(obs_dev, terminal_obs_dev, row_bytes, sim->ended, sim->n_ended, sim->cfg.num_envs, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
-  return render_pass(sim, obs_dev, stream, sim->ended, sim->n_ended);
+  if (render_pass(sim, obs_dev, stream, sim->ended, sim->n_ended)) return 1;
+  return bev_view_pass(sim, stream, true);   // every row against the frame obs_dev shows
 }
 
 int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* reward_dev, uint8_t* done_dev,
@@ -495,8 +515,8 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   if (bev_pass(sim, stream)) return 1;
-  if (obs_dev) return render_pass(sim, obs_dev, stream, nullptr, nullptr);
-  return 0;
+  if (obs_dev && render_pass(sim, obs_dev, stream, nullptr, nullptr)) return 1;
+  return bev_view_pass(sim, stream, obs_dev != nullptr);
 }
 
 int dts_get_state(dts_sim* sim, dts_state_view* v) {
@@ -661,6 +681,8 @@ int dts_set_label_target(dts_sim* sim, int16_t* labels_dev) {
   if (!sim) return 1;
   if (reinterpret_cast<uintptr_t>(labels_dev) & 1) return sim->fail("label target is not aligned to 2 bytes");
   if (!labels_dev && sim->flow.out) return sim->fail("the flow target reads the label image: clear it (dts_set_flow_target) first");
+  if (!labels_dev && (sim->bev_view.vis || sim->bev_view.pix))
+    return sim->fail("the bird's-eye visibility reads the label image: clear it (dts_set_bev_visibility_target) first");
   if (labels_dev && check_labels_fit(sim)) return 1;
   sim->aux.labels = labels_dev;
   return 0;
@@ -668,6 +690,13 @@ int dts_set_label_target(dts_sim* sim, int16_t* labels_dev) {
 
 int dts_set_bev_target(dts_sim* sim, const dts_bev_config* cfg, int16_t* labels_dev, uint8_t* markings_dev) {
   if (!sim) return 1;
+  if (sim->bev_view.vis || sim->bev_view.pix) {   // its outputs are sized for this grid, and it reads its labels
+    if (!cfg || !labels_dev)
+      return sim->fail("the bird's-eye visibility reads the grid's labels: clear it (dts_set_bev_visibility_target) first");
+    if (cfg->width != sim->bev.cfg.width || cfg->height != sim->bev.cfg.height)
+      return sim->fail("the bird's-eye visibility target is sized for the %d x %d grid: clear it "
+                       "(dts_set_bev_visibility_target) before reshaping the grid", sim->bev.cfg.width, sim->bev.cfg.height);
+  }
   if (!cfg || (!labels_dev && !markings_dev)) {
     sim->bev = BevTarget{};
     return 0;
@@ -684,6 +713,17 @@ int dts_set_bev_target(dts_sim* sim, const dts_bev_config* cfg, int16_t* labels_
   return 0;
 }
 
+// The forward maps a flow or bird's-eye visibility target takes: one per fisheye table on a DTS_FLAG_DISTORTION handle,
+// none without
+static int check_forward_maps(dts_sim* sim, const float* fwd_x, const float* fwd_y, int n_tables) {
+  const bool fish = (sim->cfg.flags & DTS_FLAG_DISTORTION) != 0;
+  if (fish && (!fwd_x || !fwd_y || n_tables < 1))
+    return sim->fail("a DTS_FLAG_DISTORTION handle needs the forward map of every fisheye table (fwd_x, fwd_y, n_tables)");
+  if (!fish && (fwd_x || fwd_y || n_tables))
+    return sim->fail("forward maps on a handle without DTS_FLAG_DISTORTION: pass NULL, NULL, 0");
+  return 0;
+}
+
 int dts_set_flow_target(dts_sim* sim, float* flow_dev, const float* fwd_x, const float* fwd_y, int n_tables) {
   if (!sim) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
@@ -693,17 +733,14 @@ int dts_set_flow_target(dts_sim* sim, float* flow_dev, const float* fwd_x, const
     DTS_CUDA(cudaDeviceSynchronize());   // no step or render in flight still writes the record or reads the maps
     flow_record_free(sim->flow.rec);
     sim->flow = FlowTarget{};
-    renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
+    if (!sim->bev_view.vis && !sim->bev_view.pix) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
     return 0;
   }
   if (reinterpret_cast<uintptr_t>(flow_dev) & 7) return sim->fail("flow target is not aligned to 8 bytes");
   if (!sim->aux.depth || !sim->aux.labels)
     return sim->fail("the flow image is taken from the depth and label images: set both targets first");
+  if (check_forward_maps(sim, fwd_x, fwd_y, n_tables)) return 1;
   const bool fish = (sim->cfg.flags & DTS_FLAG_DISTORTION) != 0;
-  if (fish && (!fwd_x || !fwd_y || n_tables < 1))
-    return sim->fail("a DTS_FLAG_DISTORTION handle needs the forward map of every fisheye table (fwd_x, fwd_y, n_tables)");
-  if (!fish && (fwd_x || fwd_y || n_tables))
-    return sim->fail("forward maps on a handle without DTS_FLAG_DISTORTION: pass NULL, NULL, 0");
   DTS_CUDA(cudaDeviceSynchronize());
   FlowRecord rec;
   std::string e = flow_record_alloc(rec, sim->cfg.num_envs, largest_n_dyn(sim));
@@ -734,6 +771,41 @@ int dts_set_occlusion_target(dts_sim* sim, uint8_t* occ_dev) {
   }
   occlusion_free(sim->occ);
   sim->occ = occ;
+  return 0;
+}
+
+int dts_set_bev_visibility_target(dts_sim* sim, uint8_t* vis_dev, float* pix_dev, const float* fwd_x, const float* fwd_y,
+                                  int n_tables) {
+  if (!sim) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  if (!vis_dev && !pix_dev) {
+    DTS_CUDA(cudaDeviceSynchronize());   // no call in flight still reads the forward maps
+    sim->bev_view = BevViewTarget{};
+    if (!sim->flow.out) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
+    return 0;
+  }
+  if (reinterpret_cast<uintptr_t>(pix_dev) & 7) return sim->fail("bird's-eye pixel target is not aligned to 8 bytes");
+  if (!sim->bev.labels || !sim->aux.labels)
+    return sim->fail("the bird's-eye visibility compares the grid's labels with the frame's: set the bird's-eye label "
+                     "target (dts_set_bev_target) and the label target (dts_set_label_target) first");
+  if (check_forward_maps(sim, fwd_x, fwd_y, n_tables)) return 1;
+  DTS_CUDA(cudaDeviceSynchronize());
+  if (sim->cfg.flags & DTS_FLAG_DISTORTION) {
+    const std::string e = renderer_set_flow_maps(*sim->render, n_tables, fwd_x, fwd_y);
+    if (!e.empty()) return sim->fail("%s", e.c_str());
+  }
+  sim->bev_view = BevViewTarget{vis_dev, reinterpret_cast<float2*>(pix_dev)};
+  return 0;
+}
+
+int dts_get_frame_cameras(dts_sim* sim, double* V_dev, float* P_dev, void* stream) {
+  if (!sim) return 1;
+  if (!V_dev || !P_dev) return sim->fail("V_dev and P_dev must not be NULL");
+  if (!sim->drawn) return sim->fail("no frame drawn since the handle was created or a map was uploaded");
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  launch_frame_cameras(renderer_frame_ctx(*sim->render), sim->cfg.num_envs, V_dev, P_dev, (cudaStream_t)stream);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
   return 0;
 }
 

@@ -1,7 +1,9 @@
 // dts_bev.cu — the bird's-eye map (dts_set_bev_target, DESIGN.md section 5 item 12): a grid of cells fixed to every
 // agent, each point-sampled from the map's own tables at its centre — the tile under it, the class of the texel under it
 // and the first object whose footprint holds it.  No rasteriser: a thread per cell, float64 in the order the spec states
-// (-fmad=false keeps every product and sum separately rounded, as numpy's are).
+// (-fmad=false keeps every product and sum separately rounded, as numpy's are).  k_bev_view then says, cell by cell,
+// whether the frame the call drew shows the grid (dts_set_bev_visibility_target, item 15).
+#include "dts_camera.cuh"
 #include "dts_kernels.h"
 
 namespace dts {
@@ -162,12 +164,121 @@ __global__ void __launch_bounds__(kBevThreads) k_bev(DState S, const DMap* __res
   }
 }
 
+constexpr int kViewThreads = 256;
+constexpr int kViewCellsPerThread = 4;
+constexpr int kViewCellsPerCta = kViewThreads * kViewCellsPerThread;
+constexpr double kGroundY = (double)(float)(-0.8 * 0.01);   // the ground quad's height (draw_ground, S:1805-1812)
+
+// grid (env, chunk of kViewCellsPerCta cells), one thread per cell of the chunk at a time, rows stored contiguously.
+// The cell centres are k_bev's, bit for bit, so a cell's surface (road tile or ground) is the one its label was taken on.
+__global__ void __launch_bounds__(kViewThreads) k_bev_view(DState S, const DMap* __restrict__ maps, BevTarget b,
+                                                           BevViewTarget v, const FrameCtx* __restrict__ ctx,
+                                                           const int16_t* __restrict__ labels, int W, int H,
+                                                           FlowRemap rm, bool drew) {
+  __shared__ double cam[12];          // the frame's V
+  __shared__ double pose[4];          // pos_x, pos_z, cos, sin of the env's angle
+  __shared__ float proj[2];           // the frame's P00, P11
+  __shared__ const float2* fwd;       // the env's forward map, null: the pinhole frame
+  __shared__ bool known;              // a frame was drawn, not through the rectification
+  const int env = blockIdx.x;
+  if (threadIdx.x == 0) {
+    double sa, ca;
+    sincos(S.angle[env], &sa, &ca);
+    pose[0] = S.pos_x[env]; pose[1] = S.pos_z[env]; pose[2] = ca; pose[3] = sa;
+    known = drew && !rm.rectify;
+    if (known) {
+      const FrameCtx& c = ctx[env];
+      for (int k = 0; k < 12; k++) cam[k] = c.V[k];
+      proj[0] = c.P00; proj[1] = c.P11;
+      fwd = rm.fwd ? rm.fwd + (size_t)(rm.table_of_env ? __ldg(rm.table_of_env + env) : 0) * W * H : nullptr;
+    }
+  }
+  __syncthreads();
+  const dts_bev_config g = b.cfg;
+  const DMap& m = maps[S.map_id[env]];
+  const double px = pose[0], pz = pose[1], ca = pose[2], sa = pose[3], ts = m.tile_size;
+  const int gw = m.grid_w, gh = m.grid_h;
+  const int n_cells = g.width * g.height;
+  const size_t row = (size_t)env * n_cells;
+  const int16_t* frame = labels + (size_t)env * W * H;
+  const float nan = __int_as_float(0x7fc00000);
+  for (int k = 0; k < kViewCellsPerThread; k++) {
+    const int t = blockIdx.y * kViewCellsPerCta + k * kViewThreads + threadIdx.x;
+    if (t >= n_cells) break;
+    uint8_t val = DTS_BEVVIS_UNKNOWN;
+    float2 pix = make_float2(nan, nan);
+    if (known) {
+      val = DTS_BEVVIS_OUTSIDE;
+      const int r = t / g.width, c = t - r * g.width;
+      const double f = (g.origin_y - (r + 0.5)) * g.cell, l = ((c + 0.5) - g.origin_x) * g.cell;
+      const double x = px + f * ca + l * sa, z = pz - f * sa + l * ca;
+      const double fi = floor(x / ts), fj = floor(z / ts);
+      const bool road = fi >= 0.0 && fi < gw && fj >= 0.0 && fj < gh && __ldg(m.tile_kind + (int)fj * gw + (int)fi) >= 0;
+      const double y = road ? 0.0 : kGroundY;
+      const int lab = b.labels[row + t];
+      const double ex = cam[0] * x + cam[1] * y + cam[2] * z + cam[3];
+      const double ey = cam[4] * x + cam[5] * y + cam[6] * z + cam[7];
+      const double w = -(cam[8] * x + cam[9] * y + cam[10] * z + cam[11]);
+      if (w > 0.04 && w <= 100.0) {   // gluPerspective's near and far planes (S:1761)
+        const double iw = 1.0 / w;
+        double qx = ((double)proj[0] * (ex * iw) + 1.0) * (0.5 * W), qy = (1.0 - (double)proj[1] * (ey * iw)) * (0.5 * H);
+        bool in = true;
+        if (fwd) {
+          float2 o;
+          in = forward_map(fwd, W, H, (float)qx, (float)qy, o);
+          qx = o.x; qy = o.y;
+        }
+        if (in && qx >= 0.0 && qx < W && qy >= 0.0 && qy < H) {
+          const int cx = (int)floor(qx - 0.5), cy = (int)floor(qy - 0.5);
+          bool seen = false, shown = false;
+#pragma unroll
+          for (int j = 0; j < 2; j++)
+#pragma unroll
+            for (int i = 0; i < 2; i++) {
+              const int sx = cx + i, sy = cy + j;
+              if (sx < 0 || sx >= W || sy < 0 || sy >= H) continue;
+              const int s = __ldg(frame + sy * W + sx);
+              seen |= s == lab;
+              shown |= s != 0;
+            }
+          if (seen || shown) {
+            val = seen ? DTS_BEVVIS_VISIBLE : DTS_BEVVIS_OCCLUDED;
+            pix = make_float2((float)qx, (float)qy);
+          }
+        }
+      }
+    }
+    if (v.vis) v.vis[row + t] = val;
+    if (v.pix) v.pix[row + t] = pix;
+  }
+}
+
+// thread per env: the camera k_frame_setup left in frame memory
+__global__ void __launch_bounds__(128) k_frame_cameras(const FrameCtx* __restrict__ ctx, int n, double* V, float* P) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const FrameCtx& c = ctx[e];
+  for (int k = 0; k < 12; k++) V[(size_t)e * 12 + k] = c.V[k];
+  P[(size_t)e * 4] = c.P00; P[(size_t)e * 4 + 1] = c.P11; P[(size_t)e * 4 + 2] = c.P22; P[(size_t)e * 4 + 3] = c.P23;
+}
+
 }  // namespace
 
 void launch_bev(const DState& S, const DMap* maps, const BevTarget& b, cudaStream_t st) {
   const int n_cells = b.cfg.width * b.cfg.height;
   const dim3 grid(S.n, (n_cells + kBevCellsPerCta - 1) / kBevCellsPerCta);
   k_bev<<<grid, kBevThreads, 0, st>>>(S, maps, b);
+}
+
+void launch_bev_view(const DState& S, const DMap* maps, const BevTarget& b, const BevViewTarget& v, const FrameCtx* ctx,
+                     const int16_t* labels, int W, int H, const FlowRemap& rm, bool drew_frame, cudaStream_t st) {
+  const int n_cells = b.cfg.width * b.cfg.height;
+  const dim3 grid(S.n, (n_cells + kViewCellsPerCta - 1) / kViewCellsPerCta);
+  k_bev_view<<<grid, kViewThreads, 0, st>>>(S, maps, b, v, ctx, labels, W, H, rm, drew_frame);
+}
+
+void launch_frame_cameras(const FrameCtx* ctx, int n_envs, double* V, float* P, cudaStream_t st) {
+  k_frame_cameras<<<(n_envs + 127) / 128, 128, 0, st>>>(ctx, n_envs, V, P);
 }
 
 }  // namespace dts

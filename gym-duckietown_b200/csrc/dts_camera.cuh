@@ -1,6 +1,6 @@
 // dts_camera.cuh — agent camera matrices of _render_img (simulator.py:1758-1803), float64,
 // row-major 3x4 [R|t].  Shared by the render kernel and by the device reset (the reference captures
-// GL_LIGHT0's position under whatever modelview the previous frame left, S:581).
+// GL_LIGHT0's position under whatever modelview the previous frame left, S:581); and the fisheye's forward map.
 #pragma once
 #include "dts_common.cuh"
 
@@ -52,6 +52,22 @@ __host__ __device__ inline void top_down_view(double grid_w, double grid_h, doub
                         ux, uy, uz, -(ux * ex + uy * ey + uz * ez),
                         -fx, -fy, -fz, (fx * ex + fy * ey + fz * ez)};
   for (int k = 0; k < 12; k++) V[k] = L[k];
+}
+
+// Bilinear read of a forward map F [H][W] (the flow image's and the bird's-eye visibility's; OpenCV's convention: table
+// index = position - 0.5); false where the footprint leaves it
+__device__ __forceinline__ bool forward_map(const float2* __restrict__ F, int W, int H, float x, float y, float2& out) {
+  const float ix = x - 0.5f, iy = y - 0.5f;
+  if (!(ix >= 0.0f && ix <= (float)(W - 1) && iy >= 0.0f && iy <= (float)(H - 1))) return false;   // (NaN: false)
+  const int x0 = min((int)ix, max(W - 2, 0)), y0 = min((int)iy, max(H - 2, 0));
+  const int x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
+  const float ax = ix - (float)x0, ay = iy - (float)y0;
+  const float2 f00 = __ldg(F + (size_t)y0 * W + x0), f01 = __ldg(F + (size_t)y0 * W + x1);
+  const float2 f10 = __ldg(F + (size_t)y1 * W + x0), f11 = __ldg(F + (size_t)y1 * W + x1);
+  const float tx = f00.x + ax * (f01.x - f00.x), ty = f00.y + ax * (f01.y - f00.y);
+  const float bx = f10.x + ax * (f11.x - f10.x), by = f10.y + ax * (f11.y - f10.y);
+  out = make_float2(tx + ay * (bx - tx), ty + ay * (by - ty));
+  return true;
 }
 
 // Eye-space GL_POSITION for a light given under modelview V: positional (w=1) or direction (w=0).

@@ -41,21 +41,6 @@ __device__ inline void mesh_motion(float px0, float pz0, float deg0, float px1, 
   compose(A, B, W);
 }
 
-// Bilinear read of a forward map (OpenCV's convention: table index = position - 0.5); false where the footprint leaves it
-__device__ __forceinline__ bool forward_map(const float2* __restrict__ F, int W, int H, float x, float y, float2& out) {
-  const float ix = x - 0.5f, iy = y - 0.5f;
-  if (!(ix >= 0.0f && ix <= (float)(W - 1) && iy >= 0.0f && iy <= (float)(H - 1))) return false;   // (NaN: false)
-  const int x0 = min((int)ix, max(W - 2, 0)), y0 = min((int)iy, max(H - 2, 0));
-  const int x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
-  const float ax = ix - (float)x0, ay = iy - (float)y0;
-  const float2 f00 = __ldg(F + (size_t)y0 * W + x0), f01 = __ldg(F + (size_t)y0 * W + x1);
-  const float2 f10 = __ldg(F + (size_t)y1 * W + x0), f11 = __ldg(F + (size_t)y1 * W + x1);
-  const float tx = f00.x + ax * (f01.x - f00.x), ty = f00.y + ax * (f01.y - f00.y);
-  const float bx = f10.x + ax * (f11.x - f10.x), by = f10.y + ax * (f11.y - f10.y);
-  out = make_float2(tx + ay * (bx - tx), ty + ay * (by - ty));
-  return true;
-}
-
 // The render-mode bits that change a frame's depth and labels: an occlusion slot's frame is of one view
 __device__ __forceinline__ int occ_view(int mode) {
   return mode & (DTS_RENDER_TOP_DOWN | DTS_RENDER_PINHOLE | DTS_RENDER_RECTIFY);

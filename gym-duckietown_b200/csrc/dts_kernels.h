@@ -132,9 +132,9 @@ Renderer* renderer_create(const dts_config& cfg);   // on cfg.device, which must
 void renderer_destroy(Renderer* r);
 void renderer_release_frame(Renderer& r);   // the maps changed: the next render re-sizes frame memory for them
 // Before every render: reserves frame memory for the maps of `counts` unless it is reserved, and checks that a fisheye
-// LUT is set if the camera needs one, a rectification LUT if render `mode` asks for it, and (`flow`: a flow target is
-// set) the fisheye tables' forward maps if the frame goes through them.
-std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode, bool flow);
+// LUT is set if the camera needs one, a rectification LUT if render `mode` asks for it, and (`forward`: a flow or
+// bird's-eye visibility target is set) the fisheye tables' forward maps if the frame goes through them.
+std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode, bool forward);
 // The rasteriser's remap table for a LUT of the camera's size (obs[y, x] = frame[rint(rmapy), rint(rmapx)]), in the
 // fisheye slot or (`rectify`) the rectification slot; it replaces that slot's previous one, so no render may be in
 // flight.  A LUT the rasteriser cannot take leaves the previous table; NULL maps free the slot.  A fisheye pool: `count`
@@ -142,7 +142,7 @@ std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, 
 // read only when count > 1, and then kept in the table).  The rectification slot takes one LUT.
 std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* rmapx, const float* rmapy,
                              const int32_t* lut_of_env);
-// The forward maps of the fisheye tables (the flow image's F, dts_set_flow_target): `count` float32 [H][W] tables of x
+// The forward maps of the fisheye tables (F of the flow image and the bird's-eye visibility): `count` float32 [H][W] tables of x
 // and of y back to back, one per table of the fisheye pool and in its order; they replace the previous ones.  Refused
 // (error text, previous maps kept) unless the fisheye slot holds exactly `count` tables.  NULL maps free them.  A new
 // fisheye LUT (renderer_set_lut) drops them with the tables they belong to.
@@ -157,6 +157,11 @@ constexpr int kProfMarks = 6;
 int launch_render(const Renderer& r, const DState& S, const DMap* maps, const RenderCfg& rc, const AuxTargets& aux,
                   const FlowTarget& flow, const OcclusionTarget& occ, void* obs, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev,
                   cudaEvent_t* marks, int mark_level, cudaStream_t st);
+// Every env's camera of the last render (k_frame_setup's), device [n_envs]; null while no frame memory is reserved
+const FrameCtx* renderer_frame_ctx(const Renderer& r);
+struct FlowRemap;
+// The remap a render in `mode` goes through, as the passes after it read it (flow, bird's-eye visibility)
+FlowRemap renderer_remap(const Renderer& r, int mode);
 // What the last render left in frame memory for one env (dts_debug_frame), after the device has synchronised
 std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, int32_t* counts, float* lattice_by_cell,
                              int n_cells);
@@ -187,6 +192,14 @@ struct BevTarget {
 };
 // every env's grid of its current state, one launch
 void launch_bev(const DState& S, const DMap* maps, const BevTarget& b, cudaStream_t st);
+// The camera visibility of the grid (dts_set_bev_visibility_target, DESIGN.md section 5 item 15): uint8 [n_envs][height]
+// [width] and the pixel of every cell, float32 x, y; either null.  Both null: off.
+struct BevViewTarget {
+  uint8_t* vis;
+  float2* pix;
+};
+// every env's cameras V [n_envs][12] and P [n_envs][4] from `ctx` (dts_get_frame_cameras), one launch
+void launch_frame_cameras(const FrameCtx* ctx, int n_envs, double* V, float* P, cudaStream_t st);
 
 // motion flow (dts_flow.cu): the image of dts_set_flow_target, float32 [n_envs][H][W][2], and the record it is taken
 // against.  Null `out`: off, and then the record is unallocated.
@@ -212,6 +225,11 @@ struct FlowRemap {
   const float2* fwd;
   bool rectify;
 };
+// Every env's visibility of the grid `b` (its labels, written by k_bev earlier in the call) in the frame the call drew:
+// its camera in `ctx`, its label image `labels` [n_envs][H][W] and remap `rm`; drew_frame false (ctx and labels unread):
+// every cell UNKNOWN.  One launch.
+void launch_bev_view(const DState& S, const DMap* maps, const BevTarget& b, const BevViewTarget& v, const FrameCtx* ctx,
+                     const int16_t* labels, int W, int H, const FlowRemap& rm, bool drew_frame, cudaStream_t st);
 // A record for n_envs envs and max_dyn dynamic slots, every env's record invalid (episode -1); synchronous.  On failure
 // (error text) `rec` is untouched.
 std::string flow_record_alloc(FlowRecord& rec, int n_envs, int max_dyn);

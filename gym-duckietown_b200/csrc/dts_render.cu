@@ -2375,7 +2375,7 @@ void renderer_destroy(Renderer* r) {
   delete r;
 }
 
-std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode, bool flow) {
+std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode, bool forward) {
   if (!r.frame) {
     // prims k_geometry emits per road tile: the literal triangles of tile mode 0, or the quad of tile mode 1, which a
     // clip splits into two triangles and fans into a few more
@@ -2412,9 +2412,9 @@ std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, 
   }
   if ((r.flags & DTS_FLAG_DISTORTION) && !r.fish.src_xy) return "distortion enabled but no fisheye LUT set";
   if ((mode & DTS_RENDER_RECTIFY) && !r.rect.src_xy) return "DTS_RENDER_RECTIFY but no rectification LUT set";
-  if (flow && (r.flags & DTS_FLAG_DISTORTION) && !(mode & (DTS_RENDER_PINHOLE | DTS_RENDER_RECTIFY)) && !r.fish.fwd)
-    return "a flow target is set but the fisheye tables have no forward maps: a fisheye LUT set after "
-           "dts_set_flow_target drops them, so set the flow target again";
+  if (forward && (r.flags & DTS_FLAG_DISTORTION) && !(mode & (DTS_RENDER_PINHOLE | DTS_RENDER_RECTIFY)) && !r.fish.fwd)
+    return "a flow or bird's-eye visibility target is set but the fisheye tables have no forward maps: a fisheye LUT set "
+           "after dts_set_flow_target / dts_set_bev_visibility_target drops them, so set that target again";
   return "";
 }
 
@@ -2550,6 +2550,21 @@ std::string renderer_set_lut(Renderer& r, bool rectify, int count, const float* 
   return "";
 }
 
+const FrameCtx* renderer_frame_ctx(const Renderer& r) { return r.frame ? r.fm.ctx : nullptr; }
+
+// the table a render in `mode` is remapped through, if any: the rectification (DTS_RENDER_RECTIFY), none
+// (DTS_RENDER_PINHOLE or no DTS_FLAG_DISTORTION) or the fisheye
+static const RemapTab* remap_of(const Renderer& r, int flags, int mode) {
+  return (mode & DTS_RENDER_RECTIFY) ? &r.rect
+       : ((flags & DTS_FLAG_DISTORTION) && !(mode & DTS_RENDER_PINHOLE)) ? &r.fish : nullptr;
+}
+
+FlowRemap renderer_remap(const Renderer& r, int mode) {
+  const RemapTab* lut = remap_of(r, r.flags, mode);
+  const RemapTab rt = lut ? *lut : RemapTab{};
+  return FlowRemap{rt.src_xy, rt.table_of_env, rt.fwd, (mode & DTS_RENDER_RECTIFY) != 0};
+}
+
 // Test hook (dts_debug_frame): what k_frame_setup / k_geometry left in frame memory for one env of the last render —
 // the camera model-view and projection, the prim / lattice counts, and the lit 8x8 lattice of every road tile that
 // was emitted, re-ordered by grid cell (i * grid_h + j; cells that were culled stay NaN).
@@ -2605,11 +2620,9 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
                   const FlowTarget& flow, const OcclusionTarget& occ, void* obs_any, const GatherTab& gather, int32_t* err_flag, int32_t* status_dev,
                   cudaEvent_t* marks, int mark_level, cudaStream_t st) {
   uint8_t* obs = reinterpret_cast<uint8_t*>(obs_any);
-  // the table the frame is remapped through, if any: the rectification (DTS_RENDER_RECTIFY), none (DTS_RENDER_PINHOLE
-  // or no DTS_FLAG_DISTORTION) or the fisheye.  A table with a per-env index is a pool (kRemapPool); one table, of
-  // either kind, is kRemapTable.
-  const RemapTab* lut = (rc.mode & DTS_RENDER_RECTIFY) ? &r.rect
-                      : ((rc.flags & DTS_FLAG_DISTORTION) && !(rc.mode & DTS_RENDER_PINHOLE)) ? &r.fish : nullptr;
+  // the table the frame is remapped through, if any.  A table with a per-env index is a pool (kRemapPool); one table,
+  // of either kind, is kRemapTable.
+  const RemapTab* lut = remap_of(r, rc.flags, rc.mode);
   const RemapTab rt = lut ? *lut : RemapTab{};
   const int remap = !lut ? kRemapNone : rt.table_of_env ? kRemapPool : kRemapTable;
   FrameMem fm = r.fm;
@@ -2664,8 +2677,7 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   });
   mark();
   if (flow.out) {   // (inside the post-pass event bracket)
-    const FlowRemap fr{lut ? rt.src_xy : nullptr, rt.table_of_env, rt.fwd, (rc.mode & DTS_RENDER_RECTIFY) != 0};
-    launches += launch_flow(S, maps, rc, fm.ctx, aux, flow, fr, occ, st);
+    launches += launch_flow(S, maps, rc, fm.ctx, aux, flow, renderer_remap(r, rc.mode), occ, st);
   }
   mark();   // (post passes: launched by the caller)
   return launches;

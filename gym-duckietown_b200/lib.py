@@ -22,6 +22,8 @@ IN_PROGRESS, INVALID_POSE, MAX_STEPS = 0, 1, 2
 DONE_CODE_STR = {0: "in-progress", 1: "invalid-pose", 2: "max-steps-reached"}  # S:1685-1705
 # the occlusion mask's values (DTS_OCC_*, dts_set_occlusion_target), by value
 OCCLUSION_NAMES = ("none", "visible", "occluded", "outside", "unknown")
+# the bird's-eye visibility's values (DTS_BEVVIS_*, dts_set_bev_visibility_target), by value
+BEV_VISIBILITY_NAMES = ("unknown", "visible", "occluded", "outside")
 
 
 class DtsError(RuntimeError):
@@ -200,6 +202,8 @@ def load() -> C.CDLL:
     lib.dts_render_bev.argtypes = [vp, vp]
     lib.dts_set_flow_target.argtypes = [vp, vp, vp, vp, i]
     lib.dts_set_occlusion_target.argtypes = [vp, vp]
+    lib.dts_set_bev_visibility_target.argtypes = [vp, vp, vp, vp, vp, i]
+    lib.dts_get_frame_cameras.argtypes = [vp, vp, vp, vp]
     lib.dts_resize_frames.argtypes = [vp, vp, vp, vp]
     lib.dts_blend4.argtypes = [vp, vp, vp, vp, C.c_uint64, vp]
     lib.dts_set_timing.argtypes = [vp, C.c_double, i, i]
@@ -234,7 +238,7 @@ def load() -> C.CDLL:
 
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_fisheye_luts", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
-           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_set_flow_target", "dts_set_occlusion_target", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
+           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_set_flow_target", "dts_set_occlusion_target", "dts_set_bev_visibility_target", "dts_get_frame_cameras", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
            "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
 
@@ -521,27 +525,47 @@ class Sim:
         """The bird's-eye grids of the current state (dts_render_bev)."""
         self._check(self.lib.dts_render_bev(self.h, stream), "dts_render_bev")
 
+    def _forward_maps(self, fwd_x, fwd_y):
+        """(fwd_x, fwd_y, n_tables) as dts_set_flow_target and dts_set_bev_visibility_target take them"""
+        if fwd_x is None and fwd_y is None:
+            return None, None, 0
+        fx, fy = np.ascontiguousarray(fwd_x, np.float32), np.ascontiguousarray(fwd_y, np.float32)
+        if fx.ndim == 2:
+            fx, fy = fx[None], fy[None]
+        if fx.ndim != 3 or fx.shape != fy.shape or fx.shape[1:] != (self.cfg.cam_height, self.cfg.cam_width):
+            raise ValueError(f"forward maps: {fx.shape} and {fy.shape} must both be [tables, cam_height, cam_width]")
+        return fx, fy, fx.shape[0]
+
     def set_flow_target(self, flow_ptr: Optional[int], fwd_x: Optional[np.ndarray] = None,
                         fwd_y: Optional[np.ndarray] = None):
         """Every later render also writes float32 [num_envs, cam_height, cam_width, 2] backward flow at `flow_ptr`, which
         the caller keeps alive, from the depth and label targets (both must be set); None turns it off
         (dts_set_flow_target).  fwd_x / fwd_y: on a distortion handle, the forward maps of the fisheye tables, float32
         [tables, cam_height, cam_width] (or one [cam_height, cam_width] table) in the pool's order."""
-        if fwd_x is None and fwd_y is None:
-            self._check(self.lib.dts_set_flow_target(self.h, flow_ptr, None, None, 0), "dts_set_flow_target")
-            return
-        fx, fy = np.ascontiguousarray(fwd_x, np.float32), np.ascontiguousarray(fwd_y, np.float32)
-        if fx.ndim == 2:
-            fx, fy = fx[None], fy[None]
-        if fx.ndim != 3 or fx.shape != fy.shape or fx.shape[1:] != (self.cfg.cam_height, self.cfg.cam_width):
-            raise ValueError(f"flow forward maps: {fx.shape} and {fy.shape} must both be [tables, cam_height, cam_width]")
-        self._check(self.lib.dts_set_flow_target(self.h, flow_ptr, _ptr(fx), _ptr(fy), fx.shape[0]), "dts_set_flow_target")
+        fx, fy, n = self._forward_maps(fwd_x, fwd_y)
+        self._check(self.lib.dts_set_flow_target(self.h, flow_ptr, _ptr(fx), _ptr(fy), n), "dts_set_flow_target")
 
     def set_occlusion_target(self, occ_ptr: Optional[int]):
         """Every later render that writes flow also writes the uint8 [num_envs, cam_height, cam_width] occlusion mask
         (OCCLUSION_NAMES) at `occ_ptr`, which the caller keeps alive; needs the flow target.  None turns it off
         (dts_set_occlusion_target)."""
         self._check(self.lib.dts_set_occlusion_target(self.h, occ_ptr), "dts_set_occlusion_target")
+
+    def set_bev_visibility_target(self, vis_ptr: Optional[int], pix_ptr: Optional[int],
+                                  fwd_x: Optional[np.ndarray] = None, fwd_y: Optional[np.ndarray] = None):
+        """Every later call that writes the bird's-eye grid also writes, for each cell, whether the frame the call drew
+        shows it (uint8 [num_envs, height, width], BEV_VISIBILITY_NAMES) at `vis_ptr` and where it lands in that frame
+        (float32 [num_envs, height, width, 2], camera pixels) at `pix_ptr`, which the caller keeps alive; needs the
+        bird's-eye and camera label targets.  fwd_x / fwd_y as set_flow_target's.  None, None turns it off
+        (dts_set_bev_visibility_target)."""
+        fx, fy, n = self._forward_maps(fwd_x, fwd_y)
+        self._check(self.lib.dts_set_bev_visibility_target(self.h, vis_ptr, pix_ptr, _ptr(fx), _ptr(fy), n),
+                    "dts_set_bev_visibility_target")
+
+    def get_frame_cameras(self, V_ptr: int, P_ptr: int, stream: int = 0):
+        """Every env's camera of its last frame -> device float64 [num_envs, 12] at `V_ptr` and float32 [num_envs, 4]
+        (P00, P11, P22, P23) at `P_ptr`, stream-ordered (dts_get_frame_cameras)."""
+        self._check(self.lib.dts_get_frame_cameras(self.h, V_ptr, P_ptr, stream), "dts_get_frame_cameras")
 
     def set_resize(self, out_w: int, out_h: int, filter: int = 0):
         """filter RESIZE_CV2_CUBIC (dts_set_resize) or RESIZE_PIL_BILINEAR (dts_set_resize_filter)."""

@@ -72,7 +72,7 @@ class Simulator(Env):
                  color_ground=(0.15, 0.15, 0.15), color_sky=(0.45, 0.82, 1), style: str = "photos",
                  enable_leds: bool = False, device: int = 0, depth: bool = False, labels: bool = False,
                  markings: bool = False, bev: bool = False, flow: bool = False, flow_occlusion: bool = False,
-                 **env_kwargs):
+                 bev_visibility: bool = False, **env_kwargs):
         if draw_curve or draw_bbox or enable_leds:
             raise NotImplementedError("draw_curve / draw_bbox / enable_leds are debug modes outside the hot path "
                                       "(SURVEY 8f-4)")
@@ -99,7 +99,7 @@ class Simulator(Env):
             camera_rand_pool=env_kwargs.pop("camera_rand_pool", 1),   # one camera per Simulator (distortion.py:46-47)
             color_ground=color_ground, color_sky=color_sky, num_tris_distractors=num_tris_distractors,
             action_mode=self._action_mode, depth=depth, labels=labels, markings=markings, bev=bev, flow=flow,
-            flow_occlusion=flow_occlusion, **env_kwargs)
+            flow_occlusion=flow_occlusion, bev_visibility=bev_visibility, **env_kwargs)
         self._b = BatchedDuckietownEnv(1, map_arg, **self._env_kwargs)
         self._adopt_map()
         self.action_space = spaces.Box(low=-1, high=1, shape=(2,), dtype=np.float32)              # S:309
@@ -162,7 +162,7 @@ class Simulator(Env):
         if getattr(self, "_human", None) is None:
             kw = dict(self._env_kwargs, camera_width=WINDOW_WIDTH, camera_height=WINDOW_HEIGHT, distortion=False,
                       terminal_obs=False, depth=False, labels=False, markings=False, bev=False, flow=False,
-                      flow_occlusion=False)
+                      flow_occlusion=False, bev_visibility=False)
             self._human = BatchedDuckietownEnv(1, list(self._b.maps), **kw)
         self._human.load_state(self._b.save_state())
         return self._human
@@ -252,6 +252,21 @@ class Simulator(Env):
         flow_occlusion=True also turns on flow, depth and labels."""
         o = self._b.flow_occlusion
         return None if o is None else o[0].cpu().numpy()
+
+    @property
+    def bev_visibility(self) -> Optional[np.ndarray]:
+        """With bev_visibility=True: uint8 [height, width], whether the frame last returned by reset / step / render_obs
+        shows each cell of the bird's-eye grid, named by BEV_VISIBILITY_NAMES (BatchedDuckietownEnv.bev_visibility);
+        else None.  bev_visibility=True also turns on bev and labels."""
+        v = self._b.bev_visibility
+        return None if v is None else v[0].cpu().numpy()
+
+    @property
+    def bev_pixels(self) -> Optional[np.ndarray]:
+        """With bev_visibility=True: float32 [height, width, 2], where each cell lands in that frame, in camera pixels
+        (BatchedDuckietownEnv.bev_pixels); else None."""
+        p = self._b.bev_pixels
+        return None if p is None else p[0].cpu().numpy()
 
     @property
     def cur_pos(self):

@@ -444,6 +444,39 @@ int dts_set_flow_target(dts_sim* sim, float* flow_dev, const float* fwd_x, const
  * not state: snapshots and the gathers carry neither it nor the slots. */
 enum { DTS_OCC_NONE = 0, DTS_OCC_VISIBLE = 1, DTS_OCC_OCCLUDED = 2, DTS_OCC_OUTSIDE = 3, DTS_OCC_UNKNOWN = 4 };
 int dts_set_occlusion_target(dts_sim* sim, uint8_t* occ_dev);
+/* Camera visibility of the bird's-eye grid (DESIGN.md section 5, item 15): for every cell of dts_set_bev_target's grid,
+ * whether the frame drawn for its env shows it, and where it lands in that frame.  In float64: the cell centre (x, z) of
+ * dts_bev_config at height y = 0 on a road tile (i, j) = (floor(x / tile_size), floor(z / tile_size)) and the ground
+ * quad's (float)(-0.8 * 0.01) elsewhere — for a cell whose label is an object, the surface under it — goes through the
+ * frame's camera V to the eye point e = V (x, y, z, 1) and, with the frame's float32 P00 / P11, to
+ * x1 = (P00 ex / -ez + 1) W / 2, y1 = (1 - P11 ey / -ez) H / 2.  Outside unless 0.04 < -ez <= 100 (gluPerspective's
+ * planes).  Without a remap q = (x1, y1); under the fisheye (one table or a camera_rand pool) q is the env's forward map
+ * F at (x1, y1), read as dts_set_flow_target reads it, and the cell is outside where F's footprint leaves the table.
+ * Outside unless q lies in [0, W) x [0, H).  Then the up to four pixels (floor(q - 0.5) + {0, 1}) clipped to the frame,
+ * in the frame's label image, decide, in this order:
+ *   DTS_BEVVIS_VISIBLE   one of them shows the cell's grid label
+ *   DTS_BEVVIS_OUTSIDE   all of them show 0 (sky, no fisheye source pixel, beyond the ground quad)
+ *   DTS_BEVVIS_OCCLUDED  otherwise
+ *   DTS_BEVVIS_UNKNOWN   every cell of an env this call drew no frame for, or drew DTS_RENDER_RECTIFY
+ * vis_dev: uint8 [num_envs][height][width]; pix_dev: float32 [num_envs][height][width][2] (8-byte aligned), q in camera
+ * pixels with pixel centres at +0.5 as the flow image's, NaN for UNKNOWN and OUTSIDE.  Either may be NULL; both NULL
+ * turns it off, and then every call launches exactly what it launches without it.  fwd_x / fwd_y / n_tables: as
+ * dts_set_flow_target's, and the two share the forward maps: clearing one keeps them for the other, and a fisheye LUT
+ * set afterwards drops them for both.  Refused (non-zero, the previous setting kept) unless a bird's-eye label target and
+ * a label target are set, with a wrong n_tables or a pix_dev not 8-byte aligned; while it is set, clearing either label
+ * target and a dts_set_bev_target of another width or height are refused.  With it set, every call that writes the grid
+ * (dts_step, dts_step_terminal, dts_render, dts_render_bev) launches one more kernel, k_bev_view, last in the call: after
+ * dts_step with obs_dev and dts_render against the frame just drawn (in its mode), after dts_step_terminal with obs_dev
+ * against the frame in obs_dev row e (the respawned first frame where the episode ended); after dts_step without obs_dev,
+ * dts_step_terminal without obs_dev and dts_render_bev every cell is UNKNOWN.  Sticky; the memory is the caller's and
+ * must stay valid while it is set.  Synchronises.  An output, not state: snapshots and the gathers do not carry it. */
+enum { DTS_BEVVIS_UNKNOWN = 0, DTS_BEVVIS_VISIBLE = 1, DTS_BEVVIS_OCCLUDED = 2, DTS_BEVVIS_OUTSIDE = 3 };
+int dts_set_bev_visibility_target(dts_sim* sim, uint8_t* vis_dev, float* pix_dev, const float* fwd_x, const float* fwd_y,
+                                  int n_tables);
+/* The camera of every env's last frame, as k_frame_setup built it: V_dev float64 [num_envs][12] (row-major 3x4 [R|t]) and
+ * P_dev float32 [num_envs][4] (P00, P11, P22, P23 of gluPerspective), device memory.  Stream-ordered, one launch; fails
+ * before the handle's first render (and after a map upload, until the next render). */
+int dts_get_frame_cameras(dts_sim* sim, double* V_dev, float* P_dev, void* stream);
 /* Select the fused wrapper behaviour for subsequent dts_step / dts_render calls (default: all zero, scale 1).
  * obs_dev then holds num_envs * 3 * H * W elements of uint8 or float32 in the chosen layout. */
 int dts_set_output_format(dts_sim* sim, const dts_output_format* fmt);

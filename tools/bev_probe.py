@@ -13,6 +13,14 @@ Reports the median and spread over the rounds and prints one JSON line with the 
 read before and after in the same run.
 
     python tools/bev_probe.py [--configs c2,c3] [--steps 100] [--warmup 10] [--rounds 5] [--out FILE.json]
+
+--visibility measures the camera visibility of the grid instead (dts_set_bev_visibility_target: one k_bev_view launch
+per step, after the render).  For each shape, with the pinhole camera and with --distortion's fisheye, one env with a
+64x64 grid and the label image on is stepped in two alternating arms: the grid alone and the grid plus visibility.
+Per arm: ms per step of step() with rendering, and render_obs() alone timed with CUDA events over `steps` calls; the
+difference of the second between the arms is k_bev_view's time.
+
+    python tools/bev_probe.py --visibility [--configs c2,c3] [--steps 100] [--warmup 10] [--rounds 5] [--out FILE.json]
 """
 import argparse
 import json
@@ -81,6 +89,69 @@ def kernel_ms(env, arm, steps):
     return a.elapsed_time(b) / steps
 
 
+def render_ms(env, steps):
+    for _ in range(5):
+        env.render_obs()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(steps):
+        env.render_obs()
+    b.record()
+    b.synchronize()
+    return a.elapsed_time(b) / steps
+
+
+def visibility(a):
+    res = {"card": card(), "steps": a.steps, "warmup": a.warmup, "rounds": a.rounds, "actions": "uniform [-1, 1]",
+           "grid": [64, 64], "cell_m": CELL, "configs": {}}
+    arms = ["grid", "grid+vis"]
+    for cfg in a.configs.split(","):
+        for fish in (False, True):
+            c = dict(SHAPES[cfg])
+            env = BatchedDuckietownEnv(c["envs"], c["map"], camera_width=c["width"], camera_height=c["height"],
+                                       domain_rand=False, seed=1, device_reset=True, auto_reset=True,
+                                       bev_shape=(64, 64), bev_cell=CELL, bev_visibility=True, distortion=fish)
+            env.reset()
+            fwd = (env.camera_model.mapx, env.camera_model.mapy) if fish else ()
+
+            def set_vis(on):
+                if on:
+                    env.sim.set_bev_visibility_target(env.bev_visibility.data_ptr(), env.bev_pixels.data_ptr(), *fwd)
+                else:
+                    env.sim.set_bev_visibility_target(None, None)
+
+            g = torch.Generator(device="cuda").manual_seed(0)
+            acts = torch.rand((16, c["envs"], 2), device="cuda", generator=g) * 2 - 1
+            step = {k: [] for k in arms}
+            rend = {k: [] for k in arms}
+            for r in range(a.rounds):
+                for arm in arms[r % 2:] + arms[:r % 2]:
+                    set_vis(arm == "grid+vis")
+                    run(env, acts, a.warmup, True)
+                    torch.cuda.synchronize()
+                    t0 = time.perf_counter()
+                    run(env, acts, a.steps, True, a.warmup)
+                    torch.cuda.synchronize()
+                    step[arm].append((time.perf_counter() - t0) / a.steps * 1e3)
+                    rend[arm].append(render_ms(env, a.steps))
+                print(f"{cfg} {'fisheye' if fish else 'pinhole'} round {r}: " +
+                      ", ".join(f"{k} {step[k][-1]:.3f} / {rend[k][-1]:.4f}" for k in arms) +
+                      " ms (step / render_obs)", file=sys.stderr, flush=True)
+            env.check()
+            med = lambda d: {k: float(np.median(v)) for k, v in d.items()}
+            spread = lambda d: {k: [float(min(v)), float(max(v))] for k, v in d.items()}
+            diffs = [v - g_ for v, g_ in zip(rend["grid+vis"], rend["grid"])]
+            res["configs"][f"{cfg}_{'fisheye' if fish else 'pinhole'}"] = {
+                **c, "ms_per_step": med(step), "spread_ms_per_step": spread(step), "render_obs_ms": med(rend),
+                "spread_render_obs_ms": spread(rend), "k_bev_view_ms": float(np.median(diffs)),
+                "spread_k_bev_view_ms": [float(min(diffs)), float(max(diffs))]}
+            env.close()
+            del env
+            torch.cuda.empty_cache()
+    res["card_after"] = card()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", default="c2,c3")
@@ -88,9 +159,13 @@ def main():
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--visibility", action="store_true")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("needs a CUDA device")
+    if a.visibility:
+        emit(visibility(a), a.out)
+        return
     arms = list(GRIDS)
     res = {"card": card(), "steps": a.steps, "warmup": a.warmup, "rounds": a.rounds, "actions": "uniform [-1, 1]",
            "cell_m": CELL, "configs": {}}
@@ -133,11 +208,15 @@ def main():
         del env
         torch.cuda.empty_cache()
     res["card_after"] = card()
+    emit(res, a.out)
+
+
+def emit(res, out):
     line = json.dumps(res)
     print(line, flush=True)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
+    if out:
+        os.makedirs(os.path.dirname(os.path.abspath(out)), exist_ok=True)
+        with open(out, "w") as f:
             f.write(line + "\n")
 
 
