@@ -979,6 +979,9 @@ struct FrameMem {
   uint2* geo_list;      // [N * items_max] (env, draw item) pairs that passed k_cull
   uint2* solo;          // [N * cbins] (env, coarse bin | prim << 16): coarse bins lying inside one prim (k_bin -> k_raster_solo)
   uint2* flat;          // [N * cbins] (env, coarse bin | record count << 16): flat bins, only road tiles and ground (k_bin -> k_raster_flat)
+  uint2* empty;         // [N * cbins] (env, coarse bin): bins without records, cleared by k_raster_solo (k_bin, no LUT)
+  uint2* rows;          // [N * cbins_y] (env, coarse row): the rows k_raster still has to draw (k_bin, k_raster_flat -> k_raster)
+  int* row_flag;        // [N][cbins_y] nonzero once the row is on `rows` (cleared by k_bin for its env)
   int* work;            // global counters, zeroed per frame: the kWork* slots
   int32_t* status;      // mapped host word (dts_status): bit 0 = a frame ran out of frame memory
 };
@@ -987,6 +990,8 @@ constexpr int kWorkPairPool = 1;   // pair-pool cursor (k_bin)
 constexpr int kWorkGeoList = 2;    // geo_list length (k_cull -> k_geometry)
 constexpr int kWorkSoloList = 3;   // solo list length (k_bin -> k_raster_solo)
 constexpr int kWorkFlatList = 4;   // flat list length (k_bin -> k_raster_flat)
+constexpr int kWorkRowList = 5;    // row list length (k_bin, k_raster_flat's hand-backs -> k_raster)
+constexpr int kWorkEmptyList = 6;  // empty list length (k_bin -> k_raster_solo)
 
 __host__ __device__ inline size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
 
@@ -1023,6 +1028,10 @@ __host__ size_t carve(const Renderer& r, uintptr_t base, FrameMem& f) {
   take(f.geo_list, n * r.items_max);
   take(f.solo, n * r.cbins);
   take(f.flat, n * r.cbins);
+  const size_t cbins_y = (r.H + kCoarseH - 1) / kCoarseH;
+  take(f.empty, n * r.cbins);
+  take(f.rows, n * cbins_y);
+  take(f.row_flag, n * cbins_y);
   return o + 256;   // (+ 256 B of slack past the last list)
 }
 
@@ -1390,13 +1399,22 @@ k_tiles(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm
 // pairs — count (shared-memory atomics), scan, scatter; prims with a small bounding box are binned by it, larger ones
 // test each bin of the box against their edges, one bin per lane.  Pass 2, dense over the pairs (one per thread, so a
 // screen-filling prim costs no more lanes than a sliver): the pair's BinRec.
+// Then, for lean output only: the lists of the bins k_raster_solo and k_raster_flat draw, and the list of the rows
+// k_raster still has to draw.
 constexpr int kBinWarps = 4;
 constexpr int kCountMask = 0xfffff, kGroundInc = 1 << 20;   // a bin's counter: records | ground-quad records << 20
 constexpr int kFlatBin = -0x7fffffff - 1;   // bin_count of a flat bin (k_raster_flat); solo bins hold -(prim + 1) >= -65536
+constexpr int kEmptyBin = kFlatBin + 1;     // bin_count of an empty bin (no records) that k_raster_solo clears
+constexpr int kSoloMark = 2;   // no_flat[] bit of a solo bin (bit 0: not flat)
+// Row `cby` of `env` onto k_raster's list, unless it is there already (`row_flag`: k_bin clears its env's flags)
+__device__ __forceinline__ void row_to_list(const FrameMem& fm, int env, int cby, int cbins_y) {
+  if (atomicOr(fm.row_flag + (size_t)env * cbins_y + cby, 1) == 0)
+    fm.rows[atomicAdd(fm.work + kWorkRowList, 1)] = make_uint2((unsigned)env, (unsigned)cby);
+}
 // kListed: the frame draws the envs of rc.env_list.  (Its own instance: an env id loaded from the list stays live across
 // the kernel, where blockIdx.x is re-read for free, and would cost the remap instances registers and spills.)
 template <int kRemap, bool kListed>   // kRemap other than kRemapNone: bins are the LUT's source boxes of the output bins
-__global__ void __launch_bounds__(kBinWarps * 32)
+__global__ void __launch_bounds__(kBinWarps * 32, 8)   // 64 registers: 32 one-warp CTAs per SM at small cameras
 k_bin(RenderCfg rc, FrameMem fm, RemapTab rts, int max_prims, int max_pairs, int32_t* __restrict__ err) {
   extern __shared__ int bin_smem[];
   __shared__ int s_total, s_base, s_ok;
@@ -1534,6 +1552,12 @@ k_bin(RenderCfg rc, FrameMem fm, RemapTab rts, int max_prims, int max_pairs, int
       }
       if (!ok) {
         if (tid == 0) { fm.ctx[env].overflow = 1; atomicOr(err, 1); *reinterpret_cast<volatile int32_t*>(fm.status) = 1; }
+        // every bin holds count 0: k_raster clears the whole frame
+        if (lean_output(rc.obs_layout, rc.obs_dtype, W))
+          for (int r = tid; r < cbins_y; r += nthr) {
+            fm.row_flag[(size_t)env * cbins_y + r] = 1;
+            fm.rows[atomicAdd(fm.work + kWorkRowList, 1)] = make_uint2((unsigned)env, (unsigned)r);
+          }
         return;
       }
     }
@@ -1543,10 +1567,11 @@ k_bin(RenderCfg rc, FrameMem fm, RemapTab rts, int max_prims, int max_pairs, int
   const int pair0 = s_base, total = s_total;
   const bool lean_fmt = lean_output(rc.obs_layout, rc.obs_dtype, W);
   // start[] is free from here on: per coarse bin, nonzero once a record rules the bin out of k_raster_flat (a mesh
-  // triangle, a tiny triangle, or a solo bin)
+  // triangle, a tiny triangle, or a solo bin, which also sets kSoloMark)
   int* no_flat = start;
   if (lean_fmt) {
     for (int b = tid; b < cbins; b += nthr) no_flat[b] = 0;
+    for (int r = tid; r < cbins_y; r += nthr) fm.row_flag[(size_t)env * cbins_y + r] = 0;
     __syncthreads();
   }
   BinRec* recs = fm.recs;
@@ -1572,27 +1597,41 @@ k_bin(RenderCfg rc, FrameMem fm, RemapTab rts, int max_prims, int max_pairs, int
         fm.bin_count[(size_t)env * cbins + b] = -(p + 1);
         const int slot = atomicAdd(fm.work + kWorkSoloList, 1);
         fm.solo[slot] = make_uint2((unsigned)env, (unsigned)b | ((unsigned)p << 16));
-        atomicOr(&no_flat[b], 1);
+        atomicOr(&no_flat[b], 1 | kSoloMark);
       }
       if (!(r & kRecFlatOk)) atomicOr(&no_flat[b], 1);
     }
   }
   if (!lean_fmt) return;
   // flat bins: 1..kStage records, every one a flat road tile or the ground quad, not solo -> k_raster_flat's list, and
-  // k_raster skips them (kFlatBin) unless k_raster_flat hands one back
+  // k_raster skips them (kFlatBin) unless k_raster_flat hands one back.  Empty bins, without a LUT -> k_raster_solo's
+  // empty list, which clears them, and k_raster skips them (kEmptyBin).  A row holding any other bin -> k_raster's list.
   __syncthreads();
   for (int b0 = wib * 32; b0 < cbins; b0 += nthr) {
     const int b = b0 + lane, c = b < cbins ? (cnt[b] & kCountMask) : 0;
     const bool flat = c >= 1 && c <= kStage && !no_flat[b];
-    const unsigned m = __ballot_sync(0xffffffffu, flat);
-    if (!m) continue;
-    int base = 0;
-    if (lane == 0) base = atomicAdd(fm.work + kWorkFlatList, __popc(m));
-    base = __shfl_sync(0xffffffffu, base, 0);
-    if (flat) {
-      fm.bin_count[(size_t)env * cbins + b] = kFlatBin;
-      fm.flat[base + __popc(m & ((1u << lane) - 1u))] = make_uint2((unsigned)env, (unsigned)b | ((unsigned)c << 16));
+    const bool empty = kRemap == kRemapNone && b < cbins && c == 0;   // (under a LUT k_raster clears them, per pixel)
+    const unsigned m = __ballot_sync(0xffffffffu, flat), me = __ballot_sync(0xffffffffu, empty);
+    if (m) {
+      int base = 0;
+      if (lane == 0) base = atomicAdd(fm.work + kWorkFlatList, __popc(m));
+      base = __shfl_sync(0xffffffffu, base, 0);
+      if (flat) {
+        fm.bin_count[(size_t)env * cbins + b] = kFlatBin;
+        fm.flat[base + __popc(m & ((1u << lane) - 1u))] = make_uint2((unsigned)env, (unsigned)b | ((unsigned)c << 16));
+      }
     }
+    if (me) {
+      DTS_COUNT(30, __popc(me));
+      int base = 0;
+      if (lane == 0) base = atomicAdd(fm.work + kWorkEmptyList, __popc(me));
+      base = __shfl_sync(0xffffffffu, base, 0);
+      if (empty) {
+        fm.bin_count[(size_t)env * cbins + b] = kEmptyBin;
+        fm.empty[base + __popc(me & ((1u << lane) - 1u))] = make_uint2((unsigned)env, (unsigned)b);
+      }
+    }
+    if (b < cbins && !flat && !empty && !(no_flat[b] & kSoloMark)) row_to_list(fm, env, b / cbins_x, cbins_y);
   }
 }
 
@@ -1738,8 +1777,9 @@ template <bool kWrapFmt, int kRemap, int kAux>
                                        // kRemap other than kRemapNone: every lane renders the SOURCE pixel the LUT names
                                        // for its output pixel;
                                        // kAux: the images written beside obs (AuxTargets)
+                                       // row_list: the work items are the rows on fm.rows (launch_render)
 __global__ void __launch_bounds__(kThreads, kRasterMinCtas)
-k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, RemapTab rts, GatherTab gt,
+k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, RemapTab rts, GatherTab gt, bool row_list,
          uint8_t* __restrict__ obs, int max_prims, int max_pairs, int max_lat, int32_t* __restrict__ err, AuxTargets aux) {
   // dynamic shared memory (kRasterSmem bytes): per warp two chunks of records in flight, their mbarriers, and a 128-sample
   // depth / winner buffer for the tiny triangles of the fine bin being drawn
@@ -1764,15 +1804,23 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
   __syncwarp();
   uint32_t parity = 0;   // bit s: the phase the next wait on slot s completes
   int cs = 0, ps = 0;    // consumer / producer slot
-  const int n_work = n_listed(rc.env_list, rc.env_count, rc.n_envs) * cbins_y;   // work item = one row of coarse bins of one env
+  // work item = one row of coarse bins of one env: every row of every (listed) env, or the rows on the list
+  const int n_work = row_list ? fm.work[kWorkRowList] : n_listed(rc.env_list, rc.env_count, rc.n_envs) * cbins_y;
   int work = 0;
   if (lane == 0) work = atomicAdd(fm.work + kWorkRaster, 1);
   work = __shfl_sync(0xffffffffu, work, 0);
   while (work < n_work) {
     int next_work = 0;
     if (lane == 0) next_work = atomicAdd(fm.work + kWorkRaster, 1);   // consumed after this row: latency hidden
-    const int slot = work / cbins_y, cby = work - slot * cbins_y;
-    const int env = listed_env(rc.env_list, slot);
+    int env, cby;
+    if (row_list) {
+      const uint2 r = fm.rows[work];
+      env = (int)r.x; cby = (int)r.y;
+    } else {
+      const int slot = work / cbins_y;
+      cby = work - slot * cbins_y;
+      env = listed_env(rc.env_list, slot);
+    }
     const RemapTab rt = kRemap == kRemapPool ? remap_of_env(rts, env, W, H, cbins) : rts;
     const DMap& m = maps[S.map_id[env]];
     const uint8_t* tex_pool = m.tex_pool;
@@ -1849,7 +1897,7 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
     issue();
     for (int cbx = 0; cbx < cbins_x; cbx++) {
       const int count = __shfl_sync(0xffffffffu, my_cnt, cbx);
-      if (count < 0) continue;   // drawn by k_raster_solo (a bin inside one prim) or k_raster_flat (kFlatBin)
+      if (count < 0) continue;   // drawn by k_raster_solo (a bin inside one prim, or kEmptyBin) or k_raster_flat (kFlatBin)
       const unsigned fvalid = fine_in_image(cbx, rows_in, W);
       DTS_COUNT(8, 1);
       if (count == 0) {
@@ -2088,10 +2136,58 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
 }
 
 // ------------------------------------------------------------------------------------------------ k_raster_solo
+// k_bin's empty bins (no LUT): the clear colour in obs, 0 in every image.  A bin waits on two dependent loads (its
+// entry, then its env's horizon), so a warp takes eight bins at once, one lane loading each, and then stores them one
+// after the other, a whole image row of the bin per store: the row's pixels of obs as words (lean output: the row starts
+// on a word and its 3 * 32 bytes, or 3 * a multiple of 4 at the right border, are whole words), cycling through the
+// three words of the packed colour, and each image's row, a lane per pixel.
+template <int kAux>
+__device__ __forceinline__ void clear_empty_bins(const DState& S, const RenderCfg& rc, const FrameMem& fm, uint8_t* __restrict__ obs,
+                                                 const AuxTargets& aux) {
+  constexpr int kBatch = 8;
+  const int W = rc.width, H = rc.height;
+  const int cbins_x = (W + kCoarseW - 1) / kCoarseW;
+  const int lane = threadIdx.x & 31, n = fm.work[kWorkEmptyList];
+  const int warps = (gridDim.x * blockDim.x) >> 5;
+  for (int i0 = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * kBatch; i0 < n; i0 += warps * kBatch) {
+    uint2 e = make_uint2(0u, 0u);
+    unsigned rgb = 0u;
+    if (lane < kBatch && i0 + lane < n) {
+      e = fm.empty[i0 + lane];
+      float clr[3];
+      clear_colour(S, rc, (int)e.x, clr);
+      rgb = pack_rgb(clr[0], clr[1], clr[2]);   // bytes r g b 0
+    }
+#pragma unroll 1
+    for (int j = 0; j < min(kBatch, n - i0); j++) {
+      const int env = (int)__shfl_sync(0xffffffffu, e.x, j), b = (int)__shfl_sync(0xffffffffu, e.y, j);
+      const unsigned c = __shfl_sync(0xffffffffu, rgb, j);
+      const int cby = b / cbins_x, x0 = (b - cby * cbins_x) * kCoarseW;
+      const int px = min(kCoarseW, W - x0), rows = min(kCoarseH, H - cby * kCoarseH);
+      // word k of a row holds channels k, k+1, k+2, k+3 (mod 3) of the colour
+      const int k3 = lane % 3;
+      const unsigned word = k3 == 0 ? (c | (c << 24)) : (k3 == 1 ? ((c >> 8) | (c << 16)) : ((c >> 16) | (c << 8)));
+      const size_t pix0 = (size_t)env * W * H + (size_t)(cby * kCoarseH) * W + x0;
+#pragma unroll 1
+      for (int r = 0; r < rows; r++) {
+        const size_t pix = pix0 + (size_t)r * W;
+        if (lane < px * 3 / 4) reinterpret_cast<unsigned*>(obs + pix * 3)[lane] = word;
+        if (lane < px) {
+          if (stores_depth<kAux>(aux.depth)) aux.depth[pix + lane] = 0.0f;
+          if (kAux & kAuxLabels) aux.labels[pix + lane] = 0;
+          if (kAux & kAuxMarks) aux.marks[pix + lane] = 0;
+        }
+      }
+    }
+  }
+}
+
 // Coarse bins that lie inside ONE prim (k_bin found: one record besides the ground quad, covering every sample of every
 // fine bin — 22 of the 55 non-empty coarse bins of a c2 frame, 40 % of the shaded pixels) need no records, no staging, no
 // visibility state: a warp fetches the prim's planes once and shades the bin's 256 pixels.  A separate kernel so that the
 // lean loop gets its own register allocation (the same fast path inside k_raster cost more than it saved).
+// Without a LUT the empty bins come here first (k_bin's empty list: the sky, 20 of a c2 frame's 75 bins), so that
+// k_raster does not walk their rows: the clear colour, and 0 in every image, as k_raster writes them (clear_empty_bins).
 // Packed u8 HWC output with whole-word rows only (k_bin marks no bin otherwise).  Runs before k_raster.
 // Images: the 1/w the shading divides by gives the depth, the bin's one prim the label of every pixel with a source, and
 // the texel it shows there the marking.
@@ -2104,6 +2200,7 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
   const int lane = threadIdx.x & 31;
   const StoreLane sl = make_store_lane(lane, W);
   const size_t frame_bytes = (size_t)W * H * 3;
+  if (kRemap == kRemapNone) clear_empty_bins<kAux>(S, rc, fm, obs, aux);
   const int n = fm.work[kWorkSoloList];
   const int warps = (gridDim.x * blockDim.x) >> 5;
   for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
@@ -2112,18 +2209,18 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
     const unsigned p = e.y >> 16;
     const int cby = b / cbins_x, cbx = b - cby * cbins_x;
     const RemapTab rt = kRemap == kRemapPool ? remap_of_env(rts, env, W, H, cbins_x * ((H + kCoarseH - 1) / kCoarseH)) : rts;
+    uint8_t* out = obs + (size_t)env * frame_bytes;
+    // fine bins inside the image as loop bounds rather than fine_in_image(): the mask test costs this loop machine code
+    const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);
+    const int ny = ((cby * kCFY + 1) * kBinH < H) ? 2 : 1;
     const uint8_t* tex_pool = maps[S.map_id[env]].tex_pool;
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
     const ShadeIn si = load_shade(fm.prims + (size_t)env * max_prims, p);
-    uint8_t* out = obs + (size_t)env * frame_bytes;
     int lab = 0;
     if constexpr ((kAux & kAuxLabels) != 0)
       lab = label_of_id(label_map(maps[S.map_id[env]], rc.tessellate), __ldg(&fm.prims[(size_t)env * max_prims + p].id));
     const uint8_t* cls_pool = (kAux & kAuxMarks) ? tex_pool + maps[S.map_id[env]].tex_class_off : nullptr;
     const AuxFrames af = aux_frames(aux, env, W, H);
-    // fine bins inside the image as loop bounds rather than fine_in_image(): the mask test costs this loop machine code
-    const int nx = min(kCFX, (W - cbx * kCoarseW + kBinW - 1) / kBinW);
-    const int ny = ((cby * kCFY + 1) * kBinH < H) ? 2 : 1;
 #pragma unroll 1
     for (int fy = 0; fy < ny; fy++)
 #pragma unroll 1
@@ -2162,8 +2259,8 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
 // lane takes one and shades its other winners (resolve_edge: the same bits whichever lane shades them).  The bin's
 // colours collect in shared memory and are stored once the bin is done.
 // Hand-back: a sample covered by two tiles (or by two ground records) is not resolved here.  The warp drops the bin's
-// queue and colours, restores its record count, and k_raster, launched next on the stream, draws the whole bin
-// depth-tested.
+// queue and colours, restores its record count, puts its row on k_raster's list, and k_raster, launched next on the
+// stream, draws the whole bin depth-tested.
 // Images need no plane in shared memory.  A lane stores a one-winner pixel's images as soon as it has shaded it, and a
 // queued pixel's when its other winners are resolved; the queue carries the first winner's 1/w in a third array (2 KB:
 // 46 KB per CTA, still four CTAs per SM) and its class in the high half of the entry's slot word, and the first label
@@ -2288,7 +2385,10 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
         }
         if (__any_sync(0xffffffffu, twice != 0)) {   // rare: k_raster draws the bin, depth-tested
           DTS_COUNT(25, 1);
-          if (lane == 0) fm.bin_count[(size_t)env * cbins + b] = count;
+          if (lane == 0) {
+            fm.bin_count[(size_t)env * cbins + b] = count;
+            row_to_list(fm, env, cby, (H + kCoarseH - 1) / kCoarseH);
+          }
           break;
         }
       }
@@ -2658,12 +2758,16 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   });
   mark();
   const bool wrap = (rc.obs_layout | rc.obs_dtype) != 0;
+  const bool lean = lean_output(rc.obs_layout, rc.obs_dtype, rc.width);
+  // k_raster walks only the rows k_bin and k_raster_flat listed, unless the solo and flat bins were not drawn apart or a
+  // gathering step ships every row, the ones they drew included, from k_raster
+  const bool row_list = lean && gather.n == 0;
   const int aux_run = aux_set(aux);   // the rasterisers' instances for the images asked for (no target: the plain ones)
   for_each_of<kAuxSets>([&](auto aux_c) {
     for_each_of<kRemapModes>([&](auto remap_c) {
       constexpr int A = decltype(aux_c)::value, R = decltype(remap_c)::value;
       if (A != aux_run || R != remap) return;
-      if (lean_output(rc.obs_layout, rc.obs_dtype, rc.width)) {   // (inside the k_raster event bracket: it is rasterisation time)
+      if (lean) {   // (inside the k_raster event bracket: it is rasterisation time)
         k_raster_solo<R, A><<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, rt, obs, r.max_prims, r.max_lat, aux);
         // before k_raster, which draws the bins k_raster_flat hands back
         k_raster_flat<R, A><<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, rt, obs, r.max_prims, r.max_lat,
@@ -2671,8 +2775,8 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
         launches += 2;
       }
       const auto raster = wrap ? k_raster<true, R, A> : k_raster<false, R, A>;
-      raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, rt, gather, obs, r.max_prims, r.pool,
-                                                                    r.max_lat, err_flag, aux);
+      raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, rt, gather, row_list, obs, r.max_prims,
+                                                                    r.pool, r.max_lat, err_flag, aux);
     });
   });
   mark();

@@ -12,7 +12,8 @@ torch.cuda.synchronize()
 c0 = env.sim.debug_counters().astype(np.int64)
 env.render_obs(); torch.cuda.synchronize()
 c = env.sim.debug_counters().astype(np.int64) - c0
-names = {8: "coarse bins", 9: "  empty (cleared)", 10: "sum of list lengths (records)", 14: "coarse bins with > 32 records", 15: "  their records",
+names = {8: "coarse bins on the rows k_raster draws", 9: "  empty, cleared there (under a LUT, wrapper formats, frames out of frame memory)",
+         30: "empty coarse bins cleared by k_raster_solo (packed u8 HWC, no LUT)", 10: "sum of list lengths (records)", 14: "coarse bins with > 32 records", 15: "  their records",
          11: "fine bins shaded", 13: "  simple (one covering prim, no visibility pass)", 12: "extra shading rounds (2nd..4th winner of edge pixels)",
          26: "  k_raster_flat: edge pixels queued for their other winners", 27: "  k_raster_flat: batches of queued pixels (32, or a bin's rest)",
          16: "warp-wide prim visits", 17: "  trivially accepted (no edge tests)", 20: "general bins holding only road tiles (coverage-only visibility)", 21: "  of those redone with depth (a sample covered twice)", 22: "coarse bins inside one prim (solo)", 23: "  their fine bins",
