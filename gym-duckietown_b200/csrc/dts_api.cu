@@ -372,8 +372,7 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
   const std::string e = renderer_prepare(*sim->render, maps_counts(*sim->maps), sim->render_mode, forward);
   if (!e.empty()) return sim->fail("%s", e.c_str());
   RenderCfg rc{sim->cfg.cam_width, sim->cfg.cam_height, sim->cfg.flags, sim->cfg.num_envs,
-               (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->fmt.obs_layout, sim->fmt.obs_dtype, sim->render_mode,
-               env_list, env_count};
+               (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->render_mode, 0, env_list, env_count};
   if (*(volatile int32_t*)sim->h_status & 1)
     return sim->fail("an earlier frame overflowed its render frame memory (prim slab / bin lists) and was left incomplete");
   if (check_loaded(sim)) return 1;
@@ -386,12 +385,6 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
     sim->prof_frames++;
   }
   const int mark_level = marks ? sim->profiling : 0;
-  void* target = obs_dev;
-  const ResizeTarget rz = resizer_target(*sim->resize);
-  if (rz.ow) {   // render full size, packed u8 HWC, into the resizer's buffer; the resize writes the caller's tensor
-    rc.obs_layout = DTS_OBS_HWC; rc.obs_dtype = DTS_OBS_U8;
-    target = rz.staging;
-  }
   GatherTab gt{};
   if (sim->gather_next) {   // (check_gather: no resize target, and the batch fits the slot)
     gt.n = sim->gather_world;
@@ -399,11 +392,20 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
       gt.base[p] = reinterpret_cast<uint8_t*>(sim->gather_peer[p]) + (uint64_t)sim->gather_rank * sim->gather_bytes;
     sim->gather_next = false;
   }
-  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, sim->aux, sim->flow, sim->occ, target,
-                        gt, sim->d_err, sim->d_status, marks, mark_level, (cudaStream_t)stream);
+  // the rasterisers draw packed u8 HWC at the camera size: into obs, or into the staging frame, from which the resize or
+  // the format pass writes obs (and the gather's slots)
+  const ResizeTarget rz = resizer_target(*sim->resize);
+  const GatherTab raster_gt = rz.staging ? GatherTab{} : gt;
+  rc.all_rows = raster_gt.n > 0;
+  int k = launch_render(*sim->render, state_arrays(*sim->state), maps_table(*sim->maps), rc, sim->aux, sim->flow, sim->occ,
+                        rz.staging ? rz.staging : obs_dev, raster_gt, sim->d_err, sim->d_status, marks, mark_level,
+                        (cudaStream_t)stream);
   if (rz.ow) {
     launch_resize(*sim->resize, rz.staging, obs_dev, sim->fmt.obs_layout, sim->fmt.obs_dtype, env_list, env_count,
                   (cudaStream_t)stream);
+    k++;
+  } else if (rz.staging) {
+    launch_format(*sim->resize, obs_dev, gt, env_list, env_count, (cudaStream_t)stream);
     k++;
   }
   if (marks && mark_level >= 2) cudaEventRecord(marks[kProfMarks - 1], (cudaStream_t)stream);   // closes the "post" interval
@@ -908,6 +910,13 @@ int dts_set_output_format(dts_sim* sim, const dts_output_format* f) {
   if (f->action_map != DTS_ACTIONS_CONTINUOUS && f->action_map != DTS_ACTIONS_DISCRETE3) return sim->fail("bad action_map %d", f->action_map);
   if (f->action_map == DTS_ACTIONS_DISCRETE3 && sim->cfg.action_mode != DTS_ACTION_VEL_STEER)
     return sim->fail("discrete actions are [vel, steering] pairs (DiscreteWrapper wraps DuckietownEnv): action_mode must be VEL_STEER");
+  if (f->obs_layout != sim->fmt.obs_layout || f->obs_dtype != sim->fmt.obs_dtype) {
+    // the staging frame may be allocated or freed: no render may be using it
+    DTS_CUDA(cudaSetDevice(sim->cfg.device));
+    DTS_CUDA(cudaDeviceSynchronize());
+    const std::string e = resizer_set_format(*sim->resize, f->obs_layout, f->obs_dtype);
+    if (!e.empty()) return sim->fail("%s", e.c_str());
+  }
   sim->fmt = *f;
   sim->step_cfg.reward_mode = f->reward_mode; sim->step_cfg.action_map = f->action_map;
   sim->step_cfg.action_vel_scale = f->action_vel_scale;

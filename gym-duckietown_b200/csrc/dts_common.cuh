@@ -157,10 +157,12 @@ __device__ __forceinline__ size_t fmt_index(int layout, int x, int y, int c, int
        : layout == DTS_OBS_CWH ? ((size_t)c * W + x) * H + y
                                : ((size_t)y * W + x) * 3 + c;
 }
+// A value v (0..255) as DTS_OBS_F32_UNIT stores it: NormalizeWrapper's v / 255 (LW:66-70)
+__device__ __forceinline__ float unit_f32(unsigned v) { return (float)v / 255.0f; }
 // Channel c of it, value v (0..255): u8, or float32 v / 255
 __device__ __forceinline__ void store_elem_fmt(void* frame, int layout, int dtype, int x, int y, int c, int W, int H, unsigned v) {
   const size_t i = fmt_index(layout, x, y, c, W, H);
-  if (dtype == DTS_OBS_F32_UNIT) reinterpret_cast<float*>(frame)[i] = (float)v / 255.0f;   // NormalizeWrapper LW:66-70
+  if (dtype == DTS_OBS_F32_UNIT) reinterpret_cast<float*>(frame)[i] = unit_f32(v);
   else reinterpret_cast<uint8_t*>(frame)[i] = (uint8_t)v;
 }
 __device__ __forceinline__ void store_px_fmt(void* frame, int layout, int dtype, int x, int y, int W, int H, unsigned rgb) {

@@ -12,8 +12,8 @@ struct RenderCfg {
   int32_t flags;
   int32_t n_envs;
   int32_t tessellate;         // 1: literal 98 triangles per road tile (spec tile mode 0)
-  int32_t obs_layout, obs_dtype;   // DTS_OBS_* (dts_output_format)
   int32_t mode;               // DTS_RENDER_* (dts_set_render_mode)
+  int32_t all_rows;           // 1: k_bin puts every row on k_raster's list (a gathering step, which ships every row)
   // Optional device list of the envs to draw: env_list[0 .. *env_count).  NULL: all n_envs.  The host never reads the
   // count: grids stay sized for n_envs and slots at or past the count exit.  Frame memory stays indexed by env id, so
   // the envs left out keep what the previous pass put there.  (n_envs stays the SoA stride of the per-env state.)
@@ -65,9 +65,10 @@ void launch_query(const DMap* maps, int map_id, int dyn_env, int n_envs, int n, 
 // dts_debug_draw: every env runs ops[0 .. n_ops) (device copy) from its stream; out[env][0 .. total)
 void launch_debug_draw(const DState& S, const dts_draw_op* ops, int n_ops, int64_t total, uint64_t* out, cudaStream_t st);
 
-// Fused end-of-rollout observation gather (SURVEY 8e): on the rollout's last step the rasteriser's resolve stores every
-// frame, besides the caller's tensor, straight into the gather buffers of all GPUs of the box — peer memory mapped with
-// cudaIpc, written over NVLink while the frame is being rasterised — instead of a separate all-gather pass afterwards.
+// Fused end-of-rollout observation gather (SURVEY 8e): on the rollout's last step every frame is stored, besides the
+// caller's tensor, straight into the gather buffers of all GPUs of the box — peer memory mapped with cudaIpc, written
+// over NVLink — instead of a separate all-gather pass afterwards: by k_raster as it finishes each row of a packed u8 HWC
+// frame, or by the format pass (launch_format) for the other layouts and dtypes.
 // base[p] = (rank p's gather buffer) + my_rank * bytes_per_rank.
 #define DTS_MAX_PEERS 8
 struct GatherTab {
@@ -166,19 +167,29 @@ FlowRemap renderer_remap(const Renderer& r, int mode);
 std::string debug_frame_copy(const Renderer& r, int env, double* V, float* P, int32_t* counts, float* lattice_by_cell,
                              int n_cells);
 
-// post passes (dts_post.cu).  The ResizeWrapper of one handle (dts_set_resize_filter): filter, tables, staging frames.
+// post passes (dts_post.cu).  The rasterisers draw packed u8 HWC at the camera size.  Where the caller's obs is anything
+// else, they draw into a staging frame and a post pass writes obs: the ResizeWrapper (dts_set_resize_filter) or the
+// format pass (dts_set_output_format).  A Resizer is the one handle's setting of both, their tables and the staging frame.
 struct Resizer;
-Resizer* resizer_create(const dts_config& cfg);   // off
+Resizer* resizer_create(const dts_config& cfg);   // no resize, packed u8 HWC
 void resizer_destroy(Resizer* z);
-// `filter` (DTS_RESIZE_*) from the camera to ow x oh, 0 x 0: off; on the handle's device, with no resize in flight.  A
+// `filter` (DTS_RESIZE_*) from the camera to ow x oh, 0 x 0: off; on the handle's device, with no render in flight.  A
 // target the filter refuses (Pillow: less than 1/32 of the camera size) or a failed allocation returns the error text
 // and leaves the previous setting.
 std::string resizer_set(Resizer& z, int filter, int ow, int oh);
-struct ResizeTarget { int ow, oh; uint8_t* staging; };   // 0 x 0: off; staging: u8[N][H][W][3], the full-size frames
+// The caller's obs layout and dtype (DTS_OBS_*), with no render in flight.  A failed allocation of the staging frame
+// returns the error text and leaves the previous setting.
+std::string resizer_set_format(Resizer& z, int layout, int dtype);
+// 0 x 0: no resize.  staging: u8[N][H][W][3], the full-size frames; null while the rasterisers write obs themselves.
+struct ResizeTarget { int ow, oh; uint8_t* staging; };
 ResizeTarget resizer_target(const Resizer& z);
 // src u8[N][H][W][3] -> dst [N] x (ow x oh) in `layout` / `dtype`, over an optional device env list like RenderCfg's
 void launch_resize(const Resizer& z, const uint8_t* src, void* dst, int layout, int dtype, const int32_t* env_list,
                    const int32_t* env_count, cudaStream_t st);
+// The staging frames -> dst at the camera size in z's layout / dtype (no resize target), and on a gathering step
+// (gt.n > 0) into every peer's gather slot as well, over an optional device env list like RenderCfg's
+void launch_format(const Resizer& z, void* dst, const GatherTab& gt, const int32_t* env_list, const int32_t* env_count,
+                   cudaStream_t st);
 // dst row e = src row e (row_bytes each) for every env e of list[0 .. *count), count <= n_envs
 void launch_copy_rows(const void* src, void* dst, size_t row_bytes, const int32_t* list, const int32_t* count, int n_envs,
                       cudaStream_t st);

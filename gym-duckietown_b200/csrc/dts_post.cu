@@ -1,5 +1,6 @@
-// dts_post.cu — the passes over finished frames: the ResizeWrappers (k_resize_band, k_resize, k_resize_pil) and the
-// Resizer that owns their tables and staging frame, MotionBlurWrapper's k_blend4, dts_step_terminal's k_copy_rows.
+// dts_post.cu — the passes over finished frames: the ResizeWrappers (k_resize_band, k_resize, k_resize_pil), the output
+// format pass (k_format) and the Resizer that owns their tables and staging frame, MotionBlurWrapper's k_blend4,
+// dts_step_terminal's k_copy_rows.
 #include <algorithm>
 #include <cstdlib>
 #include <vector>
@@ -29,11 +30,16 @@ struct PilTab {
 struct Resizer {
   int n, W, H;                         // envs and camera of the handle
   int filter = DTS_RESIZE_CV2_CUBIC, ow = 0, oh = 0;   // DTS_RESIZE_* and the target; 0 x 0: off
-  uint8_t* staging = nullptr;          // [n][H][W][3] the full-size frames (null while off)
+  int layout = DTS_OBS_HWC, dtype = DTS_OBS_U8;        // the caller's obs (dts_set_output_format)
+  uint8_t* staging = nullptr;          // [n][H][W][3] the full-size frames (null unless staged())
   int16_t* cubic = nullptr;            // cv2: the tap tables [ow][8] then [oh][8] (null unless cv2 is set), and
   int band = 0, cap = 0;               // k_resize_band's plan (plan_resize_bands; band 0: the untiled k_resize)
   PilTab pil{};                        // Pillow: tap tables and band plan (null unless Pillow is set)
 };
+
+// The rasterisers draw into the staging frame, and a post pass writes obs, whenever obs is not their packed u8 HWC frame
+// at the camera size
+static bool staged(const Resizer& z) { return z.ow || z.layout != DTS_OBS_HWC || z.dtype != DTS_OBS_U8; }
 
 constexpr size_t kSmemOptInMax = 200 * 1024;   // dynamic shared memory of the largest band plan either filter makes
 
@@ -455,21 +461,38 @@ static std::string pil_tables(Resizer& z) {
 
 Resizer* resizer_create(const dts_config& cfg) { return new Resizer{cfg.num_envs, cfg.cam_width, cfg.cam_height}; }
 
-void resizer_destroy(Resizer* z) { if (z) resizer_set(*z, 0, 0, 0); delete z; }
+void resizer_destroy(Resizer* z) {
+  if (z) { cudaFree(z->staging); cudaFree(z->cubic); cudaFree(z->pil.tab); }
+  delete z;
+}
 
-std::string resizer_set(Resizer& z, int filter, int ow, int oh) {
-  Resizer t{z.n, z.W, z.H, filter, ow, oh, ow ? z.staging : nullptr};   // built beside z, sharing its full-size frames
-  std::string e = !ow ? "" : filter == DTS_RESIZE_PIL_BILINEAR ? pil_tables(t) : cubic_tables(t);
-  if (e.empty() && ow && !t.staging) {
+// z <- t, a setting built beside it (`e`: the error building it failed with, if any): t keeps z's staging frame or gets a
+// new one if staged(t) needs one.  What the setting that is left over holds and z does not is freed.
+static std::string replace(Resizer& z, Resizer& t, std::string e) {
+  t.staging = staged(t) ? z.staging : nullptr;
+  if (e.empty() && staged(t) && !t.staging) {
     void* p = nullptr;
     const cudaError_t ce = cudaMalloc(&p, (size_t)t.n * t.W * t.H * 3);
     if (ce == cudaSuccess) t.staging = reinterpret_cast<uint8_t*>(p);
-    else e = std::string("resize staging frame cudaMalloc failed: ") + cudaGetErrorString(ce);
+    else e = std::string("staging frame cudaMalloc failed: ") + cudaGetErrorString(ce);
   }
   if (e.empty()) std::swap(z, t);   // t: the setting to release, the previous one or the one that failed
   if (t.staging != z.staging) cudaFree(t.staging);
-  cudaFree(t.cubic); cudaFree(t.pil.tab);
+  if (t.cubic != z.cubic) cudaFree(t.cubic);
+  if (t.pil.tab != z.pil.tab) cudaFree(t.pil.tab);
   return e;
+}
+
+std::string resizer_set(Resizer& z, int filter, int ow, int oh) {
+  Resizer t{z.n, z.W, z.H, filter, ow, oh, z.layout, z.dtype};
+  const std::string e = !ow ? "" : filter == DTS_RESIZE_PIL_BILINEAR ? pil_tables(t) : cubic_tables(t);
+  return replace(z, t, e);
+}
+
+std::string resizer_set_format(Resizer& z, int layout, int dtype) {
+  Resizer t = z;   // (the same tables)
+  t.layout = layout; t.dtype = dtype;
+  return replace(z, t, "");
 }
 
 ResizeTarget resizer_target(const Resizer& z) { return ResizeTarget{z.ow, z.oh, z.staging}; }
@@ -492,6 +515,44 @@ void launch_resize(const Resizer& z, const uint8_t* src, void* dst, int layout, 
   const size_t cap = device_sms() * 16;
   const int blocks = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
   k_resize<<<blocks, 256, 0, st>>>(src, z.W, z.H, z.ow, z.oh, z.n, xtab, ytab, dst, layout, dtype, env_list, env_count);
+}
+
+// ------------------------------------------------------------------------------------------------ k_format
+// The staging frames at the camera size -> the caller's layout / dtype (dts_set_output_format) and, on a gathering step,
+// every peer's gather slot at the same offset: a thread per pixel, grid-stride over the listed envs' pixels.  HWC
+// (float32 here: packed u8 HWC is not staged without a resize) where W * H % 32 == 0, so that a warp's 32 pixels are
+// consecutive in one frame: the lanes take the warp's 96 elements interleaved, each the staging byte of the same index,
+// so that a warp's stores are contiguous instead of three 12-byte-strided float stores.
+__global__ void __launch_bounds__(256) k_format(const uint8_t* __restrict__ src, int W, int H, int n_envs, void* __restrict__ dst,
+                                                int layout, int dtype, GatherTab gt, const int32_t* __restrict__ env_list,
+                                                const int32_t* __restrict__ env_count) {
+  const size_t px = (size_t)W * H, frame_bytes = px * 3 * (dtype == DTS_OBS_F32_UNIT ? 4 : 1);
+  const bool interleave = layout == DTS_OBS_HWC && px % 32 == 0;
+  const size_t total = (size_t)n_listed(env_list, env_count, n_envs) * px;
+  const int lane = threadIdx.x & 31;
+  for (size_t g = blockIdx.x * (size_t)blockDim.x + threadIdx.x; g < total; g += (size_t)gridDim.x * blockDim.x) {
+    const size_t env = (size_t)listed_env(env_list, (int)(g / px)), i = g % px;
+    const uint8_t* s = src + env * px * 3;
+    const unsigned rgb = interleave ? 0u : (unsigned)s[3 * i] | ((unsigned)s[3 * i + 1] << 8) | ((unsigned)s[3 * i + 2] << 16);
+#pragma unroll
+    for (int p = -1; p < DTS_MAX_PEERS; p++) {   // obs, then the peers' slots (constant indices: gt stays in the parameter space)
+      if (p >= gt.n) break;
+      uint8_t* out = (p < 0 ? reinterpret_cast<uint8_t*>(dst) : gt.base[p < 0 ? 0 : p]) + env * frame_bytes;
+      if (interleave) {
+#pragma unroll
+        for (size_t j = 0, e = (i - lane) * 3 + lane; j < 3; j++, e += 32) reinterpret_cast<float*>(out)[e] = unit_f32(s[e]);
+      } else {
+        store_px_fmt(out, layout, dtype, (int)(i % W), (int)(i / W), W, H, rgb);
+      }
+    }
+  }
+}
+
+void launch_format(const Resizer& z, void* dst, const GatherTab& gt, const int32_t* env_list, const int32_t* env_count,
+                   cudaStream_t st) {
+  const size_t blocks = ((size_t)z.n * z.W * z.H + 255) / 256, cap = device_sms() * 16;
+  k_format<<<(unsigned)std::min(blocks, cap), 256, 0, st>>>(z.staging, z.W, z.H, z.n, dst, z.layout, z.dtype, gt, env_list,
+                                                            env_count);
 }
 
 // ------------------------------------------------------------------------------------------------ k_blend4

@@ -770,60 +770,13 @@ __device__ __forceinline__ void store_bin_fast(uint8_t* __restrict__ bin0, const
   const unsigned word = __funnelshift_r(lo | (hi << 24), hi >> 8, sl.sh8);   // (lo | hi << 24) >> sh8, low 32 bits
   if (sl.j < 6 && sl.row < rows_ok) *reinterpret_cast<unsigned*>(bin0 + sl.off) = word;
 }
-// general form (any width, bins cut by the right border)
-__device__ __forceinline__ void store_bin(uint8_t* __restrict__ out, unsigned rgb, int lane, int bx, int by, int W, int H) {
+// byte form (any width, bins cut by the right border): a lane stores its own pixel
+__device__ __forceinline__ void store_bin_bytes(uint8_t* __restrict__ out, unsigned rgb, int lane, int bx, int by, int W, int H) {
   const int gx = bx * kBinW + (lane & 7), gy = by * kBinH + (lane >> 3);
-  if ((W & 3) == 0 && bx * kBinW + kBinW <= W) {
-    const int j = lane & 7, rowbase = lane & ~7;
-    const int p0 = (4 * j) / 3, sh8 = (4 * j - 3 * p0) * 8;
-    const unsigned lo = __shfl_sync(0xffffffffu, rgb, rowbase + min(p0, 7));
-    const unsigned hi = __shfl_sync(0xffffffffu, rgb, rowbase + min(p0 + 1, 7));
-    const unsigned long long both = (unsigned long long)lo | ((unsigned long long)hi << 24);
-    if (j < 6 && gy < H)
-      *reinterpret_cast<unsigned*>(out + ((size_t)gy * W + bx * kBinW) * 3 + 4 * j) = (unsigned)(both >> sh8);
-  } else if (gx < W && gy < H) {
+  if (gx < W && gy < H) {
     uint8_t* d = out + ((size_t)gy * W + gx) * 3;
     d[0] = (uint8_t)(rgb & 255); d[1] = (uint8_t)((rgb >> 8) & 255); d[2] = (uint8_t)(rgb >> 16);
   }
-}
-
-// One whole 8x4 bin in a PLANAR u8 layout (ImgWrapper's CHW, PyTorchObsWrapper's CWH) as 24 aligned 32-bit words, one per
-// lane: a word is four horizontally (CHW) or vertically (CWH) adjacent pixels of one channel plane, collected from the
-// four lanes holding them by shuffles and two byte permutes — instead of three scattered byte stores per lane.
-// Needs the bin inside the image and W % 4 == 0 (CHW) / H % 4 == 0 (CWH).
-__device__ __forceinline__ void store_bin_planar_u8(uint8_t* __restrict__ out, int layout, unsigned rgb, int lane, int bx, int by,
-                                                    int W, int H) {
-  const int j = lane < 24 ? lane : 0, c = j >> 3;
-  int s0, step;
-  size_t addr;
-  if (layout == DTS_OBS_CHW) {
-    const int r = (j & 7) >> 1, h = j & 1;
-    s0 = r * 8 + 4 * h; step = 1;
-    addr = ((size_t)c * H + by * kBinH + r) * W + bx * kBinW + 4 * h;
-  } else {
-    const int xi = j & 7;
-    s0 = xi; step = 8;
-    addr = ((size_t)c * W + bx * kBinW + xi) * H + by * kBinH;
-  }
-  const unsigned p0 = __shfl_sync(0xffffffffu, rgb, s0), p1 = __shfl_sync(0xffffffffu, rgb, s0 + step);
-  const unsigned p2 = __shfl_sync(0xffffffffu, rgb, s0 + 2 * step), p3 = __shfl_sync(0xffffffffu, rgb, s0 + 3 * step);
-  const unsigned sel = (unsigned)c | ((unsigned)(4 + c) << 4);   // byte c of the first operand, byte c of the second
-  const unsigned word = __byte_perm(__byte_perm(p0, p1, sel), __byte_perm(p2, p3, sel), 0x5410);
-  if (lane < 24) *reinterpret_cast<unsigned*>(out + addr) = word;
-}
-
-// Fine-bin store: the packed u8 HWC fast path, or the wrapper format straight from the resolve registers.
-__device__ __forceinline__ void store_bin_any(uint8_t* __restrict__ out, int fmt, unsigned rgb, int lane, int bx, int by,
-                                              int W, int H) {
-  if (fmt == 0) { store_bin(out, rgb, lane, bx, by, W, H); return; }
-  const int gx = bx * kBinW + (lane & 7), gy = by * kBinH + (lane >> 3);
-  if (gx < W && gy < H) store_px_fmt(out, fmt & 3, fmt >> 2, gx, gy, W, H, rgb);
-}
-
-// Packed u8 HWC whose rows are whole 32-bit words: the only output k_raster_solo and k_raster_flat write.  k_bin lists
-// bins for them, and launch_render launches them, under exactly this test; a bin listed but not drawn would stay unwritten.
-__host__ __device__ __forceinline__ bool lean_output(int layout, int dtype, int W) {
-  return layout == DTS_OBS_HWC && dtype == DTS_OBS_U8 && (W & 3) == 0;
 }
 
 // The fine bins of coarse bin (cbx, cby) that lie inside the image, as bits f = column | row << 2: all 8 except on the
@@ -856,11 +809,14 @@ __device__ __forceinline__ RemapTab remap_of_env(RemapTab rt, int env, int W, in
   return rt;
 }
 
-// One fine bin of a lean_output() frame: whole words if the bin lies inside the image, else the general form
-__device__ __forceinline__ void store_bin_lean(uint8_t* __restrict__ out, const StoreLane& sl, unsigned rgb, int lane, int bx, int by,
-                                               int W, int H) {
-  if (bx * kBinW + kBinW <= W) store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
-  else store_bin(out, rgb, lane, bx, by, W, H);
+// One fine bin of a packed u8 HWC frame, the store all three rasterisers share: whole words where the image's rows are
+// (W % 4 == 0) and the bin lies inside it, else a byte per channel
+__device__ __forceinline__ void store_bin(uint8_t* __restrict__ out, const StoreLane& sl, unsigned rgb, int lane, int bx, int by,
+                                          int W, int H) {
+  if ((W & 3) == 0 && bx * kBinW + kBinW <= W)
+    store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
+  else
+    store_bin_bytes(out, rgb, lane, bx, by, W, H);
 }
 
 // Depth target (render spec item 9): the eye-space depth of a pixel is 1 / (the largest 1/w among the distinct winners
@@ -1399,8 +1355,7 @@ k_tiles(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm
 // pairs — count (shared-memory atomics), scan, scatter; prims with a small bounding box are binned by it, larger ones
 // test each bin of the box against their edges, one bin per lane.  Pass 2, dense over the pairs (one per thread, so a
 // screen-filling prim costs no more lanes than a sliver): the pair's BinRec.
-// Then, for lean output only: the lists of the bins k_raster_solo and k_raster_flat draw, and the list of the rows
-// k_raster still has to draw.
+// Then the lists of the bins k_raster_solo and k_raster_flat draw, and the list of the rows k_raster still has to draw.
 constexpr int kBinWarps = 4;
 constexpr int kCountMask = 0xfffff, kGroundInc = 1 << 20;   // a bin's counter: records | ground-quad records << 20
 constexpr int kFlatBin = -0x7fffffff - 1;   // bin_count of a flat bin (k_raster_flat); solo bins hold -(prim + 1) >= -65536
@@ -1410,6 +1365,13 @@ constexpr int kSoloMark = 2;   // no_flat[] bit of a solo bin (bit 0: not flat)
 __device__ __forceinline__ void row_to_list(const FrameMem& fm, int env, int cby, int cbins_y) {
   if (atomicOr(fm.row_flag + (size_t)env * cbins_y + cby, 1) == 0)
     fm.rows[atomicAdd(fm.work + kWorkRowList, 1)] = make_uint2((unsigned)env, (unsigned)cby);
+}
+// Every row of `env` onto k_raster's list, its flags set (the CTA's threads tid of nthr)
+__device__ __forceinline__ void list_every_row(const FrameMem& fm, int env, int cbins_y, int tid, int nthr) {
+  for (int r = tid; r < cbins_y; r += nthr) {
+    fm.row_flag[(size_t)env * cbins_y + r] = 1;
+    fm.rows[atomicAdd(fm.work + kWorkRowList, 1)] = make_uint2((unsigned)env, (unsigned)r);
+  }
 }
 // kListed: the frame draws the envs of rc.env_list.  (Its own instance: an env id loaded from the list stays live across
 // the kernel, where blockIdx.x is re-read for free, and would cost the remap instances registers and spills.)
@@ -1552,12 +1514,7 @@ k_bin(RenderCfg rc, FrameMem fm, RemapTab rts, int max_prims, int max_pairs, int
       }
       if (!ok) {
         if (tid == 0) { fm.ctx[env].overflow = 1; atomicOr(err, 1); *reinterpret_cast<volatile int32_t*>(fm.status) = 1; }
-        // every bin holds count 0: k_raster clears the whole frame
-        if (lean_output(rc.obs_layout, rc.obs_dtype, W))
-          for (int r = tid; r < cbins_y; r += nthr) {
-            fm.row_flag[(size_t)env * cbins_y + r] = 1;
-            fm.rows[atomicAdd(fm.work + kWorkRowList, 1)] = make_uint2((unsigned)env, (unsigned)r);
-          }
+        list_every_row(fm, env, cbins_y, tid, nthr);   // every bin holds count 0: k_raster clears the whole frame
         return;
       }
     }
@@ -1565,15 +1522,12 @@ k_bin(RenderCfg rc, FrameMem fm, RemapTab rts, int max_prims, int max_pairs, int
   // pass 2: one pair per thread -> its visibility record (the pairs were written by other threads of this CTA: the
   // barrier above orders those writes before these reads)
   const int pair0 = s_base, total = s_total;
-  const bool lean_fmt = lean_output(rc.obs_layout, rc.obs_dtype, W);
   // start[] is free from here on: per coarse bin, nonzero once a record rules the bin out of k_raster_flat (a mesh
   // triangle, a tiny triangle, or a solo bin, which also sets kSoloMark)
   int* no_flat = start;
-  if (lean_fmt) {
-    for (int b = tid; b < cbins; b += nthr) no_flat[b] = 0;
-    for (int r = tid; r < cbins_y; r += nthr) fm.row_flag[(size_t)env * cbins_y + r] = 0;
-    __syncthreads();
-  }
+  for (int b = tid; b < cbins; b += nthr) no_flat[b] = 0;
+  for (int r = tid; r < cbins_y; r += nthr) fm.row_flag[(size_t)env * cbins_y + r] = 0;
+  __syncthreads();
   BinRec* recs = fm.recs;
   for (int i = pair0 + tid; i < pair0 + total; i += nthr) {
     const uint32_t pair = pairs[i];
@@ -1586,31 +1540,30 @@ k_bin(RenderCfg rc, FrameMem fm, RemapTab rts, int max_prims, int max_pairs, int
     } else {
       r = build_binrec(prims + p, p, cbx * kCoarseW * kSub, cby * kCoarseH * kSub, recs + i);
     }
-    if (lean_fmt) {
-      // the coarse bin lies inside this prim and holds no other (besides the ground, hidden below it): no visibility
-      // work at all -> the bin goes to k_raster_solo, and k_raster skips it (negative count)
-      const int c = cnt[b];
-      const unsigned valid = fine_in_image(cbx, fine_rows_in_image(cby, H), W);
-      // (... or it is the bin's only record: a stretch of bare ground)
-      const bool alone = (r & kRecGround) ? (c & kCountMask) == 1 : (c & kCountMask) - (c >> 20) == 1;
-      if (alone && (r & valid) == valid) {
-        fm.bin_count[(size_t)env * cbins + b] = -(p + 1);
-        const int slot = atomicAdd(fm.work + kWorkSoloList, 1);
-        fm.solo[slot] = make_uint2((unsigned)env, (unsigned)b | ((unsigned)p << 16));
-        atomicOr(&no_flat[b], 1 | kSoloMark);
-      }
-      if (!(r & kRecFlatOk)) atomicOr(&no_flat[b], 1);
+    // the coarse bin lies inside this prim and holds no other (besides the ground, hidden below it): no visibility
+    // work at all -> the bin goes to k_raster_solo, and k_raster skips it (negative count)
+    const int c = cnt[b];
+    const unsigned valid = fine_in_image(cbx, fine_rows_in_image(cby, H), W);
+    // (... or it is the bin's only record: a stretch of bare ground)
+    const bool alone = (r & kRecGround) ? (c & kCountMask) == 1 : (c & kCountMask) - (c >> 20) == 1;
+    if (alone && (r & valid) == valid) {
+      fm.bin_count[(size_t)env * cbins + b] = -(p + 1);
+      const int slot = atomicAdd(fm.work + kWorkSoloList, 1);
+      fm.solo[slot] = make_uint2((unsigned)env, (unsigned)b | ((unsigned)p << 16));
+      atomicOr(&no_flat[b], 1 | kSoloMark);
     }
+    if (!(r & kRecFlatOk)) atomicOr(&no_flat[b], 1);
   }
-  if (!lean_fmt) return;
   // flat bins: 1..kStage records, every one a flat road tile or the ground quad, not solo -> k_raster_flat's list, and
-  // k_raster skips them (kFlatBin) unless k_raster_flat hands one back.  Empty bins, without a LUT -> k_raster_solo's
-  // empty list, which clears them, and k_raster skips them (kEmptyBin).  A row holding any other bin -> k_raster's list.
+  // k_raster skips them (kFlatBin) unless k_raster_flat hands one back.  Empty bins, without a LUT and where the image's
+  // rows are whole words -> k_raster_solo's empty list, which clears them, and k_raster skips them (kEmptyBin).  A row
+  // holding any other bin -> k_raster's list.
   __syncthreads();
   for (int b0 = wib * 32; b0 < cbins; b0 += nthr) {
     const int b = b0 + lane, c = b < cbins ? (cnt[b] & kCountMask) : 0;
     const bool flat = c >= 1 && c <= kStage && !no_flat[b];
-    const bool empty = kRemap == kRemapNone && b < cbins && c == 0;   // (under a LUT k_raster clears them, per pixel)
+    // (otherwise k_raster clears them, per pixel: clear_empty_bins stores whole words, and the LUT can name no source)
+    const bool empty = kRemap == kRemapNone && (W & 3) == 0 && b < cbins && c == 0;
     const unsigned m = __ballot_sync(0xffffffffu, flat), me = __ballot_sync(0xffffffffu, empty);
     if (m) {
       int base = 0;
@@ -1631,17 +1584,11 @@ k_bin(RenderCfg rc, FrameMem fm, RemapTab rts, int max_prims, int max_pairs, int
         fm.empty[base + __popc(me & ((1u << lane) - 1u))] = make_uint2((unsigned)env, (unsigned)b);
       }
     }
-    if (b < cbins && !flat && !empty && !(no_flat[b] & kSoloMark)) row_to_list(fm, env, b / cbins_x, cbins_y);
+    // (a gathering step ships every row from k_raster: all of them on its list)
+    if (b < cbins && (rc.all_rows || (!flat && !empty && !(no_flat[b] & kSoloMark)))) row_to_list(fm, env, b / cbins_x, cbins_y);
   }
 }
 
-// Everything the inline store does not cover — wrapper layouts / dtypes, widths that are no multiple of 4, bins cut
-// by the right border, and the gathering step's extra stores into every peer's buffer — out of line.
-__device__ __noinline__ void emit_general(uint8_t* __restrict__ out, const GatherTab& gt, int n_peers, size_t env_off, int out_fmt,
-                                          unsigned rgb, int lane, int bx, int by, int W, int H) {
-  store_bin_any(out, out_fmt, rgb, lane, bx, by, W, H);
-  for (int p = 0; p < n_peers; p++) store_bin_any(gt.base[p] + env_off, out_fmt, rgb, lane, bx, by, W, H);
-}
 // A finished run of image rows -> every rank's gather buffer (peer memory over NVLink): 16-byte vectors, 512 contiguous
 // bytes per warp store.  The rows were written by this very warp (__syncwarp orders those stores before these loads).
 __device__ __noinline__ void gather_rows_out(const uint8_t* __restrict__ src, const GatherTab& gt, size_t off, size_t nbytes, int lane) {
@@ -1772,14 +1719,13 @@ __device__ __forceinline__ unsigned shade_resolve(const unsigned wn[4], bool sim
 }
 
 // ------------------------------------------------------------------------------------------------ k_raster
-template <bool kWrapFmt, int kRemap, int kAux>
-                                       // kWrapFmt: a dts_output_format other than packed u8 HWC is written by the resolve;
-                                       // kRemap other than kRemapNone: every lane renders the SOURCE pixel the LUT names
+// A work item is one row of coarse bins of one env, from the list k_bin and k_raster_flat built: the rows holding a bin
+// that neither k_raster_solo nor k_raster_flat drew, or on a gathering step every row.
+template <int kRemap, int kAux>        // kRemap other than kRemapNone: every lane renders the SOURCE pixel the LUT names
                                        // for its output pixel;
                                        // kAux: the images written beside obs (AuxTargets)
-                                       // row_list: the work items are the rows on fm.rows (launch_render)
 __global__ void __launch_bounds__(kThreads, kRasterMinCtas)
-k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, RemapTab rts, GatherTab gt, bool row_list,
+k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem fm, RemapTab rts, GatherTab gt,
          uint8_t* __restrict__ obs, int max_prims, int max_pairs, int max_lat, int32_t* __restrict__ err, AuxTargets aux) {
   // dynamic shared memory (kRasterSmem bytes): per warp two chunks of records in flight, their mbarriers, and a 128-sample
   // depth / winner buffer for the tiny triangles of the fine bin being drawn
@@ -1792,67 +1738,39 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
   const int cbins_x = (W + kCoarseW - 1) / kCoarseW, cbins_y = (H + kCoarseH - 1) / kCoarseH, cbins = cbins_x * cbins_y;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const size_t frame_bytes = (size_t)W * H * 3;
-  const int out_fmt = !kWrapFmt ? 0 : (rc.obs_layout | (rc.obs_dtype << 2));   // wrapper output format (0 = packed u8 HWC)
-  const size_t out_elem = (kWrapFmt && rc.obs_dtype == DTS_OBS_F32_UNIT) ? 4 : 1;
   const int pxs = (lane & 7) * kSub, pys = (lane >> 3) * kSub;   // this lane's pixel inside a fine bin (sub-pixels)
   const StoreLane sl = make_store_lane(lane, W);
-  const bool fast_fmt = !kWrapFmt && lean_output(DTS_OBS_HWC, DTS_OBS_U8, W);   // (k_raster<false, *> writes packed u8 HWC)
-  const bool planar_u8 = kWrapFmt && rc.obs_dtype == DTS_OBS_U8 &&
-                         ((rc.obs_layout == DTS_OBS_CHW && (W & 3) == 0) || (rc.obs_layout == DTS_OBS_CWH && (H & 3) == 0));
   uint64_t* bar = bars[warp];
   if (lane == 0) { mbar_init(&bar[0], 1); mbar_init(&bar[1], 1); mbar_fence_init(); }
   __syncwarp();
   uint32_t parity = 0;   // bit s: the phase the next wait on slot s completes
   int cs = 0, ps = 0;    // consumer / producer slot
-  // work item = one row of coarse bins of one env: every row of every (listed) env, or the rows on the list
-  const int n_work = row_list ? fm.work[kWorkRowList] : n_listed(rc.env_list, rc.env_count, rc.n_envs) * cbins_y;
+  const int n_work = fm.work[kWorkRowList];
   int work = 0;
   if (lane == 0) work = atomicAdd(fm.work + kWorkRaster, 1);
   work = __shfl_sync(0xffffffffu, work, 0);
   while (work < n_work) {
     int next_work = 0;
     if (lane == 0) next_work = atomicAdd(fm.work + kWorkRaster, 1);   // consumed after this row: latency hidden
-    int env, cby;
-    if (row_list) {
-      const uint2 r = fm.rows[work];
-      env = (int)r.x; cby = (int)r.y;
-    } else {
-      const int slot = work / cbins_y;
-      cby = work - slot * cbins_y;
-      env = listed_env(rc.env_list, slot);
-    }
+    const uint2 row = fm.rows[work];
+    const int env = (int)row.x, cby = (int)row.y;
     const RemapTab rt = kRemap == kRemapPool ? remap_of_env(rts, env, W, H, cbins) : rts;
     const DMap& m = maps[S.map_id[env]];
     const uint8_t* tex_pool = m.tex_pool;
     const PrimRec* prims = fm.prims + (size_t)env * max_prims;
     const BinRec* recs = fm.recs;   // bin_start holds pool indices
     const float4* lat_tab = fm.lat + (size_t)env * max_lat * 64;
-    const size_t env_off = (size_t)env * frame_bytes * out_elem;
+    const size_t env_off = (size_t)env * frame_bytes;
     uint8_t* out = obs + env_off;
     const AuxFrames af = aux_frames(aux, env, W, H);
     const uint8_t* cls_pool = (kAux & kAuxMarks) ? tex_pool + m.tex_class_off : nullptr;
     LabelMap lm{};
     if constexpr (takes_winner(kAux)) lm = label_map(m, rc.tessellate);
     auto label_of = [&](unsigned w) { return label_of_id(lm, __ldg(&prims[w].id)); };
-    // one fine bin -> the caller's tensor and, on a gathering step, every peer's gather buffer (NVLink stores)
-    // On a gathering step (gt.n > 0) the packed u8 HWC frame goes to the peers in BLOCKS: a work item is 8 whole image rows =
-    // one contiguous run of bytes, copied to every rank's gather buffer with 16-byte vector stores once the item is drawn
-    // (NVLink wants long writes: per-bin 4-byte stores reach a fifth of the link rate).  Other layouts store per bin.
-    const bool gather_rows = gt.n > 0 && !kWrapFmt;
+    // one fine bin -> obs and the images (the caller's tensors only: the gather carries obs)
     auto emit = [&](unsigned rgb, float depth, int label, int mark, int bx, int by) {
-      store_aux<kAux>(af, depth, label, mark, lane, bx, by, W, H);   // (the caller's tensors only: the gather carries obs)
-      if (fast_fmt && (gt.n == 0 || gather_rows) && bx * kBinW + kBinW <= W) {   // the common case inline: packed u8 HWC, whole bin inside
-        store_bin_fast(out + ((size_t)(by * kBinH) * W + bx * kBinW) * 3, sl, rgb, min(kBinH, H - by * kBinH));
-      } else if (kWrapFmt && gt.n == 0) {
-        if (planar_u8 && bx * kBinW + kBinW <= W && by * kBinH + kBinH <= H) {
-          store_bin_planar_u8(out, out_fmt & 3, rgb, lane, bx, by, W, H);   // CHW / CWH u8: 24 packed words per bin
-        } else {
-          const int gx = bx * kBinW + (lane & 7), gy = by * kBinH + (lane >> 3);
-          if (gx < W && gy < H) store_px_fmt(out, out_fmt & 3, out_fmt >> 2, gx, gy, W, H, rgb);   // wrapper layout / dtype, inline
-        }
-      } else {
-        emit_general(out, gt, gather_rows ? 0 : gt.n, env_off, out_fmt, rgb, lane, bx, by, W, H);
-      }
+      store_aux<kAux>(af, depth, label, mark, lane, bx, by, W, H);
+      store_bin(out, sl, rgb, lane, bx, by, W, H);
     };
     float clr[3];
     clear_colour(S, rc, env, clr);
@@ -2127,7 +2045,10 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
         }
       }
     }
-    if (gather_rows) {   // the item's rows are complete: ship them to every rank
+    // On a gathering step the frame goes to the peers in BLOCKS: a work item is 8 whole image rows = one contiguous run of
+    // bytes, copied to every rank's gather buffer with 16-byte vector stores once the item is drawn (NVLink wants long
+    // writes: per-bin 4-byte stores reach a fifth of the link rate)
+    if (gt.n > 0) {   // the item's rows are complete: ship them to every rank
       const int rows = min(kCoarseH, H - cby * kCoarseH);
       gather_rows_out(obs, gt, env_off + (size_t)cby * kCoarseH * W * 3, (size_t)rows * W * 3, lane);
     }
@@ -2136,11 +2057,11 @@ k_raster(const DState S, const DMap* __restrict__ maps, RenderCfg rc, FrameMem f
 }
 
 // ------------------------------------------------------------------------------------------------ k_raster_solo
-// k_bin's empty bins (no LUT): the clear colour in obs, 0 in every image.  A bin waits on two dependent loads (its
-// entry, then its env's horizon), so a warp takes eight bins at once, one lane loading each, and then stores them one
-// after the other, a whole image row of the bin per store: the row's pixels of obs as words (lean output: the row starts
-// on a word and its 3 * 32 bytes, or 3 * a multiple of 4 at the right border, are whole words), cycling through the
-// three words of the packed colour, and each image's row, a lane per pixel.
+// k_bin's empty bins (no LUT, W % 4 == 0): the clear colour in obs, 0 in every image.  A bin waits on two dependent
+// loads (its entry, then its env's horizon), so a warp takes eight bins at once, one lane loading each, and then stores
+// them one after the other, a whole image row of the bin per store: the row's pixels of obs as words (W % 4 == 0: the
+// row starts on a word and its 3 * 32 bytes, or 3 * a multiple of 4 at the right border, are whole words), cycling
+// through the three words of the packed colour, and each image's row, a lane per pixel.
 template <int kAux>
 __device__ __forceinline__ void clear_empty_bins(const DState& S, const RenderCfg& rc, const FrameMem& fm, uint8_t* __restrict__ obs,
                                                  const AuxTargets& aux) {
@@ -2186,9 +2107,9 @@ __device__ __forceinline__ void clear_empty_bins(const DState& S, const RenderCf
 // fine bin — 22 of the 55 non-empty coarse bins of a c2 frame, 40 % of the shaded pixels) need no records, no staging, no
 // visibility state: a warp fetches the prim's planes once and shades the bin's 256 pixels.  A separate kernel so that the
 // lean loop gets its own register allocation (the same fast path inside k_raster cost more than it saved).
-// Without a LUT the empty bins come here first (k_bin's empty list: the sky, 20 of a c2 frame's 75 bins), so that
-// k_raster does not walk their rows: the clear colour, and 0 in every image, as k_raster writes them (clear_empty_bins).
-// Packed u8 HWC output with whole-word rows only (k_bin marks no bin otherwise).  Runs before k_raster.
+// Without a LUT, where the image's rows are whole words, the empty bins come here first (k_bin's empty list: the sky, 20
+// of a c2 frame's 75 bins), so that k_raster does not walk their rows: the clear colour, and 0 in every image, as
+// k_raster writes them (clear_empty_bins).  Runs before k_raster.
 // Images: the 1/w the shading divides by gives the depth, the bin's one prim the label of every pixel with a source, and
 // the texel it shows there the marking.
 template <int kRemap, int kAux>   // kRemap other than kRemapNone: each lane shades the source pixel the LUT names for its output pixel
@@ -2239,7 +2160,7 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
                  (kAux & kAuxMarks) ? &mk : nullptr);
       unsigned rgb = pack_rgb(c3[0], c3[1], c3[2]);
       if (kRemap != kRemapNone && !px_valid) rgb = 0u;
-      store_bin_lean(out, sl, rgb, lane, bx, by, W, H);
+      store_bin(out, sl, rgb, lane, bx, by, W, H);
       store_aux<kAux>(af, depth_of(qq, px_valid), px_valid ? lab : 0, px_valid ? mk : 0, lane, bx, by, W, H);
     }
   }
@@ -2252,7 +2173,7 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
 // no depth arithmetic.  The ground quad lies below every tile and takes the samples no tile covers, where its depth
 // passes GL_LESS against the cleared 1.0; samples nothing covers keep the clear colour.  The answer is k_raster's
 // coverage-only path, in a kernel of its own so that it is not held to k_raster's register allocation
-// (depth state, the tiny-triangle buffer, chunk streaming, wrapper layouts, the gather).
+// (depth state, the tiny-triangle buffer, chunk streaming, the gather).
 // Edge pixels are shaded across the whole coarse bin: each fine bin shades every pixel's first winner, and a pixel with
 // more than one distinct winner (about a quarter of a general fine bin's lanes) joins a per-warp queue instead of keeping
 // the warp for a round at a quarter of its lanes.  Whenever 32 pixels are queued, and after the bin's last fine bin, each
@@ -2267,7 +2188,7 @@ __global__ void __launch_bounds__(kThreads, kSoloMinCtas) k_raster_solo(const DS
 // is looked up again from the first winner, which the queue holds.  Only the ground and road tiles come here, so a label
 // is arithmetic on the draw id (tile_label).  A bin handed back may have stored some images already: k_raster rewrites
 // the whole bin, colour and images.
-// Packed u8 HWC output with whole-word rows only (k_bin lists no bin otherwise).  Runs after k_raster_solo.
+// Runs after k_raster_solo.
 constexpr int kEdgeQ = 64;   // queue ring: flushed at 32 entries, so at most 31 + 32 wait at once
 template <int kRemap, int kAux>   // kRemap other than kRemapNone: each lane covers and shades the source pixel the LUT names
                                   // for its output pixel
@@ -2453,7 +2374,7 @@ __global__ void __launch_bounds__(kThreads, kFlatMinCtas) k_raster_flat(const DS
 #pragma unroll 1
     for (int f = 0; f < kCFX * kCFY; f++) {
       if ((f & 3) >= nx || (f >> 2) >= ny) continue;
-      store_bin_lean(out, sl, rgb_buf[f * 32 + lane], lane, cbx * kCFX + (f & 3), cby * kCFY + (f >> 2), W, H);
+      store_bin(out, sl, rgb_buf[f * 32 + lane], lane, cbx * kCFX + (f & 3), cby * kCFY + (f >> 2), W, H);
     }
   }
 }
@@ -2737,7 +2658,7 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
   mark();
   const size_t pairs_total = (size_t)rc.n_envs * r.items_max;
   k_cull<<<(unsigned)((pairs_total + 255) / 256), 256, 0, st>>>(S, maps, rc, fm, r.items_max, err_flag);
-  int launches = 5;
+  int launches = 7;
   if (!rc.tessellate) {   // (inside the k_geometry event bracket: it is geometry time)
     k_tiles<<<(rc.n_envs + kTileWarps - 1) / kTileWarps, kTileWarps * 32, 0, st>>>(S, maps, rc, fm, r.max_prims, r.max_lat, err_flag);
     launches++;
@@ -2757,26 +2678,18 @@ int launch_render(const Renderer& r, const DState& S, const DMap* maps, const Re
     bin<<<bin_grid, bin_threads, bin_smem_bytes, st>>>(rc, fm, rt, r.max_prims, r.pool, err_flag);
   });
   mark();
-  const bool wrap = (rc.obs_layout | rc.obs_dtype) != 0;
-  const bool lean = lean_output(rc.obs_layout, rc.obs_dtype, rc.width);
-  // k_raster walks only the rows k_bin and k_raster_flat listed, unless the solo and flat bins were not drawn apart or a
-  // gathering step ships every row, the ones they drew included, from k_raster
-  const bool row_list = lean && gather.n == 0;
   const int aux_run = aux_set(aux);   // the rasterisers' instances for the images asked for (no target: the plain ones)
   for_each_of<kAuxSets>([&](auto aux_c) {
     for_each_of<kRemapModes>([&](auto remap_c) {
       constexpr int A = decltype(aux_c)::value, R = decltype(remap_c)::value;
       if (A != aux_run || R != remap) return;
-      if (lean) {   // (inside the k_raster event bracket: it is rasterisation time)
-        k_raster_solo<R, A><<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, rt, obs, r.max_prims, r.max_lat, aux);
-        // before k_raster, which draws the bins k_raster_flat hands back
-        k_raster_flat<R, A><<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, rt, obs, r.max_prims, r.max_lat,
-                                                                        err_flag, aux);
-        launches += 2;
-      }
-      const auto raster = wrap ? k_raster<true, R, A> : k_raster<false, R, A>;
-      raster<<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, rt, gather, row_list, obs, r.max_prims,
-                                                                    r.pool, r.max_lat, err_flag, aux);
+      // (all three inside the k_raster event bracket: it is rasterisation time)
+      k_raster_solo<R, A><<<r.sms * kSoloMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, rt, obs, r.max_prims, r.max_lat, aux);
+      // before k_raster, which draws the bins k_raster_flat hands back
+      k_raster_flat<R, A><<<r.sms * kFlatMinCtas, kThreads, 0, st>>>(S, maps, rc, fm, rt, obs, r.max_prims, r.max_lat,
+                                                                      err_flag, aux);
+      k_raster<R, A><<<r.sms * kRasterMinCtas, kThreads, kRasterSmem, st>>>(S, maps, rc, fm, rt, gather, obs, r.max_prims,
+                                                                            r.pool, r.max_lat, err_flag, aux);
     });
   });
   mark();
@@ -2798,8 +2711,7 @@ Renderer* renderer_create(const dts_config& cfg) {
   for_each_of<kAuxSets>([](auto aux_c) {
     for_each_of<kRemapModes>([&](auto remap_c) {
       constexpr int A = decltype(aux_c)::value, R = decltype(remap_c)::value;
-      for (const auto raster : {k_raster<false, R, A>, k_raster<true, R, A>})
-        cudaFuncSetAttribute(raster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
+      cudaFuncSetAttribute(k_raster<R, A>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRasterSmem);
     });
   });
   return r;

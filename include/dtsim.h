@@ -478,7 +478,11 @@ int dts_set_bev_visibility_target(dts_sim* sim, uint8_t* vis_dev, float* pix_dev
  * before the handle's first render (and after a map upload, until the next render). */
 int dts_get_frame_cameras(dts_sim* sim, double* V_dev, float* P_dev, void* stream);
 /* Select the fused wrapper behaviour for subsequent dts_step / dts_render calls (default: all zero, scale 1).
- * obs_dev then holds num_envs * 3 * H * W elements of uint8 or float32 in the chosen layout. */
+ * obs_dev then holds num_envs * 3 * H * W elements of uint8 or float32 in the chosen layout.  The renderer draws packed
+ * uint8 HWC; for any other layout or dtype without a resize (dts_set_resize) it draws into a library staging frame of
+ * num_envs * cam_height * cam_width * 3 bytes, and a format pass writes obs_dev.  A call that changes the layout or dtype
+ * synchronises the device first, as it may allocate or free that frame; a failed allocation returns an error and leaves
+ * the previous format in effect. */
 int dts_set_output_format(dts_sim* sim, const dts_output_format* fmt);
 /* ResizeWrapper (wrappers.py:111-141: cv2.resize(obs, (resize_w, resize_h), interpolation=cv2.INTER_CUBIC)) on the device:
  * subsequent dts_step / dts_render calls render at the camera size into a library buffer and write obs_dev as

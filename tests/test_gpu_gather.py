@@ -200,9 +200,9 @@ def test_packed_u8_odd_sizes_equal_obs_and_oracle(W, H, torch_cuda):
 @pytest.mark.parametrize("W,H", [(160, 120), (101, 75)])
 @pytest.mark.parametrize("layout,dtype", [("hwc", "float32"), ("chw", "uint8"), ("chw", "float32"), ("cwh", "uint8"),
                                           ("cwh", "float32")])
-def test_wrapper_formats_are_stored_per_bin(layout, dtype, W, H, torch_cuda):
-    """Every layout / dtype other than packed u8 HWC: the resolve stores each bin into the caller's tensor and into
-    every peer's slot (the planar u8 fast store is not used while a gather is armed)."""
+def test_wrapper_formats_are_written_by_the_format_pass(layout, dtype, W, H, torch_cuda):
+    """Every layout / dtype other than packed u8 HWC: the rasterisers draw packed u8 HWC into the staging frame, and
+    the format pass writes the caller's tensor and every peer's slot from it."""
     torch = torch_cuda
     env = make_env(40, "loop_obstacles", W, H)
     env.set_output_format(obs_layout=layout, obs_dtype=dtype)

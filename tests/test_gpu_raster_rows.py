@@ -1,11 +1,11 @@
-"""k_raster's two ways of picking its work: the rows k_bin and k_raster_flat put on its list, or every row of every env.
+"""k_raster's two row lists: the rows k_bin and k_raster_flat put on it, or on a gathering step every row.
 
-With packed u8 HWC output k_raster_solo clears the empty coarse bins (without a LUT) and draws the bins inside one prim,
+k_raster_solo clears the empty coarse bins (without a LUT, where W % 4 == 0) and draws the bins inside one prim,
 k_raster_flat the flat ones, so k_raster draws only the rows k_bin listed (a bin that neither took) and the rows of the
-bins k_raster_flat hands back.  On a gathering step k_raster walks every row instead, since it ships each finished row,
-the ones the others drew included, to every rank.  The same state drawn both ways must give the same bytes in obs and
-in every image: a row missing from the list would keep the previous contents there.  Each case draws once without a
-gather (the list) and once with FusedObsGather(env, 0, 1) armed (every row), over buffers filled with other bytes."""
+bins k_raster_flat hands back.  On a gathering step k_bin lists every row instead, since k_raster ships each finished
+row, the ones the others drew included, to every rank.  The same state drawn both ways must give the same bytes in obs
+and in every image: a row missing from the list would keep the previous contents there.  Each case draws once without a
+gather and once with FusedObsGather(env, 0, 1) armed, over buffers filled with other bytes."""
 import numpy as np
 import pytest
 
@@ -58,8 +58,7 @@ def images(env, torch):
 
 def assert_both_walks_agree(env, torch, render=None, gather=None):
     """Draws the env's current state twice through `render` (default: dts_render in the env's own mode, fisheye and
-    rectification included): from k_raster's row list, then on a gathering step, each over targets filled with other
-    bytes.  obs and every image must be equal byte for byte, and the gather's slot must be obs."""
+    rectification included): unarmed, then on a gathering step, each over targets filled with other bytes.  obs and every image must be equal byte for byte, and the gather's slot must be obs."""
     from gym_duckietown_b200.dist import FusedObsGather
     render = render or (lambda: env.sim.render(env.obs.data_ptr(), env._stream()))
     g = gather or FusedObsGather(env, 0, 1)
@@ -77,7 +76,7 @@ def assert_both_walks_agree(env, torch, render=None, gather=None):
     assert listed.keys() == full.keys()
     for k in listed:
         diff = int((listed[k] != full[k]).sum())
-        assert diff == 0, f"{k}: {diff} bytes differ between the row list and the walk over every row"
+        assert diff == 0, f"{k}: {diff} bytes differ between the row list and the list of every row"
     assert float(env.obs.float().std()) > 5, "not a rendered frame"
     return g
 
@@ -125,10 +124,11 @@ def test_cameras_at_the_horizon(torch_cuda):
     env.close()
 
 
-@pytest.mark.parametrize("W,H", [(100, 76), (96, 60)])
+@pytest.mark.parametrize("W,H", [(100, 76), (96, 60), (101, 75)])
 def test_border_bins(W, H, torch_cuda):
     """Cameras whose right column of coarse bins is narrower than 32 pixels and whose last row of bins is 4 rows high:
-    the empty bins there are cleared row by row up to the image's edge"""
+    the empty bins there are cleared row by row up to the image's edge.  101x75: rows that are not whole words, so the
+    lean rasterisers store bytes and k_raster clears the empty bins."""
     torch = torch_cuda
     env = make_env(256, "small_loop", W, H, depth=True, labels=True, markings=True)
     place(env, *random_poses(env, 256, 13))
@@ -179,7 +179,7 @@ def test_remapped_frames(lens, torch_cuda):
 
 def test_terminal_step_second_pass(torch_cuda):
     """dts_step_terminal with envs ending: its second pass draws the listed envs from their rows on the list.  What obs
-    holds after the step is the frame of every env's current state, which a gathering render draws over every row."""
+    holds after the step is the frame of every env's current state, which a gathering render draws from every row."""
     torch = torch_cuda
     n = 256
     env = make_env(n, "loop_obstacles", auto_reset=True, device_reset=True, terminal_obs=True, max_steps=6,
@@ -206,8 +206,8 @@ def test_terminal_step_second_pass(torch_cuda):
 
 
 def test_frame_memory_overflow_still_raises(monkeypatch, torch_cuda):
-    """A pair pool of one env's bound for 64 envs: the frames that did not fit are the clear colour everywhere whether
-    k_raster walks its list or every row, the overflow is flagged, env.check() raises, and the next render is refused."""
+    """A pair pool of one env's bound for 64 envs: the frames that did not fit are the clear colour everywhere, unarmed
+    and on a gathering step, the overflow is flagged, env.check() raises, and the next render is refused."""
     torch = torch_cuda
     from gym_duckietown_b200.dist import FusedObsGather
     from gym_duckietown_b200.lib import DtsError

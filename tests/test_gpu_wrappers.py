@@ -21,19 +21,32 @@ def make_env(name, n, **kw):
     return BatchedDuckietownEnv(n, name, **args)
 
 
-@pytest.mark.parametrize("size,distortion", [((160, 120), False), ((84, 84), False), ((100, 76), False), ((160, 120), True)])
+@pytest.mark.parametrize("size,distortion", [((160, 120), False), ((84, 84), False), ((100, 76), False), ((160, 120), True),
+                                           ((101, 75), False), ((160, 120), "camera_rand_pool"), ((160, 120), "rectified")])
 def test_observation_layouts_and_normalisation(size, distortion, torch_cuda):
-    """ImgWrapper transpose(2,0,1) LW:86, PyTorchObsWrapper transpose(2,1,0) W:110, NormalizeWrapper obs/255 LW:66-70."""
+    """ImgWrapper transpose(2,0,1) LW:86, PyTorchObsWrapper transpose(2,1,0) W:110, NormalizeWrapper obs/255 LW:66-70.
+    101x75: a width that is no multiple of 4; also a camera_rand pool of four fisheye tables and the rectification."""
     torch = torch_cuda
     W, H = size
-    env = make_env("udem1", 12, camera_width=W, camera_height=H, distortion=distortion, domain_rand=True)
+    kw = dict(distortion=bool(distortion))
+    if distortion == "camera_rand_pool":
+        kw.update(camera_rand=True, camera_rand_pool=4)
+    env = make_env("udem1", 12, camera_width=W, camera_height=H, domain_rand=True, **kw)
+    if distortion == "rectified":
+        from gym_duckietown_b200.distortion import rectify_maps
+        env.set_rectification(*rectify_maps(W, H))
+        env.undistort = True
+
+    def render():   # in the env's own render mode (under undistort render_obs() would draw the pinhole frame)
+        env.sim.render(env.obs.data_ptr(), env._stream())
+        return env.obs.cpu().numpy()
     env.reset(render=False)
-    base = env.render_obs().cpu().numpy().copy()          # u8 [N,H,W,3]
+    base = render().copy()                                # u8 [N,H,W,3]
     assert base.std() > 10
     for layout, perm in (("hwc", (0, 1, 2)), ("chw", (2, 0, 1)), ("cwh", (2, 1, 0))):
         for dtype in ("uint8", "float32"):
             env.set_output_format(obs_layout=layout, obs_dtype=dtype)
-            got = env.render_obs().cpu().numpy()
+            got = render()
             want = np.stack([f.transpose(perm) for f in base])
             if dtype == "float32":
                 ref64 = want / 255.0                         # what NormalizeWrapper computes (float64)
@@ -45,7 +58,7 @@ def test_observation_layouts_and_normalisation(size, distortion, torch_cuda):
     acts = torch.zeros(12, 2, device=env.device)
     obs, *_ = env.step(acts)
     env.set_output_format(obs_layout="hwc", obs_dtype="uint8")
-    plain = env.render_obs().cpu().numpy()
+    plain = render()
     assert np.array_equal(obs.cpu().numpy(), (plain.transpose(0, 3, 1, 2) / 255.0).astype(np.float32))
     env.close()
 
