@@ -5,7 +5,7 @@ observation buffers are caller-visible torch CUDA tensors, the work runs on
 `torch.cuda.current_stream()` inside libdtsim.so, nothing synchronises.  Constructor keywords are the
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
 `auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `flow`, `flow_occlusion`,
-`camera_rand_pool` and the `bev*` keywords (`bev_visibility` among them).
+`camera_rand_pool`, the `bev*` keywords (`bev_visibility` among them) and the `scan*` keywords.
 
 `camera_rand=True` (with `distortion=True`; without it the flag does nothing, as in the reference, S:352-358) gives the
 envs a spread of lenses: `camera_rand_pool` calibrations K, D are drawn once, at construction, within the reference's
@@ -55,6 +55,19 @@ MARKING_NAMES class of the texel under it, 0 off the tiles, objects or not.  Eve
 `render=False` too (under `auto_reset`, an ended env's row is its next episode's first state, as in `obs`), and so
 does every render; `render_bev()` writes them alone, e.g. after `reset(render=False)`, `load_state` or `copy_envs`.
 They do not depend on the camera, the render modes, sizes or formats, and snapshots and gathers do not carry them.
+
+`scan=True` allocates `env.scan_range`, float32, and `env.scan_hit`, int16, both [num_envs, scan_rays]: a range scan
+around each agent (dts_set_scan_target), cast on the map rather than rendered.  Ray k leaves at fov * (0.5 - (k + 0.5)
+/ scan_rays) to the left of the heading, for `scan_fov` radians (2 pi by default: the full circle), so ray 0 is the
+leftmost and one ray points straight ahead; the rays start `scan_origin=(forward, right)` metres from the agent's
+position.  `scan_range` holds how far each ray runs before it meets an object's footprint (hidden optional objects
+skipped, moving obstacles where they are now) or ground the reference does not drive on (an empty cell, a tile that is
+not drivable, off the map), up to `scan_range` metres (2.0 by default); 0 when the origin itself is blocked.  `scan_hit`
+names what stopped it in the label image's numbering (`label_table`): the object, the tile that is not drivable, 1
+for an empty cell or off the map, 0 for nothing within range.  Every `step` writes them, with `render=False` too
+(under `auto_reset`, an ended env's row is its next episode's first state), and so does every render;
+`render_scan()` writes them alone.  They do not depend on the camera, the render modes, sizes or formats, and
+snapshots and gathers do not carry them.
 
 `flow=True` allocates `env.flow`, float32 [num_envs, camera_height, camera_width, 2], filled by the same renders: the
 backward motion flow (dts_set_flow_target) — for each pixel, (dx, dy) in pixels, x right and y down, from where the
@@ -136,7 +149,8 @@ class BatchedDuckietownEnv:
                  randomize_maps_on_reset: bool = False, randomization_config=None, terminal_obs: bool = False,
                  depth: bool = False, labels: bool = False, camera_rand_pool: int = 16, markings: bool = False,
                  bev: bool = False, bev_shape=(64, 64), bev_cell: float = 0.03, bev_origin=None, flow: bool = False,
-                 flow_occlusion: bool = False, bev_visibility: bool = False):
+                 flow_occlusion: bool = False, bev_visibility: bool = False, scan: bool = False, scan_rays: int = 64,
+                 scan_fov: float = 2 * np.pi, scan_range: float = 2.0, scan_origin=(0.0, 0.0)):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
         camera_rand = bool(camera_rand and distortion)   # S:353-356: camera_rand only with distortion
@@ -226,6 +240,11 @@ class BatchedDuckietownEnv:
                 (num_envs, bh, bw), dtype=torch.uint8, device=self.device) if bev_visibility else None
             self.bev_pixels: Optional[torch.Tensor] = torch.zeros(
                 (num_envs, bh, bw, 2), dtype=torch.float32, device=self.device) if bev_visibility else None
+            # the range scans (scan=True); every step and render writes them on the device
+            self.scan_range: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, int(scan_rays)), dtype=torch.float32, device=self.device) if scan else None
+            self.scan_hit: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, int(scan_rays)), dtype=torch.int16, device=self.device) if scan else None
             self.reward = torch.zeros(num_envs, dtype=torch.float32, device=self.device)
             self._done_u8 = torch.zeros(num_envs, dtype=torch.uint8, device=self.device)
             self.state: Dict[str, torch.Tensor] = {
@@ -253,6 +272,10 @@ class BatchedDuckietownEnv:
             ox, oy = (bw / 2, 3 * bh / 4) if bev_origin is None else (float(v) for v in bev_origin)
             self.bev_config = L.BevConfig(bw, bh, float(bev_cell), float(ox), float(oy))
             self.sim.set_bev_target(self.bev_config, self.bev_labels.data_ptr(), self.bev_markings.data_ptr())
+        if scan:
+            fwd_off, right_off = (float(v) for v in scan_origin)
+            self.scan_config = L.ScanConfig(int(scan_rays), float(scan_fov), float(scan_range), fwd_off, right_off)
+            self.sim.set_scan_target(self.scan_config, self.scan_range.data_ptr(), self.scan_hit.data_ptr())
         # the forward maps of the fisheye tables, in the pool's order
         models = self.camera_models if camera_rand else [self.camera_model] if distortion else None
         fwd = (np.stack([m.mapx for m in models]), np.stack([m.mapy for m in models])) if models else ()
@@ -462,6 +485,13 @@ class BatchedDuckietownEnv:
             raise ValueError("render_bev needs bev=True")
         self.sim.render_bev(self._stream())
         return self.bev_labels, self.bev_markings
+
+    def render_scan(self):
+        """Write `scan_range` / `scan_hit` for the current state (dts_render_scan), without rendering a frame."""
+        if self.scan_range is None:
+            raise ValueError("render_scan needs scan=True")
+        self.sim.render_scan(self._stream())
+        return self.scan_range, self.scan_hit
 
     # labels -------------------------------------------------------------------------------------
     def label_table(self, map_id: int = 0) -> list:

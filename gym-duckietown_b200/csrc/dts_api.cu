@@ -45,6 +45,7 @@ struct dts_sim {
   int render_mode = 0;                  // dts_set_render_mode             // the next dts_render also stores into the gather buffers
   AuxTargets aux{};                     // dts_set_{depth,label,marking}_target: caller-owned images, or null
   BevTarget bev{};                      // dts_set_bev_target: caller-owned grids, both null = off
+  ScanTarget scan{};                    // dts_set_scan_target: caller-owned range and hit, both null = off
   FlowTarget flow{};                    // dts_set_flow_target: caller-owned image and the record it owns, null = off
   OcclusionTarget occ{};                // dts_set_occlusion_target: caller-owned mask and the slots it owns, null = off
   BevViewTarget bev_view{};             // dts_set_bev_visibility_target: caller-owned outputs, both null = off
@@ -207,7 +208,7 @@ static int largest_n_dyn(dts_sim* sim) {
 
 int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
   if (!sim) return 1;
-  if ((sim->aux.labels || sim->bev.labels) && b && largest_label((long long)b->grid_w * b->grid_h, b->n_objects) > INT16_MAX)
+  if ((sim->aux.labels || sim->bev.labels || sim->scan.hit) && b && largest_label((long long)b->grid_w * b->grid_h, b->n_objects) > INT16_MAX)
     return sim->fail("a label target is set and this map's largest label, %lld, does not fit in int16",
                      largest_label((long long)b->grid_w * b->grid_h, b->n_objects));
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
@@ -426,6 +427,25 @@ static int bev_pass(dts_sim* sim, void* stream) {
   return 0;
 }
 
+// The range scan of every env's current state, where a target is set (dts_set_scan_target)
+static int scan_pass(dts_sim* sim, void* stream) {
+  if (!sim->scan.range && !sim->scan.hit) return 0;
+  if (check_maps(sim)) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  int max_objects = 0;
+  for (const MapCounts& c : maps_counts(*sim->maps)) max_objects = c.n_objects > max_objects ? c.n_objects : max_objects;
+  launch_scan(state_arrays(*sim->state), maps_table(*sim->maps), sim->scan, max_objects, (cudaStream_t)stream);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// The outputs sampled from the map rather than rendered, in their order: the bird's-eye grids, then the range scan
+static int map_pass(dts_sim* sim, void* stream) {
+  if (bev_pass(sim, stream)) return 1;
+  return scan_pass(sim, stream);
+}
+
 // The camera visibility of the grids bev_pass wrote, where a target is set (dts_set_bev_visibility_target): launched
 // last in the call, against the frame the call drew (its camera, labels and remap), or with none every cell UNKNOWN
 static int bev_view_pass(dts_sim* sim, void* stream, bool drew_frame) {
@@ -441,7 +461,7 @@ static int bev_view_pass(dts_sim* sim, void* stream, bool drew_frame) {
 int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
   if (!sim) return 1;
   if (render_pass(sim, obs_dev, stream, nullptr, nullptr)) return 1;
-  if (bev_pass(sim, stream)) return 1;
+  if (map_pass(sim, stream)) return 1;
   return bev_view_pass(sim, stream, true);
 }
 
@@ -450,6 +470,12 @@ int dts_render_bev(dts_sim* sim, void* stream) {
   if (!sim->bev.labels && !sim->bev.marks) return sim->fail("no bird's-eye target is set (dts_set_bev_target)");
   if (bev_pass(sim, stream)) return 1;
   return bev_view_pass(sim, stream, false);
+}
+
+int dts_render_scan(dts_sim* sim, void* stream) {
+  if (!sim) return 1;
+  if (!sim->scan.range && !sim->scan.hit) return sim->fail("no range scan target is set (dts_set_scan_target)");
+  return scan_pass(sim, stream);
 }
 
 // With a flow target: every env's camera and obstacles before the step, the previous frame of the next render's flow
@@ -489,8 +515,9 @@ int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, voi
                        sim->n_ended, st);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
-  // the grids of the state obs_dev will show: the ended envs' first states (every env's row, as the others did not move)
-  if (bev_pass(sim, stream)) return 1;
+  // the grids and scans of the state obs_dev will show: the ended envs' first states (every env's row, as the others did
+  // not move)
+  if (map_pass(sim, stream)) return 1;
   if (!obs_dev) return bev_view_pass(sim, stream, false);
   // 4. their terminal frames -> terminal_obs_dev; 5. their first frames -> obs_dev
   const ResizeTarget rz = resizer_target(*sim->resize);
@@ -516,7 +543,7 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
                     (cudaStream_t)stream);
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
-  if (bev_pass(sim, stream)) return 1;
+  if (map_pass(sim, stream)) return 1;
   if (obs_dev && render_pass(sim, obs_dev, stream, nullptr, nullptr)) return 1;
   return bev_view_pass(sim, stream, obs_dev != nullptr);
 }
@@ -712,6 +739,25 @@ int dts_set_bev_target(dts_sim* sim, const dts_bev_config* cfg, int16_t* labels_
   if (reinterpret_cast<uintptr_t>(labels_dev) & 1) return sim->fail("bird's-eye label target is not aligned to 2 bytes");
   if (labels_dev && check_labels_fit(sim)) return 1;
   sim->bev = BevTarget{*cfg, labels_dev, markings_dev};
+  return 0;
+}
+
+int dts_set_scan_target(dts_sim* sim, const dts_scan_config* cfg, float* range_dev, int16_t* hit_dev) {
+  if (!sim) return 1;
+  if (!cfg || (!range_dev && !hit_dev)) {
+    sim->scan = ScanTarget{};
+    return 0;
+  }
+  if (cfg->n_rays < 1 || cfg->n_rays > 4096) return sim->fail("range scan of %d rays: 1 to 4096 are accepted", cfg->n_rays);
+  if (!(cfg->fov > 0 && cfg->fov <= 2 * M_PI)) return sim->fail("range scan field of view %g: (0, 2 pi] is accepted", cfg->fov);
+  if (!std::isfinite(cfg->max_range) || !(cfg->max_range > 0))
+    return sim->fail("range scan max_range %g: a finite range > 0 is needed", cfg->max_range);
+  if (!std::isfinite(cfg->origin_forward) || !std::isfinite(cfg->origin_right))
+    return sim->fail("range scan origin (%g, %g) is not finite", cfg->origin_forward, cfg->origin_right);
+  if (reinterpret_cast<uintptr_t>(range_dev) & 3) return sim->fail("range scan range target is not aligned to 4 bytes");
+  if (reinterpret_cast<uintptr_t>(hit_dev) & 1) return sim->fail("range scan hit target is not aligned to 2 bytes");
+  if (hit_dev && check_labels_fit(sim)) return 1;
+  sim->scan = ScanTarget{*cfg, range_dev, hit_dev};
   return 0;
 }
 

@@ -2,9 +2,11 @@
 // agent, each point-sampled from the map's own tables at its centre — the tile under it, the class of the texel under it
 // and the first object whose footprint holds it.  No rasteriser: a thread per cell, float64 in the order the spec states
 // (-fmad=false keeps every product and sum separately rounded, as numpy's are).  k_bev_view then says, cell by cell,
-// whether the frame the call drew shows the grid (dts_set_bev_visibility_target, item 15).
+// whether the frame the call drew shows the grid (dts_set_bev_visibility_target, item 15).  k_scan casts the range scan
+// (dts_set_scan_target, item 16) from the same footprints and the reference's drivability rule.
 #include "dts_camera.cuh"
 #include "dts_kernels.h"
+#include "dts_logic.cuh"
 
 namespace dts {
 namespace {
@@ -60,6 +62,49 @@ __device__ __forceinline__ bool box_meets(const double box[4], double wx, double
   return box[0] <= wx + m && box[1] >= wx - m && box[2] <= wz + m && box[3] >= wz - m;
 }
 
+// Called by one whole warp: the footprints of env `env`'s objects that are not hidden this episode and whose box meets
+// the disc (wx, wz, wr), in index order, into foot / foot_box / foot_obj, which have room for every object of the map.
+// Returns how many, on every lane.
+__device__ __forceinline__ int gather_footprints(const DState& S, const DMap& m, int env, int lane, double wx, double wz,
+                                                 double wr, BevFootprint* foot, double (*foot_box)[4], int16_t* foot_obj) {
+  int count = 0;
+  const uint32_t* hidden = S.rep[env].hidden;
+  const size_t nd = m.n_dyn, ne = S.n;
+  for (int base = 0; base < m.n_objects; base += 32) {
+    const int o = base + lane;
+    BevFootprint q;
+    double box[4];
+    bool keep = false;
+    if (o < m.n_objects && !(hidden[o >> 5] >> (o & 31) & 1u)) {
+      const int slot = m.objects[o].dyn_slot;
+      if (slot >= 0) {   // this env's copy of the obstacle's corners
+        for (int k = 0; k < 4; k++) {
+          q.x[k] = m.dyn_state[((size_t)(DTS_DYN_CORNERS + 2 * k) * nd + slot) * ne + env];
+          q.z[k] = m.dyn_state[((size_t)(DTS_DYN_CORNERS + 2 * k + 1) * nd + slot) * ne + env];
+        }
+        keep = true;
+      } else if (m.obj_corners) {
+        for (int k = 0; k < 4; k++) {
+          q.x[k] = __ldg(m.obj_corners + (size_t)o * 8 + 2 * k);
+          q.z[k] = __ldg(m.obj_corners + (size_t)o * 8 + 2 * k + 1);
+        }
+        keep = true;
+      }
+      if (keep) footprint_box(q, box);
+      keep = keep && box_meets(box, wx, wz, wr);
+    }
+    const unsigned ball = __ballot_sync(0xffffffffu, keep);
+    if (keep) {
+      const int at = count + __popc(ball & ((1u << lane) - 1u));
+      foot[at] = q;
+      for (int k = 0; k < 4; k++) foot_box[at][k] = box[k];
+      foot_obj[at] = (int16_t)o;
+    }
+    count += __popc(ball);
+  }
+  return count;
+}
+
 // grid (env, chunk of kBevCellsPerCta cells), one thread per cell of the chunk at a time, rows stored contiguously
 __global__ void __launch_bounds__(kBevThreads) k_bev(DState S, const DMap* __restrict__ maps, BevTarget b) {
   __shared__ BevFootprint foot[DTS_MAX_OBJECTS];   // the objects whose footprint can meet the window, in index order
@@ -82,40 +127,7 @@ __global__ void __launch_bounds__(kBevThreads) k_bev(DState S, const DMap* __res
       const double fc = (g.origin_y - 0.5 * g.height) * g.cell, lc = (0.5 * g.width - g.origin_x) * g.cell;
       const double wx = px + fc * ca + lc * sa, wz = pz - fc * sa + lc * ca;
       const double wr = 0.5 * g.cell * sqrt((double)g.width * g.width + (double)g.height * g.height);
-      const uint32_t* hidden = S.rep[env].hidden;
-      const size_t nd = m.n_dyn, ne = S.n;
-      for (int base = 0; base < m.n_objects; base += 32) {
-        const int o = base + lane;
-        BevFootprint q;
-        double box[4];
-        bool keep = false;
-        if (o < m.n_objects && !(hidden[o >> 5] >> (o & 31) & 1u)) {
-          const int slot = m.objects[o].dyn_slot;
-          if (slot >= 0) {   // this env's copy of the obstacle's corners
-            for (int k = 0; k < 4; k++) {
-              q.x[k] = m.dyn_state[((size_t)(DTS_DYN_CORNERS + 2 * k) * nd + slot) * ne + env];
-              q.z[k] = m.dyn_state[((size_t)(DTS_DYN_CORNERS + 2 * k + 1) * nd + slot) * ne + env];
-            }
-            keep = true;
-          } else if (m.obj_corners) {
-            for (int k = 0; k < 4; k++) {
-              q.x[k] = __ldg(m.obj_corners + (size_t)o * 8 + 2 * k);
-              q.z[k] = __ldg(m.obj_corners + (size_t)o * 8 + 2 * k + 1);
-            }
-            keep = true;
-          }
-          if (keep) footprint_box(q, box);
-          keep = keep && box_meets(box, wx, wz, wr);
-        }
-        const unsigned ball = __ballot_sync(0xffffffffu, keep);
-        if (keep) {
-          const int at = count + __popc(ball & ((1u << lane) - 1u));
-          foot[at] = q;
-          for (int k = 0; k < 4; k++) foot_box[at][k] = box[k];
-          foot_obj[at] = (int16_t)o;
-        }
-        count += __popc(ball);
-      }
+      count = gather_footprints(S, m, env, lane, wx, wz, wr, foot, foot_box, foot_obj);
     }
     if (lane == 0) n_foot = count;
   }
@@ -162,6 +174,109 @@ __global__ void __launch_bounds__(kBevThreads) k_bev(DState S, const DMap* __res
     }
     if (b.marks) b.marks[row + t] = (uint8_t)mark;
   }
+}
+
+constexpr int kScanThreads = 256;          // the most threads of a CTA, and the most rays of one env it casts
+constexpr int kScanMaxEnvs = 32;           // the most envs of a CTA
+constexpr int kScanSmem = 40 * 1024;       // the most bytes of gathered footprints a CTA holds
+
+// The shared memory of one env's gathered footprints, in doubles: foot[cap], foot_box[cap][4], foot_obj[cap]
+__host__ __device__ __forceinline__ int scan_slot_doubles(int cap) { return cap * 12 + (cap + 3) / 4; }
+
+// Where ray (ox, oz) + t (dx, dz), t >= 0, enters the strictly convex footprint q (its four edge half-planes, Cyrus-Beck,
+// the side taken from the corners' orientation): max(t_in, 0) where t_in <= t_out and t_out >= 0, else INFINITY.
+__device__ __forceinline__ double footprint_entry(const BevFootprint& q, double ox, double oz, double dx, double dz) {
+  const double side = edge_cross(q.x[0], q.z[0], q.x[1], q.z[1], q.x[2], q.z[2]) > 0.0 ? 1.0 : -1.0;
+  double t0 = -INFINITY, t1 = INFINITY;
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    const int n = (k + 1) & 3;
+    const double num = side * edge_cross(q.x[k], q.z[k], q.x[n], q.z[n], ox, oz);   // inside: num + t den >= 0
+    const double den = side * ((q.x[n] - q.x[k]) * dz - (q.z[n] - q.z[k]) * dx);
+    if (den > 0.0) t0 = fmax(t0, -num / den);
+    else if (den < 0.0) t1 = fmin(t1, -num / den);
+    else if (num < 0.0) t1 = -INFINITY;   // parallel to the edge, outside it
+  }
+  return t0 <= t1 && t1 >= 0.0 ? fmax(t0, 0.0) : INFINITY;
+}
+
+// grid (CTAs of `envs` consecutive envs, chunks of kScanThreads rays): thread (slot, k) casts ray k of env
+// blockIdx.x * envs + slot, its rays stored contiguously.  A warp gathers each env's footprints within max_range of
+// the origin once, into `cap` entries of dynamic shared memory per env (cap: the most objects of an uploaded map).
+__global__ void __launch_bounds__(kScanThreads) k_scan(DState S, const DMap* __restrict__ maps, ScanTarget sc, int cap,
+                                                       int envs) {
+  extern __shared__ double scan_mem[];
+  __shared__ double origin[kScanMaxEnvs][2];
+  __shared__ int n_foot[kScanMaxEnvs];
+  const dts_scan_config g = sc.cfg;
+  const int R = g.n_rays, per = R < kScanThreads ? R : kScanThreads;
+  const int stride = scan_slot_doubles(cap);
+  const int lane = threadIdx.x & 31;
+  for (int s = threadIdx.x >> 5; s < envs; s += blockDim.x >> 5) {
+    const int env = blockIdx.x * envs + s;
+    if (env >= S.n) break;
+    const DMap& m = maps[S.map_id[env]];
+    double sa, ca;
+    sincos(S.angle[env], &sa, &ca);
+    const double f = g.origin_forward, r = g.origin_right;
+    const double ox = S.pos_x[env] + f * ca + r * sa, oz = S.pos_z[env] - f * sa + r * ca;
+    double* slot = scan_mem + (size_t)s * stride;
+    const int count = gather_footprints(S, m, env, lane, ox, oz, g.max_range, reinterpret_cast<BevFootprint*>(slot),
+                                        reinterpret_cast<double(*)[4]>(slot + cap * 8),
+                                        reinterpret_cast<int16_t*>(slot + cap * 12));
+    if (lane == 0) { origin[s][0] = ox; origin[s][1] = oz; n_foot[s] = count; }
+  }
+  __syncthreads();
+  const int s = threadIdx.x / per, k = blockIdx.y * per + (threadIdx.x - s * per);
+  const int env = blockIdx.x * envs + s;
+  if (s >= envs || env >= S.n || k >= R) return;
+  const DMap& m = maps[S.map_id[env]];
+  const double* slot = scan_mem + (size_t)s * stride;
+  const BevFootprint* foot = reinterpret_cast<const BevFootprint*>(slot);
+  const double(*foot_box)[4] = reinterpret_cast<const double(*)[4]>(slot + cap * 8);
+  const int16_t* foot_obj = reinterpret_cast<const int16_t*>(slot + cap * 12);
+  const double ox = origin[s][0], oz = origin[s][1];
+  double sd, cd;
+  sincos(S.angle[env] + g.fov * (0.5 - (k + 0.5) / R), &sd, &cd);
+  const double dx = cd, dz = -sd;   // get_dir_vec
+  // objects: the first footprint entered, the smallest index among equals
+  double t_obj = INFINITY;
+  int hit = 0;
+  for (int q = 0, n = n_foot[s]; q < n; q++) {
+    if (foot_box[q][0] == -INFINITY) continue;   // not strictly convex: stops no ray
+    const double t = footprint_entry(foot[q], ox, oz, dx, dz);
+    if (t < t_obj) { t_obj = t; hit = 2 + m.n_tiles + foot_obj[q]; }
+  }
+  // tiles: the cells the ray crosses, from the origin's, up to the first that is not drivable (_drivable_pos S:1411);
+  // it leaves the grid within grid_w + grid_h steps, and off the grid nothing is drivable
+  const double ts = m.tile_size, limit = fmin(t_obj, g.max_range);
+  double fi = floor(ox / ts), fj = floor(oz / ts), t_tile = INFINITY;
+  if (!drivable_at(m, ox, oz)) {
+    t_tile = 0.0;
+  } else {
+    int i = (int)fi, j = (int)fj;
+    const int si = dx > 0.0 ? 1 : -1, sj = dz > 0.0 ? 1 : -1;
+    for (int step = 0; step < m.grid_w + m.grid_h + 2; step++) {
+      const double tx = dx != 0.0 ? ((i + (si > 0)) * ts - ox) / dx : INFINITY;
+      const double tz = dz != 0.0 ? ((j + (sj > 0)) * ts - oz) / dz : INFINITY;
+      const double t = fmax(fmin(tx, tz), 0.0);
+      if (t > limit) break;
+      if (tx <= tz) i += si;
+      if (tz <= tx) j += sj;
+      if (!drivable_at(m, (i + 0.5) * ts, (j + 0.5) * ts)) { t_tile = t; fi = i; fj = j; break; }
+    }
+  }
+  double t = t_obj;
+  if (t_tile < t_obj) {   // an object wins a tie
+    t = t_tile;
+    const bool road = fi >= 0.0 && fi < m.grid_w && fj >= 0.0 && fj < m.grid_h &&
+                      __ldg(m.tile_kind + (int)fj * m.grid_w + (int)fi) >= 0;
+    hit = road ? 2 + (int)fi * m.grid_h + (int)fj : 1;
+  }
+  if (!(t <= g.max_range)) { t = g.max_range; hit = 0; }
+  const size_t at = (size_t)env * R + k;
+  if (sc.range) sc.range[at] = (float)t;
+  if (sc.hit) sc.hit[at] = (int16_t)hit;
 }
 
 constexpr int kViewThreads = 256;
@@ -268,6 +383,19 @@ void launch_bev(const DState& S, const DMap* maps, const BevTarget& b, cudaStrea
   const int n_cells = b.cfg.width * b.cfg.height;
   const dim3 grid(S.n, (n_cells + kBevCellsPerCta - 1) / kBevCellsPerCta);
   k_bev<<<grid, kBevThreads, 0, st>>>(S, maps, b);
+}
+
+void launch_scan(const DState& S, const DMap* maps, const ScanTarget& sc, int max_objects, cudaStream_t st) {
+  const int R = sc.cfg.n_rays, per = R < kScanThreads ? R : kScanThreads;
+  const int cap = max_objects > 1 ? max_objects : 1;
+  const size_t slot_bytes = sizeof(double) * scan_slot_doubles(cap);
+  const int fit = (int)(kScanSmem / slot_bytes);   // >= 1: DTS_MAX_OBJECTS footprints take 25,088 B
+  int envs = kScanThreads / per;
+  if (envs > kScanMaxEnvs) envs = kScanMaxEnvs;
+  if (envs > fit) envs = fit;
+  const int threads = (envs * per + 31) / 32 * 32;
+  const dim3 grid((S.n + envs - 1) / envs, (R + per - 1) / per);
+  k_scan<<<grid, threads, envs * slot_bytes, st>>>(S, maps, sc, cap, envs);
 }
 
 void launch_bev_view(const DState& S, const DMap* maps, const BevTarget& b, const BevViewTarget& v, const FrameCtx* ctx,

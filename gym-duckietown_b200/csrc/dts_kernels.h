@@ -209,6 +209,15 @@ struct BevViewTarget {
   uint8_t* vis;
   float2* pix;
 };
+// The range scan of dts_set_scan_target (DESIGN.md section 5 item 16): float32 range and int16 hit, each
+// [n_envs][n_rays] or null
+struct ScanTarget {
+  dts_scan_config cfg;
+  float* range;
+  int16_t* hit;
+};
+// every env's scan of its current state, one launch; max_objects: the most objects of an uploaded map
+void launch_scan(const DState& S, const DMap* maps, const ScanTarget& sc, int max_objects, cudaStream_t st);
 // every env's cameras V [n_envs][12] and P [n_envs][4] from `ctx` (dts_get_frame_cameras), one launch
 void launch_frame_cameras(const FrameCtx* ctx, int n_envs, double* V, float* P, cudaStream_t st);
 

@@ -129,6 +129,13 @@ class BevConfig(C.Structure):
                 ("origin_y", C.c_double)]
 
 
+class ScanConfig(C.Structure):
+    """dts_scan_config: the range scan (rays, field of view in radians, range in metres, the origin's offset ahead of and
+    to the right of the agent in metres)"""
+    _fields_ = [("n_rays", C.c_int32), ("fov", C.c_double), ("max_range", C.c_double), ("origin_forward", C.c_double),
+                ("origin_right", C.c_double)]
+
+
 # dts_episode_params, in its order: (member, dtype, values per env)
 _EP_FIELDS = [("map_id", np.int32, 1), ("pos_x", np.float64, 1), ("pos_z", np.float64, 1), ("angle", np.float64, 1),
               ("wheel_dist", np.float64, 1), ("trim", np.float64, 1), ("cam_height", np.float32, 1),
@@ -200,6 +207,8 @@ def load() -> C.CDLL:
     lib.dts_set_marking_target.argtypes = [vp, vp]
     lib.dts_set_bev_target.argtypes = [vp, C.POINTER(BevConfig), vp, vp]
     lib.dts_render_bev.argtypes = [vp, vp]
+    lib.dts_set_scan_target.argtypes = [vp, C.POINTER(ScanConfig), vp, vp]
+    lib.dts_render_scan.argtypes = [vp, vp]
     lib.dts_set_flow_target.argtypes = [vp, vp, vp, vp, i]
     lib.dts_set_occlusion_target.argtypes = [vp, vp]
     lib.dts_set_bev_visibility_target.argtypes = [vp, vp, vp, vp, vp, i]
@@ -238,7 +247,7 @@ def load() -> C.CDLL:
 
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_fisheye_luts", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
-           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_set_flow_target", "dts_set_occlusion_target", "dts_set_bev_visibility_target", "dts_get_frame_cameras", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
+           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_set_scan_target", "dts_render_scan", "dts_set_flow_target", "dts_set_occlusion_target", "dts_set_bev_visibility_target", "dts_get_frame_cameras", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
            "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
 
@@ -524,6 +533,16 @@ class Sim:
     def render_bev(self, stream: int = 0):
         """The bird's-eye grids of the current state (dts_render_bev)."""
         self._check(self.lib.dts_render_bev(self.h, stream), "dts_render_bev")
+
+    def set_scan_target(self, cfg: Optional[ScanConfig], range_ptr: Optional[int], hit_ptr: Optional[int]):
+        """Write the range scan of cfg (float32 range / int16 hit [num_envs][cfg.n_rays], at caller-kept device
+        pointers) on every later step and render; None for both, or cfg None, turns it off (dts_set_scan_target)."""
+        self._check(self.lib.dts_set_scan_target(self.h, None if cfg is None else C.byref(cfg), range_ptr, hit_ptr),
+                    "dts_set_scan_target")
+
+    def render_scan(self, stream: int = 0):
+        """The range scan of the current state (dts_render_scan)."""
+        self._check(self.lib.dts_render_scan(self.h, stream), "dts_render_scan")
 
     def _forward_maps(self, fwd_x, fwd_y):
         """(fwd_x, fwd_y, n_tables) as dts_set_flow_target and dts_set_bev_visibility_target take them"""

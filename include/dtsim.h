@@ -292,7 +292,8 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
  * (the respawn, state and draws bit for bit those of dts_step, and a device list of the ended envs), k_copy_rows (their
  * rows -> terminal_obs_dev) and a second render into obs_dev over the listed envs only, whose kernels exit at once when
  * nothing ended.  Launches: 2 R + 3, R being dts_render's (5, or 7 when the rasteriser writes packed u8 HWC of a width divisible by 4, +1
- * with a resize), plus a 4-byte memset; obs_dev = NULL (no render): 2; one more with a bird's-eye target (dts_set_bev_target).  Fails without DTS_FLAG_AUTO_RESET, with
+ * with a resize), plus a 4-byte memset; obs_dev = NULL (no render): 2; one more with a bird's-eye target (dts_set_bev_target),
+ * and one more with a range scan target (dts_set_scan_target).  Fails without DTS_FLAG_AUTO_RESET, with
  * terminal_obs_dev == obs_dev, and while a fused gather is armed (dts_gather_next), which it does not write.  The
  * second pass is not timed by dts_profile_*.  Never synchronises. */
 int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, void* terminal_obs_dev, float* reward_dev,
@@ -387,6 +388,40 @@ int dts_set_bev_target(dts_sim* sim, const dts_bev_config* cfg, int16_t* labels_
 /* The bird's-eye targets of the current state (after dts_reset without a render, dts_load_state, ...): one launch,
  * stream-ordered.  Fails while no target is set. */
 int dts_render_bev(dts_sim* sim, void* stream);
+/* Range scan around every agent (DESIGN.md section 5, item 16): n_rays rays on the ground plane, each cast from one
+ * origin until an object or undrivable ground stops it.  In float64, with px, pz, a the env's pos_x, pos_z, angle and
+ * ca, sa = cos a, sin a: the origin is ox = px + f ca + r sa, oz = pz - f sa + r ca (f, r = origin_forward,
+ * origin_right: dts_bev_config's formulas); ray k (0 <= k < n_rays) leaves at phi_k = fov (0.5 - (k + 0.5) / n_rays) to
+ * the left of the heading, along get_dir_vec(a + phi_k) = (cos(a + phi_k), -sin(a + phi_k)), so ray 0 is the leftmost
+ * and one ray points straight ahead; fov = 2 pi covers the circle with no ray twice.  A point p blocks a ray when (a) its
+ * bird's-eye label (dts_set_bev_target) is an object: a footprint of an object not hidden this episode holds it, which
+ * is what the camera sees (traffic lights included), not the reference's collision set; or (b) _drivable_pos(p)
+ * (S:1411-1428) is false: off the grid, an empty cell or a tile that is not drivable.  A footprint that is not strictly
+ * convex (its four corners do not turn one way) stops no ray; no shipped map has one.
+ * range_dev float32 [num_envs][n_rays]: t* = inf { t >= 0 : origin + t dir blocked }, max_range when no point within
+ * max_range is blocked, 0 when the origin is.  hit_dev int16 [num_envs][n_rays], in dts_set_label_target's numbering:
+ * 2 + n_cells + o for the smallest object index o whose footprint the ray enters at t* (an object wins over a cell
+ * boundary at the same t); else 2 + i * grid_h + j for the tile at (i, j) that is not drivable and that the ray enters;
+ * else 1 (an empty cell or off the grid); 0 when nothing is met within max_range; when the origin is blocked, the
+ * origin's own bird's-eye label.
+ * Written once per dts_step and dts_step_terminal (after the respawn: a row shows the state the returned obs row shows,
+ * whether or not obs_dev is NULL), once per dts_render and by dts_render_scan; not by a call refused before it launches.
+ * Independent of the render mode, fisheye, rectification, resize, output format and every other target. */
+typedef struct {
+  int32_t n_rays;           /* 1 to 4096 */
+  double fov;               /* radians, in (0, 2 pi] */
+  double max_range;         /* metres, finite and > 0 */
+  double origin_forward, origin_right;   /* metres, finite */
+} dts_scan_config;
+/* Sets the range scan targets range_dev (4-byte aligned) and hit_dev (2-byte aligned), either of them NULL.  Sticky;
+ * the memory is the caller's and must stay valid while it is set.  A NULL config, or both pointers NULL, turns it off,
+ * and then no call launches anything for it.  A refused config returns 1 and leaves the previous target in effect.
+ * Refused with hit_dev while an uploaded map's largest label exceeds 32767, and while so set dts_upload_map refuses
+ * such a map.  An output, not state: snapshots and the gathers do not carry it. */
+int dts_set_scan_target(dts_sim* sim, const dts_scan_config* cfg, float* range_dev, int16_t* hit_dev);
+/* The range scan of the current state (after dts_reset without a render, dts_load_state, ...): one launch,
+ * stream-ordered.  Fails while no target is set. */
+int dts_render_scan(dts_sim* sim, void* stream);
 /* Motion-flow image beside every observation (DESIGN.md section 5, item 13): every later render of this handle that
  * writes obs — dts_render, dts_step, dts_step_terminal, whatever the render mode — also writes flow_dev, float32
  * [num_envs][cam_height][cam_width][2], always in that layout and at the camera size whatever dts_set_output_format and
