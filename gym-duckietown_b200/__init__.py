@@ -7,11 +7,12 @@ Public surface (mirrors gym_duckietown's, SURVEY.md 8b):
   MARKING_NAMES                              names of the lane-marking image's values (markings=True)
   OCCLUSION_NAMES                            names of the occlusion mask's values (flow_occlusion=True)
   BEV_VISIBILITY_NAMES                       names of the bird's-eye visibility's values (bev_visibility=True)
+  OBJECT_STATE_NAMES                         names of the object boxes' states (objects=True)
 """
 __version__ = "0.1.0"
 
 from .assets import MARKING_NAMES  # noqa: F401
-from .lib import BEV_VISIBILITY_NAMES, OCCLUSION_NAMES  # noqa: F401
+from .lib import BEV_VISIBILITY_NAMES, OBJECT_STATE_NAMES, OCCLUSION_NAMES  # noqa: F401
 from .maps import InvalidMapException, list_maps, load_map  # noqa: F401
 
 

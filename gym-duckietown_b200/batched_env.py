@@ -5,7 +5,7 @@ observation buffers are caller-visible torch CUDA tensors, the work runs on
 `torch.cuda.current_stream()` inside libdtsim.so, nothing synchronises.  Constructor keywords are the
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
 `auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `flow`, `flow_occlusion`,
-`camera_rand_pool`, the `bev*` keywords (`bev_visibility` among them) and the `scan*` keywords.
+`camera_rand_pool`, the `bev*` keywords (`bev_visibility` among them), the `scan*` keywords and `objects`.
 
 `camera_rand=True` (with `distortion=True`; without it the flag does nothing, as in the reference, S:352-358) gives the
 envs a spread of lenses: `camera_rand_pool` calibrations K, D are drawn once, at construction, within the reference's
@@ -106,6 +106,21 @@ pixels show nothing: sky or no fisheye source), 2 occluded (something else is in
 for unknown and outside.  Under `auto_reset` a row matches its `obs` row.  A visibility env refuses
 `set_rectification`, whose remap has no forward map.  `frame_cameras()` returns every env's camera of its last frame,
 on the device, to turn `bev_pixels` or `depth` into rays.  Snapshots and gathers do not carry them.
+
+`objects=True` allocates, for O = the most objects any of the env's maps has (object_boxes()'s O), `env.object_boxes3d`,
+float32 [num_envs, O, 7], `env.object_state`, uint8 [num_envs, O], and `env.object_corners_px`, float32 [num_envs, O,
+9, 2] (dts_set_object_target): every object's 3D box around each agent, slot o being object o of the env's map.  A box
+is the object's footprint of the bird's-eye map (moving obstacles where they are now), raised over the mesh's height;
+its row holds the centre's (forward, right, up) in metres from the agent, as the bird's-eye grid's axes, then length
+(along the object's heading; for a Duckiebot that has turned, its collision box's robot_length), width, height and yaw,
+the object's heading minus the agent's in (-pi, pi], counter-clockwise from above.  `object_state` names each slot by OBJECT_STATE_NAMES: 0 none (the map has fewer
+objects; the box is NaN), 1 shown, 2 hidden this episode (the box is still given: the reference still collides with
+it).  `object_corners_px` holds where the box's 8 corners (the four footprint corners at the bottom, then at the top)
+and its centre land in the frame in `obs`, in camera pixels as `bev_pixels`: NaN behind the camera or beyond its near
+or far plane, kept outside the frame for the pinhole and top-down views, NaN where the fisheye's forward map has no
+value; every point NaN after `step(render=False)`, under the rectification and in `render_objects()`, which writes the
+boxes and states alone, e.g. after `reset(render=False)`, `load_state` or `copy_envs`.  Every `step` and render writes
+them, last in the call; under `auto_reset` a row matches its `obs` row.  Snapshots and gathers do not carry them.
 """
 from __future__ import annotations
 
@@ -117,6 +132,7 @@ import torch
 from . import lib as L
 from .assets import MARKING_NAMES  # noqa: F401  (the names of env.markings' values)
 from .lib import BEV_VISIBILITY_NAMES  # noqa: F401  (the names of env.bev_visibility's values)
+from .lib import OBJECT_STATE_NAMES  # noqa: F401  (the names of env.object_state's values)
 from .lib import OCCLUSION_NAMES  # noqa: F401  (the names of env.flow_occlusion's values)
 from .episode import EpisodeSampler
 from .maps import TILE_KINDS, MapData, load_map
@@ -150,7 +166,7 @@ class BatchedDuckietownEnv:
                  depth: bool = False, labels: bool = False, camera_rand_pool: int = 16, markings: bool = False,
                  bev: bool = False, bev_shape=(64, 64), bev_cell: float = 0.03, bev_origin=None, flow: bool = False,
                  flow_occlusion: bool = False, bev_visibility: bool = False, scan: bool = False, scan_rays: int = 64,
-                 scan_fov: float = 2 * np.pi, scan_range: float = 2.0, scan_origin=(0.0, 0.0)):
+                 scan_fov: float = 2 * np.pi, scan_range: float = 2.0, scan_origin=(0.0, 0.0), objects: bool = False):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
         camera_rand = bool(camera_rand and distortion)   # S:353-356: camera_rand only with distortion
@@ -245,6 +261,14 @@ class BatchedDuckietownEnv:
                 (num_envs, int(scan_rays)), dtype=torch.float32, device=self.device) if scan else None
             self.scan_hit: Optional[torch.Tensor] = torch.zeros(
                 (num_envs, int(scan_rays)), dtype=torch.int16, device=self.device) if scan else None
+            # the object boxes (objects=True), OBJECT_STATE_NAMES; every step and render writes them on the device
+            n_obj = self._max_objects()
+            self.object_boxes3d: Optional[torch.Tensor] = torch.full(
+                (num_envs, n_obj, 7), float("nan"), dtype=torch.float32, device=self.device) if objects else None
+            self.object_state: Optional[torch.Tensor] = torch.zeros(
+                (num_envs, n_obj), dtype=torch.uint8, device=self.device) if objects else None
+            self.object_corners_px: Optional[torch.Tensor] = torch.full(
+                (num_envs, n_obj, 9, 2), float("nan"), dtype=torch.float32, device=self.device) if objects else None
             self.reward = torch.zeros(num_envs, dtype=torch.float32, device=self.device)
             self._done_u8 = torch.zeros(num_envs, dtype=torch.uint8, device=self.device)
             self.state: Dict[str, torch.Tensor] = {
@@ -285,6 +309,9 @@ class BatchedDuckietownEnv:
             self.sim.set_occlusion_target(self.flow_occlusion.data_ptr())
         if bev_visibility:
             self.sim.set_bev_visibility_target(self.bev_visibility.data_ptr(), self.bev_pixels.data_ptr(), *fwd)
+        if objects and n_obj:   # (maps without objects: nothing to write)
+            self.sim.set_object_target(n_obj, self.object_boxes3d.data_ptr(), self.object_state.data_ptr(),
+                                       self.object_corners_px.data_ptr(), *fwd)
         self.seed(seed)
 
     def set_output_format(self, obs_layout: Optional[str] = None, obs_dtype: Optional[str] = None,
@@ -493,6 +520,15 @@ class BatchedDuckietownEnv:
         self.sim.render_scan(self._stream())
         return self.scan_range, self.scan_hit
 
+    def render_objects(self):
+        """Write `object_boxes3d` / `object_state` for the current state (dts_render_objects), without rendering a
+        frame; `object_corners_px` becomes NaN."""
+        if self.object_boxes3d is None:
+            raise ValueError("render_objects needs objects=True")
+        if self.object_boxes3d.shape[1]:
+            self.sim.render_objects(self._stream())
+        return self.object_boxes3d, self.object_state, self.object_corners_px
+
     # labels -------------------------------------------------------------------------------------
     def label_table(self, map_id: int = 0) -> list:
         """What each label value of map `map_id` stands for (module-level `label_table`)."""
@@ -504,29 +540,17 @@ class BatchedDuckietownEnv:
         x1, y1 (inclusive); -1 where the object shows no pixel.  max_objects is the most objects any of the maps has."""
         if self.labels is None:
             raise ValueError("object_boxes needs labels=True")
-        n, h, w = self.labels.shape
-        n_obj = max((len(md.objects) for md in self.maps), default=0)
-        dev = self.device
-        cells = torch.tensor([md.grid_w * md.grid_h for md in self.maps], dtype=torch.int64, device=dev)
-        nobj = torch.tensor([len(md.objects) for md in self.maps], dtype=torch.int64, device=dev)
-        mid = self.state["map_id"].to(torch.int64)
-        o = self.labels.to(torch.int64) - 2 - cells[mid].view(n, 1, 1)        # object index, where the label is one
-        hit = (o >= 0) & (o < nobj[mid].view(n, 1, 1))
-        env = torch.arange(n, device=dev).view(n, 1, 1).expand(n, h, w)
-        ys = torch.arange(h, device=dev).view(1, h, 1).expand(n, h, w)
-        xs = torch.arange(w, device=dev).view(1, 1, w).expand(n, h, w)
-        slot = (env * max(n_obj, 1) + o)[hit]
-        pixels = torch.zeros(n * max(n_obj, 1), dtype=torch.int64, device=dev).scatter_add_(
-            0, slot, torch.ones_like(slot))
-        big = torch.iinfo(torch.int64).max
-        lo_x = torch.full_like(pixels, big).scatter_reduce_(0, slot, xs[hit], "amin")
-        lo_y = torch.full_like(pixels, big).scatter_reduce_(0, slot, ys[hit], "amin")
-        hi_x = torch.full_like(pixels, -1).scatter_reduce_(0, slot, xs[hit], "amax")
-        hi_y = torch.full_like(pixels, -1).scatter_reduce_(0, slot, ys[hit], "amax")
-        boxes = torch.stack([lo_x, lo_y, hi_x, hi_y], dim=1)
-        boxes[pixels == 0] = -1
-        return (pixels.view(n, -1)[:, :n_obj].to(torch.int32),
-                boxes.view(n, -1, 4)[:, :n_obj].to(torch.int32))
+        n, n_obj = self.num_envs, self._max_objects()
+        with torch.cuda.device(self.device):
+            pixels = torch.empty((n, n_obj), dtype=torch.int32, device=self.device)
+            boxes = torch.empty((n, n_obj, 4), dtype=torch.int32, device=self.device)
+        if n_obj:
+            self.sim.object_pixels(self.labels.data_ptr(), pixels.data_ptr(), boxes.data_ptr(), n_obj, self._stream())
+        return pixels, boxes
+
+    def _max_objects(self) -> int:
+        """The most objects any of the env's maps has: object_boxes()'s and the object boxes' O"""
+        return max((len(md.objects) for md in self.maps), default=0)
 
     # snapshots ----------------------------------------------------------------------------------
     @property

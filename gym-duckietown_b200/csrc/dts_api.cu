@@ -49,6 +49,7 @@ struct dts_sim {
   FlowTarget flow{};                    // dts_set_flow_target: caller-owned image and the record it owns, null = off
   OcclusionTarget occ{};                // dts_set_occlusion_target: caller-owned mask and the slots it owns, null = off
   BevViewTarget bev_view{};             // dts_set_bev_visibility_target: caller-owned outputs, both null = off
+  ObjectTarget objects{};               // dts_set_object_target: caller-owned outputs, max_objects 0 = off
   bool drawn = false;                   // frame memory holds a frame of every env (dts_get_frame_cameras)
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
   int profiling = 0;                    // 0 off, 1 events around k_raster only, 2 around every render kernel
@@ -211,6 +212,8 @@ int dts_upload_map(dts_sim* sim, int map_id, const dts_map_blob* b) {
   if ((sim->aux.labels || sim->bev.labels || sim->scan.hit) && b && largest_label((long long)b->grid_w * b->grid_h, b->n_objects) > INT16_MAX)
     return sim->fail("a label target is set and this map's largest label, %lld, does not fit in int16",
                      largest_label((long long)b->grid_w * b->grid_h, b->n_objects));
+  if (sim->objects.max_objects && b && b->n_objects > sim->objects.max_objects)
+    return sim->fail("an object target of %d objects is set and this map has %d", sim->objects.max_objects, b->n_objects);
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
   const std::string e = maps_upload(*sim->maps, map_id, b);
   if (!e.empty()) return sim->fail("%s", e.c_str());
@@ -369,7 +372,8 @@ static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t*
   if (check_gather(sim)) return 1;
   if (check_maps(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  const bool forward = sim->flow.out || sim->bev_view.vis || sim->bev_view.pix;   // a pass reads the forward maps
+  // a pass reads the forward maps
+  const bool forward = sim->flow.out || sim->bev_view.vis || sim->bev_view.pix || sim->objects.max_objects;
   const std::string e = renderer_prepare(*sim->render, maps_counts(*sim->maps), sim->render_mode, forward);
   if (!e.empty()) return sim->fail("%s", e.c_str());
   RenderCfg rc{sim->cfg.cam_width, sim->cfg.cam_height, sim->cfg.flags, sim->cfg.num_envs,
@@ -458,11 +462,32 @@ static int bev_view_pass(dts_sim* sim, void* stream, bool drew_frame) {
   return 0;
 }
 
+// The object boxes of every env's current state, where a target is set (dts_set_object_target), and where they land in
+// the frame the call drew (none: every corner NaN)
+static int objects_pass(dts_sim* sim, void* stream, bool drew_frame) {
+  if (!sim->objects.max_objects) return 0;
+  if (check_maps(sim)) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  launch_objects(state_arrays(*sim->state), maps_table(*sim->maps), maps_extent_table(*sim->maps), sim->objects,
+                 drew_frame ? renderer_frame_ctx(*sim->render) : nullptr, sim->cfg.cam_width, sim->cfg.cam_height,
+                 renderer_remap(*sim->render, sim->render_mode), drew_frame, (cudaStream_t)stream);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// The passes that read the frame the call drew, last in the call and in this order: the grids' visibility, then the
+// object boxes
+static int view_passes(dts_sim* sim, void* stream, bool drew_frame) {
+  if (bev_view_pass(sim, stream, drew_frame)) return 1;
+  return objects_pass(sim, stream, drew_frame);
+}
+
 int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
   if (!sim) return 1;
   if (render_pass(sim, obs_dev, stream, nullptr, nullptr)) return 1;
   if (map_pass(sim, stream)) return 1;
-  return bev_view_pass(sim, stream, true);
+  return view_passes(sim, stream, true);
 }
 
 int dts_render_bev(dts_sim* sim, void* stream) {
@@ -476,6 +501,30 @@ int dts_render_scan(dts_sim* sim, void* stream) {
   if (!sim) return 1;
   if (!sim->scan.range && !sim->scan.hit) return sim->fail("no range scan target is set (dts_set_scan_target)");
   return scan_pass(sim, stream);
+}
+
+int dts_render_objects(dts_sim* sim, void* stream) {
+  if (!sim) return 1;
+  if (!sim->objects.max_objects) return sim->fail("no object target is set (dts_set_object_target)");
+  return objects_pass(sim, stream, false);
+}
+
+int dts_object_pixels(dts_sim* sim, const int16_t* labels_dev, int32_t* pixels_dev, int32_t* boxes_dev, int max_objects,
+                      void* stream) {
+  if (!sim) return 1;
+  if (max_objects < 1 || max_objects > DTS_MAX_OBJECTS)
+    return sim->fail("object pixels for %d objects: 1 to %d are accepted", max_objects, DTS_MAX_OBJECTS);
+  if (!labels_dev || !pixels_dev || !boxes_dev) return sim->fail("labels_dev, pixels_dev and boxes_dev must not be NULL");
+  if (reinterpret_cast<uintptr_t>(labels_dev) & 1) return sim->fail("labels_dev is not aligned to 2 bytes");
+  if ((reinterpret_cast<uintptr_t>(pixels_dev) | reinterpret_cast<uintptr_t>(boxes_dev)) & 3)
+    return sim->fail("pixels_dev and boxes_dev must be aligned to 4 bytes");
+  if (check_maps(sim)) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  launch_object_pixels(state_arrays(*sim->state), maps_table(*sim->maps), labels_dev, sim->cfg.cam_width,
+                       sim->cfg.cam_height, pixels_dev, boxes_dev, max_objects, (cudaStream_t)stream);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  return 0;
 }
 
 // With a flow target: every env's camera and obstacles before the step, the previous frame of the next render's flow
@@ -518,7 +567,7 @@ int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, voi
   // the grids and scans of the state obs_dev will show: the ended envs' first states (every env's row, as the others did
   // not move)
   if (map_pass(sim, stream)) return 1;
-  if (!obs_dev) return bev_view_pass(sim, stream, false);
+  if (!obs_dev) return view_passes(sim, stream, false);
   // 4. their terminal frames -> terminal_obs_dev; 5. their first frames -> obs_dev
   const ResizeTarget rz = resizer_target(*sim->resize);
   const size_t px = rz.ow ? (size_t)rz.ow * rz.oh : (size_t)sim->cfg.cam_width * sim->cfg.cam_height;
@@ -527,7 +576,7 @@ int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, voi
   sim->launches++;
   DTS_CUDA(cudaGetLastError());
   if (render_pass(sim, obs_dev, stream, sim->ended, sim->n_ended)) return 1;
-  return bev_view_pass(sim, stream, true);   // every row against the frame obs_dev shows
+  return view_passes(sim, stream, true);   // every row against the frame obs_dev shows
 }
 
 int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* reward_dev, uint8_t* done_dev,
@@ -545,7 +594,7 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
   DTS_CUDA(cudaGetLastError());
   if (map_pass(sim, stream)) return 1;
   if (obs_dev && render_pass(sim, obs_dev, stream, nullptr, nullptr)) return 1;
-  return bev_view_pass(sim, stream, obs_dev != nullptr);
+  return view_passes(sim, stream, obs_dev != nullptr);
 }
 
 int dts_get_state(dts_sim* sim, dts_state_view* v) {
@@ -781,7 +830,8 @@ int dts_set_flow_target(dts_sim* sim, float* flow_dev, const float* fwd_x, const
     DTS_CUDA(cudaDeviceSynchronize());   // no step or render in flight still writes the record or reads the maps
     flow_record_free(sim->flow.rec);
     sim->flow = FlowTarget{};
-    if (!sim->bev_view.vis && !sim->bev_view.pix) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
+    if (!sim->bev_view.vis && !sim->bev_view.pix && !sim->objects.max_objects)
+      renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
     return 0;
   }
   if (reinterpret_cast<uintptr_t>(flow_dev) & 7) return sim->fail("flow target is not aligned to 8 bytes");
@@ -829,7 +879,7 @@ int dts_set_bev_visibility_target(dts_sim* sim, uint8_t* vis_dev, float* pix_dev
   if (!vis_dev && !pix_dev) {
     DTS_CUDA(cudaDeviceSynchronize());   // no call in flight still reads the forward maps
     sim->bev_view = BevViewTarget{};
-    if (!sim->flow.out) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
+    if (!sim->flow.out && !sim->objects.max_objects) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
     return 0;
   }
   if (reinterpret_cast<uintptr_t>(pix_dev) & 7) return sim->fail("bird's-eye pixel target is not aligned to 8 bytes");
@@ -843,6 +893,34 @@ int dts_set_bev_visibility_target(dts_sim* sim, uint8_t* vis_dev, float* pix_dev
     if (!e.empty()) return sim->fail("%s", e.c_str());
   }
   sim->bev_view = BevViewTarget{vis_dev, reinterpret_cast<float2*>(pix_dev)};
+  return 0;
+}
+
+int dts_set_object_target(dts_sim* sim, int max_objects, float* boxes_dev, uint8_t* state_dev, float* corners_dev,
+                          const float* fwd_x, const float* fwd_y, int n_tables) {
+  if (!sim) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  if (!boxes_dev && !state_dev && !corners_dev) {
+    DTS_CUDA(cudaDeviceSynchronize());   // no call in flight still reads the forward maps
+    sim->objects = ObjectTarget{};
+    if (!sim->flow.out && !sim->bev_view.vis && !sim->bev_view.pix) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
+    return 0;
+  }
+  if (max_objects < 1 || max_objects > DTS_MAX_OBJECTS)
+    return sim->fail("object target of %d objects: 1 to %d are accepted", max_objects, DTS_MAX_OBJECTS);
+  const std::vector<MapCounts>& counts = maps_counts(*sim->maps);
+  for (size_t s = 0; s < counts.size(); s++)
+    if (counts[s].n_objects > max_objects)
+      return sim->fail("map slot %zu has %d objects, more than the object target's %d", s, counts[s].n_objects, max_objects);
+  if ((reinterpret_cast<uintptr_t>(boxes_dev) | reinterpret_cast<uintptr_t>(corners_dev)) & 3)
+    return sim->fail("object box and corner targets must be aligned to 4 bytes");
+  if (check_forward_maps(sim, fwd_x, fwd_y, n_tables)) return 1;
+  DTS_CUDA(cudaDeviceSynchronize());
+  if (sim->cfg.flags & DTS_FLAG_DISTORTION) {
+    const std::string e = renderer_set_flow_maps(*sim->render, n_tables, fwd_x, fwd_y);
+    if (!e.empty()) return sim->fail("%s", e.c_str());
+  }
+  sim->objects = ObjectTarget{max_objects, boxes_dev, state_dev, reinterpret_cast<float2*>(corners_dev)};
   return 0;
 }
 

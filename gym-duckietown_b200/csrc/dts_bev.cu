@@ -76,20 +76,7 @@ __device__ __forceinline__ int gather_footprints(const DState& S, const DMap& m,
     double box[4];
     bool keep = false;
     if (o < m.n_objects && !(hidden[o >> 5] >> (o & 31) & 1u)) {
-      const int slot = m.objects[o].dyn_slot;
-      if (slot >= 0) {   // this env's copy of the obstacle's corners
-        for (int k = 0; k < 4; k++) {
-          q.x[k] = m.dyn_state[((size_t)(DTS_DYN_CORNERS + 2 * k) * nd + slot) * ne + env];
-          q.z[k] = m.dyn_state[((size_t)(DTS_DYN_CORNERS + 2 * k + 1) * nd + slot) * ne + env];
-        }
-        keep = true;
-      } else if (m.obj_corners) {
-        for (int k = 0; k < 4; k++) {
-          q.x[k] = __ldg(m.obj_corners + (size_t)o * 8 + 2 * k);
-          q.z[k] = __ldg(m.obj_corners + (size_t)o * 8 + 2 * k + 1);
-        }
-        keep = true;
-      }
+      keep = object_footprint(m, nd, ne, env, o, q.x, q.z);
       if (keep) footprint_box(q, box);
       keep = keep && box_meets(box, wx, wz, wr);
     }

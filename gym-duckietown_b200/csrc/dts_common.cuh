@@ -170,6 +170,27 @@ __device__ __forceinline__ void store_px_fmt(void* frame, int layout, int dtype,
   for (int c = 0; c < 3; c++) store_elem_fmt(frame, layout, dtype, x, y, c, W, H, (rgb >> (8 * c)) & 255u);
 }
 
+// Object o's footprint in env `env` of `ne` (DESIGN.md section 5 items 12 and 17): the env's copy of the obstacle's
+// corners for an object with a dynamic slot, else the map's obj_corners; false when the map has no footprints.  nd: the
+// map's n_dyn (callers looping over objects read it once)
+__device__ __forceinline__ bool object_footprint(const DMap& m, size_t nd, size_t ne, int env, int o, double x[4],
+                                                 double z[4]) {
+  const int slot = m.objects[o].dyn_slot;
+  if (slot >= 0) {
+    for (int k = 0; k < 4; k++) {
+      x[k] = m.dyn_state[((size_t)(DTS_DYN_CORNERS + 2 * k) * nd + slot) * ne + env];
+      z[k] = m.dyn_state[((size_t)(DTS_DYN_CORNERS + 2 * k + 1) * nd + slot) * ne + env];
+    }
+    return true;
+  }
+  if (!m.obj_corners) return false;
+  for (int k = 0; k < 4; k++) {
+    x[k] = __ldg(m.obj_corners + (size_t)o * 8 + 2 * k);
+    z[k] = __ldg(m.obj_corners + (size_t)o * 8 + 2 * k + 1);
+  }
+  return true;
+}
+
 // A pass over a device env list (RenderCfg::env_list): the number of slots drawn, and the env of slot s < that number
 __device__ __forceinline__ int n_listed(const int32_t* list, const int32_t* count, int n_envs) { return list ? __ldg(count) : n_envs; }
 __device__ __forceinline__ int listed_env(const int32_t* list, int slot) { return list ? __ldg(list + slot) : slot; }

@@ -89,6 +89,8 @@ void maps_destroy(MapSlots* m);
 // slot, on the host and on the device, as it was.
 std::string maps_upload(MapSlots& m, int slot, const dts_map_blob* b);
 const DMap* maps_table(const MapSlots& m);           // device [max_maps]
+// device [max_maps]: each slot's objects' (least, largest) object-space mesh y, [n_objects] (null: an empty slot)
+const float2* const* maps_extent_table(const MapSlots& m);
 const DMap* maps_get(const MapSlots& m, int slot);   // the slot's host record; null if out of range or empty
 const std::vector<MapCounts>& maps_counts(const MapSlots& m);   // [max_maps]
 int maps_slot_count(const MapSlots& m);                           // max_maps
@@ -133,8 +135,8 @@ Renderer* renderer_create(const dts_config& cfg);   // on cfg.device, which must
 void renderer_destroy(Renderer* r);
 void renderer_release_frame(Renderer& r);   // the maps changed: the next render re-sizes frame memory for them
 // Before every render: reserves frame memory for the maps of `counts` unless it is reserved, and checks that a fisheye
-// LUT is set if the camera needs one, a rectification LUT if render `mode` asks for it, and (`forward`: a flow or
-// bird's-eye visibility target is set) the fisheye tables' forward maps if the frame goes through them.
+// LUT is set if the camera needs one, a rectification LUT if render `mode` asks for it, and (`forward`: a flow, bird's-eye
+// visibility or object target is set) the fisheye tables' forward maps if the frame goes through them.
 std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode, bool forward);
 // The rasteriser's remap table for a LUT of the camera's size (obs[y, x] = frame[rint(rmapy), rint(rmapx)]), in the
 // fisheye slot or (`rectify`) the rectification slot; it replaces that slot's previous one, so no render may be in
@@ -250,6 +252,23 @@ struct FlowRemap {
 // every cell UNKNOWN.  One launch.
 void launch_bev_view(const DState& S, const DMap* maps, const BevTarget& b, const BevViewTarget& v, const FrameCtx* ctx,
                      const int16_t* labels, int W, int H, const FlowRemap& rm, bool drew_frame, cudaStream_t st);
+// objects (dts_objects.cu).  The object boxes of dts_set_object_target (DESIGN.md section 5 item 17), each
+// [n_envs][max_objects][...] or null: float32 boxes [7], uint8 state, float32 corner pixels [9][2].  All null: off.
+struct ObjectTarget {
+  int32_t max_objects;
+  float* boxes;
+  uint8_t* state;
+  float2* corners;
+};
+// Every env's object boxes of its current state and, where drew_frame (ctx read), where their corners land in the frame
+// the call drew: its camera in `ctx` and remap `rm` at W x H; else every corner NaN.  `extent`: maps_extent_table.
+// One launch.
+void launch_objects(const DState& S, const DMap* maps, const float2* const* extent, const ObjectTarget& t,
+                    const FrameCtx* ctx, int W, int H, const FlowRemap& rm, bool drew_frame, cudaStream_t st);
+// Every env's object pixel statistics (dts_object_pixels) from its label image labels [n_envs][H][W]: pixels int32
+// [n_envs][max_objects] and boxes int32 [n_envs][max_objects][4].  One launch.
+void launch_object_pixels(const DState& S, const DMap* maps, const int16_t* labels, int W, int H, int32_t* pixels,
+                          int32_t* boxes, int max_objects, cudaStream_t st);
 // A record for n_envs envs and max_dyn dynamic slots, every env's record invalid (episode -1); synchronous.  On failure
 // (error text) `rec` is untouched.
 std::string flow_record_alloc(FlowRecord& rec, int n_envs, int max_dyn);

@@ -14,6 +14,7 @@ namespace dts {
 
 struct MapSlot {
   DMap rec{};                   // host copy of the device table's entry (valid = 0: empty)
+  const float2* extent = nullptr;   // host copy of the extent table's entry (maps_extent_table)
   std::vector<void*> allocs;    // the device memory behind it
   uint64_t hash = 0;            // content hash of the blob it was built from (0: empty)
 };
@@ -21,17 +22,20 @@ struct MapSlot {
 struct MapSlots {
   int n_envs;
   DMap* table = nullptr;          // device [max_maps]
+  const float2** extent = nullptr;   // device [max_maps]: each slot's object extents (maps_extent_table)
   std::vector<MapSlot> slots;     // [max_maps]
   std::vector<MapCounts> counts;  // [max_maps]
 };
 
 MapSlots* maps_create(const dts_config& cfg) {
-  const size_t bytes = sizeof(DMap) * cfg.max_maps;
-  void* t = nullptr;
+  const size_t bytes = sizeof(DMap) * cfg.max_maps, ext_bytes = sizeof(float2*) * cfg.max_maps;
+  void *t = nullptr, *x = nullptr;
   if (cudaMalloc(&t, bytes) != cudaSuccess) return nullptr;
+  if (cudaMalloc(&x, ext_bytes) != cudaSuccess) { cudaFree(t); return nullptr; }
   cudaMemset(t, 0, bytes);
-  return new MapSlots{cfg.num_envs, static_cast<DMap*>(t), std::vector<MapSlot>(cfg.max_maps),
-                      std::vector<MapCounts>(cfg.max_maps)};
+  cudaMemset(x, 0, ext_bytes);
+  return new MapSlots{cfg.num_envs, static_cast<DMap*>(t), static_cast<const float2**>(x),
+                      std::vector<MapSlot>(cfg.max_maps), std::vector<MapCounts>(cfg.max_maps)};
 }
 
 void maps_destroy(MapSlots* m) {
@@ -39,10 +43,13 @@ void maps_destroy(MapSlots* m) {
   for (const MapSlot& s : m->slots)
     for (void* p : s.allocs) cudaFree(p);
   cudaFree(m->table);
+  cudaFree(m->extent);
   delete m;
 }
 
 const DMap* maps_table(const MapSlots& m) { return m.table; }
+
+const float2* const* maps_extent_table(const MapSlots& m) { return m.extent; }
 
 const DMap* maps_get(const MapSlots& m, int slot) {
   return slot >= 0 && slot < (int)m.slots.size() && m.slots[slot].rec.valid ? &m.slots[slot].rec : nullptr;
@@ -173,8 +180,9 @@ static std::string validate(const dts_map_blob* b, int slot, int n_slots) {
 }
 
 // A DObject drawing mesh `mesh_id`: its triangles, segment texture and object-space bounding sphere.  `top` = the
-// largest coordinate of its bounding box, for the spawn radius.
-static DObject mesh_object(const dts_map_blob& b, int mesh_id, float& top) {
+// largest coordinate of its bounding box, for the spawn radius; `y_extent` = its least and largest y, ObjMesh's
+// min_coords[1] / max_coords[1] (objmesh.py:228-232).
+static DObject mesh_object(const dts_map_blob& b, int mesh_id, float& top, float2& y_extent) {
   const dts_mesh& me = b.meshes[mesh_id];
   DObject d{};
   d.mesh_id = mesh_id; d.tri_offset = me.tri_offset; d.tri_count = me.tri_count;
@@ -188,6 +196,7 @@ static DObject mesh_object(const dts_map_blob& b, int mesh_id, float& top) {
     }
   top = hi[0] > hi[1] ? hi[0] : hi[1];
   top = top > hi[2] ? top : hi[2];
+  y_extent = make_float2(lo[1], hi[1]);
   float r2 = 0.f;
   for (int k = 0; k < 3; k++) { d.centre[k] = 0.5f * (lo[k] + hi[k]); const float h = 0.5f * (hi[k] - lo[k]); r2 += h * h; }
   d.bound_rad = sqrtf(r2);
@@ -231,10 +240,11 @@ std::string maps_upload(MapSlots& ms, int slot, const dts_map_blob* blob) {
   // objects: add spawn radius (S:1467) and a bounding sphere per placed mesh
   MapCounts counts{m.n_tiles, b.n_objects, 0};
   std::vector<DObject> objs(b.n_objects);
+  std::vector<float2> y_extent(b.n_objects);
   for (int o = 0; o < b.n_objects; o++) {
     const dts_object& s = b.objects[o];
     float top;
-    DObject& d = objs[o] = mesh_object(b, s.mesh_id, top);
+    DObject& d = objs[o] = mesh_object(b, s.mesh_id, top, y_extent[o]);
     d.tri_base = (int32_t)counts.n_tris;   // (the objects' triangles so far: the agent's are added after the loop)
     for (int k = 0; k < 3; k++) { d.pos[k] = (float)s.pos[k]; d.dpos[k] = s.pos[k]; }   // glTranslatef takes floats
     d.dyn_slot = s.dyn_slot;
@@ -247,7 +257,8 @@ std::string maps_upload(MapSlots& ms, int slot, const dts_map_blob* blob) {
   m.n_tris = b.n_tris;
   if (b.agent_mesh >= 0 && b.agent_mesh < b.n_meshes) {   // self.mesh, drawn by top-down views at cur_pos (S:1923-1929)
     float top;
-    m.agent = mesh_object(b, b.agent_mesh, top);
+    float2 y_extent_agent;
+    m.agent = mesh_object(b, b.agent_mesh, top, y_extent_agent);
     m.agent.scale = 1.0f; m.agent.dyn_slot = -1; m.agent.alt_from = m.agent.alt_to = -1;
   }
   m.agent.tri_base = (int32_t)counts.n_tris;   // the agent's draw ids follow every object's
@@ -345,15 +356,25 @@ std::string maps_upload(MapSlots& ms, int slot, const dts_map_blob* blob) {
   put(m.dyn_state, st.data(), st.size());
   put(m.dyn_init, init.data(), init.size());
   if (b.obj_corners) put(m.obj_corners, b.obj_corners, (size_t)b.n_objects * 8);
+  const float2* extent = nullptr;
+  put(extent, y_extent.data(), y_extent.size());
   m.valid = 1;
   // 3. once no kernel still reads the slot's old map: the table entry, the host record, and the old map's memory
   if (err.empty()) {
     cudaError_t e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpy(ms.table + slot, &m, sizeof(DMap), cudaMemcpyHostToDevice);
+    // the extent entry first, and back to the old one if the map entry cannot follow: either both entries name the
+    // new map or both the old one
+    if (e == cudaSuccess) e = cudaMemcpy(ms.extent + slot, &extent, sizeof(extent), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+      e = cudaMemcpy(ms.table + slot, &m, sizeof(DMap), cudaMemcpyHostToDevice);
+      if (e != cudaSuccess)
+        cudaMemcpy(ms.extent + slot, &ms.slots[slot].extent, sizeof(extent), cudaMemcpyHostToDevice);
+    }
     if (e != cudaSuccess) err = format("map table update failed: %s", cudaGetErrorString(e));
   }
   if (err.empty()) {
     fresh.rec = m;
+    fresh.extent = extent;
     fresh.hash = blob_hash(b);
     std::swap(ms.slots[slot], fresh);   // fresh: what to release, the old map or the new one that failed
     ms.counts[slot] = counts;

@@ -24,6 +24,8 @@ DONE_CODE_STR = {0: "in-progress", 1: "invalid-pose", 2: "max-steps-reached"}  #
 OCCLUSION_NAMES = ("none", "visible", "occluded", "outside", "unknown")
 # the bird's-eye visibility's values (DTS_BEVVIS_*, dts_set_bev_visibility_target), by value
 BEV_VISIBILITY_NAMES = ("unknown", "visible", "occluded", "outside")
+# the object boxes' states (DTS_OBJECT_*, dts_set_object_target), by value
+OBJECT_STATE_NAMES = ("none", "shown", "hidden")
 
 
 class DtsError(RuntimeError):
@@ -213,6 +215,9 @@ def load() -> C.CDLL:
     lib.dts_set_occlusion_target.argtypes = [vp, vp]
     lib.dts_set_bev_visibility_target.argtypes = [vp, vp, vp, vp, vp, i]
     lib.dts_get_frame_cameras.argtypes = [vp, vp, vp, vp]
+    lib.dts_set_object_target.argtypes = [vp, i, vp, vp, vp, vp, vp, i]
+    lib.dts_render_objects.argtypes = [vp, vp]
+    lib.dts_object_pixels.argtypes = [vp, vp, vp, vp, i, vp]
     lib.dts_resize_frames.argtypes = [vp, vp, vp, vp]
     lib.dts_blend4.argtypes = [vp, vp, vp, vp, C.c_uint64, vp]
     lib.dts_set_timing.argtypes = [vp, C.c_double, i, i]
@@ -247,7 +252,7 @@ def load() -> C.CDLL:
 
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_fisheye_luts", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
-           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_set_scan_target", "dts_render_scan", "dts_set_flow_target", "dts_set_occlusion_target", "dts_set_bev_visibility_target", "dts_get_frame_cameras", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
+           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_set_scan_target", "dts_render_scan", "dts_set_flow_target", "dts_set_occlusion_target", "dts_set_bev_visibility_target", "dts_get_frame_cameras", "dts_set_object_target", "dts_render_objects", "dts_object_pixels", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
            "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
 
@@ -585,6 +590,28 @@ class Sim:
         """Every env's camera of its last frame -> device float64 [num_envs, 12] at `V_ptr` and float32 [num_envs, 4]
         (P00, P11, P22, P23) at `P_ptr`, stream-ordered (dts_get_frame_cameras)."""
         self._check(self.lib.dts_get_frame_cameras(self.h, V_ptr, P_ptr, stream), "dts_get_frame_cameras")
+
+    def set_object_target(self, max_objects: int, boxes_ptr: Optional[int], state_ptr: Optional[int],
+                          corners_ptr: Optional[int], fwd_x: Optional[np.ndarray] = None,
+                          fwd_y: Optional[np.ndarray] = None):
+        """Every later step and render also writes, for each env and object slot < max_objects, the object's 3D box
+        (float32 [num_envs, max_objects, 7]) at `boxes_ptr`, its state (uint8 [num_envs, max_objects],
+        OBJECT_STATE_NAMES) at `state_ptr` and where its corners land in the frame the call drew (float32 [num_envs,
+        max_objects, 9, 2]) at `corners_ptr`, which the caller keeps alive.  fwd_x / fwd_y as set_flow_target's.  All
+        None turns it off (dts_set_object_target)."""
+        fx, fy, n = self._forward_maps(fwd_x, fwd_y)
+        self._check(self.lib.dts_set_object_target(self.h, int(max_objects), boxes_ptr, state_ptr, corners_ptr, _ptr(fx),
+                                                   _ptr(fy), n), "dts_set_object_target")
+
+    def render_objects(self, stream: int = 0):
+        """The object boxes and states of the current state, every corner NaN (dts_render_objects)."""
+        self._check(self.lib.dts_render_objects(self.h, stream), "dts_render_objects")
+
+    def object_pixels(self, labels_ptr: int, pixels_ptr: int, boxes_ptr: int, max_objects: int, stream: int = 0):
+        """Each env's object pixel counts (int32 [num_envs, max_objects]) and inclusive bounds (int32 [num_envs,
+        max_objects, 4], -1 where the count is 0) from the label image at `labels_ptr` (dts_object_pixels)."""
+        self._check(self.lib.dts_object_pixels(self.h, labels_ptr, pixels_ptr, boxes_ptr, int(max_objects), stream),
+                    "dts_object_pixels")
 
     def set_resize(self, out_w: int, out_h: int, filter: int = 0):
         """filter RESIZE_CV2_CUBIC (dts_set_resize) or RESIZE_PIL_BILINEAR (dts_set_resize_filter)."""

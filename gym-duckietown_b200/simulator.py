@@ -72,7 +72,7 @@ class Simulator(Env):
                  color_ground=(0.15, 0.15, 0.15), color_sky=(0.45, 0.82, 1), style: str = "photos",
                  enable_leds: bool = False, device: int = 0, depth: bool = False, labels: bool = False,
                  markings: bool = False, bev: bool = False, flow: bool = False, flow_occlusion: bool = False,
-                 bev_visibility: bool = False, scan: bool = False, **env_kwargs):
+                 bev_visibility: bool = False, scan: bool = False, objects: bool = False, **env_kwargs):
         if draw_curve or draw_bbox or enable_leds:
             raise NotImplementedError("draw_curve / draw_bbox / enable_leds are debug modes outside the hot path "
                                       "(SURVEY 8f-4)")
@@ -99,7 +99,7 @@ class Simulator(Env):
             camera_rand_pool=env_kwargs.pop("camera_rand_pool", 1),   # one camera per Simulator (distortion.py:46-47)
             color_ground=color_ground, color_sky=color_sky, num_tris_distractors=num_tris_distractors,
             action_mode=self._action_mode, depth=depth, labels=labels, markings=markings, bev=bev, flow=flow,
-            flow_occlusion=flow_occlusion, bev_visibility=bev_visibility, scan=scan, **env_kwargs)
+            flow_occlusion=flow_occlusion, bev_visibility=bev_visibility, scan=scan, objects=objects, **env_kwargs)
         self._b = BatchedDuckietownEnv(1, map_arg, **self._env_kwargs)
         self._adopt_map()
         self.action_space = spaces.Box(low=-1, high=1, shape=(2,), dtype=np.float32)              # S:309
@@ -162,7 +162,7 @@ class Simulator(Env):
         if getattr(self, "_human", None) is None:
             kw = dict(self._env_kwargs, camera_width=WINDOW_WIDTH, camera_height=WINDOW_HEIGHT, distortion=False,
                       terminal_obs=False, depth=False, labels=False, markings=False, bev=False, flow=False,
-                      flow_occlusion=False, bev_visibility=False, scan=False)
+                      flow_occlusion=False, bev_visibility=False, scan=False, objects=False)
             self._human = BatchedDuckietownEnv(1, list(self._b.maps), **kw)
         self._human.load_state(self._b.save_state())
         return self._human
@@ -250,6 +250,28 @@ class Simulator(Env):
         (BatchedDuckietownEnv.scan_hit); else None."""
         h = self._b.scan_hit
         return None if h is None else h[0].cpu().numpy()
+
+    @property
+    def object_boxes3d(self) -> Optional[np.ndarray]:
+        """With objects=True: float32 [O, 7], every object's 3D box around the agent (forward, right, up of its centre,
+        length, width, height, yaw) in the state last returned by reset / step / render_obs
+        (BatchedDuckietownEnv.object_boxes3d); else None."""
+        b = self._b.object_boxes3d
+        return None if b is None else b[0].cpu().numpy()
+
+    @property
+    def object_state(self) -> Optional[np.ndarray]:
+        """With objects=True: uint8 [O], each slot's OBJECT_STATE_NAMES value (BatchedDuckietownEnv.object_state);
+        else None."""
+        s = self._b.object_state
+        return None if s is None else s[0].cpu().numpy()
+
+    @property
+    def object_corners_px(self) -> Optional[np.ndarray]:
+        """With objects=True: float32 [O, 9, 2], where each box's 8 corners and centre land in the frame last returned
+        (BatchedDuckietownEnv.object_corners_px); else None."""
+        c = self._b.object_corners_px
+        return None if c is None else c[0].cpu().numpy()
 
     @property
     def flow(self) -> Optional[np.ndarray]:

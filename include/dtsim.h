@@ -293,7 +293,8 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
  * rows -> terminal_obs_dev) and a second render into obs_dev over the listed envs only, whose kernels exit at once when
  * nothing ended.  Launches: 2 R + 3, R being dts_render's (5, or 7 when the rasteriser writes packed u8 HWC of a width divisible by 4, +1
  * with a resize), plus a 4-byte memset; obs_dev = NULL (no render): 2; one more with a bird's-eye target (dts_set_bev_target),
- * and one more with a range scan target (dts_set_scan_target).  Fails without DTS_FLAG_AUTO_RESET, with
+ * one more with a range scan target (dts_set_scan_target), and one more with an object target (dts_set_object_target).
+ * Fails without DTS_FLAG_AUTO_RESET, with
  * terminal_obs_dev == obs_dev, and while a fused gather is armed (dts_gather_next), which it does not write.  The
  * second pass is not timed by dts_profile_*.  Never synchronises. */
 int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, void* terminal_obs_dev, float* reward_dev,
@@ -512,6 +513,50 @@ int dts_set_bev_visibility_target(dts_sim* sim, uint8_t* vis_dev, float* pix_dev
  * P_dev float32 [num_envs][4] (P00, P11, P22, P23 of gluPerspective), device memory.  Stream-ordered, one launch; fails
  * before the handle's first render (and after a map upload, until the next render). */
 int dts_get_frame_cameras(dts_sim* sim, double* V_dev, float* P_dev, void* stream);
+/* Object boxes around every agent (DESIGN.md section 5, item 17): for each env e and object slot o < max_objects, the
+ * 3D box of object o of e's map and where it lands in the frame drawn for e.  Box: its four corners in x-z are the
+ * object's footprint of the bird's-eye map (dts_map_blob.obj_corners, or env e's DTS_DYN_CORNERS for an object with a
+ * dynamic slot), ordered so that c0 -> c1 runs along the object's heading: generate_corners' order (C:64-79), c0 (min
+ * x, min z), c1 (max x, min z), c2, c3, as the map and the load-time obstacles have them; for a Duckiebot whose turning
+ * step has rewritten them in agent_boundbox's order (back-left, back-right, front-right, front-left, collision.py:9-31),
+ * (c1, c2, c3, c0) — chosen by which of c0 -> c1 and c1 -> c2 lies along get_dir_vec(DTS_DYN_ANGLE); its span in y is pos_y + scale min_y to pos_y + scale max_y, min_y / max_y the mesh's object-space
+ * extent (ObjMesh.min_coords / max_coords, objmesh.py:228-232, over the mesh's vertices as uploaded).  In float64, with
+ * px, pz, a the env's pos_x, pos_z, angle and ca, sa = cos a, sin a (the bird's-eye grid's frame, item 12, inverted):
+ *   boxes_dev float32 [num_envs][max_objects][7]: forward, right, up of the centre (the mean of c0..c3 at the middle of
+ *     the span; forward = dx ca - dz sa, right = dx sa + dz ca for dx, dz = centre - (px, pz), up = y), then
+ *     length = |c1 - c0|, width = |c2 - c1|, height = y1 - y0, and yaw = atan2(-right(c1 - c0), forward(c1 - c0)) in
+ *     (-pi, pi]: the object's heading minus the agent's, counter-clockwise from above.  NaN for DTS_OBJECT_NONE.
+ *   state_dev uint8 [num_envs][max_objects]: DTS_OBJECT_NONE (o >= the map's object count, or a map uploaded without
+ *     footprints), DTS_OBJECT_SHOWN, or DTS_OBJECT_HIDDEN (an optional object hidden this episode; the reference still
+ *     collides with it, so its box is given).
+ *   corners_dev float32 [num_envs][max_objects][9][2]: the 8 box corners (c0..c3 at y0, then c0..c3 at y1) and the box
+ *     centre through the frame's camera as dts_set_bev_visibility_target projects a cell: x1, y1 where 0.04 < -ez <= 100,
+ *     else NaN; without a remap q = (x1, y1), kept when it lies outside the frame; under the fisheye (one table or a
+ *     camera_rand pool) q = F(x1, y1), NaN where F's footprint leaves the table.  Every point NaN for an env this call
+ *     drew no frame for, for a frame drawn with DTS_RENDER_RECTIFY, and for DTS_OBJECT_NONE.
+ * Any output may be NULL; all NULL turns it off, and then every call launches exactly what it launches without it.
+ * fwd_x / fwd_y / n_tables: as dts_set_flow_target's, shared with the flow image and the bird's-eye visibility on the same
+ * terms.  Refused (non-zero, the previous target kept) for max_objects outside 1 to DTS_MAX_OBJECTS, while an uploaded
+ * map has more objects than max_objects, with outputs not aligned to their element size, with wrong forward maps, or
+ * when an allocation fails; while it is set, dts_upload_map refuses a map with more objects than max_objects.  With it
+ * set, dts_step, dts_step_terminal and dts_render launch one more kernel, k_objects, last in the call (after
+ * k_bev_view): a row shows the state obs row e shows, the respawned first state where dts_step_terminal's episode ended,
+ * and boxes and state are written without obs_dev too.  Sticky; the memory is the caller's and must stay valid while it
+ * is set.  Synchronises.  An output, not state: snapshots and the gathers do not carry it. */
+enum { DTS_OBJECT_NONE = 0, DTS_OBJECT_SHOWN = 1, DTS_OBJECT_HIDDEN = 2 };
+int dts_set_object_target(dts_sim* sim, int max_objects, float* boxes_dev, uint8_t* state_dev, float* corners_dev,
+                          const float* fwd_x, const float* fwd_y, int n_tables);
+/* The object boxes and states of the current state (after dts_reset without a render, dts_load_state, ...), every corner
+ * NaN: one launch, stream-ordered.  Fails while no target is set. */
+int dts_render_objects(dts_sim* sim, void* stream);
+/* Every env's object pixel statistics from a caller's label image labels_dev int16 [num_envs][cam_height][cam_width]
+ * (dts_set_label_target's numbering, against the map each env has now): o = label - 2 - grid_w * grid_h is object o
+ * where 0 <= o < the map's object count.  pixels_dev int32 [num_envs][max_objects]: how many pixels show object o;
+ * boxes_dev int32 [num_envs][max_objects][4]: their inclusive bounds x0, y0, x1, y1, all -1 where the count is 0 (and
+ * for o at or past the map's object count).  Refused for max_objects outside 1 to DTS_MAX_OBJECTS, NULL or misaligned
+ * pointers.  One launch, k_object_pixels, stream-ordered. */
+int dts_object_pixels(dts_sim* sim, const int16_t* labels_dev, int32_t* pixels_dev, int32_t* boxes_dev, int max_objects,
+                      void* stream);
 /* Select the fused wrapper behaviour for subsequent dts_step / dts_render calls (default: all zero, scale 1).
  * obs_dev then holds num_envs * 3 * H * W elements of uint8 or float32 in the chosen layout.  The renderer draws packed
  * uint8 HWC; for any other layout or dtype without a resize (dts_set_resize) it draws into a library staging frame of
