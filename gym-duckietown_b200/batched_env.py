@@ -5,7 +5,8 @@ observation buffers are caller-visible torch CUDA tensors, the work runs on
 `torch.cuda.current_stream()` inside libdtsim.so, nothing synchronises.  Constructor keywords are the
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
 `auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `flow`, `flow_occlusion`,
-`camera_rand_pool`, the `bev*` keywords (`bev_visibility` among them), the `scan*` keywords and `objects`.
+`camera_rand_pool`, the `bev*` keywords (`bev_visibility` among them), the `scan*` keywords, `objects` and the
+`lane_path*` keywords.
 
 `camera_rand=True` (with `distortion=True`; without it the flag does nothing, as in the reference, S:352-358) gives the
 envs a spread of lenses: `camera_rand_pool` calibrations K, D are drawn once, at construction, within the reference's
@@ -121,6 +122,21 @@ or far plane, kept outside the frame for the pinhole and top-down views, NaN whe
 value; every point NaN after `step(render=False)`, under the rectification and in `render_objects()`, which writes the
 boxes and states alone, e.g. after `reset(render=False)`, `load_state` or `copy_envs`.  Every `step` and render writes
 them, last in the call; under `auto_reset` a row matches its `obs` row.  Snapshots and gathers do not carry them.
+
+`lane_path=True` allocates, for K = `lane_path_points` (1 to 64, default 16), `env.lane_path`, float32 [num_envs, K, 3],
+`env.lane_path_count`, int16 [num_envs], and `env.lane_path_px`, float32 [num_envs, K, 2] (dts_set_lane_path_target):
+the lane ahead of each agent as points on its lane's centre curve, found by the reference's closest_curve_point.  Point
+0 is the closest point to the agent for its heading, the anchor of the lane pose; each later point is the closest point
+to a step of `lane_path_spacing` metres (0 < spacing <= 1, default 0.1) along the previous point's tangent, so the
+spacing is nominal.  A row holds the point's (forward, right) in metres from the agent, as `object_boxes3d`'s centre,
+then the yaw of the lane's tangent there against the agent's heading in (-pi, pi], counter-clockwise from above.
+`lane_path_count` says how many points were found: the walk stops at K or where it leaves the drivable tiles (0 when
+the agent is off them); later rows are NaN.  On 3-way and 4-way tiles the curve best aligned with the heading is taken,
+as the reference's rule does, and it can switch curves within a tile: the path does not choose a route.
+`lane_path_px` holds where each point lands in the frame in `obs`, in camera pixels as `object_corners_px`, NaN as
+there: after `step(render=False)`, under the rectification and in `render_lane_path()`, which writes the points and
+counts alone.  Every `step` and render writes them, last in the call; under `auto_reset` a row matches its `obs` row.
+Snapshots and gathers do not carry them.
 """
 from __future__ import annotations
 
@@ -166,7 +182,8 @@ class BatchedDuckietownEnv:
                  depth: bool = False, labels: bool = False, camera_rand_pool: int = 16, markings: bool = False,
                  bev: bool = False, bev_shape=(64, 64), bev_cell: float = 0.03, bev_origin=None, flow: bool = False,
                  flow_occlusion: bool = False, bev_visibility: bool = False, scan: bool = False, scan_rays: int = 64,
-                 scan_fov: float = 2 * np.pi, scan_range: float = 2.0, scan_origin=(0.0, 0.0), objects: bool = False):
+                 scan_fov: float = 2 * np.pi, scan_range: float = 2.0, scan_origin=(0.0, 0.0), objects: bool = False,
+                 lane_path: bool = False, lane_path_points: int = 16, lane_path_spacing: float = 0.1):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
         camera_rand = bool(camera_rand and distortion)   # S:353-356: camera_rand only with distortion
@@ -269,6 +286,14 @@ class BatchedDuckietownEnv:
                 (num_envs, n_obj), dtype=torch.uint8, device=self.device) if objects else None
             self.object_corners_px: Optional[torch.Tensor] = torch.full(
                 (num_envs, n_obj, 9, 2), float("nan"), dtype=torch.float32, device=self.device) if objects else None
+            # the lane path (lane_path=True); every step and render writes it on the device
+            n_pts = int(lane_path_points)
+            self.lane_path: Optional[torch.Tensor] = torch.full(
+                (num_envs, n_pts, 3), float("nan"), dtype=torch.float32, device=self.device) if lane_path else None
+            self.lane_path_count: Optional[torch.Tensor] = torch.zeros(
+                num_envs, dtype=torch.int16, device=self.device) if lane_path else None
+            self.lane_path_px: Optional[torch.Tensor] = torch.full(
+                (num_envs, n_pts, 2), float("nan"), dtype=torch.float32, device=self.device) if lane_path else None
             self.reward = torch.zeros(num_envs, dtype=torch.float32, device=self.device)
             self._done_u8 = torch.zeros(num_envs, dtype=torch.uint8, device=self.device)
             self.state: Dict[str, torch.Tensor] = {
@@ -312,6 +337,9 @@ class BatchedDuckietownEnv:
         if objects and n_obj:   # (maps without objects: nothing to write)
             self.sim.set_object_target(n_obj, self.object_boxes3d.data_ptr(), self.object_state.data_ptr(),
                                        self.object_corners_px.data_ptr(), *fwd)
+        if lane_path:
+            self.sim.set_lane_path_target(n_pts, lane_path_spacing, self.lane_path.data_ptr(),
+                                          self.lane_path_count.data_ptr(), self.lane_path_px.data_ptr(), *fwd)
         self.seed(seed)
 
     def set_output_format(self, obs_layout: Optional[str] = None, obs_dtype: Optional[str] = None,
@@ -528,6 +556,14 @@ class BatchedDuckietownEnv:
         if self.object_boxes3d.shape[1]:
             self.sim.render_objects(self._stream())
         return self.object_boxes3d, self.object_state, self.object_corners_px
+
+    def render_lane_path(self):
+        """Write `lane_path` / `lane_path_count` for the current state (dts_render_lane_path), without rendering a
+        frame; `lane_path_px` becomes NaN."""
+        if self.lane_path is None:
+            raise ValueError("render_lane_path needs lane_path=True")
+        self.sim.render_lane_path(self._stream())
+        return self.lane_path, self.lane_path_count, self.lane_path_px
 
     # labels -------------------------------------------------------------------------------------
     def label_table(self, map_id: int = 0) -> list:

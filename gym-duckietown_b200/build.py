@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdtsim.so")
 SOURCES = ["dts_api.cu", "dts_maps.cu", "dts_kernels_logic.cu", "dts_render.cu", "dts_post.cu", "dts_state.cu", "dts_bev.cu",
-           "dts_flow.cu", "dts_objects.cu"]
+           "dts_flow.cu", "dts_objects.cu", "dts_path.cu"]
 # -fmad=false: no implicit FMA contraction, so fp32/fp64 arithmetic is exactly what the source says
 # (the render kernels spell out fmaf() where an FMA is wanted; the CPU oracle is built the same way).
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-fmad=false",

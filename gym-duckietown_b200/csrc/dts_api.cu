@@ -50,6 +50,7 @@ struct dts_sim {
   OcclusionTarget occ{};                // dts_set_occlusion_target: caller-owned mask and the slots it owns, null = off
   BevViewTarget bev_view{};             // dts_set_bev_visibility_target: caller-owned outputs, both null = off
   ObjectTarget objects{};               // dts_set_object_target: caller-owned outputs, max_objects 0 = off
+  LanePathTarget lane_path{};           // dts_set_lane_path_target: caller-owned outputs, n_points 0 = off
   bool drawn = false;                   // frame memory holds a frame of every env (dts_get_frame_cameras)
   // per-kernel timing (dts_profile_*): event pairs recorded around the render launches
   int profiling = 0;                    // 0 off, 1 events around k_raster only, 2 around every render kernel
@@ -367,14 +368,18 @@ static int check_gather(dts_sim* sim) {
 }
 
 // dts_render of every env, or of the envs on a device list (dts_step_terminal's second pass; not profiled)
+// Whether a target reads the fisheye tables' forward maps: flow, the bird's-eye visibility, the object boxes and the lane
+// path.  They share one set; clearing one target frees it only when no other still reads it.
+static bool reads_forward_maps(const dts_sim* sim) {
+  return sim->flow.out || sim->bev_view.vis || sim->bev_view.pix || sim->objects.max_objects || sim->lane_path.n_points;
+}
+
 static int render_pass(dts_sim* sim, void* obs_dev, void* stream, const int32_t* env_list, const int32_t* env_count) {
   if (!obs_dev) return sim->fail("obs_dev is NULL");
   if (check_gather(sim)) return 1;
   if (check_maps(sim)) return 1;
   DTS_CUDA(cudaSetDevice(sim->cfg.device));
-  // a pass reads the forward maps
-  const bool forward = sim->flow.out || sim->bev_view.vis || sim->bev_view.pix || sim->objects.max_objects;
-  const std::string e = renderer_prepare(*sim->render, maps_counts(*sim->maps), sim->render_mode, forward);
+  const std::string e = renderer_prepare(*sim->render, maps_counts(*sim->maps), sim->render_mode, reads_forward_maps(sim));
   if (!e.empty()) return sim->fail("%s", e.c_str());
   RenderCfg rc{sim->cfg.cam_width, sim->cfg.cam_height, sim->cfg.flags, sim->cfg.num_envs,
                (sim->cfg.flags & DTS_FLAG_TESSELLATE) ? 1 : 0, sim->render_mode, 0, env_list, env_count};
@@ -476,11 +481,26 @@ static int objects_pass(dts_sim* sim, void* stream, bool drew_frame) {
   return 0;
 }
 
-// The passes that read the frame the call drew, last in the call and in this order: the grids' visibility, then the
-// object boxes
+// The lane path of every env's current state, where a target is set (dts_set_lane_path_target), and where its points
+// land in the frame the call drew (none: every pixel NaN)
+static int lane_path_pass(dts_sim* sim, void* stream, bool drew_frame) {
+  if (!sim->lane_path.n_points) return 0;
+  if (check_maps(sim)) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  launch_lane_path(state_arrays(*sim->state), maps_table(*sim->maps), sim->lane_path,
+                   drew_frame ? renderer_frame_ctx(*sim->render) : nullptr, sim->cfg.cam_width, sim->cfg.cam_height,
+                   renderer_remap(*sim->render, sim->render_mode), drew_frame, (cudaStream_t)stream);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// The passes that read the frame the call drew, last in the call and in this order: the grids' visibility, the object
+// boxes, then the lane path
 static int view_passes(dts_sim* sim, void* stream, bool drew_frame) {
   if (bev_view_pass(sim, stream, drew_frame)) return 1;
-  return objects_pass(sim, stream, drew_frame);
+  if (objects_pass(sim, stream, drew_frame)) return 1;
+  return lane_path_pass(sim, stream, drew_frame);
 }
 
 int dts_render(dts_sim* sim, void* obs_dev, void* stream) {
@@ -507,6 +527,12 @@ int dts_render_objects(dts_sim* sim, void* stream) {
   if (!sim) return 1;
   if (!sim->objects.max_objects) return sim->fail("no object target is set (dts_set_object_target)");
   return objects_pass(sim, stream, false);
+}
+
+int dts_render_lane_path(dts_sim* sim, void* stream) {
+  if (!sim) return 1;
+  if (!sim->lane_path.n_points) return sim->fail("no lane path target is set (dts_set_lane_path_target)");
+  return lane_path_pass(sim, stream, false);
 }
 
 int dts_object_pixels(dts_sim* sim, const int16_t* labels_dev, int32_t* pixels_dev, int32_t* boxes_dev, int max_objects,
@@ -810,8 +836,8 @@ int dts_set_scan_target(dts_sim* sim, const dts_scan_config* cfg, float* range_d
   return 0;
 }
 
-// The forward maps a flow or bird's-eye visibility target takes: one per fisheye table on a DTS_FLAG_DISTORTION handle,
-// none without
+// The forward maps a flow, bird's-eye visibility, object or lane path target takes: one per fisheye table on a
+// DTS_FLAG_DISTORTION handle, none without
 static int check_forward_maps(dts_sim* sim, const float* fwd_x, const float* fwd_y, int n_tables) {
   const bool fish = (sim->cfg.flags & DTS_FLAG_DISTORTION) != 0;
   if (fish && (!fwd_x || !fwd_y || n_tables < 1))
@@ -830,8 +856,7 @@ int dts_set_flow_target(dts_sim* sim, float* flow_dev, const float* fwd_x, const
     DTS_CUDA(cudaDeviceSynchronize());   // no step or render in flight still writes the record or reads the maps
     flow_record_free(sim->flow.rec);
     sim->flow = FlowTarget{};
-    if (!sim->bev_view.vis && !sim->bev_view.pix && !sim->objects.max_objects)
-      renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
+    if (!reads_forward_maps(sim)) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
     return 0;
   }
   if (reinterpret_cast<uintptr_t>(flow_dev) & 7) return sim->fail("flow target is not aligned to 8 bytes");
@@ -879,7 +904,7 @@ int dts_set_bev_visibility_target(dts_sim* sim, uint8_t* vis_dev, float* pix_dev
   if (!vis_dev && !pix_dev) {
     DTS_CUDA(cudaDeviceSynchronize());   // no call in flight still reads the forward maps
     sim->bev_view = BevViewTarget{};
-    if (!sim->flow.out && !sim->objects.max_objects) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
+    if (!reads_forward_maps(sim)) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
     return 0;
   }
   if (reinterpret_cast<uintptr_t>(pix_dev) & 7) return sim->fail("bird's-eye pixel target is not aligned to 8 bytes");
@@ -903,7 +928,7 @@ int dts_set_object_target(dts_sim* sim, int max_objects, float* boxes_dev, uint8
   if (!boxes_dev && !state_dev && !corners_dev) {
     DTS_CUDA(cudaDeviceSynchronize());   // no call in flight still reads the forward maps
     sim->objects = ObjectTarget{};
-    if (!sim->flow.out && !sim->bev_view.vis && !sim->bev_view.pix) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
+    if (!reads_forward_maps(sim)) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
     return 0;
   }
   if (max_objects < 1 || max_objects > DTS_MAX_OBJECTS)
@@ -921,6 +946,32 @@ int dts_set_object_target(dts_sim* sim, int max_objects, float* boxes_dev, uint8
     if (!e.empty()) return sim->fail("%s", e.c_str());
   }
   sim->objects = ObjectTarget{max_objects, boxes_dev, state_dev, reinterpret_cast<float2*>(corners_dev)};
+  return 0;
+}
+
+int dts_set_lane_path_target(dts_sim* sim, int n_points, double spacing, float* points_dev, int16_t* count_dev,
+                             float* px_dev, const float* fwd_x, const float* fwd_y, int n_tables) {
+  if (!sim) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  if (!points_dev && !count_dev && !px_dev) {
+    DTS_CUDA(cudaDeviceSynchronize());   // no call in flight still reads the forward maps
+    sim->lane_path = LanePathTarget{};
+    if (!reads_forward_maps(sim)) renderer_set_flow_maps(*sim->render, 0, nullptr, nullptr);
+    return 0;
+  }
+  if (n_points < 1 || n_points > DTS_LANE_PATH_MAX_POINTS)
+    return sim->fail("lane path of %d points: 1 to %d are accepted", n_points, DTS_LANE_PATH_MAX_POINTS);
+  if (!(spacing > 0.0 && spacing <= 1.0)) return sim->fail("lane path spacing %g: 0 < spacing <= 1 m is accepted", spacing);
+  if ((reinterpret_cast<uintptr_t>(points_dev) | reinterpret_cast<uintptr_t>(px_dev)) & 3)
+    return sim->fail("lane path point and pixel targets must be aligned to 4 bytes");
+  if (reinterpret_cast<uintptr_t>(count_dev) & 1) return sim->fail("lane path count target is not aligned to 2 bytes");
+  if (check_forward_maps(sim, fwd_x, fwd_y, n_tables)) return 1;
+  DTS_CUDA(cudaDeviceSynchronize());
+  if (sim->cfg.flags & DTS_FLAG_DISTORTION) {
+    const std::string e = renderer_set_flow_maps(*sim->render, n_tables, fwd_x, fwd_y);
+    if (!e.empty()) return sim->fail("%s", e.c_str());
+  }
+  sim->lane_path = LanePathTarget{n_points, spacing, points_dev, count_dev, px_dev};
   return 0;
 }
 

@@ -70,6 +70,22 @@ __device__ __forceinline__ bool forward_map(const float2* __restrict__ F, int W,
   return true;
 }
 
+// A world point (x, y, z) to the pixel q of a W x H frame drawn under modelview V and gluPerspective's P00, P11, then
+// through the forward map `fwd` unless it is null (the pinhole and top-down views).  False where the point does not lie
+// within the near and far planes (0.04 < -ez <= 100, S:1761) or F's footprint leaves the table; a point outside the
+// frame is kept.
+__device__ __forceinline__ bool project_to_frame(const double* V, double P00, double P11, const float2* __restrict__ fwd,
+                                                 int W, int H, double x, double y, double z, float2& q) {
+  const double ex = V[0] * x + V[1] * y + V[2] * z + V[3];
+  const double ey = V[4] * x + V[5] * y + V[6] * z + V[7];
+  const double w = -(V[8] * x + V[9] * y + V[10] * z + V[11]);
+  if (!(w > 0.04 && w <= 100.0)) return false;
+  const double iw = 1.0 / w;
+  const double qx = (P00 * (ex * iw) + 1.0) * (0.5 * W), qy = (1.0 - P11 * (ey * iw)) * (0.5 * H);
+  q = make_float2((float)qx, (float)qy);
+  return !fwd || forward_map(fwd, W, H, (float)qx, (float)qy, q);
+}
+
 // Eye-space GL_POSITION for a light given under modelview V: positional (w=1) or direction (w=0).
 __host__ __device__ inline void light_to_eye(const double V[12], const float lp[4], float out[4]) {
   const double x = lp[0], y = lp[1], z = lp[2], w = lp[3];

@@ -136,7 +136,7 @@ void renderer_destroy(Renderer* r);
 void renderer_release_frame(Renderer& r);   // the maps changed: the next render re-sizes frame memory for them
 // Before every render: reserves frame memory for the maps of `counts` unless it is reserved, and checks that a fisheye
 // LUT is set if the camera needs one, a rectification LUT if render `mode` asks for it, and (`forward`: a flow, bird's-eye
-// visibility or object target is set) the fisheye tables' forward maps if the frame goes through them.
+// visibility, object or lane path target is set) the fisheye tables' forward maps if the frame goes through them.
 std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, int mode, bool forward);
 // The rasteriser's remap table for a LUT of the camera's size (obs[y, x] = frame[rint(rmapy), rint(rmapx)]), in the
 // fisheye slot or (`rectify`) the rectification slot; it replaces that slot's previous one, so no render may be in
@@ -269,6 +269,19 @@ void launch_objects(const DState& S, const DMap* maps, const float2* const* exte
 // [n_envs][max_objects] and boxes int32 [n_envs][max_objects][4].  One launch.
 void launch_object_pixels(const DState& S, const DMap* maps, const int16_t* labels, int W, int H, int32_t* pixels,
                           int32_t* boxes, int max_objects, cudaStream_t st);
+// lane path (dts_path.cu).  The lane path of dts_set_lane_path_target (DESIGN.md section 5 item 18), each
+// [n_envs][n_points][...] or null: float32 points [3], int16 count [n_envs], float32 pixels [2].  All null: off.
+struct LanePathTarget {
+  int32_t n_points;
+  double spacing;
+  float* points;
+  int16_t* count;
+  float* px;
+};
+// Every env's lane path from its current state and, where drew_frame (ctx read), where its points land in the frame the
+// call drew: its camera in `ctx` and remap `rm` at W x H; else every pixel NaN.  One launch.
+void launch_lane_path(const DState& S, const DMap* maps, const LanePathTarget& t, const FrameCtx* ctx, int W, int H,
+                      const FlowRemap& rm, bool drew_frame, cudaStream_t st);
 // A record for n_envs envs and max_dyn dynamic slots, every env's record invalid (episode -1); synchronous.  On failure
 // (error text) `rec` is untouched.
 std::string flow_record_alloc(FlowRecord& rec, int n_envs, int max_dyn);

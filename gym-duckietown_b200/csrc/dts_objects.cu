@@ -84,14 +84,8 @@ __global__ void __launch_bounds__(kObjThreads) k_objects(DState S, const DMap* _
             rm.fwd ? rm.fwd + (size_t)(rm.table_of_env ? __ldg(rm.table_of_env + env) : 0) * W * H : nullptr;
         for (int k = 0; k < 9; k++) {
           const double x = k < 8 ? cx[k & 3] : mx, y = k < 4 ? y0 : k < 8 ? y1 : my, z = k < 8 ? cz[k & 3] : mz;
-          const double qe_x = V[0] * x + V[1] * y + V[2] * z + V[3];
-          const double qe_y = V[4] * x + V[5] * y + V[6] * z + V[7];
-          const double w = -(V[8] * x + V[9] * y + V[10] * z + V[11]);
-          if (!(w > 0.04 && w <= 100.0)) continue;   // gluPerspective's near and far planes (S:1761)
-          const double iw = 1.0 / w;
-          const double qx = (P00 * (qe_x * iw) + 1.0) * (0.5 * W), qy = (1.0 - P11 * (qe_y * iw)) * (0.5 * H);
-          float2 q = make_float2((float)qx, (float)qy);
-          if (fwd && !forward_map(fwd, W, H, (float)qx, (float)qy, q)) continue;
+          float2 q;
+          if (!project_to_frame(V, P00, P11, fwd, W, H, x, y, z, q)) continue;
           px[2 * k] = q.x;
           px[2 * k + 1] = q.y;
         }

@@ -2434,9 +2434,9 @@ std::string renderer_prepare(Renderer& r, const std::vector<MapCounts>& counts, 
   if ((r.flags & DTS_FLAG_DISTORTION) && !r.fish.src_xy) return "distortion enabled but no fisheye LUT set";
   if ((mode & DTS_RENDER_RECTIFY) && !r.rect.src_xy) return "DTS_RENDER_RECTIFY but no rectification LUT set";
   if (forward && (r.flags & DTS_FLAG_DISTORTION) && !(mode & (DTS_RENDER_PINHOLE | DTS_RENDER_RECTIFY)) && !r.fish.fwd)
-    return "a flow, bird's-eye visibility or object target is set but the fisheye tables have no forward maps: a fisheye "
-           "LUT set after dts_set_flow_target / dts_set_bev_visibility_target / dts_set_object_target drops them, so set "
-           "that target again";
+    return "a flow, bird's-eye visibility, object or lane path target is set but the fisheye tables have no forward maps: "
+           "a fisheye LUT set after dts_set_flow_target / dts_set_bev_visibility_target / dts_set_object_target / "
+           "dts_set_lane_path_target drops them, so set that target again";
   return "";
 }
 

@@ -218,6 +218,8 @@ def load() -> C.CDLL:
     lib.dts_set_object_target.argtypes = [vp, i, vp, vp, vp, vp, vp, i]
     lib.dts_render_objects.argtypes = [vp, vp]
     lib.dts_object_pixels.argtypes = [vp, vp, vp, vp, i, vp]
+    lib.dts_set_lane_path_target.argtypes = [vp, i, C.c_double, vp, vp, vp, vp, vp, i]
+    lib.dts_render_lane_path.argtypes = [vp, vp]
     lib.dts_resize_frames.argtypes = [vp, vp, vp, vp]
     lib.dts_blend4.argtypes = [vp, vp, vp, vp, C.c_uint64, vp]
     lib.dts_set_timing.argtypes = [vp, C.c_double, i, i]
@@ -252,7 +254,7 @@ def load() -> C.CDLL:
 
 
 EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_fisheye_luts", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
-           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_set_scan_target", "dts_render_scan", "dts_set_flow_target", "dts_set_occlusion_target", "dts_set_bev_visibility_target", "dts_get_frame_cameras", "dts_set_object_target", "dts_render_objects", "dts_object_pixels", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
+           "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_set_scan_target", "dts_render_scan", "dts_set_flow_target", "dts_set_occlusion_target", "dts_set_bev_visibility_target", "dts_get_frame_cameras", "dts_set_object_target", "dts_render_objects", "dts_object_pixels", "dts_set_lane_path_target", "dts_render_lane_path", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
            "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
 
@@ -612,6 +614,22 @@ class Sim:
         max_objects, 4], -1 where the count is 0) from the label image at `labels_ptr` (dts_object_pixels)."""
         self._check(self.lib.dts_object_pixels(self.h, labels_ptr, pixels_ptr, boxes_ptr, int(max_objects), stream),
                     "dts_object_pixels")
+
+    def set_lane_path_target(self, n_points: int, spacing: float, points_ptr: Optional[int], count_ptr: Optional[int],
+                             px_ptr: Optional[int], fwd_x: Optional[np.ndarray] = None,
+                             fwd_y: Optional[np.ndarray] = None):
+        """Every later step and render also writes, for each env, n_points points of its lane path `spacing` metres
+        apart (float32 [num_envs, n_points, 3]: forward, right, yaw) at `points_ptr`, how many it found (int16
+        [num_envs]) at `count_ptr` and where they land in the frame the call drew (float32 [num_envs, n_points, 2]) at
+        `px_ptr`, which the caller keeps alive.  fwd_x / fwd_y as set_flow_target's.  All None turns it off
+        (dts_set_lane_path_target)."""
+        fx, fy, n = self._forward_maps(fwd_x, fwd_y)
+        self._check(self.lib.dts_set_lane_path_target(self.h, int(n_points), float(spacing), points_ptr, count_ptr,
+                                                      px_ptr, _ptr(fx), _ptr(fy), n), "dts_set_lane_path_target")
+
+    def render_lane_path(self, stream: int = 0):
+        """The lane path of the current state, every pixel NaN (dts_render_lane_path)."""
+        self._check(self.lib.dts_render_lane_path(self.h, stream), "dts_render_lane_path")
 
     def set_resize(self, out_w: int, out_h: int, filter: int = 0):
         """filter RESIZE_CV2_CUBIC (dts_set_resize) or RESIZE_PIL_BILINEAR (dts_set_resize_filter)."""

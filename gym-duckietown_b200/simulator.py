@@ -72,7 +72,8 @@ class Simulator(Env):
                  color_ground=(0.15, 0.15, 0.15), color_sky=(0.45, 0.82, 1), style: str = "photos",
                  enable_leds: bool = False, device: int = 0, depth: bool = False, labels: bool = False,
                  markings: bool = False, bev: bool = False, flow: bool = False, flow_occlusion: bool = False,
-                 bev_visibility: bool = False, scan: bool = False, objects: bool = False, **env_kwargs):
+                 bev_visibility: bool = False, scan: bool = False, objects: bool = False,
+                 lane_path: bool = False, **env_kwargs):
         if draw_curve or draw_bbox or enable_leds:
             raise NotImplementedError("draw_curve / draw_bbox / enable_leds are debug modes outside the hot path "
                                       "(SURVEY 8f-4)")
@@ -99,7 +100,8 @@ class Simulator(Env):
             camera_rand_pool=env_kwargs.pop("camera_rand_pool", 1),   # one camera per Simulator (distortion.py:46-47)
             color_ground=color_ground, color_sky=color_sky, num_tris_distractors=num_tris_distractors,
             action_mode=self._action_mode, depth=depth, labels=labels, markings=markings, bev=bev, flow=flow,
-            flow_occlusion=flow_occlusion, bev_visibility=bev_visibility, scan=scan, objects=objects, **env_kwargs)
+            flow_occlusion=flow_occlusion, bev_visibility=bev_visibility, scan=scan, objects=objects, lane_path=lane_path,
+            **env_kwargs)
         self._b = BatchedDuckietownEnv(1, map_arg, **self._env_kwargs)
         self._adopt_map()
         self.action_space = spaces.Box(low=-1, high=1, shape=(2,), dtype=np.float32)              # S:309
@@ -162,7 +164,7 @@ class Simulator(Env):
         if getattr(self, "_human", None) is None:
             kw = dict(self._env_kwargs, camera_width=WINDOW_WIDTH, camera_height=WINDOW_HEIGHT, distortion=False,
                       terminal_obs=False, depth=False, labels=False, markings=False, bev=False, flow=False,
-                      flow_occlusion=False, bev_visibility=False, scan=False, objects=False)
+                      flow_occlusion=False, bev_visibility=False, scan=False, objects=False, lane_path=False)
             self._human = BatchedDuckietownEnv(1, list(self._b.maps), **kw)
         self._human.load_state(self._b.save_state())
         return self._human
@@ -272,6 +274,27 @@ class Simulator(Env):
         (BatchedDuckietownEnv.object_corners_px); else None."""
         c = self._b.object_corners_px
         return None if c is None else c[0].cpu().numpy()
+
+    @property
+    def lane_path(self) -> Optional[np.ndarray]:
+        """With lane_path=True: float32 [K, 3], the lane path ahead of the agent (forward, right, yaw of each point) in
+        the state last returned by reset / step / render_obs (BatchedDuckietownEnv.lane_path); else None."""
+        p = self._b.lane_path
+        return None if p is None else p[0].cpu().numpy()
+
+    @property
+    def lane_path_count(self) -> Optional[int]:
+        """With lane_path=True: how many of lane_path's points were found (BatchedDuckietownEnv.lane_path_count);
+        else None."""
+        c = self._b.lane_path_count
+        return None if c is None else int(c[0].item())
+
+    @property
+    def lane_path_px(self) -> Optional[np.ndarray]:
+        """With lane_path=True: float32 [K, 2], where each lane path point lands in the frame last returned
+        (BatchedDuckietownEnv.lane_path_px); else None."""
+        p = self._b.lane_path_px
+        return None if p is None else p[0].cpu().numpy()
 
     @property
     def flow(self) -> Optional[np.ndarray]:

@@ -20,6 +20,7 @@ extern "C" {
 #define DTS_ABI_VERSION 3
 #define DTS_MAX_DELAY 16     /* command-delay line depth (steps): 0.15 s at up to 100 Hz (MotionBlurWrapper steps at 90 Hz) */
 #define DTS_MAX_OBJECTS 256  /* per map; visibility bitmask is 8 x u32 */
+#define DTS_LANE_PATH_MAX_POINTS 64  /* points per env of dts_set_lane_path_target */
 
 typedef struct dts_sim dts_sim; /* opaque, one per GPU, not thread-safe */
 
@@ -293,8 +294,8 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
  * rows -> terminal_obs_dev) and a second render into obs_dev over the listed envs only, whose kernels exit at once when
  * nothing ended.  Launches: 2 R + 3, R being dts_render's (5, or 7 when the rasteriser writes packed u8 HWC of a width divisible by 4, +1
  * with a resize), plus a 4-byte memset; obs_dev = NULL (no render): 2; one more with a bird's-eye target (dts_set_bev_target),
- * one more with a range scan target (dts_set_scan_target), and one more with an object target (dts_set_object_target).
- * Fails without DTS_FLAG_AUTO_RESET, with
+ * one more with a range scan target (dts_set_scan_target), one more with an object target (dts_set_object_target), and
+ * one more with a lane path target (dts_set_lane_path_target).  Fails without DTS_FLAG_AUTO_RESET, with
  * terminal_obs_dev == obs_dev, and while a fused gather is armed (dts_gather_next), which it does not write.  The
  * second pass is not timed by dts_profile_*.  Never synchronises. */
 int dts_step_terminal(dts_sim* sim, const float* actions_dev, void* obs_dev, void* terminal_obs_dev, float* reward_dev,
@@ -549,6 +550,42 @@ int dts_set_object_target(dts_sim* sim, int max_objects, float* boxes_dev, uint8
 /* The object boxes and states of the current state (after dts_reset without a render, dts_load_state, ...), every corner
  * NaN: one launch, stream-ordered.  Fails while no target is set. */
 int dts_render_objects(dts_sim* sim, void* stream);
+/* The lane path ahead of every agent (DESIGN.md section 5, item 18): points along its lane's centre curve, in the
+ * agent's frame and in the frame drawn for it.  ccp(p, a) below is closest_curve_point (S:1337-1369) as the step's lane
+ * pose takes it: the tile under p (get_grid_coords), none off the grid or on a tile that is not drivable; the curve of
+ * that tile whose chord P3 - P0, every chord divided by the one Frobenius norm of them all, has the largest dot product
+ * with get_dir_vec(a) (the first at a tie); then bezier_closest's 8-level bisection for p and the point and unit
+ * tangent there.  Per env e, in float64, with px, pz, a its pos_x, pos_z, angle:
+ *   (q0, t0) = ccp((px, 0, pz), a); for k = 0, 1, ...: a_k = atan2(-t_k.z, t_k.x) (the tangent's heading, so that
+ *   get_dir_vec(a_k) lies along t_k) and (q_{k+1}, t_{k+1}) = ccp(q_k + spacing t_k, a_k); the walk ends at n_points
+ *   points or at the first call that finds none, and count is how many it found.
+ * Point 0 takes the agent's heading, so it is the anchor of get_lane_pos2 (the lane pose); each later point takes the
+ * previous tangent's, so the walk follows the lane around curves.  On 3-way and 4-way tiles the best-aligned chord picks
+ * the curve as the reference's rule does, and it can switch curves partway through a tile: the walk does not choose a
+ * route.  Spacing is nominal: a point is the bisection's closest point to a step of `spacing` along the tangent.
+ *   points_dev float32 [num_envs][n_points][3]: forward, right of q_k (dx ca - dz sa, dx sa + dz ca for dx, dz =
+ *     q_k - (px, pz), ca, sa = cos a, sin a, item 17's formulas), then yaw = atan2(-right(t_k), forward(t_k)) in
+ *     (-pi, pi], -pi given as pi: the tangent's heading minus the agent's, counter-clockwise from above.  NaN for k >=
+ *     count.  Point 0's lane pose: dist = -forward sin(yaw) - right cos(yaw) and angle_rad = yaw.
+ *   count_dev int16 [num_envs].
+ *   px_dev float32 [num_envs][n_points][2]: q_k (at its own y: 0, the curves are flat) through the frame's camera as
+ *     dts_set_object_target projects a box corner: where 0.04 < -ez <= 100, kept outside the frame for the pinhole and
+ *     top-down views, through F under the fisheye or a camera_rand pool (NaN where F's footprint leaves the table).
+ *     NaN under DTS_RENDER_RECTIFY, for an env the call drew no frame for, and for k >= count.
+ * Any output may be NULL; all NULL turns it off, and then every call launches exactly what it launches without it.
+ * fwd_x / fwd_y / n_tables: as dts_set_flow_target's, shared with the flow image, the bird's-eye visibility and the
+ * object target on the same terms.  Refused (non-zero, the previous target kept) for n_points outside 1 to
+ * DTS_LANE_PATH_MAX_POINTS, spacing outside (0, 1] m or not finite, points_dev / px_dev not aligned to 4 bytes or
+ * count_dev to 2, or wrong forward maps.  With it set, dts_step, dts_step_terminal and dts_render launch one more
+ * kernel, k_lane_path, last in the call (after k_objects): a row shows the state obs row e shows, the respawned first
+ * state where dts_step_terminal's episode ended, and points and count are written without obs_dev too.  Sticky; the
+ * memory is the caller's and must stay valid while it is set.  Synchronises.  An output, not state: snapshots and the
+ * gathers do not carry it. */
+int dts_set_lane_path_target(dts_sim* sim, int n_points, double spacing, float* points_dev, int16_t* count_dev,
+                             float* px_dev, const float* fwd_x, const float* fwd_y, int n_tables);
+/* The lane path of the current state (after dts_reset without a render, dts_load_state, ...), every pixel NaN: one
+ * launch, stream-ordered.  Fails while no target is set. */
+int dts_render_lane_path(dts_sim* sim, void* stream);
 /* Every env's object pixel statistics from a caller's label image labels_dev int16 [num_envs][cam_height][cam_width]
  * (dts_set_label_target's numbering, against the map each env has now): o = label - 2 - grid_w * grid_h is object o
  * where 0 <= o < the map's object count.  pixels_dev int32 [num_envs][max_objects]: how many pixels show object o;
