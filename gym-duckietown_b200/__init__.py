@@ -2,17 +2,19 @@
 
 Public surface (mirrors gym_duckietown's, SURVEY.md 8b):
   Simulator, DuckietownEnv, MultiMapEnv      single-env gym.Env adapters (old 4-tuple API)
+  DuckietownLF, DuckietownNav                the lane-following and navigation tasks (envs/duckietown_env.py)
   BatchedDuckietownEnv                       N envs per GPU, torch tensors in/out
   load_map, list_maps                        MapFormat1 loader
   MARKING_NAMES                              names of the lane-marking image's values (markings=True)
   OCCLUSION_NAMES                            names of the occlusion mask's values (flow_occlusion=True)
   BEV_VISIBILITY_NAMES                       names of the bird's-eye visibility's values (bev_visibility=True)
   OBJECT_STATE_NAMES                         names of the object boxes' states (objects=True)
+  DONE_CODE_NAMES                            names of the done codes (the state's done_code)
 """
 __version__ = "0.1.0"
 
 from .assets import MARKING_NAMES  # noqa: F401
-from .lib import BEV_VISIBILITY_NAMES, OBJECT_STATE_NAMES, OCCLUSION_NAMES  # noqa: F401
+from .lib import BEV_VISIBILITY_NAMES, DONE_CODE_NAMES, OBJECT_STATE_NAMES, OCCLUSION_NAMES  # noqa: F401
 from .maps import InvalidMapException, list_maps, load_map  # noqa: F401
 
 
@@ -20,7 +22,7 @@ def __getattr__(name):  # lazy: importing the package must not require torch/CUD
     if name in ("BatchedDuckietownEnv", "HostPipeline"):
         from . import batched_env
         return getattr(batched_env, name)
-    if name in ("Simulator", "DuckietownEnv", "MultiMapEnv", "NotInLane"):
+    if name in ("Simulator", "DuckietownEnv", "DuckietownLF", "DuckietownNav", "MultiMapEnv", "NotInLane"):
         from . import simulator
         return getattr(simulator, name)
     raise AttributeError(name)

@@ -6,7 +6,7 @@ observation buffers are caller-visible torch CUDA tensors, the work runs on
 reference's (simulator.py:207-232, envs/duckietown_env.py:15) plus `num_envs`, `device`,
 `auto_reset`, `device_reset`, `terminal_obs`, `depth`, `labels`, `markings`, `flow`, `flow_occlusion`,
 `camera_rand_pool`, the `bev*` keywords (`bev_visibility` among them), the `scan*` keywords, `objects` and the
-`lane_path*` keywords.
+`lane_path*` keywords and `nav`.
 
 `camera_rand=True` (with `distortion=True`; without it the flag does nothing, as in the reference, S:352-358) gives the
 envs a spread of lenses: `camera_rand_pool` calibrations K, D are drawn once, at construction, within the reference's
@@ -137,6 +137,15 @@ as the reference's rule does, and it can switch curves within a tile: the path d
 there: after `step(render=False)`, under the rectification and in `render_lane_path()`, which writes the points and
 counts alone.  Every `step` and render writes them, last in the call; under `auto_reset` a row matches its `obs` row.
 Snapshots and gathers do not carry them.
+
+`nav=True` poses the reference's navigation task, DuckietownNav (envs/duckietown_env.py:89-127, its two calls to itself
+read as calls to DuckietownEnv and its `randint` as `integers`), for every env: each reset, host or device, draws a
+goal tile from the env's own stream after everything else the reset draws, uniformly among the map's drivable tiles
+and again until it is not the tile the agent starts on; `env.goal_tile`, int16 [num_envs, 2], holds (i, j).  A step
+that ends on the goal tile ends the episode with reward 1000 (1010 under the `dt` reward) and done_code 3,
+"goal-reached" (DONE_CODE_NAMES), whatever the step would have ended with otherwise; auto-reset and `terminal_obs`
+then treat it as any other ended episode.  Every map needs at least two drivable tiles and at most 255 tiles a side.
+The goal is part of the env's state: snapshots carry it.  Without `nav` nothing is drawn and no goal is tested.
 """
 from __future__ import annotations
 
@@ -148,6 +157,7 @@ import torch
 from . import lib as L
 from .assets import MARKING_NAMES  # noqa: F401  (the names of env.markings' values)
 from .lib import BEV_VISIBILITY_NAMES  # noqa: F401  (the names of env.bev_visibility's values)
+from .lib import DONE_CODE_NAMES  # noqa: F401  (the names of the done codes)
 from .lib import OBJECT_STATE_NAMES  # noqa: F401  (the names of env.object_state's values)
 from .lib import OCCLUSION_NAMES  # noqa: F401  (the names of env.flow_occlusion's values)
 from .episode import EpisodeSampler
@@ -183,7 +193,8 @@ class BatchedDuckietownEnv:
                  bev: bool = False, bev_shape=(64, 64), bev_cell: float = 0.03, bev_origin=None, flow: bool = False,
                  flow_occlusion: bool = False, bev_visibility: bool = False, scan: bool = False, scan_rays: int = 64,
                  scan_fov: float = 2 * np.pi, scan_range: float = 2.0, scan_origin=(0.0, 0.0), objects: bool = False,
-                 lane_path: bool = False, lane_path_points: int = 16, lane_path_spacing: float = 0.1):
+                 lane_path: bool = False, lane_path_points: int = 16, lane_path_spacing: float = 0.1,
+                 nav: bool = False):
         if not torch.cuda.is_available():
             raise L.DtsError("BatchedDuckietownEnv needs a CUDA device; there is no CPU implementation")
         camera_rand = bool(camera_rand and distortion)   # S:353-356: camera_rand only with distortion
@@ -213,7 +224,9 @@ class BatchedDuckietownEnv:
         self._keep_terminal = terminal_obs
         flags = (L.FLAG_AUTO_RESET if auto_reset else 0) | (L.FLAG_DOMAIN_RAND if domain_rand else 0) | \
                 (L.FLAG_DISTORTION if distortion else 0) | (L.FLAG_DYNAMICS_RAND if dynamics_rand else 0) | \
-                (L.FLAG_TESSELLATE if tessellate_tiles else 0) | (L.FLAG_CAMERA_RAND if camera_rand else 0)
+                (L.FLAG_TESSELLATE if tessellate_tiles else 0) | (L.FLAG_CAMERA_RAND if camera_rand else 0) | \
+                (L.FLAG_NAV if nav else 0)
+        self.nav = nav
         self.cfg = L.default_config(
             num_envs=num_envs, device=device, cam_width=camera_width, cam_height=camera_height, max_steps=max_steps,
             frame_skip=int(frame_skip), action_mode=L.ACTION_VEL_STEER if action_mode == "vel_steer" else L.ACTION_PWM,
@@ -298,11 +311,13 @@ class BatchedDuckietownEnv:
             self._done_u8 = torch.zeros(num_envs, dtype=torch.uint8, device=self.device)
             self.state: Dict[str, torch.Tensor] = {
                 k_: torch.as_tensor(v, device=self.device) for k_, v in self.sim.state_arrays().items()}
+            # the goal tiles (nav=True), library-owned uint8 [num_envs] each
+            self._goal = {k_: torch.as_tensor(v, device=self.device) for k_, v in self.sim.goal_arrays().items()}
         self.sampler = EpisodeSampler(
             num_envs, domain_rand=domain_rand, dynamics_rand=dynamics_rand, camera_rand=camera_rand,
             accept_start_angle_deg=accept_start_angle_deg,
             num_tris_distractors=num_tris_distractors, color_ground=color_ground, color_sky=color_sky,
-            user_tile_start=user_tile_start, randomization_config=randomization_config)
+            user_tile_start=user_tile_start, randomization_config=randomization_config, nav=nav)
         self.map_ids = np.zeros(num_envs, np.int32)
         self._first_reset = True
         self.resize = None
@@ -478,11 +493,22 @@ class BatchedDuckietownEnv:
                     full[envs] = val
                     params[key] = full
                 params["map_id"] = self.map_ids.copy()
+                goals = params.pop("goal", None)
                 self.sim.reset(mask_ptr, params, self._stream())
+                if goals is not None:   # stream-ordered after the reset it belongs to
+                    g = torch.from_numpy(goals.astype(np.int16)).to(self.device)
+                    self.sim.set_goals(mask_ptr, g.data_ptr(), self._stream())
         self._first_reset = False
         if render:
             self.sim.render(self.obs.data_ptr(), self._stream())
         return self.obs
+
+    @property
+    def goal_tile(self) -> torch.Tensor:
+        """int16 [num_envs, 2]: every env's goal tile (i, j) under nav=True (a copy, on the current stream)."""
+        if not self.nav:
+            raise ValueError("goal_tile needs nav=True")
+        return torch.stack([self._goal["goal_i"], self._goal["goal_j"]], 1).to(torch.int16)
 
     def _query_for(self, envs):
         def query(k, x, z, a, safety, hidden):

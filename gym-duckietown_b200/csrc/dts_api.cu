@@ -287,10 +287,13 @@ int dts_set_rectify_lut(dts_sim* sim, const float* mapx, const float* mapy, int 
 // > 0: round-robin over that many slots; < 0: uniform draw over -n slots; 0: the env keeps its map
 static int map_select(const dts_sim* sim) { return sim->cfg.random_maps > 0 ? -sim->cfg.random_maps : sim->cfg.cycle_maps; }
 
-// status bit 1: a dts_load_state was handed a record naming no uploaded map (that env kept its state)
+// status bit 1: a dts_load_state was handed a record naming no uploaded map (that env kept its state); bit 2: a
+// dts_set_goals was handed a goal that is not a drivable tile of its env's map (that env kept its goal)
 static int check_loaded(dts_sim* sim) {
   if (((volatile int32_t*)sim->h_status)[1])
     return sim->fail("an earlier dts_load_state met a record whose map_id names no uploaded map; that env was not loaded");
+  if (((volatile int32_t*)sim->h_status)[2])
+    return sim->fail("an earlier dts_set_goals met a goal that is not a drivable tile of its env's map; that env kept its goal");
   return 0;
 }
 
@@ -626,6 +629,26 @@ int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* rewar
 int dts_get_state(dts_sim* sim, dts_state_view* v) {
   if (!sim || !v) return 1;
   *v = state_view(*sim->state);
+  return 0;
+}
+
+int dts_set_goals(dts_sim* sim, const uint8_t* mask_dev, const int16_t* goals_dev, void* stream) {
+  if (!sim) return 1;
+  if (!(sim->cfg.flags & DTS_FLAG_NAV)) return sim->fail("dts_set_goals on a handle created without DTS_FLAG_NAV");
+  if (!goals_dev || (uintptr_t)goals_dev % 2) return sim->fail("goals_dev must be a 2-byte aligned device pointer");
+  if (check_maps(sim)) return 1;
+  DTS_CUDA(cudaSetDevice(sim->cfg.device));
+  launch_set_goals(state_arrays(*sim->state), maps_table(*sim->maps), mask_dev, goals_dev, sim->d_status + 2,
+                   (cudaStream_t)stream);
+  sim->launches++;
+  DTS_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int dts_get_goals(dts_sim* sim, uint8_t** goal_i_dev, uint8_t** goal_j_dev) {
+  if (!sim || !goal_i_dev || !goal_j_dev) return 1;
+  *goal_i_dev = state_arrays(*sim->state).goal_i;
+  *goal_j_dev = state_arrays(*sim->state).goal_j;
   return 0;
 }
 
@@ -1006,7 +1029,7 @@ int dts_resize_frames(dts_sim* sim, const uint8_t* src_dev, void* dst_dev, void*
 int dts_status(dts_sim* sim) {
   if (!sim || !sim->h_status) return 0;
   const volatile int32_t* w = sim->h_status;
-  return (w[0] ? 1 : 0) | (w[1] ? 2 : 0);
+  return (w[0] ? 1 : 0) | (w[1] ? 2 : 0) | (w[2] ? 4 : 0);
 }
 
 // ---- snapshots: every env's state as one record, out of and back into the library's arrays (dts_state.cu) --------

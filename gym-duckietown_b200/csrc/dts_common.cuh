@@ -117,6 +117,7 @@ struct DState {
   uint8_t *done_code, *in_lane, *collided;
   uint64_t* rng;         // [6][n] numpy PCG64 stream per env: state hi, lo, inc hi, lo, has_uint32, cached uint32
   struct RenderEp* rep;  // [n] per-episode render parameters (AoS: one CTA reads one record)
+  uint8_t *goal_i, *goal_j;   // DTS_FLAG_NAV: the episode's goal tile (such maps are at most 255 tiles a side); else 0
 };
 
 // Per-episode render inputs (simulator.py:546-614, 1768): 144 bytes, seven 16-byte groups and the hidden mask, read by

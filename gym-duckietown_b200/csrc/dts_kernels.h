@@ -55,6 +55,10 @@ void launch_reset_random(const DState& S, const DMap* maps, const StepCfg& c, in
 // `p` holds DEVICE copies of the host's episode parameters (state_stage); NULL members keep the defaults
 void launch_reset_params(const DState& S, const DMap* maps, const StepCfg& c, const uint8_t* mask,
                          const dts_episode_params& p, cudaStream_t st);
+// dts_set_goals: goals int16 [n][2] (device) -> the goal tiles of the envs with mask[e] (null: all); an entry that is not
+// a drivable tile of the env's map is not taken and sets *refused (device address of a status word) to 1
+void launch_set_goals(const DState& S, const DMap* maps, const uint8_t* mask, const int16_t* goals, int32_t* refused,
+                      cudaStream_t st);
 void launch_assign_maps(const DState& S, const DMap* maps, const uint8_t* mask, const int32_t* map_id, cudaStream_t st);
 // The auto-reset k_step_logic does in place, deferred (dts_step_terminal): every env whose episode ended re-spawns, and
 // is appended to ended[0 .. *n_ended), which the caller zeroes first.  The list's order is not deterministic.

@@ -19,8 +19,9 @@ __device__ __forceinline__ void default_render_ep(RenderEp& r) {
 }
 
 // Fill the per-step outputs for the env's current pose: get_agent_info fields + _compute_done_reward S:1685-1705.
+// `arrival`: DuckietownNav.step's goal test, which overrides whatever _compute_done_reward decided (a step's only).
 __device__ inline void evaluate_pose(const DState& S, const DMap& m, const StepCfg& c, int e, double px, double pz,
-                                     double ang, int step_count, float* reward, uint8_t* done) {
+                                     double ang, int step_count, float* reward, uint8_t* done, bool arrival = false) {
   int ti, tj;
   tile_at(m, px, pz, ti, tj);
   const DynRef dyn = dyn_ref(m, S.n, e);
@@ -36,6 +37,7 @@ __device__ inline void evaluate_pose(const DState& S, const DMap& m, const StepC
     code = DTS_IN_PROGRESS;
     rew = lp.in_lane ? (+1.0 * c.robot_speed * lp.dot_dir + -10 * fabs(lp.dist) + +40 * pen) : 40 * pen;  // S:1654-1667
   }
+  if (arrival && ti == S.goal_i[e] && tj == S.goal_j[e]) { rew = kRewardGoal; code = DTS_GOAL_REACHED; }   // envs/duckietown_env.py:119-125
   S.tile_i[e] = ti; S.tile_j[e] = tj;
   S.lane_dist[e] = lp.dist; S.lane_dot[e] = lp.dot_dir; S.lane_angle[e] = lp.angle_rad; S.in_lane[e] = lp.in_lane;
   S.prox[e] = pen; S.collided[e] = hit; S.reward[e] = rew; S.done_code[e] = code;
@@ -183,6 +185,15 @@ __device__ inline void respawn(const DState& S, const DMap* maps, const StepCfg&
     px = x; pz = z; ang = a;
     break;
   }
+  if (c.flags & DTS_FLAG_NAV) {   // DuckietownNav.reset: a goal tile other than the start's (upload keeps n_drivable >= 2)
+    int si, sj, gi, gj;
+    tile_at(m, px, pz, si, sj);
+    do {
+      const int t = rs.integers(0, m.n_drivable);
+      gi = m.drivable_ij[2 * t]; gj = m.drivable_ij[2 * t + 1];
+    } while (gi == si && gj == sj);
+    S.goal_i[e] = (uint8_t)gi; S.goal_j[e] = (uint8_t)gj;
+  }
   set_pose(S, m, e, px, pz, ang);
   S.rep[e] = r;
   store_stream(S, e, rs);
@@ -239,7 +250,7 @@ __global__ void __launch_bounds__(128) k_step_logic(DState S, const DMap* __rest
   if (dyn_rand) store_stream(S, e, rs);
   S.cx[e] = x; S.cy[e] = y; S.ctheta[e] = th; S.vu[e] = u; S.vw[e] = w;
   S.pos_x[e] = px; S.pos_z[e] = pz; S.angle[e] = ang; S.speed[e] = speed; S.step_count[e] = steps;
-  evaluate_pose(S, m, c, e, px, pz, ang, steps, reward, done);
+  evaluate_pose(S, m, c, e, px, pz, ang, steps, reward, done, (c.flags & DTS_FLAG_NAV) != 0);
   if ((c.flags & DTS_FLAG_AUTO_RESET) && S.done_code[e] != DTS_IN_PROGRESS) respawn(S, maps, c, n_maps_cycle, e);
 }
 
@@ -306,6 +317,22 @@ __global__ void __launch_bounds__(128) k_reset_params(DState S, const DMap* __re
   S.rep[e] = r;
   S.episode[e] += 1;
   evaluate_pose(S, m, c, e, px, pz, ang, 0, nullptr, nullptr);
+}
+
+// dts_set_goals: a host reset's goal tiles.  One that is not a drivable tile of its env's map is not taken: the env
+// keeps its goal and `refused` (a status word) is set
+__global__ void __launch_bounds__(128) k_set_goals(DState S, const DMap* __restrict__ maps, const uint8_t* __restrict__ mask,
+                                                   const int16_t* __restrict__ goals, int32_t* refused) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= S.n || (mask && !mask[e])) return;
+  const DMap& m = maps[S.map_id[e]];
+  const int gi = goals[2 * e], gj = goals[2 * e + 1];
+  const int idx = gj * m.grid_w + gi;
+  if (gi < 0 || gi >= m.grid_w || gj < 0 || gj >= m.grid_h || m.tile_kind[idx] < 0 || !m.tile_drivable[idx]) {
+    *reinterpret_cast<volatile int32_t*>(refused) = 1;
+    return;
+  }
+  S.goal_i[e] = (uint8_t)gi; S.goal_j[e] = (uint8_t)gj;
 }
 
 // randomize_maps_on_reset with a host-drawn map (S:541-544): new map id + its obstacles re-created (_load_map),
@@ -389,6 +416,10 @@ void launch_respawn_ended(const DState& S, const DMap* maps, const StepCfg& c, i
 void launch_reset_params(const DState& S, const DMap* maps, const StepCfg& c, const uint8_t* mask,
                          const dts_episode_params& p, cudaStream_t st) {
   k_reset_params<<<(S.n + 127) / 128, 128, 0, st>>>(S, maps, c, mask, p);
+}
+void launch_set_goals(const DState& S, const DMap* maps, const uint8_t* mask, const int16_t* goals, int32_t* refused,
+                      cudaStream_t st) {
+  k_set_goals<<<(S.n + 127) / 128, 128, 0, st>>>(S, maps, mask, goals, refused);
 }
 void launch_assign_maps(const DState& S, const DMap* maps, const uint8_t* mask, const int32_t* map_id, cudaStream_t st) {
   k_assign_maps<<<(S.n + 127) / 128, 128, 0, st>>>(S, maps, mask, map_id);

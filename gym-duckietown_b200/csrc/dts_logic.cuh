@@ -15,6 +15,7 @@ constexpr double kCamForward = 0.066;
 constexpr double kCentreOff = kCamForward - (kRobotLength / 2);          // _actual_center S:2109
 constexpr double kAgentSafetyRad = ((kRobotLength > kRobotWidth ? kRobotLength : kRobotWidth) / 2) * 1.8;  // S:153
 constexpr double kRewardInvalidPose = -1000.0;                           // S:175
+constexpr double kRewardGoal = 1000.0;                                   // DuckietownNav.step envs/duckietown_env.py:125
 constexpr int kMaxSpawnAttempts = 5000;                                  // S:177
 
 struct LanePose { double dist, dot_dir, angle_rad; bool in_lane; };

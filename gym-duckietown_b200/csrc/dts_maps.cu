@@ -21,6 +21,7 @@ struct MapSlot {
 
 struct MapSlots {
   int n_envs;
+  bool nav;                       // DTS_FLAG_NAV: every map needs two drivable tiles and at most 255 tiles a side
   DMap* table = nullptr;          // device [max_maps]
   const float2** extent = nullptr;   // device [max_maps]: each slot's object extents (maps_extent_table)
   std::vector<MapSlot> slots;     // [max_maps]
@@ -34,7 +35,7 @@ MapSlots* maps_create(const dts_config& cfg) {
   if (cudaMalloc(&x, ext_bytes) != cudaSuccess) { cudaFree(t); return nullptr; }
   cudaMemset(t, 0, bytes);
   cudaMemset(x, 0, ext_bytes);
-  return new MapSlots{cfg.num_envs, static_cast<DMap*>(t), static_cast<const float2**>(x),
+  return new MapSlots{cfg.num_envs, (cfg.flags & DTS_FLAG_NAV) != 0, static_cast<DMap*>(t), static_cast<const float2**>(x),
                       std::vector<MapSlot>(cfg.max_maps), std::vector<MapCounts>(cfg.max_maps)};
 }
 
@@ -237,6 +238,11 @@ std::string maps_upload(MapSlots& ms, int slot, const dts_map_blob* blob) {
   m.has_start_pose = b.has_start_pose != 0;
   for (int k = 0; k < 3; k++) m.start_pose[k] = b.start_pose[k];
   m.n_drivable = (int)drv.size() / 2;
+  // the goal draw needs a drivable tile other than the start's (assert, envs/duckietown_env.py:106), and the snapshot
+  // records keep the goal's coordinates in one byte each
+  if (ms.nav && (b.grid_w > 255 || b.grid_h > 255))
+    return format("DTS_FLAG_NAV: the map is %d x %d tiles, at most 255 a side are supported", b.grid_w, b.grid_h);
+  if (ms.nav && m.n_drivable < 2) return format("DTS_FLAG_NAV: the map has %d drivable tiles, a goal needs 2", m.n_drivable);
   // objects: add spawn radius (S:1467) and a bounding sphere per placed mesh
   MapCounts counts{m.n_tiles, b.n_objects, 0};
   std::vector<DObject> objs(b.n_objects);

@@ -21,7 +21,7 @@
 namespace dts {
 
 namespace {
-constexpr uint64_t kLayoutVersion = 1;   // bump whenever the rows below change
+constexpr uint64_t kLayoutVersion = 2;   // bump whenever the rows below change
 constexpr int kGroup = 32;               // envs per CTA
 constexpr int kChunkBytes = 1024;        // record bytes per env one CTA stages (a chunk ends at a row boundary)
 constexpr int kThreads = 256;
@@ -48,7 +48,8 @@ constexpr StateArray kStateArrays[] = {
     DTS_STATE_ARRAY(fifo, 2 * DTS_MAX_DELAY), DTS_STATE_ARRAY(rng, 6),
     DTS_STATE_ARRAY(step_count, 1), DTS_STATE_ARRAY(tile_i, 1), DTS_STATE_ARRAY(tile_j, 1), DTS_STATE_ARRAY(map_id, 1),
     DTS_STATE_ARRAY(episode, 1),
-    DTS_STATE_ARRAY(done_code, 1), DTS_STATE_ARRAY(in_lane, 1), DTS_STATE_ARRAY(collided, 1)};
+    DTS_STATE_ARRAY(done_code, 1), DTS_STATE_ARRAY(in_lane, 1), DTS_STATE_ARRAY(collided, 1),
+    DTS_STATE_ARRAY(goal_i, 1), DTS_STATE_ARRAY(goal_j, 1)};
 #undef DTS_STATE_ARRAY
 constexpr int kNumArrays = sizeof(kStateArrays) / sizeof(kStateArrays[0]);
 

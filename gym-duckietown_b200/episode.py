@@ -64,8 +64,10 @@ def np_random(seed=None) -> np.random.Generator:
 class EpisodeSampler:
     def __init__(self, num_envs: int, *, domain_rand: bool, dynamics_rand: bool = False, camera_rand: bool = False,
                  accept_start_angle_deg: float = 60.0, num_tris_distractors: int = 12,
-                 color_ground=(0.15, 0.15, 0.15), color_sky=BLUE_SKY, user_tile_start=None, randomization_config=None):
+                 color_ground=(0.15, 0.15, 0.15), color_sky=BLUE_SKY, user_tile_start=None, randomization_config=None,
+                 nav: bool = False):
         self.n = num_envs
+        self.nav = nav   # DuckietownNav.reset: a goal tile drawn after the spawn loop
         self.domain_rand = domain_rand
         self.dynamics_rand = dynamics_rand
         self.camera_rand = camera_rand
@@ -239,7 +241,21 @@ class EpisodeSampler:
                         nxt.append(k)
                     off += m
             todo = nxt
+        if self.nav:   # DuckietownNav.reset (envs/duckietown_env.py:97-111, randint read as integers)
+            for k, e in enumerate(envs):
+                recs[k]["goal"] = self._draw_goal(self.rngs[e], maps[k], recs[k]["pos_x"], recs[k]["pos_z"])
         keys = ["pos_x", "pos_z", "angle", "wheel_dist", "trim", "cam_height", "cam_angle_deg", "cam_fov_y_deg",
                 "cam_noise", "horizon_color", "light_ambient", "light_diffuse", "light_pos", "light_stale",
-                "ground_color", "obj_hidden"]
+                "ground_color", "obj_hidden"] + (["goal"] if self.nav else [])
         return {k: np.array([r[k] for r in recs]) for k in keys}
+
+    @staticmethod
+    def _draw_goal(rng, md: MapData, x: float, z: float) -> tuple:
+        """A drivable tile other than get_grid_coords((x, 0, z)) (S:1134), drawn until one is."""
+        if len(md.drivable_tiles) < 2:   # assert len(self.drivable_tiles) > 1, envs/duckietown_env.py:106
+            raise ValueError("navigation needs a map with at least two drivable tiles")
+        start = (math.floor(x / md.tile_size), math.floor(z / md.tile_size))
+        while True:
+            goal = tuple(md.drivable_tiles[int(rng.integers(0, len(md.drivable_tiles)))])
+            if goal != start:
+                return goal

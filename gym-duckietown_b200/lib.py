@@ -18,8 +18,12 @@ DTS_ABI_VERSION = 3
 ACTION_PWM, ACTION_VEL_STEER = 0, 1
 FLAG_AUTO_RESET, FLAG_DOMAIN_RAND, FLAG_DISTORTION, FLAG_DYNAMICS_RAND, FLAG_TESSELLATE = 1, 2, 4, 8, 16
 FLAG_CAMERA_RAND = 32
-IN_PROGRESS, INVALID_POSE, MAX_STEPS = 0, 1, 2
-DONE_CODE_STR = {0: "in-progress", 1: "invalid-pose", 2: "max-steps-reached"}  # S:1685-1705
+FLAG_NAV = 64
+IN_PROGRESS, INVALID_POSE, MAX_STEPS, GOAL_REACHED = 0, 1, 2, 3
+# the done codes' names, by value (S:1685-1705; "goal-reached" is DuckietownNav's arrival, DTS_GOAL_REACHED, which the
+# reference reports through done and the reward alone)
+DONE_CODE_NAMES = ("in-progress", "invalid-pose", "max-steps-reached", "goal-reached")
+DONE_CODE_STR = dict(enumerate(DONE_CODE_NAMES))
 # the occlusion mask's values (DTS_OCC_*, dts_set_occlusion_target), by value
 OCCLUSION_NAMES = ("none", "visible", "occluded", "outside", "unknown")
 # the bird's-eye visibility's values (DTS_BEVVIS_*, dts_set_bev_visibility_target), by value
@@ -195,6 +199,8 @@ def load() -> C.CDLL:
     lib.dts_reset.argtypes = [vp, vp, C.POINTER(EpisodeParams), vp]
     lib.dts_reset_random.argtypes = [vp, vp, vp]
     lib.dts_seed_streams.argtypes = [vp, vp, vp]
+    lib.dts_set_goals.argtypes = [vp, vp, vp, vp]
+    lib.dts_get_goals.argtypes = [vp, C.POINTER(vp), C.POINTER(vp)]
     lib.dts_step.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.dts_step_terminal.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.dts_render.argtypes = [vp, vp, vp]
@@ -253,7 +259,7 @@ def load() -> C.CDLL:
     return lib
 
 
-EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_fisheye_luts", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_step",
+EXPORTS = ["dts_create", "dts_upload_map", "dts_set_fisheye_lut", "dts_set_fisheye_luts", "dts_set_rectify_lut", "dts_reset", "dts_seed_streams", "dts_reset_random", "dts_set_goals", "dts_get_goals", "dts_step",
            "dts_step_terminal", "dts_render", "dts_get_state", "dts_query_poses", "dts_assign_maps", "dts_set_resize", "dts_set_resize_filter", "dts_set_render_mode", "dts_set_depth_target", "dts_set_label_target", "dts_set_marking_target", "dts_set_bev_target", "dts_render_bev", "dts_set_scan_target", "dts_render_scan", "dts_set_flow_target", "dts_set_occlusion_target", "dts_set_bev_visibility_target", "dts_get_frame_cameras", "dts_set_object_target", "dts_render_objects", "dts_object_pixels", "dts_set_lane_path_target", "dts_render_lane_path", "dts_resize_frames", "dts_blend4", "dts_set_timing", "dts_status", "dts_state_info", "dts_save_state", "dts_load_state", "dts_profile_enable", "dts_profile_read", "dts_get_dyn_state", "dts_set_output_format", "dts_gather_alloc", "dts_gather_open", "dts_gather_next", "dts_comm_load", "dts_comm_unique_id", "dts_comm_init",
            "dts_allgather_obs", "dts_launch_count", "dts_debug_counters", "dts_debug_episode", "dts_debug_frame",
            "dts_debug_streams", "dts_debug_draw", "dts_last_error", "dts_destroy"]
@@ -468,6 +474,17 @@ class Sim:
     def reset_random(self, mask_ptr: Optional[int], stream: int = 0):
         self._check(self.lib.dts_reset_random(self.h, mask_ptr, stream), "dts_reset_random")
 
+    def set_goals(self, mask_ptr: Optional[int], goals_ptr: int, stream: int = 0):
+        """The goal tiles of a host reset, int16 [num_envs][2] on the device, for the masked envs (dts_set_goals)."""
+        self._check(self.lib.dts_set_goals(self.h, mask_ptr, goals_ptr, stream), "dts_set_goals")
+
+    def goal_arrays(self) -> dict:
+        """Every env's goal tile, the library's uint8 [num_envs] arrays goal_i and goal_j (dts_get_goals)."""
+        gi, gj = C.c_void_p(), C.c_void_p()
+        self._check(self.lib.dts_get_goals(self.h, C.byref(gi), C.byref(gj)), "dts_get_goals")
+        return {"goal_i": _CudaArray(gi.value, self.cfg.num_envs, np.uint8),
+                "goal_j": _CudaArray(gj.value, self.cfg.num_envs, np.uint8)}
+
     def step(self, actions_ptr: int, obs_ptr: Optional[int], reward_ptr: int, done_ptr: int, stream: int = 0):
         self._check(self.lib.dts_step(self.h, actions_ptr, obs_ptr, reward_ptr, done_ptr, stream), "dts_step")
 
@@ -651,7 +668,7 @@ class Sim:
 
     def status(self) -> int:
         """Sticky status bits, read without synchronising (bit 0: a frame overflowed its render frame memory; bit 1: a
-        load_state met a record naming no uploaded map)."""
+        load_state met a record naming no uploaded map; bit 2: set_goals met a goal that is not a drivable tile)."""
         return int(self.lib.dts_status(self.h))
 
     def state_info(self):

@@ -2,7 +2,8 @@
 one-env `BatchedDuckietownEnv` on the GPU.  Same constructor keywords, attributes and helper methods
 callers rely on (SURVEY.md 1 / 8b): simulator.py:188-232 (Simulator), envs/duckietown_env.py
 (DuckietownEnv), envs/multimap_env.py (MultiMapEnv).  Observations come back as numpy uint8 HxWx3,
-so the reference's wrappers (wrappers.py) work unchanged on top of these classes.
+so the reference's wrappers (wrappers.py) work unchanged on top of these classes.  DuckietownLF and DuckietownNav are
+the two tasks of envs/duckietown_env.py.
 """
 from __future__ import annotations
 
@@ -149,7 +150,8 @@ class Simulator(Env):
         misc = self.get_agent_info(st)
         code = int(st["done_code"])
         misc["Simulator"]["msg"] = {0: "", 1: "Stopping the simulator because we are at an invalid pose.",
-                                    2: "Stopping the simulator because we reached max_steps = %s" % self.max_steps}[code]
+                                    2: "Stopping the simulator because we reached max_steps = %s" % self.max_steps,
+                                    3: ""}[code]   # DuckietownNav's arrival sets no message
         return o, float(st["reward"]), bool(code != 0), misc
 
     def render_obs(self, segment: bool = False):
@@ -411,6 +413,38 @@ class DuckietownEnv(Simulator):
         omega_l = (vel - 0.5 * angle * baseline) / self.radius
         info["DuckietownEnv"] = {"k": self.k, "gain": self.gain, "train": self.trim, "radius": self.radius,
                                  "omega_r": omega_r, "omega_l": omega_l}
+        return obs, reward, done, info
+
+
+class DuckietownLF(DuckietownEnv):
+    """The lane-following task (envs/duckietown_env.py:75-86): DuckietownEnv itself."""
+
+
+class DuckietownNav(DuckietownEnv):
+    """The navigation task (envs/duckietown_env.py:89-127) as its author meant it: every reset also draws a goal tile
+    other than the start tile, and the episode ends with reward 1000 when the agent reaches it.  The reference's class
+    cannot run (its reset and step call themselves, and its Generator has no randint); here they are read as calls to
+    DuckietownEnv and `integers`, and the draw and the arrival test run inside the batched env (nav=True)."""
+
+    def __init__(self, **kwargs):
+        DuckietownEnv.__init__(self, nav=True, **kwargs)
+
+    @property
+    def goal_tile(self) -> dict:
+        """The episode's goal tile as the reference's tile dict holds it (S:838-860): "coords" (i, j), one of
+        `drivable_tiles`, "kind", "angle" (0..3) and "drivable".  The reference's dict also holds the tile's GL texture
+        and colour and its curves, which are not given here; and a new dict is returned on every access, so compare
+        goals by their coords, not with `is`."""
+        from .maps import TILE_KINDS
+        i, j = (int(v) for v in self._b.goal_tile[0].tolist())
+        md = self._b.maps[self._map_index()]
+        t = j * md.grid_w + i
+        return {"coords": (i, j), "kind": TILE_KINDS[int(md.tile_kind[t])], "angle": int(md.tile_angle[t]),
+                "drivable": bool(md.tile_drivable[t])}
+
+    def step(self, action):
+        obs, reward, done, info = DuckietownEnv.step(self, action)
+        info["goal_tile"] = self.goal_tile
         return obs, reward, done, info
 
 

@@ -25,7 +25,8 @@ extern "C" {
 typedef struct dts_sim dts_sim; /* opaque, one per GPU, not thread-safe */
 
 /* done_code values (simulator.py:1685-1705 DoneRewardInfo.done_code) */
-enum { DTS_IN_PROGRESS = 0, DTS_INVALID_POSE = 1, DTS_MAX_STEPS = 2 };
+enum { DTS_IN_PROGRESS = 0, DTS_INVALID_POSE = 1, DTS_MAX_STEPS = 2,
+       DTS_GOAL_REACHED = 3 /* DTS_FLAG_NAV: the step ended on the env's goal tile (envs/duckietown_env.py:119-125) */ };
 /* action_mode */
 enum { DTS_ACTION_PWM = 0,      /* Simulator.step(action=[u_left,u_right])        simulator.py:1669 */
        DTS_ACTION_VEL_STEER = 1 /* DuckietownEnv.step(action=[vel, steering])  envs/duckietown_env.py:36-59 */ };
@@ -36,9 +37,12 @@ enum { DTS_FLAG_AUTO_RESET = 1,   /* done envs are re-spawned on device inside d
        DTS_FLAG_DYNAMICS_RAND = 8,/* simulator.py:224  per-env trim on the motor gains (S:746-748) */
        DTS_FLAG_TESSELLATE = 16,  /* draw every road tile as the literal 7x7 quads of simulator.py:386-507
                                      instead of one quad + analytic lattice lighting (DESIGN.md render spec) */
-       DTS_FLAG_CAMERA_RAND = 32  /* simulator.py:225 camera_rand: device resets apply the drawn camera height / angle
+       DTS_FLAG_CAMERA_RAND = 32, /* simulator.py:225 camera_rand: device resets apply the drawn camera height / angle
                                      / FOV without DTS_FLAG_DOMAIN_RAND too (S:611-614); the calibrations are the
-                                     caller's (dts_set_fisheye_luts) */ };
+                                     caller's (dts_set_fisheye_luts) */
+       DTS_FLAG_NAV = 64          /* DuckietownNav (envs/duckietown_env.py:89-127, its two self-calls read as the parent's
+                                     and randint as integers): every reset also draws a goal tile, and a step that ends
+                                     on it ends the episode with reward 1000 (dts_set_goals, DESIGN.md section 6c) */ };
 
 /* One entry of the reference's domain-randomization table (randomization/randomizer.py:19-89): Randomizer.randomize
  * draws every key of the JSON config in SORTED key order from the env's np_random, whether or not domain_rand is on
@@ -281,6 +285,22 @@ int dts_seed_streams(dts_sim* sim, const uint8_t* mask_host, const uint64_t* str
 /* Simulator.reset() with pose / DR drawn ON THE DEVICE from the env's numpy-compatible stream, draw for draw
  * in the reference's order (np_random.cuh): same seeds -> same episodes as the reference. */
 int dts_reset_random(dts_sim* sim, const uint8_t* mask_dev, void* stream);
+/* DuckietownNav's goal tiles (DTS_FLAG_NAV, DESIGN.md section 6c).  Every reset of a DTS_FLAG_NAV handle draws one for
+ * the env on the device (dts_reset_random and the auto-reset of dts_step / dts_step_terminal), from the env's stream
+ * right after the reset's other draws: repeat (i, j) = drivable_tiles[integers(0, n_drivable)] until (i, j) is not
+ * get_grid_coords of the pose the reset chose.  dts_reset takes host-drawn parameters and draws nothing, so a host reset
+ * hands its goals over with dts_set_goals: goals_dev int16 [num_envs][2] (i, j), DEVICE memory, 2-byte aligned; the
+ * envs of mask_dev (device u8[num_envs]; NULL = all) take theirs.  An entry that is not a drivable tile of its env's
+ * map (off the grid, an empty cell or an undrivable tile) is not taken: that env keeps its goal and status bit 2 is
+ * set (dts_status), after which dts_step and dts_render fail, as for bit 1.  A goal on the start tile is the caller's
+ * choice: the reference's draw never makes it, and the first step then ends the episode.  One launch, stream-ordered
+ * (after the dts_reset it follows on the same stream).
+ * Refused without DTS_FLAG_NAV.  A step of a DTS_FLAG_NAV handle whose pose ends on the goal tile (tile_i, tile_j of
+ * dts_get_state) ends the episode with done_code DTS_GOAL_REACHED and reward 1000 (1010 under DTS_REWARD_DT), whatever
+ * the step's done_code was.  The goal is env state: the snapshot records carry it. */
+int dts_set_goals(dts_sim* sim, const uint8_t* mask_dev, const int16_t* goals_dev, void* stream);
+/* Device pointers to every env's goal tile, uint8 [num_envs] each (0 on a handle without DTS_FLAG_NAV). */
+int dts_get_goals(dts_sim* sim, uint8_t** goal_i_dev, uint8_t** goal_j_dev);
 /* Simulator.step() (simulator.py:1669-1683) for all envs: actions f32[N][2] -> obs u8[N][H][W][3]
  * (NULL = skip rendering), reward f32[N], done u8[N]. All DEVICE pointers. */
 int dts_step(dts_sim* sim, const float* actions_dev, void* obs_dev, float* reward_dev, uint8_t* done_dev,
@@ -650,7 +670,9 @@ int dts_allgather_obs(dts_sim* sim, const void* send_dev, void* recv_dev, uint64
 /* Sticky status, readable WITHOUT synchronising (mapped host words the kernels write): bit 0 = some frame since
  * creation overflowed its render frame memory (prim slab / bin lists) and was left incomplete; bit 1 = a
  * dts_load_state was handed a record whose map_id names no uploaded map (that env was not loaded).  dts_step and
- * dts_render return non-zero once either is set (the call that set it may be one or two calls back). */
+ * dts_render return non-zero once either is set (the call that set it may be one or two calls back); bit 2 = a
+ * dts_set_goals was handed a goal that is not a drivable tile of its env's map (that env kept its goal), with the same
+ * effect. */
 int dts_status(dts_sim* sim);
 /* Snapshots: every env's complete simulator state as one record, saved from and loaded into the library's own arrays
  * on the device, for resuming a run exactly or branching envs from a state.  A record holds everything a step, a reset
@@ -659,7 +681,7 @@ int dts_status(dts_sim* sim);
  *     fifo[DTS_MAX_DELAY][2], pending duty cycles included;
  *   - the simulator-frame pose and the per-step outputs that dts_get_state points to: pos_x pos_z angle speed reward
  *     lane_dist lane_dot lane_angle_rad prox_penalty wheel_dist step_count tile_i tile_j map_id episode done_code
- *     in_lane collided;
+ *     in_lane collided, and the goal tile goal_i goal_j (dts_get_goals; 0 without DTS_FLAG_NAV);
  *   - the env's numpy PCG64 stream (as dts_seed_streams takes it);
  *   - the per-episode render record (camera height / angle / fov and noise, horizon, light, ground colour, hidden
  *     objects: dts_debug_episode's 144 bytes);
